@@ -35,12 +35,14 @@ ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 
 METRIC = "input Msamples/s through forward+filter+inverse at N channels"
-L2_BYTES = 126e6   # B200 L2 (B200_PROFILING.md); the resident input a rank cycles through must exceed it
+L2_BYTES = 50e6    # H100 L2; the resident input a rank cycles through must exceed it
+HBM_GBS = 3350.0   # H100 SXM data-sheet HBM3 bandwidth, the roofline's peak unless MEASURED_PEAKS.json gives a measured one
+DUMP_BYTES = 64_000_000
 
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region (read-only queries every 20 ms)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -483,6 +485,9 @@ def run_ours(args) -> None:
     stride = max(1, nchan // 22)
     chans_chk = sorted(set(list(range(0, nchan, stride)) + [nchan - 1] + _tone_channels(w)))
     o_host = out.cpu().numpy()
+    if args.dump_outputs:
+        cols = np.concatenate([np.arange(cz.bank.out_offset(c), cz.bank.out_offset(c) + w.channels[c].olen) for c in range(nchan)])
+        dump_outputs(args.dump_outputs, o_host[:, cols], rank, world)
     pairs = {}
     for b in blocks_chk:
         for c in chans_chk:
@@ -520,8 +525,8 @@ def run_ours(args) -> None:
     pk = ROOT / "MEASURED_PEAKS.json"
     if pk.exists():
         peaks = json.loads(pk.read_text())
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "6650 GB/s (of fallback, B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", HBM_GBS))
+    peak_src = "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else f"{HBM_GBS:.0f} GB/s (H100 SXM data sheet, not measured)"
     blocks_fwd = B // world if mode in ("allgather", "a2a") else B
     alg_per_kernel = {"fwd_cols": alg_fwd_in * blocks_fwd, "fwd_rows": alg_fwd_out * blocks_fwd, "chan": alg_chan * B}
     kernels = {}
@@ -534,14 +539,10 @@ def run_ours(args) -> None:
                              "alg_gbs": alg_per_kernel.get(name, 0.0) / (per_step * 1e-3) / 1e9 if per_step > 0 else None}
     cand = {k: v for k, v in kernels.items() if k in alg_per_kernel}
     dom = max(cand, key=lambda k: cand[k]["ms_per_step"]) if cand else None
-    traffic = TRAFFIC_NCU.get(w.name, TRAFFIC_NCU if w.name == "cfg2" else {})
     roof = None
     if dom:
         a = kernels[dom]["alg_gbs"]
-        tr = traffic.get(dom) if isinstance(traffic, dict) else None
         roof = {"kernel": dom, "bound": "hbm", "achieved": a, "peak": peak, "unit": "GB/s", "frac": a / peak,
-                "traffic": (tr * blocks_fwd if dom != "chan" else tr * B) if isinstance(tr, (int, float)) else None,
-                "traffic_note": "ncu dram__bytes_read+write per block (profiles/traffic.json) x blocks per step",
                 "peak_source": peak_src,
                 "note": "algorithmic bytes attributed per kernel: fwd_cols = window read, fwd_rows = spectrum "
                         "write (bins*8 B), chan = slices+responses+outputs; the inter-pass buffer earns no credit"}
@@ -566,7 +567,7 @@ def run_ours(args) -> None:
         "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": w.description + (" per GPU" if world > 1 else ""),
                    "blocks_per_step": B, "input_stream_MB": round(host.nbytes / 1e6, 1),
-                   "l2_policy": f"input stream larger than L2 (126 MB) -- this rank cycles through {rank_reads * (nstream // B) / 1e6:.0f} MB "
+                   "l2_policy": f"input stream larger than L2 ({L2_BYTES / 1e6:.0f} MB) -- this rank cycles through {rank_reads * (nstream // B) / 1e6:.0f} MB "
                                 "of it --, consecutive groups cycled; no explicit flush",
                    "plan": cz.master.describe(), "parallelism": par,
                    "value_definition": ("input stream rate" if world == 1 else
@@ -594,12 +595,22 @@ class _Multi:
             self.then()
 
 
-# ncu --set full dram__bytes_read.sum + dram__bytes_write.sum per block and kernel (filled from profiles/ once captured)
-TRAFFIC_NCU: dict = {}
-try:
-    TRAFFIC_NCU = json.loads((ROOT / "profiles" / "traffic.json").read_text())
-except Exception:
-    pass
+def dump_outputs(dirname: str, o_host: np.ndarray, rank: int, world: int) -> None:
+    """The channel outputs of the last timed step, [block][sample] complex with this rank's channels in index order and
+    olen samples each (the row padding left out), as float32 (..., 2) = (re, im) in DIR/outputs.npy.  Above DUMP_BYTES
+    (shared equally by the ranks) a fixed seeded sample of whole blocks is written instead, with their indices in
+    DIR/output_blocks.npy.  With several GPUs every rank writes its own channel group: DIR/outputs_rank<r>.npy, ..."""
+    d = Path(dirname)
+    d.mkdir(parents=True, exist_ok=True)
+    cap = DUMP_BYTES // world
+    per_block = o_host[0].size * 8
+    blocks = np.arange(o_host.shape[0])
+    if o_host.nbytes > cap:
+        keep = max(1, cap // per_block)
+        blocks = np.sort(np.random.default_rng(0).choice(o_host.shape[0], size=keep, replace=False))
+    sfx = f"_rank{rank}" if world > 1 else ""
+    np.save(d / f"outputs{sfx}.npy", np.ascontiguousarray(o_host[blocks]).view(np.float32).reshape(len(blocks), -1, 2))
+    np.save(d / f"output_blocks{sfx}.npy", blocks.astype(np.float64))
 
 
 def run_e2e(args, torch, cz, hpin, dev, rank, world, dist, B, ngroups, w, hist) -> dict:
@@ -749,8 +760,10 @@ def main():
     ap.add_argument("--no-filter-h", action="store_true", help="skip the e2e leg through the filter.h symbols")
     ap.add_argument("--filter-h-blocks", type=int, default=96)
     ap.add_argument("--filter-h-blocks-per-write", type=int, default=1,
-                    help="blocks completed per write_i16filter call (1..ND-1); 1 keeps ND launches in flight: 13.7 GS/s against 7.9-9.1 (2) and 10.0 (3)")
+                    help="blocks completed per write_i16filter call (1..ND-1); 1 keeps ND launches in flight")
     ap.add_argument("--quick", action="store_true", help="sweeps: skip the parity self-check and the e2e legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write the last step's channel outputs to DIR/*.npy (float32, <= 64 MB in all; one file per rank)")
     ap.add_argument("--depth", type=int, default=2, help="spectrum ring depth of the multi-GPU pipeline")
     ap.add_argument("--mg-mode", default="a2a", choices=["spectrum", "spectrum-mc", "input", "allgather", "slices", "a2a"],
                     help="multi-GPU hand-off of the shared forward spectrum, one NCCL collective per step: `allgather` (default) = every "

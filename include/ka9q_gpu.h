@@ -1,4 +1,4 @@
-/* include/ka9q_gpu.h -- low-level C-ABI of libka9qgpu.so: the B200 overlap-save channelizer.
+/* include/ka9q_gpu.h -- low-level C-ABI of libka9qgpu.so: the H100 overlap-save channelizer.
  *
  * Plain pointers and sizes only; no CUDA or torch types in the signatures (streams are passed
  * as void* holding a cudaStream_t, device buffers as void*).  The reference-compatible
@@ -9,7 +9,7 @@
  * Every entry point names the reference code it replaces (paths relative to the ka9q-radio
  * tree, commit 4e0033b4).  All functions return 0 on success, -1 on error (the reference's
  * convention, filter.h:99-118) unless stated; kgpu_last_error() gives the text.
- * There is NO CPU fallback: if no sm_100 device is usable the calls fail.
+ * There is NO CPU fallback: if no sm_90 device is usable the calls fail.
  */
 #ifndef KA9Q_GPU_H
 #define KA9Q_GPU_H 1
@@ -158,11 +158,10 @@ int kgpu_bank_commit(kgpu_bank *b, void *stream);
 int kgpu_use_static_kernels(int on);
 
 /* A/B knobs (0 = shipped default everywhere).  key 13: 4 = column pass of the 1296 x n2 transform on the round-1 12 x 12 x 9
- * kernel instead of the 36 x 36 one; key 10: 6 = row pass of a REAL n1 x 1250 transform on the 10 x 25 x 5 kernel instead of the
- * 50 x 25 one; key 14: 1 = row pass takes the blocks first-to-last (default last-to-first: L2 reuse of the column pass's
- * output); key 15: row pass's L2 prefetch distance in CTAs (0 = one SM count, -1 = off).  The experiments that lost
- * (tile widths, TMA tile store, sub-batched forward, prefetches elsewhere ...) are listed with their numbers in
- * profiles/README.md and are no longer in the library. */
+ * kernel instead of the 36 x 36 one; key 10: 5 = row pass of a REAL n1 x 1250 transform on the 50 x 25 kernel instead of the
+ * 10 x 25 x 5 one; key 14: 1 = row pass takes the blocks first-to-last (default last-to-first: L2 reuse of the column pass's
+ * output); key 15: n > 0 = row pass prefetches the rows of the CTA n later into L2 (default off).  The experiments that lost
+ * (tile widths, TMA tile store, sub-batched forward, prefetches elsewhere ...) are no longer in the library. */
 int kgpu_set_tuning(int key, int value);
 
 /* Diagnostics: device buffer (6 uint64 per CTA of the cols kernel) receiving globaltimer stamps

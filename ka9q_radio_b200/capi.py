@@ -1,6 +1,6 @@
 """ctypes binding of libka9qgpu.so (the C-ABI in include/ka9q_gpu.h).
 
-The shipped path: every call lands in the hand-written sm_100a kernels.  There is no CPU
+The shipped path: every call lands in the hand-written sm_90a kernels.  There is no CPU
 fallback here -- if the shared library is missing or no CUDA device is usable, import/launch
 fails loudly (see load()).  torch is only used by callers for device memory and streams.
 """
@@ -27,7 +27,7 @@ class KgpuError(RuntimeError):
 
 
 def build(force: bool = False) -> None:
-    """Compile the CUDA library in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA library in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     if force or not LIB_PATH.exists():
         subprocess.run(["make", "-C", str(PKG / "csrc"), "-s"], check=True)
 

@@ -1,4 +1,4 @@
-// fft_radix.cuh -- in-register DFT butterflies for the Stockham/DIF stages (sm_100a).
+// fft_radix.cuh -- in-register DFT butterflies for the Stockham/DIF stages (sm_90a).
 //
 // Everything here works on a thread-private float2 x[R] that the compiler keeps in registers
 // (all indices are literals after unrolling).  Primitive radices 2,3,4,5,7 are written out;
@@ -14,33 +14,28 @@
 
 namespace kfft {
 
-// ---- packed complex arithmetic ----------------------------------------------------------------
-// sm_100 has two-wide fp32 instructions (FADD2 / FMUL2 / FFMA2 on an aligned register pair) whose
-// operands take a half swap (.LO_HI), a per-half sign and a scalar broadcast for free.  A float2 IS
-// such a pair, so a complex add is ONE instruction and a complex multiply TWO (instead of 2 and 4):
-// the lane throughput of the FMA pipe is unchanged, but these kernels are bound by instruction
-// issue, not by the pipe (ncu: issue 45-69 %, FMA pipe 34-41 %).  On the host (tests) and with
-// KFFT_PACKED=0 the three primitives are plain scalar code with the same rounding (fmaf / mul / add).
-#ifndef KFFT_PACKED
-#define KFFT_PACKED 1
-#endif
+// ---- complex arithmetic on float2 pairs -------------------------------------------------------
+// Every butterfly is built from three per-half primitives: add, multiply and fused multiply-add,
+// one rounding each.  Hopper has no two-wide fp32 instructions, so each is two scalar instructions;
+// on the device they are the _rn intrinsics, which the compiler never contracts or reassociates, so
+// the rounding of every result is fixed by the source (the host build used by the tests matches it).
 KFFT_HD float2 p_add(float2 a, float2 b) {
-#if defined(__CUDA_ARCH__) && KFFT_PACKED
-  return __fadd2_rn(a, b);
+#if defined(__CUDA_ARCH__)
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 #else
   return make_float2(a.x + b.x, a.y + b.y);
 #endif
 }
 KFFT_HD float2 p_mul(float2 a, float2 b) {
-#if defined(__CUDA_ARCH__) && KFFT_PACKED
-  return __fmul2_rn(a, b);
+#if defined(__CUDA_ARCH__)
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 #else
   return make_float2(a.x * b.x, a.y * b.y);
 #endif
 }
 KFFT_HD float2 p_fma(float2 a, float2 b, float2 c) {  // a*b + c per half, one rounding each
-#if defined(__CUDA_ARCH__) && KFFT_PACKED
-  return __ffma2_rn(a, b, c);
+#if defined(__CUDA_ARCH__)
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 #else
   return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 #endif

@@ -1,4 +1,4 @@
-/* filter_abi.c -- the reference's filter.h surface served by the B200 kernels.
+/* filter_abi.c -- the reference's filter.h surface served by the H100 kernels.
  *
  * Host code stays C, exactly as north_star asks: this file owns the caller-visible state the
  * untouched ka9q-radio sources expect (mirrored input ring, ND-deep job bookkeeping, per-slave

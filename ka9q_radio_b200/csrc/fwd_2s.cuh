@@ -3,8 +3,7 @@
 // fwd_cols_r36.cuh showed (cfg-2, 1296 = 36 x 36) that these kernels are paced by trips through shared memory, not by
 // arithmetic: with two stages a point crosses shared memory once per pass.  This file is the same design with the radices
 // as template parameters, instantiated for the c2c front ends of BASELINE.json (cfg-4, Airspy-class 20 MS/s I/Q:
-// 500 000 = 800 x 625 = (25 x 32) x (25 x 25)), which until now ran on the runtime-plan kernels of fwd_kernels.cuh
-// (10.2 us per block for 0.5 M points, against 11.8 us for the 1.62 M points of cfg-2).
+// 500 000 = 800 x 625 = (25 x 32) x (25 x 25)), which otherwise run on the runtime-plan kernels of fwd_kernels.cuh.
 //
 // Column pass  fwd_cols_2s<FMT, RA, RB>:  column n2 of the n1 x n2 matrix, n1 = RA x RB
 //   stage 0 (fused with the global load, int16 pairs -> float in registers): butterfly j < RB takes x[j + RB m], m < RA,

@@ -1,8 +1,7 @@
 // fwd_cols_r36.cuh -- column pass of the 1296 x n2 two-pass forward transform with TWO fat stages (36 x 36).
 //
-// ncu on fwd_cols_v2 (12 x 12 x 9, profiles/ncu_r02a_summary.txt): the L1TEX data pipe is the busiest unit (57 % of peak on
-// average, `mio_throttle` 4.2 stalls per issue); 53 % of its wavefronts are shared-memory traffic: one store, one
-// load + store and one load per point, plus stage twiddles.  With 1296 = 36 x 36 a point crosses shared memory ONCE
+// fwd_cols_v2 (12 x 12 x 9) is paced by the L1TEX data pipe, and most of its wavefronts are shared-memory traffic: one
+// store, one load + store and one load per point, plus stage twiddles.  With 1296 = 36 x 36 a point crosses shared memory ONCE
 // (stage 0 store, stage 1 load), there is one block barrier instead of two, and the 36-point butterfly is a Good-Thomas
 // 4 x 9 split with no inner twiddles (fft_radix.cuh).  Stage 0 still reads its 36 inputs straight from global memory
 // (int16 pairs -> float in registers) and stage 1 still stores X[k1] * W^{n2 k1} straight to the inter-pass buffer, so the
@@ -13,8 +12,7 @@
 // W_nc^{n2 (t + 36 k')} = A[n2][t] * (W_nc^{36 n2})^{k'}.
 // Shared-memory layout: a column is 36 blocks of 36 points padded to 38 (V128, default) or 37, column pitch = 2 mod 16:
 // stage 0's stores (8 columns x 2 consecutive j) and stage 1's loads are bank-conflict free either way.
-// Measured (tools/kbench.py, cfg-2, us per block): v2 12x12x9 6.32 -> 36x36 5.62 -> + inter-pass rows padded to 128 B 5.39
-// -> + LDS.128 in stage 1 5.30.
+// Inter-pass rows are padded to 128 B and stage 1 loads with LDS.128 (tools/kbench.py compares it with fwd_cols_v2).
 #pragma once
 #include "static_kernels_v2.cuh"
 

@@ -2,8 +2,7 @@
 // real-input split fused into the second.
 //
 // fwd_rows_v2 (10 x 25 x 5) moves every point through shared memory five times (stage 0 load + store, stage 1 load + store,
-// stage 2 load) on top of the TMA fill; ncu (profiles/ncu_r02_final_summary.txt) shows it paced by exactly that traffic
-// (23.6 M shared wavefronts per 32 blocks, `mio_throttle` + `long_scoreboard` the top stalls).  1250 = 50 x 25 needs three:
+// stage 2 load) on top of the TMA fill and is paced by exactly that traffic.  1250 = 50 x 25 needs three:
 //   stage 0, in place:  butterfly j < 25 takes x[j + 25 m], m < 50; output t, times W_1250^{j t}, goes back to x[25 t + j];
 //   stage 1 + split:    the thread of (row pair i, sub-transform t) transforms block t of row a = k1 and block 49 - t of
 //                       row b = n1 - k1 (25 contiguous points each).  Output k' of the first is Z[k], k = k1 + n1 (t + 50 k'),

@@ -1,6 +1,6 @@
 // kgpu.cu -- host side of libka9qgpu.so: plan registry, forward-transform and channel-bank
 // launchers behind the C-ABI declared in include/ka9q_gpu.h.  No CPU fallback anywhere: every
-// entry point either launches the sm_100a kernels or fails with -1.
+// entry point either launches the sm_90a kernels or fails with -1.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdarg.h>
@@ -37,7 +37,7 @@ static int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;  // H100 SXM
   }
   return n;
 }      // experiment knobs (kgpu_set_tuning), 0 = default
@@ -737,11 +737,10 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
   a2.dbg = g_dbg_buf2 ? (unsigned long long *)g_dbg_buf2 : nullptr;
   a2.mid_ld = a1.mid_ld;
   // The row pass reads what the column pass has just written: taking the blocks last-to-first finds the most recent ones
-  // still in L2, and every CTA pulls the rows of the CTA one SM-count later in launch order into L2 while it works, so
-  // that CTA's TMA fill is an L2 hit instead of a DRAM round trip (6.53 -> 6.16 us/block on the 10 x 25 x 5 kernel,
-  // 5.92 on the 50 x 25 one; distances 8 / 32 / 74 / 148 / 222 / 296 / 600: 6.33 / 6.22 / 6.16 / 6.16 / 6.19 / 6.22 / 6.75).
-  a2.rev = g_tuning[14].load() != 1;                                                    // 14=1: first-to-last (A/B)
-  a2.pf_ctas = g_tuning[15].load() == 0 ? sm_count() : std::max(0, g_tuning[15].load());  // 15=-1: off, 15=n: n CTAs ahead
+  // still in L2.  Key 15 = n makes every CTA pull the rows of the CTA n later in launch order into L2 while it works; on
+  // H100 that prefetch costs row-pass time at every distance tried (tools/kbench.py), so it is off by default.
+  a2.rev = g_tuning[14].load() != 1;                   // 14=1: first-to-last (A/B)
+  a2.pf_ctas = std::max(0, g_tuning[15].load());       // 15=n: prefetch n CTAs ahead (A/B)
   dim3 const g2((unsigned)m->n_item_ctas, (unsigned)nblocks);
   {
     ProfScope ps(K_FWD_ROWS, st);
@@ -751,7 +750,7 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
       fwd_rows_2s<25, 25><<<g2s, RS::T, RS::smem, st>>>(a2, m->d_2s_rtw0);
     } else if (use_static && m->static_rows == 1250) {
       size_t const sv2 = sizeof(float2) * (8 * 1250 + 1246);
-      if (a2.real_split && g_tuning[10].load() == 0) {  // default: two fat stages (50 x 25); 10=6: the 10 x 25 x 5 kernel (A/B)
+      if (a2.real_split && g_tuning[10].load() == 5) {  // 10=5: two fat stages (50 x 25) (A/B); default: the 10 x 25 x 5 kernel
         using RS = RowsR50Shape;
         if (halved) fwd_rows_r50<1296, true><<<g2, RS::T, RS::smem, st>>>(a2, tb, m->d_r50_tw0);  // halved <=> 36 x 36 columns in front
         else fwd_rows_r50<0, false><<<g2, RS::T, RS::smem, st>>>(a2, tb, m->d_r50_tw0);

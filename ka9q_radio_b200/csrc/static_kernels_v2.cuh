@@ -1,7 +1,7 @@
 // static_kernels_v2.cuh -- forward passes with the first and last butterfly stage fused into the
 // global load / store.
 //
-// ncu showed the v1 kernels bound by the L1/shared-memory LSU data pipe (77 % of peak): an
+// The v1 kernels are bound by the L1/shared-memory LSU data pipe: an
 // in-shared-memory DIF moves every point through shared memory twice per stage plus once on the
 // way in and once on the way out.  Here the lanes of a warp are interleaved over the tile's 8
 // columns (lane = 8*u' + column), so a warp-wide global access still covers 8 adjacent columns
@@ -75,9 +75,8 @@ __device__ __forceinline__ float i32_to_f32(int v) {
 }
 
 // Round-1 column pass (12 x 12 x 9, two and a half trips through shared memory); fwd_cols_r36.cuh replaced it as the default,
-// it stays selectable (kgpu_set_tuning(13, 4)) as the A/B partner.  Variants measured on it and removed again: 16- and 6-column
-// tiles (7.82 / 10.93 us per block against 6.32), a TMA tensor store of the tile (6.87), table twiddles, an L2 prefetch of
-// the next block's input (no change) -- profiles/README.md.
+// it stays selectable (kgpu_set_tuning(13, 4)) as the A/B partner.  Variants tried on it and removed again: 16- and 6-column
+// tiles, a TMA tensor store of the tile, table twiddles, an L2 prefetch of the next block's input.
 template <int FMT, int N2C = 0>
 __global__ void __launch_bounds__(288, 2) fwd_cols_v2(Pass1Args const a, ColsV2Tables const tb) {
   using P = SPlan<1296, 12, 12, 9>;
@@ -265,8 +264,8 @@ __device__ constexpr float kRowsTw0[3][4][2] = {
 };
 
 // Stage-0 twiddles W^{j t}, j = ul + 32 it, are (4 values loaded once per thread) x (literal W^{32 it t}) instead of 4 loads per
-// butterfly (6.80 -> 6.55 us per block).  Variants measured and removed again: warp-per-column stages 0/1 (6.93), stage-0
-// butterflies in groups of 2 / 4 (6.71 / 6.73), stage-1 twiddles by products (6.62), a persistent double-buffered form (7.37).
+// butterfly.  Variants tried and removed again: warp-per-column stages 0/1, stage-0 butterflies in groups of 2 / 4,
+// stage-1 twiddles by products, a persistent double-buffered form.
 // For REAL masters fwd_rows_r50.cuh is the default now; this kernel serves COMPLEX 1296 x 1250 masters and
 // kgpu_set_tuning(10, 6).
 template <bool REAL_SPLIT, int N1C = 0, bool HALVED = false>
@@ -496,8 +495,7 @@ __global__ void __launch_bounds__(256, 2) fwd_rows_v2(Pass2Args const a, FwdTabl
 // (20) lanes of a warp write contiguous runs.  Shared-memory traffic per point drops from eight
 // accesses to three.  ISB channels need the whole product first and take the v1 path.
 // OSC: instantiated twice so that the default path carries none of the oscillator's registers
-// Measured and removed again: stage-0 twiddles by products (2.12 vs 2.13 us per block at 90 instead of 72 registers), an L2
-// prefetch of a later CTA's slices (2.19 .. 2.36 against 2.12).
+// Tried and removed again: stage-0 twiddles by products (more registers, no gain), an L2 prefetch of a later CTA's slices.
 template <class P, bool OSC = false>
 __global__ void __launch_bounds__(kChanWarps * 32) chan_v2(ChanArgs const a) {
   static_assert(P::nst == 2, "two-stage plans only");

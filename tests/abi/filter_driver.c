@@ -1,9 +1,9 @@
 /* tests/abi/filter_driver.c -- flat, ctypes-friendly driver over the filter.h surface.
  *
- * Compiled twice (tests/abi/Makefile):
- *   driver_gpuhdr.so  against include/ka9q_gpu_filter.h (our header)
- *   driver_refhdr.so  against the REFERENCE's own src/filter.h (only where /root/reference
- *                     exists) -- proves that code built with the reference header, i.e. the
+ * Compiled twice:
+ *   driver_gpuhdr.so  against include/ka9q_gpu_filter.h (our header; tests/abi/Makefile)
+ *   driver_refhdr.so  against the REFERENCE's own src/filter.h (oracle/Makefile, into oracle/_ref/, only where
+ *                     the reference sources exist) -- proves that code built with the reference header, i.e. the
  *                     untouched radiod sources, binds to libka9qgpu.so unchanged.
  * Both link libka9qgpu.so.  Function names match oracle/ref_driver.c so the same Python session
  * class drives the reference library and the GPU library: the parity tests read like the

@@ -1,5 +1,5 @@
-// Host-side check of the butterfly templates (fft_radix.cuh): on the host the packed primitives are plain
-// scalar code with the rounding of FADD2 / FMUL2 / FFMA2, so the algebra (index maps, signs, quarter turns,
+// Host-side check of the butterfly templates (fft_radix.cuh): on the host the add / multiply / fma primitives are
+// plain scalar code with the rounding of the device's __fadd_rn / __fmul_rn / __fmaf_rn, so the algebra (index maps, signs, quarter turns,
 // Good-Thomas / Cooley-Tukey splits) is verified without a GPU.  Built and run by tests/test_capi_cpu.py.
 #include <cmath>
 #include <complex>

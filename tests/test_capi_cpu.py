@@ -78,26 +78,8 @@ def test_no_oracle_in_product():
         assert "oracle" not in txt.replace("no oracle", ""), p
 
 
-def test_bench_reference_arm_runs_on_cpu():
-    """`bench.py --impl reference` (the driver's reference arm) times oracle/_ref (or the port) on the
-    host cores and prints the contract's JSON line; no GPU involved."""
-    import json
-    import subprocess
-    import sys
-    from pathlib import Path
-
-    root = Path(__file__).resolve().parent.parent
-    out = subprocess.run([sys.executable, str(root / "bench.py"), "--impl", "reference", "--steps", "1", "--warmup", "1",
-                          "--ref-blocks", "2"], capture_output=True, text=True, timeout=600, check=True)
-    line = json.loads(out.stdout.strip().splitlines()[-1])
-    assert line["impl"] == "reference" and line["unit"] == "Msamples/s" and line["value"] > 0
-    assert line["e2e"]["value"] == line["value"] and line["e2e"]["h2d_bytes_per_step"] == 0
-    cb = line["cpu_baseline"]
-    assert cb["kind"] in ("reference", "port") and cb["cores"] >= 1 and "sample" in cb
-
-
 def test_butterfly_templates_on_host(tmp_path):
-    """fft_radix.cuh compiled for the HOST (the packed f32x2 primitives fall back to scalar code with the same
+    """fft_radix.cuh compiled for the HOST (the add / multiply / fma primitives are scalar code with the device's
     rounding): every radix the planner can pick, forward and inverse, against a float64 DFT."""
     import shutil
     import subprocess
@@ -108,7 +90,7 @@ def test_butterfly_templates_on_host(tmp_path):
         pytest.skip("nvcc not available")
     src = Path(__file__).resolve().parent / "host" / "dft_host_test.cu"
     exe = tmp_path / "dft_host_test"
-    subprocess.run([nvcc, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_100a,code=sm_100a",
+    subprocess.run([nvcc, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_90a,code=sm_90a",
                     "-o", str(exe), str(src)], check=True, capture_output=True, timeout=600)
     out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0 and "all butterflies ok" in out.stdout, out.stdout[-2000:]

@@ -80,10 +80,8 @@ def test_cfg2_all_channels_32_block_launch(oracle, cuda_dev):
 
 def test_cfg2_quiet_channels_no_worse_than_the_float32_oracle(oracle, cuda_dev):
     """The justification of the -40 dB floor above: against a float64 transform of the same block, the GPU's error on
-    noise-only channels is the same rounding-noise floor as the float32 oracle's.  Measured on a B200 (tools/diag_floor.py,
-    nine quiet channels): oracle max 1.09e-9 / rms 2.9e-10; GPU 1.41e-9 / 3.8e-10 (50 x 25 rows), 1.03e-9 / 3.8e-10
-    (10 x 25 x 5 rows), 0.98e-9 / 3.5e-10 (runtime-plan kernels); spectrum rms error 3.97e-5 (GPU) vs 4.39e-5 (oracle) on
-    max|X| = 7.2e4.  The rms is the statistic (the max of ~4000 noise-like samples moves by +-30 % between kernel variants)."""
+    noise-only channels is the same rounding-noise floor as the float32 oracle's (tools/diag_floor.py prints both).
+    The rms is the statistic (the max of ~4000 noise-like samples moves by +-30 % between kernel variants)."""
     from ka9q_radio_b200 import workloads
     from ka9q_radio_b200.channelizer import Channelizer
 

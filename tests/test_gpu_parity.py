@@ -152,9 +152,9 @@ def test_forward_full_size_vs_oracle(oracle, cuda_dev, static):
 
 @pytest.mark.parametrize("L,M,shape", [(2560000, 640001, "1280 x 1250"), (2592000, 648001, "1296 x 1250")])
 def test_forward_real_1250_columns_row_kernel_variants(oracle, cuda_dev, L, M, shape):
-    """The 50 x 25 row kernel serves every REAL master with 1250 columns: with the 36 x 36 column kernel in front of it
-    (1296 rows, the 1/2 of the split pre-folded) and with the runtime-plan column kernel (any other row count, here 1280);
-    both also against the 10 x 25 x 5 kernel it replaced (tuning 10 = 6).  Two blocks, float input."""
+    """Both row kernels of a REAL master with 1250 columns, the default 10 x 25 x 5 one and the 50 x 25 one (tuning 10 = 5):
+    with the 36 x 36 column kernel in front of them (1296 rows, the 1/2 of the split pre-folded) and with the runtime-plan
+    column kernel (any other row count, here 1280), against the oracle and against each other.  Two blocks, float input."""
     from ka9q_radio_b200 import capi
 
     lib = capi.load()
@@ -167,7 +167,7 @@ def test_forward_real_1250_columns_row_kernel_variants(oracle, cuda_dev, L, M, s
     d = cz.stage_stream(x)
     spec, spec_old = cz.alloc_spectra(2), cz.alloc_spectra(2)
     cz.forward(d, 2, spec)
-    lib.kgpu_set_tuning(10, 6)
+    lib.kgpu_set_tuning(10, 5)
     cz.forward(d, 2, spec_old)
     lib.kgpu_set_tuning(10, 0)
     torch.cuda.synchronize()

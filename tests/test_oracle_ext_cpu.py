@@ -1,8 +1,11 @@
 """CPU suite (no GPU): pins the oracle's restatement of the slice variants and of the per-channel steps after the
-filter (SURVEY.md 8a REAL-out / beam rows, 8f-1 fine tuning + power, 8f-2 noise estimate) against the reference's OWN
-code compiled unmodified: filter.c (oracle/_ref/libka9qref.so) and radio.c's downconvert() with its static
-estimate_noise() (oracle/_ref/libka9qradio.so).  Skipped where /root/reference was never available to build them."""
+filter (SURVEY.md 8a REAL-out / beam rows, 8f-1 fine tuning + power, 8f-2 noise estimate) against the outputs of the
+reference's OWN code compiled unmodified: filter.c (oracle/_ref/libka9qref.so) and radio.c's downconvert() with its
+static estimate_noise() (oracle/_ref/libka9qradio.so), stored in tests/golden/ref_checks.npz by
+tests/golden/make_ref_golden.py (long outputs at a fixed stride)."""
 import ctypes as C
+import functools
+from pathlib import Path
 
 import numpy as np
 import pytest
@@ -10,23 +13,19 @@ import pytest
 from conftest import rel_err
 
 
-def _need_ref(oracle):
-    if not oracle.ref_available():
-        pytest.skip("oracle/_ref not built here")
 
-
-def _need_radio(oracle):
-    if not oracle.radio_available():
-        pytest.skip("oracle/_ref/libka9qradio.so not built here")
+@functools.cache
+def gold():
+    return dict(np.load(Path(__file__).resolve().parent / "golden" / "ref_checks.npz"))
 
 
 # ------------------------------------------------------------------ oscillator ---------------------------------
 @pytest.mark.parametrize("f,r", [(0.0123, 0.0), (-0.25, 0.0), (1e-3, 1e-9), (0.0, 0.0)])
 def test_osc_restatement_vs_reference_osc(oracle, f, r):
-    _need_radio(oracle)
     n = 40000  # crosses two renormalisations (osc.c:15: every 16384 steps)
-    ref = np.empty(n, np.complex128)
-    oracle.radio_lib().rr_osc_run(f, r, n, ref.ctypes.data)
+    j = [(0.0123, 0.0), (-0.25, 0.0), (1e-3, 1e-9), (0.0, 0.0)].index((f, r))
+    st_ref = int(gold()["osc_stride"])
+    ref = gold()[f"osc{j}"]   # the reference's osc.c, every st_ref-th step
     st = oracle.FineTune._S()
     o = oracle.lib()
     o.ko_osc_set(C.byref(st), f, r)
@@ -40,17 +39,36 @@ def test_osc_restatement_vs_reference_osc(oracle, f, r):
     for i in range(n):
         v = o.ko_osc_step(C.byref(st))
         got[i] = complex(v.re, v.im)
+    got = got[::st_ref]
     assert np.abs(got - ref).max() < 1e-10  # FMA contraction differs between the two builds; 4e4 recursive products
     # closed form the GPU epilogue uses: phase_n = n f + r n (n+1) / 2 cycles
-    k = np.arange(n, dtype=np.float64)
+    k = np.arange(n, dtype=np.float64)[::st_ref]
     closed = np.exp(2j * np.pi * ((k * f + r * k * (k + 1) / 2) % 1.0))
     assert np.abs(closed - ref).max() < 1e-8
 
 
 # ------------------------------------------------------------------ downconvert: fine tuning, power, noise ------
-def _downconvert_case(oracle, in_type, L, M, fs, fe_freq, chans, freq_plan, nb):
-    """chans: list of (olen, out_rate, low, high, beta); freq_plan[b][c] = carrier frequency for block b."""
+def downconvert_plan(tag, nb):
+    """freq_plan[b][c] = carrier frequency of channel c for block b"""
+    if tag == "dr":
+        base = [30_017.3, 61_234.5, 90_000.0]  # not on bin centres: non-zero remainders, shifts not divisible by V
+        plan = [list(base) for _ in range(nb)]
+        for b in range(4, nb):       # retune mid-stream: shift changes -> the one-time phase term (radio.c:1494)
+            plan[b][0] = 33_333.3
+        for b in range(6, nb):
+            plan[b][1] = 61_234.5 + 7.25  # same shift, new remainder -> set_osc only
+        return plan
+    plan = [[10.0e6 + 23_456.7, 10.0e6 - 41_234.5] for _ in range(nb)]
+    for b in range(3, nb):
+        plan[b][1] = 10.0e6 - 12_000.0
+    return plan
+
+
+def _downconvert_case(oracle, tag, in_type, L, M, fs, fe_freq, chans, nb):
+    """chans: list of (olen, out_rate, low, high, beta); compared with the reference's downconvert() outputs of the same
+    stream and frequency plan (golden prefix `tag`)."""
     N = L + M - 1
+    freq_plan = downconvert_plan(tag, nb)
     if in_type == oracle.KO_REAL:
         x = oracle.siggen_real(nb * L, 0.1, 0.02, 0.1234, 1.0)
     else:
@@ -59,53 +77,38 @@ def _downconvert_case(oracle, in_type, L, M, fs, fe_freq, chans, freq_plan, nb):
     fts = [oracle.FineTune(L, M, c[1]) for c in chans]
     n0 = [float("nan")] * len(chans)
     worst = dict(bb=0.0, pw=0.0, n0=0.0)
-    with oracle.RadioRef(L, M, in_type, fs, fe_freq) as rr:
-        ids = [rr.add_channel(c[0], c[1], freq_plan[0][i], c[2], c[3], c[4]) for i, c in enumerate(chans)]
-        for b in range(nb):
-            assert rr.write(x[b * L:(b + 1) * L]) == 1
-            X = oracle.forward(oracle.block_window(x, L, M, b))
-            assert rel_err(rr.spectrum(), X) < 1e-6
-            for i, c in enumerate(chans):
-                rr.set_freq(ids[i], freq_plan[b][i])
-                d = rr.downconvert(ids[i])
-                # restatement: radio.c:1437-1441 -> compute_tuning -> slice/IFFT -> noise -> fine tune -> power
-                freq = -(0.0 + (fe_freq - freq_plan[b][i]))
-                rc, shift, rem = oracle.compute_tuning(N, fs, freq)
-                assert rc == 0 and shift == d["shift"] and rem == d["remainder"]
-                y = oracle.channel_block(in_type, X, resp[i], shift)[-c[0]:].copy()
-                est = oracle.estimate_noise(in_type, X, len(resp[i]), shift, fs)
-                n0[i] = est if np.isnan(n0[i]) else n0[i] + 0.10 * (est - n0[i])  # radio.c:1468-1474, Power_alpha
-                pw = fts[i].block(y, shift, rem)
-                worst["bb"] = max(worst["bb"], rel_err(y, d["baseband"]))
-                worst["pw"] = max(worst["pw"], abs(pw - d["bb_power"]) / d["bb_power"])
-                worst["n0"] = max(worst["n0"], abs(n0[i] - d["n0"]) / d["n0"])
+    st = int(gold()["spec_stride"])
+    scal = gold()[f"{tag}_scalars"]   # per block and channel: shift, remainder, bb_power, n0
+    for b in range(nb):
+        X = oracle.forward(oracle.block_window(x, L, M, b))
+        assert np.abs(X[::st] - gold()[f"{tag}_spec"][b]).max() / gold()[f"{tag}_spec_absmax"][b] < 1e-6
+        for i, c in enumerate(chans):
+            d_shift, d_rem, d_pw, d_n0 = scal[b, i]
+            # restatement: radio.c:1437-1441 -> compute_tuning -> slice/IFFT -> noise -> fine tune -> power
+            freq = -(0.0 + (fe_freq - freq_plan[b][i]))
+            rc, shift, rem = oracle.compute_tuning(N, fs, freq)
+            assert rc == 0 and shift == int(d_shift) and rem == d_rem
+            y = oracle.channel_block(in_type, X, resp[i], shift)[-c[0]:].copy()
+            est = oracle.estimate_noise(in_type, X, len(resp[i]), shift, fs)
+            n0[i] = est if np.isnan(n0[i]) else n0[i] + 0.10 * (est - n0[i])  # radio.c:1468-1474, Power_alpha
+            pw = fts[i].block(y, shift, rem)
+            worst["bb"] = max(worst["bb"], rel_err(y[::int(gold()["bb_stride"])], gold()[f"{tag}_bb{i}"][b]))
+            worst["pw"] = max(worst["pw"], abs(pw - d_pw) / d_pw)
+            worst["n0"] = max(worst["n0"], abs(n0[i] - d_n0) / d_n0)
     return worst
 
 
 def test_downconvert_real_master_vs_reference_radio(oracle):
-    _need_radio(oracle)
     L, M, fs = 4800, 1201, 240e3
     chans = [(480, 24000.0, -1 / 3, 1 / 3, 11.0), (240, 12000.0, 50 / 12000, 3000 / 12000, 11.0), (960, 48000.0, -0.4, 0.4, 7.0)]
-    nb = 9
-    base = [30_017.3, 61_234.5, 90_000.0]  # not on bin centres: non-zero remainders, shifts not divisible by V
-    plan = [list(base) for _ in range(nb)]
-    for b in range(4, nb):       # retune mid-stream: shift changes -> the one-time phase term (radio.c:1494)
-        plan[b][0] = 33_333.3
-    for b in range(6, nb):
-        plan[b][1] = 61_234.5 + 7.25  # same shift, new remainder -> set_osc only
-    w = _downconvert_case(oracle, oracle.KO_REAL, L, M, fs, 0.0, chans, plan, nb)
+    w = _downconvert_case(oracle, "dr", oracle.KO_REAL, L, M, fs, 0.0, chans, 9)
     assert w["bb"] < 2e-6 and w["pw"] < 1e-5 and w["n0"] < 1e-5, w
 
 
 def test_downconvert_complex_master_vs_reference_radio(oracle):
-    _need_radio(oracle)
     L, M, fs = 4000, 1001, 200e3
     chans = [(480, 24000.0, -1 / 3, 1 / 3, 11.0), (480, 24000.0, -0.3, 0.2, 9.0)]
-    nb = 7
-    plan = [[10.0e6 + 23_456.7, 10.0e6 - 41_234.5] for _ in range(nb)]
-    for b in range(3, nb):
-        plan[b][1] = 10.0e6 - 12_000.0
-    w = _downconvert_case(oracle, oracle.KO_COMPLEX, L, M, fs, 10.0e6, chans, plan, nb)
+    w = _downconvert_case(oracle, "dc", oracle.KO_COMPLEX, L, M, fs, 10.0e6, chans, 7)
     assert w["bb"] < 2e-6 and w["pw"] < 1e-5 and w["n0"] < 1e-5, w
 
 
@@ -142,47 +145,38 @@ def _ref_exec(oracle, s, ch, shift, olen, real_out):
     return dst, full
 
 
+# (olen, low, high, beta, shift)
+REALOUT_CASES = [(480, 50 / 24000, 0.3, 11.0, 0), (960, 0.01, 0.45, 7.0, 0), (480, -0.2, 0.25, 11.0, 40), (240, 0.05, 0.3, 5.0, -7)]
+# (olen, shift, i weight, q weight)
+BEAM_CASES = [(480, 615, 1.0, 0.0), (480, -615, 0.0, 1.0), (160, 300, 0.6 - 0.2j, 0.3 + 0.7j), (80, 0, 1.0, 1j), (480, 2100, 0.5, -0.5j),
+              (480, -2150, 0.2j, 0.9)]
+
+
 @pytest.mark.parametrize("in_type", ["real", "complex"])
 def test_realout_slaves_vs_reference_library(oracle, in_type):
-    _need_ref(oracle)
     it = oracle.KO_REAL if in_type == "real" else oracle.KO_COMPLEX
     L, M, nb = 4800, 1201, 3
     N = L + M - 1
     x = oracle.siggen_real(nb * L, 0.1, 0.02, 0.0123, 1.0) if it == oracle.KO_REAL else oracle.siggen_complex(nb * L, 0.1, 0.02, 0.0123, 1.0)
-    cases = [(480, 50 / 24000, 0.3, 11.0, 0), (960, 0.01, 0.45, 7.0, 0), (480, -0.2, 0.25, 11.0, 40), (240, 0.05, 0.3, 5.0, -7)]
-    with oracle.RefSession(L, M, it) as s:
-        ids = [s.add_channel(c[0], c[1], c[2], c[3], out_type=oracle.KO_REAL) for c in cases]
-        for b in range(nb):
-            assert s.write(x[b * L:(b + 1) * L]) == 1
-            X = oracle.forward(oracle.block_window(x, L, M, b))
-            for i, c in zip(ids, cases):
-                pts = c[0] * N // L
-                R = oracle.design_response_realout(pts, c[0], N, it == oracle.KO_REAL, c[1], c[2], c[3])
-                assert rel_err(R[: pts // 2 + 1], s.response(i)[: pts // 2 + 1]) < 1e-6
-                dst, full = _ref_exec(oracle, s, i, c[4], c[0], True)
-                mine = oracle.channel_block_realout(it, X, R, c[4])
-                assert rel_err(mine, full) < 2e-6, (b, c)
-                assert np.array_equal(full[-c[0]:], dst)
+    for b in range(nb):
+        X = oracle.forward(oracle.block_window(x, L, M, b))
+        for i, c in enumerate(REALOUT_CASES):
+            pts = c[0] * N // L
+            R = oracle.design_response_realout(pts, c[0], N, it == oracle.KO_REAL, c[1], c[2], c[3])
+            assert rel_err(R[: pts // 2 + 1][::int(gold()["bb_stride"])], gold()[f"ro_{in_type}_R{i}"]) < 1e-6
+            mine = oracle.channel_block_realout(it, X, R, c[4])
+            assert rel_err(mine[::int(gold()["bb_stride"])], gold()[f"ro_{in_type}_out{i}"][b]) < 2e-6, (b, c)
 
 
 def test_beam_slaves_vs_reference_library(oracle):
-    _need_ref(oracle)
     L, M, nb = 4000, 1001, 3
     N = L + M - 1
     x = oracle.siggen_complex(nb * L, 0.1, 0.02, 0.0123, 1.0)
-    cases = [(480, 615, 1.0, 0.0), (480, -615, 0.0, 1.0), (160, 300, 0.6 - 0.2j, 0.3 + 0.7j), (80, 0, 1.0, 1j), (480, 2100, 0.5, -0.5j), (480, -2150, 0.2j, 0.9)]
     # (a slice that runs into the master's Nyquist bin is left unfinished by the reference's beam loop, filter.c:775: stale memory)
-    with oracle.RefSession(L, M, oracle.KO_COMPLEX) as s:
-        s.R.ref_set_beam.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_double] * 4
-        ids = [s.add_channel(c[0], -0.3, 0.35, 11.0) for c in cases]
-        for i, c in zip(ids, cases):
-            s.R.ref_set_beam(s.h, i, 1, complex(c[2]).real, complex(c[2]).imag, complex(c[3]).real, complex(c[3]).imag)
-        for b in range(nb):
-            assert s.write(x[b * L:(b + 1) * L]) == 1
-            X = oracle.forward(oracle.block_window(x, L, M, b))
-            for i, c in zip(ids, cases):
-                pts = c[0] * N // L
-                R = oracle.design_response(pts, c[0], N, False, -0.3, 0.35, 11.0)
-                dst, full = _ref_exec(oracle, s, i, c[1], c[0], False)
-                mine = oracle.channel_block_beam(X, R, c[1], c[2], c[3])
-                assert rel_err(mine[-c[0]:], dst) < 2e-6, (b, c)
+    for b in range(nb):
+        X = oracle.forward(oracle.block_window(x, L, M, b))
+        for i, c in enumerate(BEAM_CASES):
+            pts = c[0] * N // L
+            R = oracle.design_response(pts, c[0], N, False, -0.3, 0.35, 11.0)
+            mine = oracle.channel_block_beam(X, R, c[1], c[2], c[3])
+            assert rel_err(mine[-c[0]:][::int(gold()["bb_stride"])], gold()[f"beam_out{i}"][b]) < 2e-6, (b, c)

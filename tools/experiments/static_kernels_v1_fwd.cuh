@@ -1,5 +1,5 @@
 // NOT BUILT.  Round-1 forward kernels (in-shared-memory DIF, every stage through shared memory), superseded by
-// static_kernels_v2.cuh (cols 7.99 -> 6.3 us, rows 8.32 -> 6.8 us per block).  Kept for the record of profiles/README.md.
+// static_kernels_v2.cuh.  Kept for the record.
 #pragma once
 namespace kfft {
 // largest divisor of n that is <= cap (compile-time batch sizes without remainders)

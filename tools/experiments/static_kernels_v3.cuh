@@ -1,8 +1,7 @@
 // static_kernels_v3.cuh -- persistent forward passes.
 //
 // The per-CTA timeline of the v2 kernels (tools/phase_trace.py) shows each 8-row / 8-column tile
-// waiting 2.3-2.8 us (rows, TMA) or ~3 us (columns, gather) for its input before a single
-// butterfly issues, and with two CTAs per SM about half of the time only one of them is past that
+// waiting for its input (rows: TMA, columns: gather) before a single butterfly issues, and with two CTAs per SM about half of the time only one of them is past that
 // wait.  Here one CTA stays on each SM and walks over the tiles:
 //   cols  : 288 threads x 2 CTAs per SM as before, but the 36 raw int16 words a thread needs for the
 //           NEXT tile are requested into the (by then dead) registers right after stage 0 of the

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""A/B micro-benchmark of the three kernels on cfg-2 (run under gpurun).
+"""A/B micro-benchmark of the three kernels on cfg-2 (needs a GPU).
 
 usage: kbench.py [--blocks B] [--iters K] variant [variant ...]
 a variant is a comma list of key=value tuning knobs (kgpu_set_tuning), e.g. "10=6" "13=4" "14=1,15=-1" (include/ka9q_gpu.h);

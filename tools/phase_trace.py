@@ -55,7 +55,7 @@ def report(name, raw, labels):
         st = np.sort(u[:, 0]); en = np.sort(u[:, 3])
     tot = occ[:3].sum()
     print("  SM time with 0/1/2 CTAs past the load wait: %.1f %% / %.1f %% / %.1f %%   (no CTA resident: %.1f %%)" % tuple(100 * occ / tot))
-    per_sm = np.bincount(sm, minlength=148)
+    per_sm = np.bincount(sm, minlength=torch.cuda.get_device_properties(dev).multi_processor_count)
     print("  CTAs per SM: min %d max %d" % (per_sm.min(), per_sm.max()))
 
 report("COLS v2", dbg, ("load + stage 0", "stage 1", "stage 2 + store", "total"))

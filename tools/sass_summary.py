@@ -1,14 +1,14 @@
 #!/usr/bin/env python3
-"""Static SASS evidence for the default kernels of libka9qgpu.so: opcode mix and the Blackwell-specific mnemonics
-(UBLKCP = cp.async.bulk / TMA, SYNCS = mbarrier, FFMA2/FADD2/FMUL2 = packed f32x2, LDS.128).  No GPU needed."""
+"""Static SASS evidence for the default kernels of libka9qgpu.so: opcode mix and the Hopper-specific mnemonics
+(UBLKCP = cp.async.bulk / TMA, SYNCS = mbarrier, LDS.128).  No GPU needed."""
 import collections, re, subprocess, sys
 from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
 so = ROOT / "ka9q_radio_b200" / "libka9qgpu.so"
 names = subprocess.run(["cuobjdump", "-elf", str(so)], capture_output=True, text=True).stdout
 want = {"fwd_cols_r36<int16, 1250> (column pass, default)": r"_ZN4kfft12fwd_cols_r36ILi1ELi1250ELb1EE\w+",
-        "fwd_rows_r50<1296, halved> (row pass 50 x 25 + real split, default)": r"_ZN4kfft12fwd_rows_r50ILi1296ELb1EE\w+",
-        "fwd_rows_v2<real, 1296, halved> (row pass 10 x 25 x 5, tuning 10=6)": r"_ZN4kfft11fwd_rows_v2ILb1ELi1296ELb1ELb0ELi0ELb1ELb0EE\w+",
+        "fwd_rows_r50<1296, halved> (row pass 50 x 25 + real split, tuning 10=5)": r"_ZN4kfft12fwd_rows_r50ILi1296ELb1EE\w+",
+        "fwd_rows_v2<real, 1296, halved> (row pass 10 x 25 x 5, default)": r"_ZN4kfft11fwd_rows_v2ILb1ELi1296ELb1ELb0ELi0ELb1ELb0EE\w+",
         "fwd_cols_2s<int16, 25, 32> (cfg-4 column pass)": r"_ZN4kfft11fwd_cols_2sILi1ELi25ELi32EE\w+",
         "fwd_rows_2s<25, 25> (cfg-4 row pass)": r"_ZN4kfft11fwd_rows_2sILi25ELi25EE\w+",
         "chan_v2<600 = 24 x 25> (channels, default)": r"_ZN4kfft7chan_v2INS_5SPlanILi600EJLi24ELi25EEEELb0ELb0EE\w+"}
@@ -28,5 +28,5 @@ for title, pat in want.items():
     print("  symbol", sym)
     print("  instructions", sum(ops.values()))
     print("  opcode mix", ", ".join(f"{k} {v}" for k, v in ops.most_common(18)))
-    ev = {k: v for k, v in full.items() if k.startswith(("UBLKCP", "SYNCS", "LDS.128", "LDS.64", "STS.64", "LDG", "STG", "FFMA2", "FADD2", "FMUL2", "UTMA", "I2FP"))}
+    ev = {k: v for k, v in full.items() if k.startswith(("UBLKCP", "SYNCS", "LDS.128", "LDS.64", "STS.64", "LDG", "STG", "UTMA", "I2FP"))}
     print("  evidence", ", ".join(f"{k} {v}" for k, v in sorted(ev.items())))
