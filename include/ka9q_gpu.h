@@ -154,20 +154,10 @@ int kgpu_bank_fm_front(kgpu_bank *b, const void *d_out, long out_pitch, int nblo
 /* Push pending channel changes (shift/filter/enable) to the device now, ordered after `stream`. */
 int kgpu_bank_commit(kgpu_bank *b, void *stream);
 /* Testing aid: 0 forces the generic runtime-plan kernels even where a compile-time specialised
- * kernel exists (both are parity-tested). Default 1. */
+ * kernel exists (both are parity-tested); it takes effect at the next launch, also for existing masters. Default 1.
+ * A master's forward kernel pair (specialised where its split has one, generic otherwise) is chosen when it is created;
+ * kgpu_master_describe prints it.  Kernel variants that lost on H100 are not in the library. */
 int kgpu_use_static_kernels(int on);
-
-/* A/B knobs (0 = shipped default everywhere).  key 13: 4 = column pass of the 1296 x n2 transform on the round-1 12 x 12 x 9
- * kernel instead of the 36 x 36 one; key 10: 5 = row pass of a REAL n1 x 1250 transform on the 50 x 25 kernel instead of the
- * 10 x 25 x 5 one; key 14: 1 = row pass takes the blocks first-to-last (default last-to-first: L2 reuse of the column pass's
- * output); key 15: n > 0 = row pass prefetches the rows of the CTA n later into L2 (default off).  The experiments that lost
- * (tile widths, TMA tile store, sub-batched forward, prefetches elsewhere ...) are no longer in the library. */
-int kgpu_set_tuning(int key, int value);
-
-/* Diagnostics: device buffer (6 uint64 per CTA of the cols kernel) receiving globaltimer stamps
- * at the phase boundaries; NULL (default) disables. */
-int kgpu_set_debug_buffer(void *d_buf);
-int kgpu_set_debug_buffer_rows(void *d_buf); /* same for the rows kernel */
 
 /* Planner introspection, pure host code (works without a GPU): the in-register radices chosen for
  * a column transform of length len (returns their count, -1 if unplannable) and the two-pass split

@@ -89,9 +89,6 @@ def load() -> C.CDLL:
     L.kgpu_bank_noise.argtypes = [vp, vp, i, d, vp, vp]
     L.kgpu_bank_fm_front.argtypes = [vp, vp, l, i, vp, vp, vp]
     L.kgpu_use_static_kernels.argtypes = [i]
-    L.kgpu_set_tuning.argtypes = [i, i]
-    L.kgpu_set_debug_buffer.argtypes = [vp]
-    L.kgpu_set_debug_buffer_rows.argtypes = [vp]
     L.kgpu_profile_enable.argtypes = [i]
     L.kgpu_profile_name.argtypes = [i]
     L.kgpu_profile_name.restype = C.c_char_p

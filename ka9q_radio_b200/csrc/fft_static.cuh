@@ -13,7 +13,6 @@ namespace kfft {
 
 template <int LEN, int... RS> struct SPlan {
   static constexpr int len = LEN;
-  static constexpr int PB = 0;  // padding block: see Padded<>
   static constexpr int nst = sizeof...(RS);
   static constexpr int rad_arr[sizeof...(RS) > 0 ? sizeof...(RS) : 1] = {RS...};
   static constexpr int rad(int i) { return rad_arr[i]; }
@@ -35,15 +34,6 @@ template <int LEN, int... RS> struct SPlan {
     return p == LEN;
   }
 };
-
-// Same plan with one spare element after every PB_ points of a column (physical index
-// p + p/PB_): turns the even unit-stride of a last stage of radix PB_ into an odd one (no bank
-// conflicts).  Supported when every stage has stride % PB_ == 0 or sub-length <= PB_.
-template <int PB_, class Base> struct Padded : Base {
-  static constexpr int PB = PB_;
-};
-template <class P> constexpr int phys_len() { return P::PB ? P::len + P::len / P::PB : P::len; }
-template <class P> __device__ __forceinline__ int phys_of(int p) { return P::PB ? p + p / P::PB : p; }
 
 // slot holding X[k] after the last stage: digits of k in the mixed radix (r0, r1, ...)
 template <class P, int I = 0> struct SlotOf {
@@ -90,34 +80,11 @@ template <class P, int I> struct StageGeom {
 // TWS: the twiddle table pointer is in shared memory (plain loads) instead of global (__ldg).
 // ILP: butterflies of consecutive loop iterations handled together (loads of all first, then the
 // arithmetic, then the stores) so one warp keeps ILP independent chains in flight.
-// Stage 1 of the 1296 = 12*12*9 plan (sub-length 108, stride 9): with the plain u -> (u/9, u%9)
-// split a half-warp straddles two 108-blocks whose bases differ by 12 (mod 16) and collides.
-// Walk the 12 x 9 (block, j) grid in 4 x 4 patches instead: 108*b mod 16 takes {0,12,8,4} over four
-// consecutive b, plus j in a run of four -> 16 distinct bank pairs.  j = 8 (12 butterflies) is
-// left over and costs three wavefronts per access instead of one.
-template <> struct StageGeom<SPlan<1296, 12, 12, 9>, 1> {
-  static constexpr int R = 12, NSUB = 108, S = 9, NB = 108;
-  static __device__ __forceinline__ void split(int u, int &b, int &j) {
-    if (u < 96) {
-      int const p = u >> 4, w = u & 15;
-      b = 4 * (p >> 1) + (w >> 2);
-      j = 4 * (p & 1) + (w & 3);
-    } else {
-      b = u - 96;
-      j = 8;
-    }
-  }
-};
-
-// TWC: load only the stage twiddles W^{j*t} for t = 1,2,4,8 and form the others as products of two
-// of them (depth <= 2): shared-memory loads are the scarce resource in these kernels, FMAs are not.
-template <class P, bool INV, int I, bool TWS, int ILP, int NL = 32, bool TWC = false>
+template <class P, bool INV, int I, bool TWS, int ILP>
 __device__ __forceinline__ void static_stage(float2 *__restrict__ col, float2 const *__restrict__ tw, int lane) {
   using G = StageGeom<P, I>;
-  constexpr int R = G::R, NSUB = G::NSUB, S = G::S, NB = G::NB;
+  constexpr int R = G::R, NSUB = G::NSUB, S = G::S, NB = G::NB, NL = 32;
   constexpr int ITERS = (NB + NL - 1) / NL;
-  static_assert(P::PB == 0 || S % P::PB == 0 || NSUB <= P::PB, "padding block does not fit this stage");
-  constexpr int SP = (P::PB && S % P::PB == 0) ? S + S / P::PB : S;  // physical element stride
   float2 const *twi = tw + P::tw_off(I);
 #pragma unroll
   for (int it0 = 0; it0 < ITERS; it0 += ILP) {
@@ -132,10 +99,10 @@ __device__ __forceinline__ void static_stage(float2 *__restrict__ col, float2 co
       int b, j;
       G::split(ok[q] ? u : 0, b, j);
       jj[q] = j;
-      p[q] = col + phys_of<P>(b * NSUB + j);
+      p[q] = col + b * NSUB + j;
       if (ok[q]) {
 #pragma unroll
-        for (int m = 0; m < R; m++) x[q][m] = p[q][m * SP];
+        for (int m = 0; m < R; m++) x[q][m] = p[q][m * S];
       }
     }
 #pragma unroll
@@ -143,23 +110,10 @@ __device__ __forceinline__ void static_stage(float2 *__restrict__ col, float2 co
       if (ok[q]) {
         Dft<R, INV>::run(x[q]);
         if (S > 1) {
-          if (TWC && R <= 16) {
-            float2 w[R];
 #pragma unroll
-            for (int t = 1; t < R; t <<= 1) w[t] = TWS ? twi[(t - 1) * S + jj[q]] : __ldg(twi + (t - 1) * S + jj[q]);
-#pragma unroll
-            for (int t = 3; t < R; t++) {
-              int const hb = (t >= 8) ? 8 : (t >= 4) ? 4 : 2;  // highest power of two <= t
-              if (t != hb) w[t] = cmul(w[hb], w[t - hb]);
-            }
-#pragma unroll
-            for (int t = 1; t < R; t++) x[q][t] = INV ? cmulc(x[q][t], w[t]) : cmul(x[q][t], w[t]);
-          } else {
-#pragma unroll
-            for (int t = 1; t < R; t++) {
-              float2 const w = TWS ? twi[(t - 1) * S + jj[q]] : __ldg(twi + (t - 1) * S + jj[q]);
-              x[q][t] = INV ? cmulc(x[q][t], w) : cmul(x[q][t], w);
-            }
+          for (int t = 1; t < R; t++) {
+            float2 const w = TWS ? twi[(t - 1) * S + jj[q]] : __ldg(twi + (t - 1) * S + jj[q]);
+            x[q][t] = INV ? cmulc(x[q][t], w) : cmul(x[q][t], w);
           }
         }
       }
@@ -168,7 +122,7 @@ __device__ __forceinline__ void static_stage(float2 *__restrict__ col, float2 co
     for (int q = 0; q < ILP; q++) {
       if (ok[q]) {
 #pragma unroll
-        for (int t = 0; t < R; t++) p[q][t * SP] = x[q][t];
+        for (int t = 0; t < R; t++) p[q][t * S] = x[q][t];
       }
     }
   }
@@ -186,22 +140,6 @@ template <class P, bool INV, bool TWS, int ILP> struct StaticFft<P, INV, TWS, IL
   static __device__ __forceinline__ void run(float2 *, float2 const *, int) {}
 };
 
-// Same, with a group of WPC warps (NL = 32*WPC lanes) sharing one column; stages are separated
-// by the named barrier `bar_id` that only the group's NL threads use.
-template <class P, bool INV, int WPC, bool TWC = false, int I = 0> struct StaticFftGroup {
-  static __device__ __forceinline__ void run(float2 *col, float2 const *tw, int glane, int bar_id) {
-    static_stage<P, INV, I, true, 1, 32 * WPC, TWC>(col, tw, glane);
-    if (WPC == 1)
-      __syncwarp();
-    else
-      asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "n"(32 * WPC) : "memory");
-    StaticFftGroup<P, INV, WPC, TWC, I + 1>::run(col, tw, glane, bar_id);
-  }
-};
-template <class P, bool INV, int WPC, bool TWC> struct StaticFftGroup<P, INV, WPC, TWC, P::nst> {
-  static __device__ __forceinline__ void run(float2 *, float2 const *, int, int) {}
-};
-
 // ---- shared-memory bulk copies (TMA, 1-D): cp.async.bulk + mbarrier -------------------------
 __device__ __forceinline__ uint32_t smem_u32(void const *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
@@ -215,10 +153,6 @@ __device__ __forceinline__ void bulk_g2s(void *dst, void const *src, uint32_t by
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
-}
-// L2-only bulk prefetch of a contiguous range (address and size multiples of 16)
-__device__ __forceinline__ void bulk_prefetch_l2(void const *src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
   asm volatile(

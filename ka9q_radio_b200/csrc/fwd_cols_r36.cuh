@@ -1,18 +1,19 @@
 // fwd_cols_r36.cuh -- column pass of the 1296 x n2 two-pass forward transform with TWO fat stages (36 x 36).
 //
-// fwd_cols_v2 (12 x 12 x 9) is paced by the L1TEX data pipe, and most of its wavefronts are shared-memory traffic: one
-// store, one load + store and one load per point, plus stage twiddles.  With 1296 = 36 x 36 a point crosses shared memory ONCE
-// (stage 0 store, stage 1 load), there is one block barrier instead of two, and the 36-point butterfly is a Good-Thomas
-// 4 x 9 split with no inner twiddles (fft_radix.cuh).  Stage 0 still reads its 36 inputs straight from global memory
-// (int16 pairs -> float in registers) and stage 1 still stores X[k1] * W^{n2 k1} straight to the inter-pass buffer, so the
-// global access pattern (8 adjacent columns per warp row) is unchanged.
+// A three-stage 12 x 12 x 9 column pass is paced by the L1TEX data pipe, and most of its wavefronts are shared-memory
+// traffic: one store, one load + store and one load per point, plus stage twiddles (on H100 it took 14.4 us per cfg-2 block
+// against 9.8 for this kernel).  With 1296 = 36 x 36 a point crosses shared memory ONCE (stage 0 store, stage 1 load), there
+// is one block barrier instead of two, and the 36-point butterfly is a Good-Thomas 4 x 9 split with no inner twiddles
+// (fft_radix.cuh).  Stage 0 reads its 36 inputs straight from global memory (int16 pairs -> float in registers) and
+// stage 1 stores X[k1] * W^{n2 k1} straight to the inter-pass buffer, 8 adjacent columns per warp row.
 //
 // Twiddles: a thread needs W^{j t}, t = 1..35.  Ten are loaded (t = 1..5 and 6, 12, .., 30), the other 25 are one product
 // each (t = 6a + b): depth 1, so the rounding error stays at one multiply.  Same for the inter-pass factors
 // W_nc^{n2 (t + 36 k')} = A[n2][t] * (W_nc^{36 n2})^{k'}.
-// Shared-memory layout: a column is 36 blocks of 36 points padded to 38 (V128, default) or 37, column pitch = 2 mod 16:
-// stage 0's stores (8 columns x 2 consecutive j) and stage 1's loads are bank-conflict free either way.
-// Inter-pass rows are padded to 128 B and stage 1 loads with LDS.128 (tools/kbench.py compares it with fwd_cols_v2).
+// Shared-memory layout: a column is 36 blocks of 36 points padded to 38, column pitch = 2 mod 16: stage 0's stores
+// (8 columns x 2 consecutive j) and stage 1's loads are bank-conflict free.  Stage 1 reads its 36 contiguous points with
+// 18 LDS.128 (a quarter-warp = the 8 columns of one butterfly: 8 x 16 B at a column pitch of 4 banks = all 32 banks once)
+// instead of 36 LDS.64.  Inter-pass rows are padded to 128 B when the row pass is fwd_rows_v2 (N2C = 1250).
 #pragma once
 #include "static_kernels_v2.cuh"
 
@@ -32,11 +33,14 @@ __device__ __forceinline__ float2 r36_power(float2 const (&wb)[6], float2 const 
   return cmul(wa[a], wb[b]);
 }
 
-// V128: blocks padded to 38 (even) so that stage 1 reads its 36 contiguous points with 18 LDS.128 (a quarter-warp = the 8
-// columns of one butterfly: 8 x 16 B at a column pitch of 4 banks = all 32 banks once) instead of 36 LDS.64.
-template <int FMT, int N2C, bool V128 = true>
-__global__ void __launch_bounds__(288, 2) fwd_cols_r36(Pass1Args const a, ColsR36Tables const tb) {
-  constexpr int R = 36, BLK = V128 ? 38 : 37, CP = V128 ? 1378 : 1346, T = 288;  // 36 * BLK <= CP, CP = 2 mod 16
+struct ColsR36Shape {
+  static constexpr int BLK = 38, CP = 1378, T = 288;  // 36 * BLK <= CP, CP = 2 mod 16; 8 columns x 36 butterflies
+  static constexpr size_t smem = sizeof(float2) * (size_t)(8 * CP + 360 + 80);  // tile, tw0, twB of the 8 columns
+};
+
+template <int FMT, int N2C>
+__global__ void __launch_bounds__(ColsR36Shape::T, 2) fwd_cols_r36(Pass1Args const a, ColsR36Tables const tb) {
+  constexpr int R = 36, BLK = ColsR36Shape::BLK, CP = ColsR36Shape::CP;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // [8][CP]
   float2 *s_tw0 = tile + 8 * CP;                        // [10][36]
@@ -125,18 +129,12 @@ __global__ void __launch_bounds__(288, 2) fwd_cols_r36(Pass1Args const a, ColsR3
   // ---- stage 1 fused with the store: sub-transform t = ul, X[t + 36 k'] * W_nc^{n2 (t + 36 k')} -> mid ------------
   if (col_ok) {
     float2 x[R];
-    float2 const *p = mycol + ul * BLK;
-    if (V128) {
-      float4 const *p4 = reinterpret_cast<float4 const *>(p);
+    float4 const *p4 = reinterpret_cast<float4 const *>(mycol + ul * BLK);
 #pragma unroll
-      for (int m = 0; m < R / 2; m++) {
-        float4 const v = p4[m];
-        x[2 * m] = make_float2(v.x, v.y);
-        x[2 * m + 1] = make_float2(v.z, v.w);
-      }
-    } else {
-#pragma unroll
-      for (int m = 0; m < R; m++) x[m] = p[m];
+    for (int m = 0; m < R / 2; m++) {
+      float4 const v = p4[m];
+      x[2 * m] = make_float2(v.x, v.y);
+      x[2 * m + 1] = make_float2(v.z, v.w);
     }
     Dft<R, false>::run(x);
     float2 wb[6], wa[6];
@@ -151,7 +149,6 @@ __global__ void __launch_bounds__(288, 2) fwd_cols_r36(Pass1Args const a, ColsR3
 #pragma unroll
     for (int k = 1; k < R; k++) dst[(long)(R * k) * ld] = cmul(x[k], cmul(w0, r36_power(wb, wa, k)));
   }
-  (void)T;
 }
 
 }  // namespace kfft

@@ -38,20 +38,9 @@ struct Pass1Args {
   long first_new;       // index (in complex elements) of the first NEW element of a window, for stats
   float2 *mid;          // [block][k1][n2]
   IngestStats *stats;   // or nullptr
-  unsigned long long *dbg;  // or nullptr: per-CTA phase timestamps (globaltimer ns) for tools/phase_trace.py
-  float out_scale;      // v2 kernels: factor folded into the inter-pass twiddle (int16 scale, x0.5 when the split is pre-halved)
-  int mid_ld;           // elements between consecutive k1 rows of `mid` (>= n2; the 36 x 36 kernel pads rows to 128 bytes)
+  float out_scale;      // specialised kernels: factor folded into the inter-pass twiddle (int16 scale, x0.5 when the split is pre-halved)
+  int mid_ld;           // elements between consecutive k1 rows of `mid` (>= n2; padded to 128 bytes for the specialised pairs)
 };
-__device__ __forceinline__ unsigned long long gtimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-__device__ __forceinline__ unsigned sm_id() {
-  unsigned s;
-  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
-  return s;
-}
 
 // exp(-2*pi*i*e/n) from a double-precision sincospi, rounded once
 __device__ __forceinline__ float2 unit_root_f(long e, long n) {
@@ -177,8 +166,26 @@ struct RowItem {   // one unit of pass-2 work: a row, or a mirrored pair of rows
   int kind;
   int row_a;       // k1 of the first row (column 2*i of the tile, or column i for plain rows)
   int row_b;       // k1 of the mirror row N1-row_a (column 2*i+1), pairs only
-  int pad;
 };
+
+// Pass-2 work item p.  REAL: row 0 | pairs (k1, n1-k1) | row n1/2 (n1 even) | empty padding, n1/2 + 1 items in all.
+// COMPLEX: row p | empty padding.
+__device__ __forceinline__ RowItem row_item(int p, int n1, bool real_split) {
+  RowItem it;
+  if (!real_split) {
+    it.kind = p < n1 ? kRowPlain : kRowEmpty;
+    it.row_a = p;
+    it.row_b = 0;
+    return it;
+  }
+  it.row_a = p;
+  it.row_b = n1 - p;
+  if (p == 0) it.kind = kRowSelf0, it.row_b = 0;
+  else if (2 * p < n1) it.kind = kRowPair;
+  else if (2 * p == n1) it.kind = kRowSelfMid, it.row_b = p;
+  else it.kind = kRowEmpty, it.row_a = it.row_b = 0;
+  return it;
+}
 
 struct Pass2Args {
   float2 const *mid;    // [block][k1][n2]
@@ -187,14 +194,10 @@ struct Pass2Args {
   int plan;             // registry index of the length-n2 row plan
   int pitch;
   int real_split;       // 1: REAL master epilogue, 0: plain complex rows
-  RowItem const *items; // [gridDim.x][items_per_cta]
   float2 const *rootD;  // REAL only: W_{2*nc}^{n1*k2} = exp(-i*pi*k2/n2), k2 < n2
   float2 *spec;         // [block][spec_stride]
   long spec_stride;
-  unsigned long long *dbg;  // or nullptr: per-CTA phase timestamps
   int mid_ld;           // see Pass1Args
-  int rev;              // v2 rows: take the blocks of the launch last-to-first (the column pass wrote the last ones most recently: L2)
-  int pf_ctas;          // v2 rows: L2-prefetch the rows of the CTA this many CTAs ahead in launch order (0 = off)
 };
 
 __global__ void __launch_bounds__(kFwdThreads, 2) fwd_rows_kernel(Pass2Args const a) {
@@ -203,12 +206,11 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fwd_rows_kernel(Pass2Args cons
   TilePlan const &pl = c_plans[a.plan];
   int const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int const blk = blockIdx.y;
-  int const ipc = a.real_split ? kTile / 2 : kTile;  // items per CTA
-  RowItem const *items = a.items + (long)blockIdx.x * ipc;
+  int const item0 = blockIdx.x * (a.real_split ? kTile / 2 : kTile);  // items per CTA: 4 row pairs or 8 plain rows
 
   // ---- each warp streams its own row into its column (contiguous 8-byte loads) ------------
   {
-    RowItem const it = items[a.real_split ? warp >> 1 : warp];
+    RowItem const it = row_item(item0 + (a.real_split ? warp >> 1 : warp), a.n1, a.real_split);
     int row = -1;
     if (a.real_split) {
       if ((warp & 1) == 0 && it.kind != kRowEmpty) row = it.row_a;
@@ -239,7 +241,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fwd_rows_kernel(Pass2Args cons
   if (!a.real_split) {
     // plain rows: X[k1 + n1*k2] = Z; 8 adjacent rows -> 64-byte segments
     int const i = tid % kTile, q0 = tid / kTile;
-    RowItem const it = items[i];
+    RowItem const it = row_item(item0 + i, a.n1, false);
     if (it.kind == kRowPlain) {
       float2 const *colp = tile + i * a.pitch;
       constexpr int V = 4, QS = kFwdThreads / kTile;
@@ -261,7 +263,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fwd_rows_kernel(Pass2Args cons
   // ---- REAL epilogue: split the packed transform, 4 adjacent rows -> 32-byte segments -----
   int const i = tid % (kTile / 2), q0 = tid / (kTile / 2);
   int const qstep = kFwdThreads / (kTile / 2);
-  RowItem const it = items[i];
+  RowItem const it = row_item(item0 + i, a.n1, true);
   if (it.kind == kRowEmpty) return;
   float2 const *ca = tile + (2 * i) * a.pitch;
   float2 const *cb = (it.kind == kRowPair) ? tile + (2 * i + 1) * a.pitch : ca;

@@ -9,6 +9,7 @@
 #include <string.h>
 #include <algorithm>
 #include <atomic>
+#include <map>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -22,7 +23,6 @@
 #include "static_kernels_v2.cuh"
 #include "fwd_cols_r36.cuh"
 #include "fwd_2s.cuh"
-#include "fwd_rows_r50.cuh"
 
 using namespace kfft;
 
@@ -30,31 +30,6 @@ using namespace kfft;
 static thread_local std::string g_err;
 static std::atomic<unsigned long long> g_launches{0};
 
-static std::atomic<int> g_tuning[16];
-static int sm_count() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;  // H100 SXM
-  }
-  return n;
-}      // experiment knobs (kgpu_set_tuning), 0 = default
-extern "C" int kgpu_set_tuning(int key, int value) {
-  if (key < 0 || key >= 16) return -1;
-  g_tuning[key].store(value);
-  return 0;
-}
-static void *g_dbg_buf = nullptr, *g_dbg_buf2 = nullptr;  // per-CTA phase timestamps (tools/phase_trace.py)
-extern "C" int kgpu_set_debug_buffer(void *d_buf) {
-  g_dbg_buf = d_buf;
-  return 0;
-}
-extern "C" int kgpu_set_debug_buffer_rows(void *d_buf) {
-  g_dbg_buf2 = d_buf;
-  return 0;
-}
 static std::atomic<int> g_static_on{1};  // tests can force the generic kernels
 extern "C" int kgpu_use_static_kernels(int on) {
   g_static_on.store(on != 0);
@@ -83,6 +58,23 @@ static int fail(char const *fmt, ...) {
       return nullptr;                                                                    \
     }                                                                                    \
   } while (0)
+
+// Lets `func` launch with up to `bytes` of dynamic shared memory.  The limit is one value per kernel and device for the
+// whole process, shared by every master and bank, so it is only ever raised: a smaller request must not take away what
+// another caller already relies on.  It is a ceiling; each launch still asks for its own size, so occupancy is unchanged.
+static int allow_smem(const void *func, size_t bytes) {
+  if (bytes <= 48 * 1024) return 0;
+  static std::mutex mu;
+  static std::map<std::pair<int, const void *>, size_t> granted;
+  int dev = 0;
+  CUDA_OK(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(mu);
+  size_t &g = granted[{dev, func}];
+  if (bytes <= g) return 0;
+  CUDA_OK(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  g = bytes;
+  return 0;
+}
 
 // ------------------------------------------------------------------ per-launch profiling -----
 // When enabled, every kernel launch is bracketed by CUDA events on the launching stream; bench.py
@@ -399,34 +391,136 @@ bool choose_split(long n, Split2 *out) {
 }  // namespace kfft
 
 // ------------------------------------------------------------------ master ------------------
+// The kernel pair of a master is chosen once, in kgpu_master_create, from its split n1 x n2:
+//   COMPLEX 800 x 625       fwd_cols_2s<f, 25, 32> + fwd_rows_2s<25, 25>     (fwd_2s.cuh)
+//   n1 = 1296               column pass fwd_cols_r36                           (fwd_cols_r36.cuh)
+//   n2 = 1250               row pass fwd_rows_v2                               (static_kernels_v2.cuh)
+//   anything else           the runtime-plan kernels fwd_cols_kernel / fwd_rows_kernel (fwd_kernels.cuh)
+// When both passes of a REAL master are specialised (1296 x 1250) the 1/2 of the real split rides on the column pass's
+// inter-pass twiddle, and the inter-pass rows of a specialised pair are padded to 128 bytes.  kgpu_use_static_kernels(0)
+// runs the generic pair instead, at launch time.
+enum ColsKernel { COLS_GENERIC, COLS_R36, COLS_2S };
+enum RowsKernel { ROWS_GENERIC, ROWS_V2, ROWS_2S };
+
 struct kgpu_master {
   int L, M, N, in_type, bins;
   long nc;           // complex points of the two-pass transform (N/2 for REAL, N for COMPLEX)
   Split2 sp;
   int plan1, plan2, pitch1, pitch2;
   long spec_stride;
-  RowItem *d_items = nullptr;
-  int n_item_ctas = 0;
-  float2 *d_rootD = nullptr;
-  float2 *d_rootC = nullptr;                                      // split roots of the row pass
-  float2 *d_twU = nullptr, *d_twT = nullptr;                      // v2 cols kernel (1296 columns)
-  float2 *d_r36_tw0 = nullptr, *d_r36_A = nullptr, *d_r36_B = nullptr;  // 36 x 36 cols kernel
-  int static_cols = 0, static_rows = 0;  // which specialised kernels apply (0 = generic)
-  int static_2s = 0;                     // 1: COMPLEX 800 x 625 on the two-fat-stage kernels of fwd_2s.cuh
-  float2 *d_2s_tw0 = nullptr, *d_2s_A = nullptr, *d_2s_B = nullptr, *d_2s_rtw0 = nullptr;
-  float2 *d_r50_tw0 = nullptr;           // 50 x 25 row kernel (REAL masters with 1250 columns)
+  int n_item_ctas = 0;             // row-pass CTAs per block of the generic and v2 kernels (row_item(): 4 pairs or 8 rows)
+  ColsKernel cols = COLS_GENERIC;
+  RowsKernel rows = ROWS_GENERIC;
+  bool halved = false;             // the 1/2 of the real split is folded into the column pass
+  int n1c = 0, n2c = 0;            // compile-time n1 of fwd_rows_v2, n2 of fwd_cols_r36 (0 = from the arguments)
+  int mid_ld = 0;                  // row pitch of the inter-pass buffer for the chosen pair
+  float2 *d_rootD = nullptr;       // REAL: split roots of the row pass
+  float2 *d_rootC = nullptr;       // REAL with fwd_rows_v2: W_{2nc}^{k1}
+  float2 *d_tw0 = nullptr, *d_twA = nullptr, *d_twB = nullptr;  // tables of fwd_cols_r36 / fwd_cols_2s
+  float2 *d_rtw0 = nullptr;        // stage-0 powers of fwd_rows_2s
   float2 *d_mid = nullptr;
   int mid_blocks = 0;
-  size_t smem1 = 0, smem2 = 0;
+  size_t smem1 = 0, smem2 = 0;     // generic kernels
   // notches
   NotchDev *d_notch = nullptr;
   int n_notch = 0;
   int notch_sequential = 0;
 };
 
-static int set_smem(const void *func, size_t bytes) {
-  if (bytes > 48 * 1024)
-    CUDA_OK(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+// the specialised kernels of a master's pair; f: 0 float input, 1 int16, 2 int16 with de-randomisation or statistics
+using ColsR36Fn = void (*)(Pass1Args, ColsR36Tables);
+using Cols2sFn = void (*)(Pass1Args, Cols2sTables);
+using RowsV2Fn = void (*)(Pass2Args, FwdTables);
+using Cols2s = Cols2sShape<25, 32>;
+using Rows2s = Rows2sShape<25, 25>;
+static ColsR36Fn cols_r36_kernel(kgpu_master const *m, int f) {
+  static ColsR36Fn const k[2][3] = {{fwd_cols_r36<0, 0>, fwd_cols_r36<1, 0>, fwd_cols_r36<2, 0>},
+                                    {fwd_cols_r36<0, 1250>, fwd_cols_r36<1, 1250>, fwd_cols_r36<2, 1250>}};
+  return k[m->n2c == 1250][f];
+}
+static Cols2sFn cols_2s_kernel(int f) {
+  static Cols2sFn const k[3] = {fwd_cols_2s<0, 25, 32>, fwd_cols_2s<1, 25, 32>, fwd_cols_2s<2, 25, 32>};
+  return k[f];
+}
+static RowsV2Fn rows_v2_kernel(kgpu_master const *m) {
+  if (m->in_type == KGPU_REAL) return m->halved ? fwd_rows_v2<true, 1296, true> : fwd_rows_v2<true, 0, false>;
+  return m->n1c ? fwd_rows_v2<false, 1296, false> : fwd_rows_v2<false, 0, false>;
+}
+
+static int upload(float2 **d, std::vector<float2> const &v) {
+  CUDA_OK(cudaMalloc(d, sizeof(float2) * v.size()));
+  CUDA_OK(cudaMemcpy(*d, v.data(), sizeof(float2) * v.size(), cudaMemcpyHostToDevice));
+  return 0;
+}
+
+// kernel choice, tables and shared-memory limits of a master whose split and plans are set
+static int master_setup(kgpu_master *m) {
+  int const n1 = m->sp.n1, n2 = m->sp.n2;
+  bool const real = m->in_type == KGPU_REAL;
+  if (!real && n1 == 800 && n2 == 625) {
+    m->cols = COLS_2S;
+    m->rows = ROWS_2S;
+  } else {
+    if (n1 == 1296) m->cols = COLS_R36, m->n2c = (n2 == 1250) ? 1250 : 0;
+    if (n2 == 1250) m->rows = ROWS_V2, m->n1c = (n1 == 1296) ? 1296 : 0;
+  }
+  m->halved = real && m->cols == COLS_R36 && m->rows == ROWS_V2;
+  bool const padded = m->cols == COLS_2S || (m->cols == COLS_R36 && m->rows == ROWS_V2);  // both kernels know the pitch
+  m->mid_ld = padded ? (n2 + 15) / 16 * 16 : n2;
+  m->n_item_ctas = real ? (n1 / 2 + 1 + 3) / 4 : (n1 + 7) / 8;
+
+  auto root = [](long e, long n) {
+    long double const ang = -2.0L * M_PIl * (long double)(e % n) / (long double)n;
+    return make_float2((float)cosl(ang), (float)sinl(ang));
+  };
+  if (real) {
+    std::vector<float2> rootD((size_t)n2);
+    for (int k2 = 0; k2 < n2; k2++) {
+      long double const ang = -M_PIl * (long double)k2 / (long double)n2;
+      rootD[(size_t)k2] = make_float2((float)cosl(ang), (float)sinl(ang));
+    }
+    if (upload(&m->d_rootD, rootD)) return -1;
+  }
+  if (real && m->rows == ROWS_V2) {
+    std::vector<float2> tC((size_t)n1 / 2 + 1);
+    for (int k1 = 0; k1 <= n1 / 2; k1++) tC[(size_t)k1] = root(k1, 2 * m->nc);
+    if (upload(&m->d_rootC, tC)) return -1;
+  }
+  if (m->cols == COLS_R36) {  // stage-0 powers, inter-pass factors A[n2][t] and the ten powers of W_nc^{36 n2}
+    static int const kPow[10] = {1, 2, 3, 4, 5, 6, 12, 18, 24, 30};
+    std::vector<float2> t0(360), tA((size_t)n2 * 36), tB((size_t)(n2 + 8) * 10, make_float2(0.f, 0.f));
+    for (int e = 0; e < 10; e++)
+      for (int j = 0; j < 36; j++) t0[(size_t)e * 36 + j] = root((long)j * kPow[e], 1296);
+    for (long c = 0; c < n2; c++) {
+      for (int t = 0; t < 36; t++) tA[(size_t)c * 36 + t] = root(c * t, m->nc);
+      for (int e = 0; e < 10; e++) tB[(size_t)c * 10 + e] = root(c * 36 * kPow[e], m->nc);
+    }
+    if (upload(&m->d_tw0, t0) || upload(&m->d_twA, tA) || upload(&m->d_twB, tB)) return -1;
+    for (int f = 0; f < 3; f++)
+      if (allow_smem((const void *)cols_r36_kernel(m, f), ColsR36Shape::smem)) return -1;
+  }
+  if (m->cols == COLS_2S) {  // (25 x 32) x (25 x 25)
+    constexpr int RA = 25, RB = 32, RC = 25, RD = 25;
+    std::vector<float2> t0((size_t)Cols2s::TW0, make_float2(0.f, 0.f)), tA((size_t)n2 * RA),
+        tB((size_t)(n2 + 8) * Cols2s::NP1, make_float2(0.f, 0.f)), r0((size_t)Rows2s::TW0, make_float2(0.f, 0.f));
+    for (int e = 0; e < Cols2s::NP0; e++)
+      for (int j = 0; j < RB; j++) t0[(size_t)e * RB + j] = root((long)j * Pow<RA>::exponent(e), n1);
+    for (long c = 0; c < n2; c++) {
+      for (int t = 0; t < RA; t++) tA[(size_t)c * RA + t] = root(c * t, m->nc);
+      for (int e = 0; e < Cols2s::NP1; e++) tB[(size_t)c * Cols2s::NP1 + e] = root(c * RA * Pow<RB>::exponent(e), m->nc);
+    }
+    for (int e = 0; e < Rows2s::NP0; e++)
+      for (int j = 0; j < RD; j++) r0[(size_t)e * RD + j] = root((long)j * Pow<RC>::exponent(e), n2);
+    if (upload(&m->d_tw0, t0) || upload(&m->d_twA, tA) || upload(&m->d_twB, tB) || upload(&m->d_rtw0, r0)) return -1;
+    for (int f = 0; f < 3; f++)
+      if (allow_smem((const void *)cols_2s_kernel(f), Cols2s::smem)) return -1;
+    if (allow_smem((const void *)fwd_rows_2s<25, 25>, Rows2s::smem)) return -1;
+  }
+  if (m->rows == ROWS_V2 && allow_smem((const void *)rows_v2_kernel(m), RowsV2Shape::smem)) return -1;
+  // the generic pair can run for every master (kgpu_use_static_kernels(0)); a master it does not fit is rejected here
+  if (allow_smem((const void *)fwd_cols_kernel<0>, m->smem1) || allow_smem((const void *)fwd_cols_kernel<1>, m->smem1) ||
+      allow_smem((const void *)fwd_rows_kernel, m->smem2))
+    return -1;
   return 0;
 }
 
@@ -466,131 +560,7 @@ extern "C" kgpu_master *kgpu_master_create(int L, int M, int in_type) {
   m->smem1 = sizeof(float2) * ((size_t)kTile * m->pitch1 + (size_t)kTile * nit);
   m->smem2 = sizeof(float2) * ((size_t)kTile * m->pitch2);
   m->spec_stride = ((long)m->bins + 3) / 4 * 4;
-
-  // pass-2 work items
-  std::vector<RowItem> items;
-  int const n1 = m->sp.n1;
-  if (in_type == KGPU_REAL) {
-    items.push_back({kRowSelf0, 0, 0, 0});
-    for (int k1 = 1; 2 * k1 < n1; k1++) items.push_back({kRowPair, k1, n1 - k1, 0});
-    if (n1 % 2 == 0 && n1 > 1) items.push_back({kRowSelfMid, n1 / 2, n1 / 2, 0});
-    int const ipc = kTile / 2;
-    while (items.size() % ipc) items.push_back({kRowEmpty, 0, 0, 0});
-    m->n_item_ctas = (int)items.size() / ipc;
-  } else {
-    for (int k1 = 0; k1 < n1; k1++) items.push_back({kRowPlain, k1, 0, 0});
-    while (items.size() % kTile) items.push_back({kRowEmpty, 0, 0, 0});
-    m->n_item_ctas = (int)items.size() / kTile;
-  }
-  CUDA_OKP(cudaMalloc(&m->d_items, sizeof(RowItem) * items.size()));
-  CUDA_OKP(cudaMemcpy(m->d_items, items.data(), sizeof(RowItem) * items.size(), cudaMemcpyHostToDevice));
-  if (in_type == KGPU_REAL) {
-    std::vector<float2> rootD((size_t)m->sp.n2);
-    for (int k2 = 0; k2 < m->sp.n2; k2++) {
-      long double const ang = -M_PIl * (long double)k2 / (long double)m->sp.n2;
-      rootD[(size_t)k2] = make_float2((float)cosl(ang), (float)sinl(ang));
-    }
-    CUDA_OKP(cudaMalloc(&m->d_rootD, sizeof(float2) * rootD.size()));
-    CUDA_OKP(cudaMemcpy(m->d_rootD, rootD.data(), sizeof(float2) * rootD.size(), cudaMemcpyHostToDevice));
-  }
-  // specialised kernels for the lengths the configured workloads use
-  {
-    TilePlan const *p1 = host_tile_plan(m->plan1), *p2 = host_tile_plan(m->plan2);
-    if (plan_is<S1296>(p1)) m->static_cols = 1296;
-    if (plan_is<S1250>(p2)) m->static_rows = 1250;
-    int const n2 = m->sp.n2;
-    std::vector<float2> tC((size_t)n1 / 2 + 1);
-    auto root = [](long e, long n) {
-      long double const ang = -2.0L * M_PIl * (long double)(e % n) / (long double)n;
-      return make_float2((float)cosl(ang), (float)sinl(ang));
-    };
-    for (int k1 = 0; k1 <= n1 / 2; k1++) tC[(size_t)k1] = root(k1, 2 * m->nc);
-    if (m->static_cols == 1296) {  // inter-pass factors in the v2 kernel's (u, t2) split
-      std::vector<float2> tU((size_t)(n2 + 8) * 144, make_float2(0.f, 0.f)), tT((size_t)(n2 + 16) * 9 + 32, make_float2(0.f, 0.f));
-      for (long c = 0; c < n2; c++) {
-        for (int u = 0; u < 144; u++) tU[(size_t)c * 144 + u] = root(c * (u / 12 + 12 * (u % 12)), m->nc);
-        for (int t = 0; t < 9; t++) tT[(size_t)c * 9 + t] = root(c * 144 * t, m->nc);
-      }
-      CUDA_OKP(cudaMalloc(&m->d_twU, sizeof(float2) * tU.size()));
-      CUDA_OKP(cudaMalloc(&m->d_twT, sizeof(float2) * tT.size()));
-      CUDA_OKP(cudaMemcpy(m->d_twU, tU.data(), sizeof(float2) * tU.size(), cudaMemcpyHostToDevice));
-      CUDA_OKP(cudaMemcpy(m->d_twT, tT.data(), sizeof(float2) * tT.size(), cudaMemcpyHostToDevice));
-      // 36 x 36 variant: stage-0 powers, inter-pass factors A[n2][t] and the ten powers of W_nc^{36 n2}
-      static int const kPow[10] = {1, 2, 3, 4, 5, 6, 12, 18, 24, 30};
-      std::vector<float2> t0(360), tA36((size_t)n2 * 36), tB10((size_t)(n2 + 8) * 10, make_float2(0.f, 0.f));
-      for (int e = 0; e < 10; e++)
-        for (int j = 0; j < 36; j++) t0[(size_t)e * 36 + j] = root((long)j * kPow[e], 1296);
-      for (long c = 0; c < n2; c++) {
-        for (int t = 0; t < 36; t++) tA36[(size_t)c * 36 + t] = root(c * t, m->nc);
-        for (int e = 0; e < 10; e++) tB10[(size_t)c * 10 + e] = root(c * 36 * kPow[e], m->nc);
-      }
-      CUDA_OKP(cudaMalloc(&m->d_r36_tw0, sizeof(float2) * t0.size()));
-      CUDA_OKP(cudaMalloc(&m->d_r36_A, sizeof(float2) * tA36.size()));
-      CUDA_OKP(cudaMalloc(&m->d_r36_B, sizeof(float2) * tB10.size()));
-      CUDA_OKP(cudaMemcpy(m->d_r36_tw0, t0.data(), sizeof(float2) * t0.size(), cudaMemcpyHostToDevice));
-      CUDA_OKP(cudaMemcpy(m->d_r36_A, tA36.data(), sizeof(float2) * tA36.size(), cudaMemcpyHostToDevice));
-      CUDA_OKP(cudaMemcpy(m->d_r36_B, tB10.data(), sizeof(float2) * tB10.size(), cudaMemcpyHostToDevice));
-    }
-    if (in_type == KGPU_COMPLEX && n1 == 800 && n2 == 625) {  // cfg-4: (25 x 32) x (25 x 25), fwd_2s.cuh
-      using CS = Cols2sShape<25, 32>;
-      using RS = Rows2sShape<25, 25>;
-      constexpr int RA = 25, RB = 32, RC = 25, RD = 25;
-      std::vector<float2> t0((size_t)CS::TW0, make_float2(0.f, 0.f)), tA((size_t)n2 * RA),
-          tB((size_t)(n2 + 8) * CS::NP1, make_float2(0.f, 0.f)), r0((size_t)RS::TW0, make_float2(0.f, 0.f));
-      for (int e = 0; e < CS::NP0; e++)
-        for (int j = 0; j < RB; j++) t0[(size_t)e * RB + j] = root((long)j * Pow<RA>::exponent(e), n1);
-      for (long c = 0; c < n2; c++) {
-        for (int t = 0; t < RA; t++) tA[(size_t)c * RA + t] = root(c * t, m->nc);
-        for (int e = 0; e < CS::NP1; e++) tB[(size_t)c * CS::NP1 + e] = root(c * RA * Pow<RB>::exponent(e), m->nc);
-      }
-      for (int e = 0; e < RS::NP0; e++)
-        for (int j = 0; j < RD; j++) r0[(size_t)e * RD + j] = root((long)j * Pow<RC>::exponent(e), n2);
-      auto up = [](float2 **d, std::vector<float2> const &v) {
-        if (cudaMalloc(d, sizeof(float2) * v.size()) != cudaSuccess) return 1;
-        return cudaMemcpy(*d, v.data(), sizeof(float2) * v.size(), cudaMemcpyHostToDevice) != cudaSuccess ? 1 : 0;
-      };
-      if (up(&m->d_2s_tw0, t0) || up(&m->d_2s_A, tA) || up(&m->d_2s_B, tB) || up(&m->d_2s_rtw0, r0) ||
-          set_smem((const void *)fwd_cols_2s<0, 25, 32>, CS::smem) || set_smem((const void *)fwd_cols_2s<1, 25, 32>, CS::smem) ||
-          set_smem((const void *)fwd_cols_2s<2, 25, 32>, CS::smem) || set_smem((const void *)fwd_rows_2s<25, 25>, RS::smem)) {
-        fail("kgpu_master_create: tables of the 800 x 625 kernels: %s", cudaGetErrorString(cudaGetLastError()));
-        kgpu_master_destroy(m);
-        return nullptr;
-      }
-      m->static_2s = 1;
-    }
-    if (in_type == KGPU_REAL && m->static_rows == 1250) {  // fwd_rows_r50.cuh
-      using RS = RowsR50Shape;
-      std::vector<float2> r0((size_t)RS::TW0, make_float2(0.f, 0.f));
-      for (int e = 0; e < RS::NP0; e++)
-        for (int j = 0; j < RS::RD; j++) r0[(size_t)e * RS::RD + j] = root((long)j * Pow<RS::RC>::exponent(e), 1250);
-      CUDA_OKP(cudaMalloc(&m->d_r50_tw0, sizeof(float2) * r0.size()));
-      CUDA_OKP(cudaMemcpy(m->d_r50_tw0, r0.data(), sizeof(float2) * r0.size(), cudaMemcpyHostToDevice));
-      if (set_smem((const void *)fwd_rows_r50<1296, true>, RS::smem) || set_smem((const void *)fwd_rows_r50<0, false>, RS::smem)) {
-        kgpu_master_destroy(m);
-        return nullptr;
-      }
-    }
-    CUDA_OKP(cudaMalloc(&m->d_rootC, sizeof(float2) * tC.size()));
-    CUDA_OKP(cudaMemcpy(m->d_rootC, tC.data(), sizeof(float2) * tC.size(), cudaMemcpyHostToDevice));
-    size_t const sv1 = sizeof(float2) * (8 * 1298 + 1288 + 80), sv2 = sizeof(float2) * (8 * 1250 + 1246);
-    if (set_smem((const void *)fwd_cols_v2<0>, sv1) || set_smem((const void *)fwd_cols_v2<1>, sv1) ||
-        set_smem((const void *)fwd_cols_v2<2>, sv1) || set_smem((const void *)fwd_rows_v2<true>, sv2) ||
-        set_smem((const void *)fwd_rows_v2<false>, sv2) ||
-        set_smem((const void *)fwd_cols_v2<0, 1250>, sv1) || set_smem((const void *)fwd_cols_v2<1, 1250>, sv1) ||
-        set_smem((const void *)fwd_cols_v2<2, 1250>, sv1) || set_smem((const void *)fwd_rows_v2<true, 1296, true>, sv2) ||
-        set_smem((const void *)fwd_cols_r36<0, 1250>, sizeof(float2) * (8 * 1378 + 440)) ||
-        set_smem((const void *)fwd_cols_r36<1, 1250>, sizeof(float2) * (8 * 1378 + 440)) ||
-        set_smem((const void *)fwd_cols_r36<2, 1250>, sizeof(float2) * (8 * 1378 + 440)) ||
-        set_smem((const void *)fwd_cols_r36<0, 0>, sizeof(float2) * (8 * 1378 + 440)) ||
-        set_smem((const void *)fwd_cols_r36<1, 0>, sizeof(float2) * (8 * 1378 + 440)) ||
-        set_smem((const void *)fwd_cols_r36<2, 0>, sizeof(float2) * (8 * 1378 + 440)) ||
-        set_smem((const void *)fwd_rows_v2<false, 1296, false>, sv2)) {
-      kgpu_master_destroy(m);
-      return nullptr;
-    }
-  }
-  if (set_smem((const void *)fwd_cols_kernel<0>, m->smem1) || set_smem((const void *)fwd_cols_kernel<1>, m->smem1) ||
-      set_smem((const void *)fwd_rows_kernel, m->smem2)) {
+  if (master_setup(m)) {
     kgpu_master_destroy(m);
     return nullptr;
   }
@@ -599,19 +569,12 @@ extern "C" kgpu_master *kgpu_master_create(int L, int M, int in_type) {
 
 extern "C" void kgpu_master_destroy(kgpu_master *m) {
   if (!m) return;
-  cudaFree(m->d_items);
   cudaFree(m->d_rootD);
   cudaFree(m->d_rootC);
-  cudaFree(m->d_twU);
-  cudaFree(m->d_r36_tw0);
-  cudaFree(m->d_r36_A);
-  cudaFree(m->d_r36_B);
-  cudaFree(m->d_2s_tw0);
-  cudaFree(m->d_2s_A);
-  cudaFree(m->d_2s_B);
-  cudaFree(m->d_2s_rtw0);
-  cudaFree(m->d_r50_tw0);
-  cudaFree(m->d_twT);
+  cudaFree(m->d_tw0);
+  cudaFree(m->d_twA);
+  cudaFree(m->d_twB);
+  cudaFree(m->d_rtw0);
   cudaFree(m->d_mid);
   cudaFree(m->d_notch);
   delete m;
@@ -621,32 +584,28 @@ extern "C" int kgpu_master_bins(kgpu_master const *m) { return m ? m->bins : -1;
 extern "C" long kgpu_master_spec_stride(kgpu_master const *m) { return m ? m->spec_stride : -1; }
 extern "C" int kgpu_master_describe(kgpu_master const *m, char *buf, int buflen) {
   if (!m || !buf) return -1;
-  std::string s;
-  char tmp[128];
-  snprintf(tmp, sizeof tmp, "N=%d %s, %ld-point complex two-pass %d x %d; cols radices [", m->N,
-           m->in_type == KGPU_REAL ? "real" : "complex", m->nc, m->sp.n1, m->sp.n2);
-  s += tmp;
-  TilePlan const *p1 = host_tile_plan(m->plan1), *p2 = host_tile_plan(m->plan2);
-  if (m->static_2s) s += "25,32";
-  else if (m->static_cols == 1296) s += "36,36";  // fwd_cols_r36 (the tile plan is what the generic kernels would run)
-  else
-    for (int i = 0; i < p1->nstages; i++) s += std::to_string(p1->radix[i]) + (i + 1 < p1->nstages ? "," : "");
-  s += "] rows radices [";
-  if (m->in_type == KGPU_REAL && m->static_rows == 1250) s += "50,25";
-  else
-  for (int i = 0; i < p2->nstages; i++) s += std::to_string(p2->radix[i]) + (i + 1 < p2->nstages ? "," : "");
-  snprintf(tmp, sizeof tmp, "]; smem %zu/%zu B; grids %d/%d CTAs per block",
-           m->static_2s ? Cols2sShape<25, 32>::smem : m->static_cols == 1296 ? sizeof(float2) * (8 * 1378 + 440) : m->smem1,
-           m->static_2s ? Rows2sShape<25, 25>::smem : (m->in_type == KGPU_REAL && m->static_rows == 1250) ? RowsR50Shape::smem : m->smem2,
-           (m->sp.n2 + kTile - 1) / kTile, m->n_item_ctas);
-  s += tmp;
-  snprintf(buf, (size_t)buflen, "%s", s.c_str());
+  auto radices = [](TilePlan const *p) {
+    std::string r;
+    for (int i = 0; i < p->nstages; i++) r += std::to_string(p->radix[i]) + (i + 1 < p->nstages ? "," : "");
+    return r;
+  };
+  // the tile plans are what the generic kernels run
+  std::string const rc = m->cols == COLS_2S ? "25,32" : m->cols == COLS_R36 ? "36,36" : radices(host_tile_plan(m->plan1));
+  std::string const rr = m->rows == ROWS_2S ? "25,25" : m->rows == ROWS_V2 ? "10,25,5" : radices(host_tile_plan(m->plan2));
+  size_t const s1 = m->cols == COLS_2S ? Cols2s::smem : m->cols == COLS_R36 ? ColsR36Shape::smem : m->smem1;
+  size_t const s2 = m->rows == ROWS_2S ? Rows2s::smem : m->rows == ROWS_V2 ? RowsV2Shape::smem : m->smem2;
+  snprintf(buf, (size_t)buflen, "N=%d %s, %ld-point complex two-pass %d x %d; cols radices [%s] rows radices [%s]; smem %zu/%zu B; "
+           "grids %d/%d CTAs per block", m->N, m->in_type == KGPU_REAL ? "real" : "complex", m->nc, m->sp.n1, m->sp.n2,
+           rc.c_str(), rr.c_str(), s1, s2, (m->sp.n2 + kTile - 1) / kTile, m->n_item_ctas);
   return 0;
 }
 
 // One launch pair (column pass, row pass) over `nblocks` consecutive blocks on stream `st`, inter-pass data in `mid`.
 static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, int derandomize, int nblocks, void *d_spec,
                         void *d_stats, cudaStream_t st, float2 *mid) {
+  bool const use_static = g_static_on.load() != 0;
+  ColsKernel const cols = use_static ? m->cols : COLS_GENERIC;
+  RowsKernel const rows = use_static ? m->rows : ROWS_GENERIC;
   Pass1Args a1;
   a1.in = d_in;
   a1.hop = (m->in_type == KGPU_REAL) ? m->L / 2 : m->L;
@@ -660,66 +619,25 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
   a1.first_new = (m->in_type == KGPU_REAL) ? (m->M - 1) / 2 : (m->M - 1);
   a1.mid = mid;
   a1.stats = (fmt == KGPU_FMT_I16) ? (IngestStats *)d_stats : nullptr;
-  a1.dbg = (unsigned long long *)g_dbg_buf;
-  a1.mid_ld = m->sp.n2;
+  // the specialised column kernels take the int16 scale (and the folded 1/2) on the inter-pass twiddle
+  a1.out_scale = (fmt == KGPU_FMT_I16 ? scale : 1.0f) * (m->halved ? 0.5f : 1.0f);
+  a1.mid_ld = use_static ? m->mid_ld : m->sp.n2;
+  int const f = (fmt != KGPU_FMT_I16) ? 0 : ((derandomize || a1.stats) ? 2 : 1);
   dim3 const g1((unsigned)((m->sp.n2 + kTile - 1) / kTile), (unsigned)nblocks);
-  FwdTables tb;
-  tb.rootC = m->d_rootC;
-  bool const use_static = g_static_on.load() != 0;
-  bool halved = false;
   {
     ProfScope ps(K_FWD_COLS, st);
-    if (use_static && m->static_2s) {
-      int const f = (fmt != KGPU_FMT_I16) ? 0 : ((derandomize || a1.stats) ? 2 : 1);
-      using CS = Cols2sShape<25, 32>;
-      Cols2sTables t4;
-      t4.tw0 = m->d_2s_tw0;
-      t4.twA = m->d_2s_A;
-      t4.twB = m->d_2s_B;
-      a1.out_scale = (fmt == KGPU_FMT_I16) ? scale : 1.0f;
-      a1.mid_ld = (m->sp.n2 + 15) / 16 * 16;
-      if (f == 0) fwd_cols_2s<0, 25, 32><<<g1, CS::T, CS::smem, st>>>(a1, t4);
-      else if (f == 1) fwd_cols_2s<1, 25, 32><<<g1, CS::T, CS::smem, st>>>(a1, t4);
-      else fwd_cols_2s<2, 25, 32><<<g1, CS::T, CS::smem, st>>>(a1, t4);
-    } else if (use_static && m->static_cols == 1296) {
-      int const f = (fmt != KGPU_FMT_I16) ? 0 : ((derandomize || a1.stats) ? 2 : 1);
-      size_t const sv1 = sizeof(float2) * (8 * 1298 + 1288 + 80);
-      ColsV2Tables t2;
-      t2.twU = m->d_twU;
-      t2.twT = m->d_twT;
-      // the int16 scale (and the 1/2 of the real split when the row pass is the v2 kernel too) is
-      // folded into the inter-pass twiddle
-      halved = (m->in_type == KGPU_REAL) && m->static_rows == 1250;
-      a1.out_scale = (fmt == KGPU_FMT_I16 ? scale : 1.0f) * (halved ? 0.5f : 1.0f);
-      if (g_tuning[13].load() == 0) {  // default: two fat stages (36 x 36), one trip through shared memory
-        if (m->sp.n2 == 1250 && m->static_rows == 1250) a1.mid_ld = (m->sp.n2 + 15) / 16 * 16;  // rows padded to 128 B (both kernels know)
-        size_t const sr = sizeof(float2) * (8 * 1378 + 440);
-        ColsR36Tables t3;
-        t3.tw0 = m->d_r36_tw0;
-        t3.twA = m->d_r36_A;
-        t3.twB = m->d_r36_B;
-        if (m->sp.n2 == 1250 && m->static_rows == 1250) {
-          if (f == 0) fwd_cols_r36<0, 1250><<<g1, 288, sr, st>>>(a1, t3);
-          else if (f == 1) fwd_cols_r36<1, 1250><<<g1, 288, sr, st>>>(a1, t3);
-          else fwd_cols_r36<2, 1250><<<g1, 288, sr, st>>>(a1, t3);
-        } else {
-          if (f == 0) fwd_cols_r36<0, 0><<<g1, 288, sr, st>>>(a1, t3);
-          else if (f == 1) fwd_cols_r36<1, 0><<<g1, 288, sr, st>>>(a1, t3);
-          else fwd_cols_r36<2, 0><<<g1, 288, sr, st>>>(a1, t3);
-        }
-      } else if (m->sp.n2 == 1250) {
-        if (f == 0) fwd_cols_v2<0, 1250><<<g1, 288, sv1, st>>>(a1, t2);
-        else if (f == 1) fwd_cols_v2<1, 1250><<<g1, 288, sv1, st>>>(a1, t2);
-        else fwd_cols_v2<2, 1250><<<g1, 288, sv1, st>>>(a1, t2);
-      } else {
-        if (f == 0) fwd_cols_v2<0><<<g1, 288, sv1, st>>>(a1, t2);
-        else if (f == 1) fwd_cols_v2<1><<<g1, 288, sv1, st>>>(a1, t2);
-        else fwd_cols_v2<2><<<g1, 288, sv1, st>>>(a1, t2);
-      }
-    } else if (fmt == KGPU_FMT_I16)
-      fwd_cols_kernel<1><<<g1, kFwdThreads, m->smem1, st>>>(a1);
-    else
-      fwd_cols_kernel<0><<<g1, kFwdThreads, m->smem1, st>>>(a1);
+    switch (cols) {
+      case COLS_2S:
+        cols_2s_kernel(f)<<<g1, Cols2s::T, Cols2s::smem, st>>>(a1, Cols2sTables{m->d_tw0, m->d_twA, m->d_twB});
+        break;
+      case COLS_R36:
+        cols_r36_kernel(m, f)<<<g1, ColsR36Shape::T, ColsR36Shape::smem, st>>>(a1, ColsR36Tables{m->d_tw0, m->d_twA, m->d_twB});
+        break;
+      case COLS_GENERIC:
+        if (f) fwd_cols_kernel<1><<<g1, kFwdThreads, m->smem1, st>>>(a1);
+        else fwd_cols_kernel<0><<<g1, kFwdThreads, m->smem1, st>>>(a1);
+        break;
+    }
   }
   g_launches++;
   Pass2Args a2;
@@ -730,36 +648,24 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
   a2.plan = m->plan2;
   a2.pitch = m->pitch2;
   a2.real_split = (m->in_type == KGPU_REAL);
-  a2.items = m->d_items;
   a2.rootD = m->d_rootD;
   a2.spec = (float2 *)d_spec;
   a2.spec_stride = m->spec_stride;
-  a2.dbg = g_dbg_buf2 ? (unsigned long long *)g_dbg_buf2 : nullptr;
   a2.mid_ld = a1.mid_ld;
-  // The row pass reads what the column pass has just written: taking the blocks last-to-first finds the most recent ones
-  // still in L2.  Key 15 = n makes every CTA pull the rows of the CTA n later in launch order into L2 while it works; on
-  // H100 that prefetch costs row-pass time at every distance tried (tools/kbench.py), so it is off by default.
-  a2.rev = g_tuning[14].load() != 1;                   // 14=1: first-to-last (A/B)
-  a2.pf_ctas = std::max(0, g_tuning[15].load());       // 15=n: prefetch n CTAs ahead (A/B)
   dim3 const g2((unsigned)m->n_item_ctas, (unsigned)nblocks);
   {
     ProfScope ps(K_FWD_ROWS, st);
-    if (use_static && m->static_2s) {
-      using RS = Rows2sShape<25, 25>;
-      dim3 const g2s((unsigned)((m->sp.n1 + 7) / 8), (unsigned)nblocks);
-      fwd_rows_2s<25, 25><<<g2s, RS::T, RS::smem, st>>>(a2, m->d_2s_rtw0);
-    } else if (use_static && m->static_rows == 1250) {
-      size_t const sv2 = sizeof(float2) * (8 * 1250 + 1246);
-      if (a2.real_split && g_tuning[10].load() == 5) {  // 10=5: two fat stages (50 x 25) (A/B); default: the 10 x 25 x 5 kernel
-        using RS = RowsR50Shape;
-        if (halved) fwd_rows_r50<1296, true><<<g2, RS::T, RS::smem, st>>>(a2, tb, m->d_r50_tw0);  // halved <=> 36 x 36 columns in front
-        else fwd_rows_r50<0, false><<<g2, RS::T, RS::smem, st>>>(a2, tb, m->d_r50_tw0);
-      } else if (a2.real_split && halved) fwd_rows_v2<true, 1296, true><<<g2, 256, sv2, st>>>(a2, tb);
-      else if (a2.real_split) fwd_rows_v2<true><<<g2, 256, sv2, st>>>(a2, tb);
-      else if (m->sp.n1 == 1296) fwd_rows_v2<false, 1296, false><<<g2, 256, sv2, st>>>(a2, tb);
-      else fwd_rows_v2<false><<<g2, 256, sv2, st>>>(a2, tb);
-    } else
-      fwd_rows_kernel<<<g2, kFwdThreads, m->smem2, st>>>(a2);
+    switch (rows) {
+      case ROWS_2S:
+        fwd_rows_2s<25, 25><<<dim3((unsigned)((m->sp.n1 + 7) / 8), (unsigned)nblocks), Rows2s::T, Rows2s::smem, st>>>(a2, m->d_rtw0);
+        break;
+      case ROWS_V2:
+        rows_v2_kernel(m)<<<g2, RowsV2Shape::T, RowsV2Shape::smem, st>>>(a2, FwdTables{m->d_rootC});
+        break;
+      case ROWS_GENERIC:
+        fwd_rows_kernel<<<g2, kFwdThreads, m->smem2, st>>>(a2);
+        break;
+    }
   }
   g_launches++;
   CUDA_OK(cudaGetLastError());
@@ -1144,7 +1050,7 @@ static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *ho
   CUDA_OK(cudaMemcpyAsync(dst, host, sizeof(float2) * (size_t)c.points, cudaMemcpyHostToDevice, st));
   if (transform) {
     size_t const sm = sizeof(float2) * (size_t)c.points;
-    if (set_smem((const void *)response_fft_kernel, sm)) return -1;
+    if (allow_smem((const void *)response_fft_kernel, sm)) return -1;
     response_fft_kernel<<<1, 32, sm, st>>>(dst, c.plan);
     g_launches++;
     CUDA_OK(cudaGetLastError());
@@ -1268,7 +1174,7 @@ template <class P> static int launch_chan_v2(ChanArgs const &a, int n, int nbloc
   size_t const sm = sizeof(float2) * ((size_t)(2 * P::len + 4) * kChanWarps + static_tw_count<P>() + 2);
   static bool attr_done = false;
   if (!attr_done) {
-    if (set_smem((const void *)chan_v2<P, false>, sm) || set_smem((const void *)chan_v2<P, true>, sm)) return -1;
+    if (allow_smem((const void *)chan_v2<P, false>, sm) || allow_smem((const void *)chan_v2<P, true>, sm)) return -1;
     attr_done = true;
   }
   dim3 const g((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks);
@@ -1281,7 +1187,7 @@ template <class P> static int launch_chan_static(ChanArgs const &a, int n, int n
   size_t const sm = sizeof(float2) * ((size_t)(2 * P::len + 4) * kChanWarps + static_tw_count<P>() + 2);
   static bool attr_done = false;
   if (!attr_done) {
-    if (set_smem((const void *)chan_static<P>, sm)) return -1;
+    if (allow_smem((const void *)chan_static<P>, sm)) return -1;
     attr_done = true;
   }
   dim3 const g((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks);
@@ -1319,7 +1225,7 @@ static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_ou
     if (plan_is<S1200>(tp)) return launch_chan_static<S1200>(a, n, nblocks, st);
   }
   size_t const sm = sizeof(float2) * (size_t)a.pitch * kChanWarps;
-  if (set_smem((const void *)chan_kernel, sm)) return -1;
+  if (allow_smem((const void *)chan_kernel, sm)) return -1;
   dim3 const g((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks);
   chan_kernel<<<g, kChanWarps * 32, sm, st>>>(a);
   return 0;

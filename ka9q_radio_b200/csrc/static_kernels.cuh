@@ -1,7 +1,6 @@
 // static_kernels.cuh -- shared pieces of the compile-time specialised kernels (fft_static.cuh) and the v1 channel kernel
-// (chan_static: 1200-point and other three-stage plans; the 600 / 300-point channels use chan_v2).  The v1 forward kernels
-// and the persistent v3 experiments live in tools/experiments/ and are not part of the library.  Same arithmetic, same tables and the
-// same argument structs as the generic kernels in fwd_kernels.cuh / chan_kernels.cuh, so parity
+// (chan_static: 1200-point and other three-stage plans; the 600 / 300-point channels use chan_v2).  Same arithmetic, same
+// tables and the same argument structs as the generic kernels in fwd_kernels.cuh / chan_kernels.cuh, so parity
 // tests cover both; what changes is everything around the butterflies:
 //   * literal strides / trip counts, unrolled stage loops, arithmetic digit reversal
 //   * rows and channel inputs arrive by TMA bulk copies (cp.async.bulk -> mbarrier) straight into
@@ -17,12 +16,6 @@ namespace kfft {
 struct FwdTables {
   float2 const *rootC;  // [n1/2+1]   W_{2nc}^{k1}   (REAL split only)
 };
-
-constexpr int static_pitch(int len) {
-  int p = len;
-  while (p % 16 != 2) p++;
-  return p;
-}
 
 // ------------------------------------------------------------------ channels ------------------
 // `order` lists the descriptors that share this plan (mixed output rates are launched per plan).
@@ -152,9 +145,6 @@ template <class P> inline bool plan_is(TilePlan const *p) {
   return true;
 }
 
-using S1296 = SPlan<1296, 12, 12, 9>;
-using S1250 = SPlan<1250, 10, 25, 5>;
-using S1296b = Padded<36, SPlan<1296, 36, 36>>;  // two fat stages; 36-blocks padded to 37 (odd stride)
 using S600 = SPlan<600, 24, 25>;
 using S300 = SPlan<300, 20, 15>;
 using S1200 = SPlan<1200, 12, 10, 10>;

@@ -1,68 +1,22 @@
-// static_kernels_v2.cuh -- forward passes with the first and last butterfly stage fused into the
-// global load / store.
+// static_kernels_v2.cuh -- the 1250-point row pass and the two-stage channel kernels, with the first and last butterfly
+// stage fused into the fill and the global store.
 //
-// The v1 kernels are bound by the L1/shared-memory LSU data pipe: an
-// in-shared-memory DIF moves every point through shared memory twice per stage plus once on the
-// way in and once on the way out.  Here the lanes of a warp are interleaved over the tile's 8
-// columns (lane = 8*u' + column), so a warp-wide global access still covers 8 adjacent columns
-// (one 32/64-byte segment per row) -- which lets
-//   * stage 0 read its R0 inputs straight from global memory (int16 -> float in registers),
-//   * the last stage write its outputs (times the inter-pass twiddle / through the real split)
-//     straight to global memory,
-// leaving one store, one load+store and one load per point in shared memory instead of eight
-// accesses.  With 288 threads the 8 x 1296 tile divides evenly (864 and 1152 butterflies per
-// stage): no idle lanes.  Column pitch = 2 mod 16 keeps every access pattern here free of bank
-// conflicts (8 even column offsets x 2 consecutive butterflies per half-warp).
+// An in-shared-memory DIF moves every point through shared memory twice per stage plus once on the way in and once on the
+// way out, and kernels built that way are bound by the L1/shared-memory LSU data pipe.  Here the lanes of a warp are
+// interleaved over the tile's 8 columns (lane = 8*u' + column), the first stage works on the data as it arrives and the last
+// stage writes its outputs (through the real split, or into the kept samples of a channel) straight to global memory.
+// Column pitch = 2 mod 16 keeps every access pattern free of bank conflicts (8 even column offsets x 2 consecutive
+// butterflies per half-warp).
 #pragma once
 #include "static_kernels.cuh"
 
 namespace kfft {
 
-using S1250v2 = SPlan<1250, 10, 25, 5>;
-
-// twiddles W^{j*t}, t = 1..R-1, for one butterfly: 4 table loads + products (see static_stage TWC)
-template <int R, int S> __device__ __forceinline__ void load_stage_twiddles(float2 const *twi, int j, float2 (&w)[R]) {
-#pragma unroll
-  for (int t = 1; t < R; t <<= 1) w[t] = twi[(t - 1) * S + j];
-#pragma unroll
-  for (int t = 3; t < R; t++) {
-    int const hb = (t >= 16) ? 16 : (t >= 8) ? 8 : (t >= 4) ? 4 : 2;
-    if (t != hb) w[t] = cmul(w[hb], w[t - hb]);
-  }
-}
-
-// pass-2 work item p of the list kgpu.cu builds (row 0 | pairs (k1, n1-k1) | row n1/2 | padding),
-// computed instead of loaded: the row fetch of a CTA does not wait for a table read
-__device__ __forceinline__ RowItem row_item(int p, int n1, bool real_split) {
-  RowItem it;
-  it.pad = 0;
-  if (!real_split) {
-    it.kind = p < n1 ? kRowPlain : kRowEmpty;
-    it.row_a = p;
-    it.row_b = 0;
-    return it;
-  }
-  it.row_a = p;
-  it.row_b = n1 - p;
-  if (p == 0) it.kind = kRowSelf0, it.row_b = 0;
-  else if (2 * p < n1) it.kind = kRowPair;
-  else if (2 * p == n1) it.kind = kRowSelfMid, it.row_b = p;
-  else it.kind = kRowEmpty, it.row_a = it.row_b = 0;
-  return it;
-}
-
-struct ColsV2Tables {
-  float2 const *twU;  // [n2][144]  W_nc^{n2 * kbase(u)}, kbase(u) = u/12 + 12*(u%12)   (u = t0*12 + t1)
-  float2 const *twT;  // [n2][9]    W_nc^{n2 * 144 * t2}
-};
-
-// ------------------------------------------------------------------ pass 1: columns -----------
+// ---- int16 ingest of the specialised column kernels (fwd_cols_r36.cuh, fwd_2s.cuh) -----------
 // FMT 0: float pairs; 1: int16 pairs; 2: int16 pairs + de-randomise + energy/clip statistics.
-// N2C: number of columns as a compile-time constant (0 = read it from the arguments): with it every
-// global address of a thread is one base register plus an immediate.
 // int16 pair -> two floats.  `(float)(short)` compiles to I2F.S16, which issues through the MIO
 // queue to the quarter-rate conversion unit -- the queue the 36 loads and 72 shared-memory accesses
-// of a thread also need (ncu: mio_throttle was the top stall of this kernel).  Sign-extend with
+// of a thread also need (ncu: mio_throttle was the top stall of the column pass).  Sign-extend with
 // PRMT / SHF and convert with I2FP.F32.S32 on the integer pipe instead.
 __device__ __forceinline__ void unpack_i16(int raw, int &lo, int &hi) {
   asm("prmt.b32 %0, %1, 0, 0x9910;" : "=r"(lo) : "r"(raw));  // bytes b0 b1 sign sign
@@ -74,181 +28,6 @@ __device__ __forceinline__ float i32_to_f32(int v) {
   return f;
 }
 
-// Round-1 column pass (12 x 12 x 9, two and a half trips through shared memory); fwd_cols_r36.cuh replaced it as the default,
-// it stays selectable (kgpu_set_tuning(13, 4)) as the A/B partner.  Variants tried on it and removed again: 16- and 6-column
-// tiles, a TMA tensor store of the tile, table twiddles, an L2 prefetch of the next block's input.
-template <int FMT, int N2C = 0>
-__global__ void __launch_bounds__(288, 2) fwd_cols_v2(Pass1Args const a, ColsV2Tables const tb) {
-  using P = SPlan<1296, 12, 12, 9>;
-  constexpr int TC = 8;
-  constexpr int N1 = 1296, PITCH = 1298, UPI = 36 /*butterflies per column per iteration*/;
-  constexpr int R0 = 12, S0 = 108, R1 = 12, NSUB1 = 108, S1 = 9, R2 = 9;
-  constexpr int XS = 1, CS = PITCH;  // element (column c, index X) at tile[X*XS + c*CS]
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // [8][PITCH]
-  float2 *s_tw = tile + TC * PITCH + (TC * PITCH) % 2;  // stage twiddles (1287 entries, padded to 1288), 16-byte aligned
-  float2 *s_twT = s_tw + 1288;                          // [TC][9] (padded to 10 TC)
-  __shared__ __align__(8) uint64_t tbar;
-  TilePlan const &pl = c_plans[a.plan];
-  int const tid = threadIdx.x;
-  int const c = tid % TC, ul = tid / TC;  // column of the tile, butterfly lane 0..35
-  int const c0 = blockIdx.x * TC, blk = blockIdx.y;
-  int const n2 = N2C ? N2C : a.n2;
-  long const nc = N2C ? (long)N1 * N2C : a.nc;
-  unsigned long long *dbg = a.dbg ? a.dbg + 6 * ((long)blockIdx.y * gridDim.x + blockIdx.x) : nullptr;
-  if (dbg && tid == 0) {
-    dbg[0] = gtimer();
-    dbg[5] = sm_id();
-  }
-  int const ncols = min(TC, n2 - c0);
-  bool const col_ok = c < ncols;
-  int const n2g = c0 + c;
-  float2 *mycol = tile + c * CS;
-  if (tid == 0) {
-    mbar_init(&tbar, 1);
-    mbar_fence_init();
-    mbar_expect_tx(&tbar, 1288 * 8 + 10 * TC * 8);
-    bulk_g2s(s_tw, pl.tw, 1288 * 8, &tbar);
-    bulk_g2s(s_twT, tb.twT + (long)c0 * 9, 10 * TC * 8, &tbar);  // table padded by 16 columns + 16 entries
-  }
-  __syncthreads();  // barrier initialised before anybody waits on it
-  // inter-pass factors B'(n2, u) for this thread's four stage-2 butterflies: issued now, used last
-  float2 twU[4];
-#pragma unroll
-  for (int it = 0; it < 4; it++)
-    twU[it] = col_ok ? ldg_stream_f2(tb.twU + (long)n2g * 144 + ul + UPI * it) : make_float2(1.f, 0.f);
-
-  // ---- stage 0 fused with the load: x[j + 108 m], m = 0..11, straight from global ------------
-  unsigned long long energy = 0;
-  unsigned int clips = 0;
-  if (col_ok) {
-    // row of butterfly j = ul + 36 it, input m: j + 108 m  ->  element (ul + 36 it + 108 m) * n2
-    if (FMT == 0) {
-      float2 const *src = reinterpret_cast<float2 const *>(a.in) + (long)blk * a.hop + n2g + (long)ul * n2;
-      float2 x[3][R0];
-#pragma unroll
-      for (int it = 0; it < 3; it++) {
-#pragma unroll
-        for (int m = 0; m < R0; m++) x[it][m] = ldg_stream_f2(src + (long)(UPI * it + S0 * m) * n2);
-      }
-      mbar_wait(&tbar, 0);
-#pragma unroll
-      for (int it = 0; it < 3; it++) {
-        int const j = ul + UPI * it;
-        Dft<R0, false>::run(x[it]);
-        float2 w[R0];
-        load_stage_twiddles<R0, S0>(s_tw, j, w);
-        float2 *d = mycol + j * XS;
-        d[0] = x[it][0];
-#pragma unroll
-        for (int t = 1; t < R0; t++) d[t * S0 * XS] = cmul(x[it][t], w[t]);
-      }
-    } else {
-      int const *src = reinterpret_cast<int const *>(a.in) + (long)blk * a.hop + n2g + (long)ul * n2;
-      int raw[3][R0];
-#pragma unroll
-      for (int it = 0; it < 3; it++) {
-#pragma unroll
-        for (int m = 0; m < R0; m++) raw[it][m] = ldg_stream_b32(src + (long)(UPI * it + S0 * m) * n2);
-      }
-      mbar_wait(&tbar, 0);
-#pragma unroll
-      for (int it = 0; it < 3; it++) {
-        int const j = ul + UPI * it;
-        float2 x[R0];
-#pragma unroll
-        for (int m = 0; m < R0; m++) {
-          int lo, hi;
-          unpack_i16(raw[it][m], lo, hi);
-          if (FMT == 2) {
-            if (a.derandomize) {  // lsb set -> flip bits 1..15 (rx888.c:707-712); on the sign-extended word: bits 1..31
-              lo ^= (lo & 1) ? 0xfffffffe : 0;
-              hi ^= (hi & 1) ? 0xfffffffe : 0;
-            }
-            if (a.stats && (long)(j + S0 * m) * n2 + n2g >= a.first_new) {
-              energy += (unsigned long long)(lo * lo) + (unsigned long long)(hi * hi);
-              clips += (lo > 32766 || lo < -32766) + (hi > 32766 || hi < -32766);
-            }
-          }
-          x[m] = make_float2(i32_to_f32(lo), i32_to_f32(hi));  // the int16 scale rides on the inter-pass twiddle
-        }
-        Dft<R0, false>::run(x);
-        float2 w[R0];
-        load_stage_twiddles<R0, S0>(s_tw, j, w);
-        float2 *d = mycol + j * XS;
-        d[0] = x[0];
-#pragma unroll
-        for (int t = 1; t < R0; t++) d[t * S0 * XS] = cmul(x[t], w[t]);
-      }
-    }
-  } else {
-    mbar_wait(&tbar, 0);
-  }
-  if (FMT == 2 && a.stats) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      energy += __shfl_xor_sync(0xffffffffu, energy, o);
-      clips += __shfl_xor_sync(0xffffffffu, clips, o);
-    }
-    if ((tid & 31) == 0 && (energy | clips)) {
-      atomicAdd(&a.stats[blk].energy, energy);
-      atomicAdd(&a.stats[blk].clips, clips);
-    }
-  }
-  __syncthreads();
-  if (dbg && tid == 0) dbg[1] = gtimer();
-
-  // ---- stage 1 in shared memory: 12 blocks of 108, stride 9 -----------------------------------
-  if (col_ok) {
-    float2 const *tw1 = s_tw + P::tw_off(1);
-    // j = u mod 9 with u = ul + 36 it: the same for the three butterflies -> twiddles formed once
-    int const b0 = ul / S1, j = ul - b0 * S1;
-    float2 w[R1];
-    load_stage_twiddles<R1, S1>(tw1, j, w);
-#pragma unroll 1
-    for (int it = 0; it < 3; it++) {
-      float2 *p = mycol + ((b0 + (UPI / S1) * it) * NSUB1 + j) * XS;
-      float2 x[R1];
-#pragma unroll
-      for (int m = 0; m < R1; m++) x[m] = p[m * S1 * XS];
-      Dft<R1, false>::run(x);
-      p[0] = x[0];
-#pragma unroll
-      for (int t = 1; t < R1; t++) p[t * S1 * XS] = cmul(x[t], w[t]);
-    }
-  }
-  __syncthreads();
-  if (dbg && tid == 0) dbg[2] = gtimer();
-
-  // ---- stage 2 fused with the store: X[k1] * W_nc^{n2 k1} -> mid[k1][n2] ------------------------
-  {
-    float2 wT[R2];
-#pragma unroll
-    for (int t = 0; t < R2; t++) wT[t] = s_twT[c * 9 + t];
-    // u = ul + 36 it = t0*12 + t1 -> k1 = kbase + 144 t2 with kbase = t0 + 12 t1 = kbase(ul) + 3 it
-    int const kb0 = ul / 12 + 12 * (ul % 12);
-    float2 *dst = a.mid + (long)blk * nc + n2g + (long)kb0 * n2;
-    float const os = a.out_scale;
-#pragma unroll
-    for (int it = 0; it < 4; it++) {
-      if (col_ok) {
-        int const u = ul + UPI * it;
-        float2 *p = mycol + u * R2 * XS;
-        float2 x[R2];
-#pragma unroll
-        for (int m = 0; m < R2; m++) x[m] = p[m * XS];
-        Dft<R2, false>::run(x);
-        float2 const wb = make_float2(twU[it].x * os, twU[it].y * os);
-#pragma unroll
-        for (int t = 0; t < R2; t++) {
-          dst[(long)(3 * it + 144 * t) * n2] = cmul(x[t], cmul(wb, wT[t]));
-        }
-      }
-    }
-  }
-  if (dbg && tid == 0) dbg[3] = gtimer();
-}
-
 // ------------------------------------------------------------------ pass 2: rows --------------
 // 1250 = 10 * 25 * 5.  Rows arrive by TMA; stages 0 and 1 run in shared memory with the lanes
 // interleaved over the 8 columns; the radix-5 last stage is fused with the real split: the thread
@@ -256,6 +35,16 @@ __global__ void __launch_bounds__(288, 2) fwd_cols_v2(Pass1Args const a, ColsV2T
 // exactly the partners Z[Nc-k] of its five outputs (digit complement: 1249-k2 <-> (9-t0,24-t1,4-t2)).
 // N1C: row count as a compile-time constant (0 = from the arguments).  HALVED: the 1/2 of the real
 // split was already folded into the column pass (Pass1Args::out_scale).
+// The row pass of every master with 1250 columns, REAL and COMPLEX.  On H100 it beat a two-stage 50 x 25 row kernel
+// (DESIGN.md section 4).  Blocks are taken last-to-first: the column pass wrote the last ones most recently, so their
+// rows are the likeliest to be still in L2.
+struct RowsV2Shape {
+  using P = SPlan<1250, 10, 25, 5>;  // what choose_radices(1250) picks: the kernel reads that registry plan's stage twiddles
+  static constexpr int N2 = 1250, PITCH = 1250, T = 256;
+  static constexpr int TW = (static_tw_count<P>() + 1) & ~1;  // stage twiddles, even (bulk copies move 16-byte multiples)
+  static constexpr size_t smem = sizeof(float2) * (size_t)(8 * PITCH + TW);
+};
+
 // W_1250^{32 it t} literals for stage 0 of the row pass
 __device__ constexpr float kRowsTw0[3][4][2] = {
     {{9.870916009e-01f, -1.601568460e-01f}, {9.486995935e-01f, -3.161789477e-01f}, {8.000617623e-01f, -5.999176502e-01f}, {2.801976204e-01f, -9.599423409e-01f}},
@@ -265,13 +54,12 @@ __device__ constexpr float kRowsTw0[3][4][2] = {
 
 // Stage-0 twiddles W^{j t}, j = ul + 32 it, are (4 values loaded once per thread) x (literal W^{32 it t}) instead of 4 loads per
 // butterfly.  Variants tried and removed again: warp-per-column stages 0/1, stage-0 butterflies in groups of 2 / 4,
-// stage-1 twiddles by products, a persistent double-buffered form.
-// For REAL masters fwd_rows_r50.cuh is the default now; this kernel serves COMPLEX 1296 x 1250 masters and
-// kgpu_set_tuning(10, 6).
+// stage-1 twiddles by products, a persistent double-buffered form, an L2 prefetch of a later CTA's rows, blocks first-to-last.
 template <bool REAL_SPLIT, int N1C = 0, bool HALVED = false>
-__global__ void __launch_bounds__(256, 2) fwd_rows_v2(Pass2Args const a, FwdTables const tb) {
-  using P = S1250v2;
-  constexpr int N2 = 1250, PITCH = 1250, T = 256;
+__global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const a, FwdTables const tb) {
+  using S = RowsV2Shape;
+  using P = S::P;
+  constexpr int N2 = S::N2, PITCH = S::PITCH, T = S::T;
   constexpr int R0 = 10, S0 = 125, R1 = 25, NSUB1 = 125, S1 = 5, R2 = 5;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // [8][PITCH]
@@ -280,18 +68,13 @@ __global__ void __launch_bounds__(256, 2) fwd_rows_v2(Pass2Args const a, FwdTabl
   __shared__ __align__(8) uint64_t tbar;
   TilePlan const &pl = c_plans[a.plan];
   int const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  int const blk = a.rev ? gridDim.y - 1 - blockIdx.y : blockIdx.y;
+  int const blk = gridDim.y - 1 - blockIdx.y;
   constexpr int IPC = REAL_SPLIT ? 4 : 8;
   int const n1 = N1C ? N1C : a.n1;
   int const item0 = blockIdx.x * IPC;
-  unsigned long long *dbg = a.dbg ? a.dbg + 6 * ((long)blockIdx.y * gridDim.x + blockIdx.x) : nullptr;
-  if (dbg && tid == 0) {
-    dbg[0] = gtimer();
-    dbg[5] = sm_id();
-  }
   // which global row sits in which tile column
-  auto row_of = [&](int col, int first = -1) -> int {
-    RowItem const it = row_item((first < 0 ? item0 : first) + (REAL_SPLIT ? col >> 1 : col), n1, REAL_SPLIT);
+  auto row_of = [&](int col) -> int {
+    RowItem const it = row_item(item0 + (REAL_SPLIT ? col >> 1 : col), n1, REAL_SPLIT);
     if (REAL_SPLIT) {
       if ((col & 1) == 0) return it.kind != kRowEmpty ? it.row_a : -1;
       return it.kind == kRowPair ? it.row_b : -1;
@@ -308,18 +91,9 @@ __global__ void __launch_bounds__(256, 2) fwd_rows_v2(Pass2Args const a, FwdTabl
       bulk_g2s(tile + warp * PITCH, a.mid + ((long)blk * n1 + row) * a.mid_ld, N2 * 8, &bars[warp]);
     }
     if (warp == 0) {
-      constexpr uint32_t TWB = (uint32_t)((static_tw_count<P>() + 1) & ~1) * 8u;
+      constexpr uint32_t TWB = (uint32_t)S::TW * 8u;
       mbar_expect_tx(&tbar, TWB);
       bulk_g2s(s_tw, pl.tw, TWB, &tbar);
-    }
-    if (a.pf_ctas) {  // pull the rows of a CTA that starts about one wave later into L2 now
-      int const lin = blockIdx.y * gridDim.x + blockIdx.x + a.pf_ctas;
-      int const ty = lin / gridDim.x, tx = lin - ty * gridDim.x;
-      if (ty < gridDim.y) {
-        int const prow = row_of(warp, tx * IPC);
-        int const pblk = a.rev ? gridDim.y - 1 - ty : ty;
-        if (prow >= 0) bulk_prefetch_l2(a.mid + ((long)pblk * n1 + prow) * a.mid_ld, N2 * 8);
-      }
     }
   }
   __syncthreads();
@@ -327,7 +101,6 @@ __global__ void __launch_bounds__(256, 2) fwd_rows_v2(Pass2Args const a, FwdTabl
   bool const col_ok = row_of(c) >= 0;
   mbar_wait(&tbar, 0);
   if (col_ok) mbar_wait(&bars[c], 0);
-  if (dbg && tid == 0) dbg[1] = gtimer();
   float2 *mycol = tile + c * PITCH;
 
   // ---- stage 0: radix 10, stride 125 (125 butterflies per column) ------------------------------
@@ -392,7 +165,6 @@ __global__ void __launch_bounds__(256, 2) fwd_rows_v2(Pass2Args const a, FwdTabl
     }
   }
   int const has_self = __syncthreads_or(self_item);
-  if (dbg && tid == 0) dbg[2] = gtimer();
 
   float2 *spec = a.spec + (long)blk * a.spec_stride;
   float const hf = HALVED ? 1.0f : 0.5f;
@@ -451,7 +223,6 @@ __global__ void __launch_bounds__(256, 2) fwd_rows_v2(Pass2Args const a, FwdTabl
     }
   }
   // rows that pair with themselves (k1 = 0 and k1 = n1/2): last stage in place, then the v1 epilogue
-  if (dbg && tid == 0) dbg[3] = gtimer();
   if (!has_self) return;  // CTA-uniform
   for (int s = 0; s < 4; s++) {
     RowItem const its = row_item(item0 + s, n1, true);

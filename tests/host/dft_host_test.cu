@@ -32,7 +32,7 @@ template <int R> static int both() {
   printf("radix %2d  forward %.2e  inverse %.2e  %s\n", R, f, i, ok ? "ok" : "FAIL");
   return ok ? 0 : 1;
 }
-// The two-fat-stage decomposition of fwd_cols_r36 / fwd_2s / fwd_rows_r50 restated on the host: stage 0 takes x[j + RD m],
+// The two-fat-stage decomposition of fwd_cols_r36 / fwd_2s restated on the host: stage 0 takes x[j + RD m],
 // m < RC, output t times W_N^{j t} goes to slot t RD + j; stage 1 transforms slots t RD .. t RD + RD - 1 and its output k' is
 // X[t + RC k'].  The twiddle W^{j t} is formed as the kernels form it: t = Q a + b, one product of two float-rounded powers.
 template <int RC, int RD> static int two_stage() {

@@ -150,35 +150,66 @@ def test_forward_full_size_vs_oracle(oracle, cuda_dev, static):
     capi.load().kgpu_use_static_kernels(1)
 
 
-@pytest.mark.parametrize("L,M,shape", [(2560000, 640001, "1280 x 1250"), (2592000, 648001, "1296 x 1250")])
-def test_forward_real_1250_columns_row_kernel_variants(oracle, cuda_dev, L, M, shape):
-    """Both row kernels of a REAL master with 1250 columns, the default 10 x 25 x 5 one and the 50 x 25 one (tuning 10 = 5):
-    with the 36 x 36 column kernel in front of them (1296 rows, the 1/2 of the split pre-folded) and with the runtime-plan
-    column kernel (any other row count, here 1280), against the oracle and against each other.  Two blocks, float input."""
+@pytest.mark.parametrize("real,L,M,split,cols,rows", [
+    (False, 400000, 100001, "800 x 625", "25,32", "25,25"),        # fwd_cols_2s + fwd_rows_2s (cfg-4)
+    (True, 2592000, 648001, "1296 x 1250", "36,36", "10,25,5"),    # fwd_cols_r36 with the 1/2 of the split + fwd_rows_v2
+    (False, 1296000, 324001, "1296 x 1250", "36,36", "10,25,5"),   # fwd_cols_r36 + fwd_rows_v2
+    (False, 1259712, 419905, "1296 x 1296", "36,36", "12,12,9"),   # fwd_cols_r36 + generic rows
+    (True, 2560000, 640001, "1280 x 1250", "16,10,8", "10,25,5"),  # generic columns + fwd_rows_v2 with the real split
+    (False, 1200000, 400001, "1280 x 1250", "16,10,8", "10,25,5"), # generic columns + fwd_rows_v2
+])
+def test_forward_specialised_kernel_pairs(oracle, cuda_dev, real, L, M, split, cols, rows):
+    """Every kernel pair kgpu_master_create can choose other than the generic one, against the oracle and against the
+    generic kernels of the same master (kgpu_use_static_kernels(0) at launch time).  Two blocks, float input."""
     from ka9q_radio_b200 import capi
 
     lib = capi.load()
     rng = np.random.default_rng(12)
-    x = (0.1 * rng.standard_normal(2 * L)).astype(np.float32)
     t = np.arange(2 * L)
-    x += (0.5 * np.cos(2 * np.pi * ((0.2345 * t) % 1.0))).astype(np.float32)
-    cz = _mk(L, M, capi.KGPU_REAL, cuda_dev)
-    assert shape in cz.master.describe()
+    if real:
+        x = (0.1 * rng.standard_normal(2 * L)).astype(np.float32)
+        x += (0.5 * np.cos(2 * np.pi * ((0.2345 * t) % 1.0))).astype(np.float32)
+    else:
+        x = (0.1 * (rng.standard_normal(2 * L) + 1j * rng.standard_normal(2 * L))).astype(np.complex64)
+        x += (0.5 * np.exp(2j * np.pi * ((0.2345 * t) % 1.0))).astype(np.complex64)
+    cz = _mk(L, M, capi.KGPU_REAL if real else capi.KGPU_COMPLEX, cuda_dev)
+    assert f"two-pass {split}; cols radices [{cols}] rows radices [{rows}]" in cz.master.describe()
     d = cz.stage_stream(x)
-    spec, spec_old = cz.alloc_spectra(2), cz.alloc_spectra(2)
+    spec, spec_gen = cz.alloc_spectra(2), cz.alloc_spectra(2)
     cz.forward(d, 2, spec)
-    lib.kgpu_set_tuning(10, 5)
-    cz.forward(d, 2, spec_old)
-    lib.kgpu_set_tuning(10, 0)
+    lib.kgpu_use_static_kernels(0)
+    try:
+        cz.forward(d, 2, spec_gen)
+    finally:
+        lib.kgpu_use_static_kernels(1)
     torch.cuda.synchronize()
     nb = cz.master.bins
-    got, old = spec.cpu().numpy()[:, :nb], spec_old.cpu().numpy()[:, :nb]
+    got, gen = spec.cpu().numpy()[:, :nb], spec_gen.cpu().numpy()[:, :nb]
     for b in range(2):
         ref = oracle.forward(oracle.block_window(x, L, M, b))
         assert rel_err(got[b], ref) < TOL, (b, rel_err(got[b], ref))
-        assert rel_err(old[b], ref) < TOL
-    assert np.abs(got - old).max() / np.abs(old).max() < 2e-6
+        assert rel_err(gen[b], ref) < TOL
+    assert np.abs(got - gen).max() / np.abs(gen).max() < 2e-6
     cz.close()
+
+
+def test_forward_after_a_smaller_master_is_created(oracle, cuda_dev):
+    """The shared-memory limit of a kernel is one value for the whole process.  Creating a master whose generic kernels
+    need less (640 000 = 800 x 800) must not take away what an existing one launches with (1 500 000 = 1250 x 1200)."""
+    from ka9q_radio_b200 import capi
+
+    L, M = 1125000, 375001
+    x = oracle.siggen_complex(L, 0.1, 0.01, -0.123, 1.0)
+    big = _mk(L, M, capi.KGPU_COMPLEX, cuda_dev)
+    small = _mk(480000, 160001, capi.KGPU_COMPLEX, cuda_dev)
+    assert "two-pass 1250 x 1200" in big.master.describe() and "two-pass 800 x 800" in small.master.describe()
+    spec = big.alloc_spectra(1)
+    big.forward(big.stage_stream(x), 1, spec)
+    torch.cuda.synchronize()
+    ref = oracle.forward(oracle.block_window(x, L, M, 0))
+    assert rel_err(spec.cpu().numpy()[0, : big.master.bins], ref) < TOL
+    small.close()
+    big.close()
 
 
 def test_notches(oracle, cuda_dev):

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Compare the spectra of two kernel variants on the same input (cfg-2 sizes, REAL int16 and COMPLEX float).
-usage: ab_check.py "8=1" ["9=1" ...]   (each variant is compared with the default)"""
+usage: ab_check.py static=0   (the generic kernels, compared with each master's default kernel pair)"""
 import sys
 from pathlib import Path
 import numpy as np, torch
@@ -11,14 +11,11 @@ W = workloads.cfg2()
 from ka9q_radio_b200 import capi
 from ka9q_radio_b200.channelizer import Channelizer
 lib = capi.load(); dev = torch.device("cuda:0")
+VARIANTS = ("default", "static=0")
+for v in sys.argv[1:]:
+    if v not in VARIANTS: sys.exit("variants: %s" % ", ".join(VARIANTS))
 def setv(v):
-    lib.kgpu_use_static_kernels(1)
-    for k in range(16): lib.kgpu_set_tuning(k, 0)
-    for kv in v.split(","):
-        if kv and kv != "default":
-            k, val = kv.split("=")
-            if k == "static": lib.kgpu_use_static_kernels(int(val))
-            else: lib.kgpu_set_tuning(int(k), int(val))
+    lib.kgpu_use_static_kernels(0 if v == "static=0" else 1)
 B = 5
 rng = np.random.default_rng(1)
 W4 = workloads.cfg4()

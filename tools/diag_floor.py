@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Rounding floor of quiet cfg-2 channels against a float64 transform: GPU kernel variants and the float32 CPU checker.
-usage: diag_floor.py [variant ...]   (variants as in kbench.py; test/diagnostic tool, not product code)"""
+usage: diag_floor.py [default] [static=0]   (variants as in kbench.py; test/diagnostic tool, not product code)"""
 import sys
 from pathlib import Path
 import numpy as np, torch
@@ -33,13 +33,8 @@ print("float32 CPU checker : max %.3e rms %.3e" % (np.abs(e).max(), np.sqrt((np.
 se = np.abs(X32[:w.N // 2 + 1] - X64[:w.N // 2 + 1])
 print("   spectrum: max %.3e rms %.3e (max|X| %.3e)" % (se.max(), np.sqrt((se ** 2).mean()), np.abs(X64).max()))
 for v in sys.argv[1:] or ["default"]:
-    lib.kgpu_use_static_kernels(1)
-    for kk in range(16): lib.kgpu_set_tuning(kk, 0)
-    for kv in v.split(","):
-        if kv and kv != "default":
-            a, b = kv.split("=")
-            if a == "static": lib.kgpu_use_static_kernels(int(b))
-            else: lib.kgpu_set_tuning(int(a), int(b))
+    if v not in ("default", "static=0"): sys.exit("variants: default, static=0")
+    lib.kgpu_use_static_kernels(0 if v == "static=0" else 1)
     cz = Channelizer(w.L, w.M, w.in_type, dev, capacity=len(w.channels))
     for c in w.channels:
         cz.add_channel(c.olen, c.shift, c.low, c.high, c.beta)

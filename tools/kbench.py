@@ -2,8 +2,8 @@
 """A/B micro-benchmark of the three kernels on cfg-2 (needs a GPU).
 
 usage: kbench.py [--blocks B] [--iters K] variant [variant ...]
-a variant is a comma list of key=value tuning knobs (kgpu_set_tuning), e.g. "10=6" "13=4" "14=1,15=-1" (include/ka9q_gpu.h);
-"static=0" selects the generic kernels.  Variants are interleaved round-robin to cancel drift."""
+a variant is "default" (the master's own kernel pair) or "static=0" (the generic kernels, kgpu_use_static_kernels(0));
+variants are interleaved round-robin to cancel drift."""
 import argparse, sys, json
 from pathlib import Path
 import numpy as np, torch
@@ -19,7 +19,7 @@ ap.add_argument("--iters", type=int, default=20)
 ap.add_argument("--rounds", type=int, default=3)
 ap.add_argument("--nchan", type=int, default=0, help="0 = the workload's own channel list")
 ap.add_argument("--config", default="cfg2", choices=["cfg2", "cfg3", "cfg4"])
-ap.add_argument("variants", nargs="+")
+ap.add_argument("variants", nargs="+", choices=["default", "static=0"])
 a = ap.parse_args()
 W = workloads.by_name(a.config)
 lib = capi.load()
@@ -37,18 +37,10 @@ host = rng.integers(-3000, 3000, (nstream * W.L + W.M - 1) * wps, dtype=np.int16
 d_stream = torch.from_numpy(host).to(dev)
 spec, out = cz.alloc_spectra(B), cz.alloc_outputs(B)
 ng = nstream // B
-def apply(v):
-    lib.kgpu_use_static_kernels(1)
-    for k in range(16): lib.kgpu_set_tuning(k, 0)
-    for kv in v.split(","):
-        if not kv or kv == "default": continue
-        k, val = kv.split("=")
-        if k == "static": lib.kgpu_use_static_kernels(int(val))
-        else: lib.kgpu_set_tuning(int(k), int(val))
 res = {v: [] for v in a.variants}
 for rnd in range(a.rounds + 1):
     for v in a.variants:
-        apply(v)
+        lib.kgpu_use_static_kernels(0 if v == "static=0" else 1)
         lib.kgpu_profile_enable(1); lib.kgpu_profile_reset()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         torch.cuda.synchronize(); e0.record()
@@ -61,6 +53,7 @@ for rnd in range(a.rounds + 1):
         row = {k: 1e3 * ms / cnt / B for k, (ms, cnt) in p.items() if cnt}
         row["wall"] = 1e3 * e0.elapsed_time(e1) / a.iters / B
         res[v].append(row)
+lib.kgpu_use_static_kernels(1)
 for v, rows in res.items():
     keys = rows[0].keys()
     print("%-28s" % v, "  ".join("%s %6.2f" % (k, np.median([r[k] for r in rows])) for k in keys), " us/block (median of %d)" % len(rows))

@@ -6,12 +6,11 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
 so = ROOT / "ka9q_radio_b200" / "libka9qgpu.so"
 names = subprocess.run(["cuobjdump", "-elf", str(so)], capture_output=True, text=True).stdout
-want = {"fwd_cols_r36<int16, 1250> (column pass, default)": r"_ZN4kfft12fwd_cols_r36ILi1ELi1250ELb1EE\w+",
-        "fwd_rows_r50<1296, halved> (row pass 50 x 25 + real split, tuning 10=5)": r"_ZN4kfft12fwd_rows_r50ILi1296ELb1EE\w+",
-        "fwd_rows_v2<real, 1296, halved> (row pass 10 x 25 x 5, default)": r"_ZN4kfft11fwd_rows_v2ILb1ELi1296ELb1ELb0ELi0ELb1ELb0EE\w+",
+want = {"fwd_cols_r36<int16, 1250> (column pass, default)": r"_ZN4kfft12fwd_cols_r36ILi1ELi1250EE\w+",
+        "fwd_rows_v2<real, 1296, halved> (row pass 10 x 25 x 5, default)": r"_ZN4kfft11fwd_rows_v2ILb1ELi1296ELb1EE\w+",
         "fwd_cols_2s<int16, 25, 32> (cfg-4 column pass)": r"_ZN4kfft11fwd_cols_2sILi1ELi25ELi32EE\w+",
         "fwd_rows_2s<25, 25> (cfg-4 row pass)": r"_ZN4kfft11fwd_rows_2sILi25ELi25EE\w+",
-        "chan_v2<600 = 24 x 25> (channels, default)": r"_ZN4kfft7chan_v2INS_5SPlanILi600EJLi24ELi25EEEELb0ELb0EE\w+"}
+        "chan_v2<600 = 24 x 25> (channels, default)": r"_ZN4kfft7chan_v2INS_5SPlanILi600EJLi24ELi25EEEELb0EE\w+"}
 for title, pat in want.items():
     m = re.search(pat, names)
     if not m:
