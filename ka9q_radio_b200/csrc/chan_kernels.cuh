@@ -15,6 +15,11 @@ namespace kfft {
 
 constexpr int kChanWarps = 4;  // (channel, block) pairs per CTA
 
+// Longest channel transform: chan_kernel holds kChanWarps columns of (points rounded up to 4) + 2 float2 in shared
+// memory, which must fit the 227 KB a block may opt into on sm_90.  7260 points.
+constexpr int kChanSmemLimit = 227 * 1024;
+constexpr int kMaxChanPoints = (kChanSmemLimit / (8 * kChanWarps) - 2) / 4 * 4;
+
 // Host-resolved description of how output bin t (in the reference's walk order, starting at the
 // most negative output bin) maps onto the master spectrum.  Covers filter.c:810-893 (REAL
 // master, upright or inverted) and :728-793 (COMPLEX master with circular wrap).

@@ -28,8 +28,13 @@ struct TilePlan {
 };
 
 // Process-wide registry of column plans (filled by get_tile_plan() in kgpu.cu; this header is
-// included by exactly one translation unit).
-constexpr int kMaxPlans = 64;
+// included by exactly one translation unit).  One entry per distinct transform length, never freed:
+// every master uses two, every channel rate one.  320 entries hold all 304 lengths the planner can
+// ever be asked for (1 .. 7260 points, factors 2, 3, 5, 7; kgpu.cu asserts it), so the registry
+// cannot fill.  The table (57.5 KB) is the library's only __constant__ data and must stay inside
+// the 64 KB constant bank.
+constexpr int kMaxPlans = 320;
+static_assert(sizeof(TilePlan) * kMaxPlans <= 60 * 1024, "plan registry must fit the 64 KB constant bank");
 __constant__ TilePlan c_plans[kMaxPlans];
 
 // One DIF stage of radix R on one column.  `lane`/`nl`: index and size of the cooperating group.

@@ -263,6 +263,23 @@ namespace kfft {
 
 static int const kRadixSet[] = {25, 24, 20, 16, 15, 12, 10, 9, 8, 7, 6, 5, 4, 3, 2};
 
+// Every length the registry accepts has prime factors 2, 3, 5, 7 only and is at most kMaxChanPoints: masters split into
+// lengths <= kMaxTileLen and kgpu_bank_define rejects channels whose transform the channel kernel cannot hold.  If all
+// of them fit, the registry can never fill, and which lengths a process has used (master rates, channel rates, test
+// order) cannot make a creation fail.
+static_assert(kMaxChanPoints >= kMaxTileLen, "every tile length must also be a valid channel length");
+constexpr int plannable_lengths(int max) {
+  int count = 0;
+  for (int n = 1; n <= max; n++) {
+    int v = n;
+    for (int p : {2, 3, 5, 7})
+      while (v % p == 0) v /= p;
+    count += (v == 1);
+  }
+  return count;
+}
+static_assert(plannable_lengths(kMaxChanPoints) <= kMaxPlans, "the plan registry must hold every plannable length");
+
 // exhaustive search over multisets of supported radices (depth <= kMaxStages): fewest stages,
 // then smallest sum.
 static void search(int n, int start, std::vector<int> &cur, std::vector<int> &best, int &best_sum) {
@@ -313,12 +330,11 @@ int get_tile_plan(int len) {
   std::lock_guard<std::mutex> lk(g_plan_mu);
   for (size_t i = 0; i < g_plans.size(); i++)
     if (g_plans[i].len == len) return (int)i;
-  if ((int)g_plans.size() >= kMaxPlans || len < 1 || len > 65535) return -1;
   std::vector<int> rad;
-  if (len > 1) {
-    rad = choose_radices(len);
-    if (rad.empty()) return -1;
-  }
+  if (len > 1) rad = choose_radices(len);
+  if (len < 1 || len > kMaxChanPoints || (len > 1 && rad.empty()))
+    return fail("%d-point transform cannot be planned (factors 2, 3, 5, 7; at most %d points)", len, kMaxChanPoints);
+  if ((int)g_plans.size() >= kMaxPlans) return fail("plan registry full (%d plans)", kMaxPlans);
   TilePlan p;
   memset(&p, 0, sizeof p);
   p.len = len;
@@ -354,14 +370,24 @@ int get_tile_plan(int len) {
   uint16_t *d_perm = nullptr;
   tw.push_back(make_float2(0.f, 0.f));  // padding: bulk (16-byte granular) copies may read one entry past the end
   tw.push_back(make_float2(0.f, 0.f));
-  if (cudaMalloc(&d_tw, sizeof(float2) * std::max<size_t>(tw.size(), 1)) != cudaSuccess) return -1;
-  if (cudaMalloc(&d_perm, sizeof(uint16_t) * (size_t)len) != cudaSuccess) return -1;
-  if (!tw.empty()) cudaMemcpy(d_tw, tw.data(), sizeof(float2) * tw.size(), cudaMemcpyHostToDevice);
-  cudaMemcpy(d_perm, perm.data(), sizeof(uint16_t) * (size_t)len, cudaMemcpyHostToDevice);
-  p.tw = d_tw;
-  p.perm = d_perm;
+  p.tw = nullptr;
+  p.perm = nullptr;
   int const idx = (int)g_plans.size();
-  if (cudaMemcpyToSymbol(c_plans, &p, sizeof p, sizeof(TilePlan) * (size_t)idx) != cudaSuccess) return -1;
+  auto upload = [&]() -> int {
+    CUDA_OK(cudaMalloc(&d_tw, sizeof(float2) * tw.size()));
+    CUDA_OK(cudaMalloc(&d_perm, sizeof(uint16_t) * (size_t)len));
+    CUDA_OK(cudaMemcpy(d_tw, tw.data(), sizeof(float2) * tw.size(), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(d_perm, perm.data(), sizeof(uint16_t) * (size_t)len, cudaMemcpyHostToDevice));
+    p.tw = d_tw;
+    p.perm = d_perm;
+    CUDA_OK(cudaMemcpyToSymbol(c_plans, &p, sizeof p, sizeof(TilePlan) * (size_t)idx));
+    return 0;
+  };
+  if (upload()) {  // the CUDA error is in kgpu_last_error()
+    cudaFree(d_tw);
+    cudaFree(d_perm);
+    return -1;
+  }
   PlanSlot sl;
   sl.len = len;
   sl.host = p;
@@ -550,7 +576,7 @@ extern "C" kgpu_master *kgpu_master_create(int L, int M, int in_type) {
   m->plan1 = get_tile_plan(m->sp.n1);
   m->plan2 = get_tile_plan(m->sp.n2);
   if (m->plan1 < 0 || m->plan2 < 0) {
-    fail("kgpu_master_create: plan registry full or length unsupported");
+    fail("kgpu_master_create: %s", std::string(g_err).c_str());
     delete m;
     return nullptr;
   }
@@ -594,9 +620,11 @@ extern "C" int kgpu_master_describe(kgpu_master const *m, char *buf, int buflen)
   std::string const rr = m->rows == ROWS_2S ? "25,25" : m->rows == ROWS_V2 ? "10,25,5" : radices(host_tile_plan(m->plan2));
   size_t const s1 = m->cols == COLS_2S ? Cols2s::smem : m->cols == COLS_R36 ? ColsR36Shape::smem : m->smem1;
   size_t const s2 = m->rows == ROWS_2S ? Rows2s::smem : m->rows == ROWS_V2 ? RowsV2Shape::smem : m->smem2;
+  char const *kc = m->cols == COLS_2S ? "fwd_cols_2s" : m->cols == COLS_R36 ? "fwd_cols_r36" : "fwd_cols_kernel";
+  char const *kr = m->rows == ROWS_2S ? "fwd_rows_2s" : m->rows == ROWS_V2 ? "fwd_rows_v2" : "fwd_rows_kernel";
   snprintf(buf, (size_t)buflen, "N=%d %s, %ld-point complex two-pass %d x %d; cols radices [%s] rows radices [%s]; smem %zu/%zu B; "
-           "grids %d/%d CTAs per block", m->N, m->in_type == KGPU_REAL ? "real" : "complex", m->nc, m->sp.n1, m->sp.n2,
-           rc.c_str(), rr.c_str(), s1, s2, (m->sp.n2 + kTile - 1) / kTile, m->n_item_ctas);
+           "grids %d/%d CTAs per block; kernels %s + %s", m->N, m->in_type == KGPU_REAL ? "real" : "complex", m->nc, m->sp.n1,
+           m->sp.n2, rc.c_str(), rr.c_str(), s1, s2, (m->sp.n2 + kTile - 1) / kTile, m->n_item_ctas, kc, kr);
   return 0;
 }
 
@@ -1002,8 +1030,12 @@ static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out) {
   if (num % b->m->L) return fail("invalid output length %d for N=%d L=%d (filter.c:312-316)", olen, b->m->N, b->m->L);
   int const points = (int)(num / b->m->L);
   if (real_out && (points & 1)) return fail("kgpu_bank_define: REAL-output slaves need an even number of points (got %d)", points);
+  // the channel kernel holds kChanWarps transforms of this length in shared memory; the bound also keeps the plan
+  // registry from filling (see kMaxPlans)
+  if (points > kMaxChanPoints)
+    return fail("kgpu_bank_define: %d-point inverse transform exceeds the %d-point maximum", points, kMaxChanPoints);
   int const plan = get_tile_plan(points);
-  if (plan < 0) return fail("kgpu_bank_define: %d-point inverse transform cannot be planned", points);
+  if (plan < 0) return fail("kgpu_bank_define: %s", std::string(g_err).c_str());
   ChanHost &c = b->ch[(size_t)idx];
   c.real_out = real_out;
   if (!(c.defined && c.points == points)) {

@@ -5,6 +5,8 @@ from pathlib import Path
 
 import pytest
 
+from accuracy_cases import CHANNEL_RADICES, CHANNELS, FORWARD, UNSERVABLE
+
 ROOT = Path(__file__).resolve().parent.parent
 
 
@@ -68,6 +70,35 @@ def test_planner_split(n):
 
     a, b = capi.plan_split(n)
     assert a * b == n and a >= b and a <= 4096
+
+
+@pytest.mark.parametrize("geo", FORWARD, ids=lambda g: g.id)
+def test_accuracy_sweep_reaches_its_split_and_radices(geo):
+    """tests/test_gpu_accuracy.py claims each forward row reaches a code path through its split and radices."""
+    from ka9q_radio_b200 import capi
+
+    n = (geo.L + geo.M - 1) // (2 if geo.real else 1)
+    n1, n2 = capi.plan_split(n)
+    assert (n1, n2) == geo.split
+    assert (capi.plan_radices(n1), capi.plan_radices(n2)) == tuple(geo.plan)
+
+
+@pytest.mark.parametrize("case", CHANNELS, ids=lambda c: c.id)
+def test_accuracy_channel_lengths_are_planned(case):
+    from ka9q_radio_b200 import capi
+
+    N = case.L + case.M - 1
+    for ns in case.points + case.real_out:
+        assert ns * case.L % N == 0, ns  # a whole output length
+        assert capi.plan_radices(ns) == CHANNEL_RADICES[ns], ns
+
+
+def test_unservable_front_end_is_rejected_at_create():
+    """AirspyHF+ at 912 kS/s, 20 ms blocks at overlap 5: N = 22 800 = 2^4 * 3 * 5^2 * 19 has no plannable split."""
+    from ka9q_radio_b200 import capi
+
+    with pytest.raises(capi.KgpuError, match="22800 points cannot be split into two plannable lengths"):
+        capi.Master(*UNSERVABLE, capi.KGPU_COMPLEX)
 
 
 def test_no_oracle_in_product():
