@@ -98,6 +98,12 @@ int kgpu_bank_define(kgpu_bank *b, int idx, int olen);
  * REAL-output slaves of wfm.c:76 / stereod.c:387 (slice filter.c:794-809, c2r inverse filter.c:386,914): olen FLOATS
  * per block, packed into (olen+1)/2 float2 of the output row.  points must be even for KGPU_REAL. */
 int kgpu_bank_define_ex(kgpu_bank *b, int idx, int olen, int out_type);
+/* Same, without the 7260-point limit of the two calls above (the reference plans any length, filter.c:298-415): at
+ * most 7260 points it is kgpu_bank_define_ex; up to 28812 points (e.g. the 384 kHz wfm downconverter, wfm.c:37-38, at
+ * 9600 or 15360 points) the channel runs a four-step inverse transform, one CTA per channel and block, provided
+ * points splits into two factors of at most 4096 with factors 2, 3, 5, 7 (every such length in range does).  Every
+ * other bank call treats such a channel like any other. */
+int kgpu_bank_define_wide(kgpu_bank *b, int idx, int olen, int out_type);
 /* set_filter (filter.c:968-1045): Kaiser-windowed sinc designed on the host in double, forward
  * transformed on the device.  low/high are fractions of the output rate. */
 int kgpu_bank_set_filter(kgpu_bank *b, int idx, double low, double high, double kaiser_beta);

@@ -78,6 +78,7 @@ def load() -> C.CDLL:
     L.kgpu_bank_commit.argtypes = [vp, vp]
     L.kgpu_unpack_airspy12.argtypes = [vp, l, vp, vp, vp]
     L.kgpu_bank_define_ex.argtypes = [vp, i, i, i]
+    L.kgpu_bank_define_wide.argtypes = [vp, i, i, i]
     L.kgpu_bank_set_weights.argtypes = [vp, i, d, d, d, d]
     L.kgpu_bank_set_osc.argtypes = [vp, i, i, d, d, d, d]
     L.kgpu_bank_get_osc_phase.argtypes = [vp, i, vp]
@@ -195,6 +196,10 @@ class Bank:
 
     def define(self, idx, olen, out_type=KGPU_COMPLEX) -> int:
         return check(self.lib.kgpu_bank_define_ex(self.h, idx, olen, out_type), "kgpu_bank_define_ex")
+
+    def define_wide(self, idx, olen, out_type=KGPU_COMPLEX) -> int:
+        """define() without its 7260-point limit: longer channels (up to 28812 points) run the four-step channel kernel."""
+        return check(self.lib.kgpu_bank_define_wide(self.h, idx, olen, out_type), "kgpu_bank_define_wide")
 
     def set_weights(self, idx, i_weight=1.0, q_weight=0.0):
         """set_filter_weights (filter.c:922-929)"""

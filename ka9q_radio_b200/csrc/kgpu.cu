@@ -16,6 +16,7 @@
 
 #include "../../include/ka9q_gpu.h"
 #include "chan_kernels.cuh"
+#include "chan_wide.cuh"
 #include "fwd_kernels.cuh"
 #include "noise_kernel.cuh"
 #include "plan.cuh"
@@ -413,6 +414,91 @@ bool choose_split(long n, Split2 *out) {
   out->n1 = (int)(n / best);
   out->n2 = (int)best;
   return true;
+}
+
+// choose_split restated at compile time (a length <= kMaxTileLen is plannable iff its factors are 2, 3, 5, 7), to pin
+// kMaxWideChanPoints: every such length above kMaxChanPoints up to it fits chan_wide's shared memory, the next does not.
+constexpr bool smooth7(long n) {
+  for (long p : {2, 3, 5, 7})
+    while (n % p == 0) n /= p;
+  return n == 1;
+}
+constexpr bool wide_fits(long n) {
+  long d = 1;
+  while ((d + 1) * (d + 1) <= n) d++;
+  for (; d >= 1; d--) {
+    if (n % d) continue;
+    if (n / d > kMaxTileLen) return false;
+    if (smooth7(n / d) && smooth7(d)) return wide_smem_bytes((int)(n / d), (int)d) <= kChanSmemLimit;
+  }
+  return false;
+}
+constexpr bool all_wide_fit(long lo, long hi) {
+  for (long n = lo; n <= hi; n++)
+    if (smooth7(n) && !wide_fits(n)) return false;
+  return true;
+}
+constexpr long next_smooth7(long n) {
+  while (!smooth7(n)) n++;
+  return n;
+}
+static_assert(all_wide_fit(kMaxChanPoints + 1, kMaxWideChanPoints), "a wide length up to the maximum does not fit");
+static_assert(!wide_fits(next_smooth7(kMaxWideChanPoints + 1)), "kMaxWideChanPoints is below what shared memory holds");
+
+// Four-step geometry of every wide length used so far (never freed, like the plan registry).  Its two plans are
+// registry plans of at most kMaxTileLen points, so wide channels add no registry entries.
+static std::mutex g_wide_mu;
+static std::map<int, WideGeom> g_wide;
+
+static int plan_slot(TilePlan const &p, int k) {  // slot holding X[k] after the plan's last stage (its perm[k])
+  int slot = 0;
+  for (int i = 0; i < p.nstages; i++) {
+    slot += (k % p.radix[i]) * p.stride[i];
+    k /= p.radix[i];
+  }
+  return slot;
+}
+
+static WideGeom const *get_wide_geom(int points) {
+  std::lock_guard<std::mutex> lk(g_wide_mu);
+  auto it = g_wide.find(points);
+  if (it != g_wide.end()) return &it->second;
+  Split2 sp;
+  if (!choose_split(points, &sp)) {
+    fail("%d-point transform cannot be split into two plannable lengths (factors 2, 3, 5, 7; each at most %d)", points,
+         kMaxTileLen);
+    return nullptr;
+  }
+  if (wide_smem_bytes(sp.n1, sp.n2) > kChanSmemLimit) {
+    fail("%d-point transform (%d x %d) does not fit in shared memory", points, sp.n1, sp.n2);
+    return nullptr;
+  }
+  WideGeom g;
+  g.n1 = sp.n1;
+  g.n2 = sp.n2;
+  g.pitch = wide_pitch(sp.n2);
+  g.plan1 = get_tile_plan(sp.n1);
+  g.plan2 = get_tile_plan(sp.n2);
+  if (g.plan1 < 0 || g.plan2 < 0) return nullptr;
+  // pass 1 leaves output j2 in column plan_slot(j2): tabulate W_Ns^{k1 j2} in column order
+  std::vector<float2> tw((size_t)points);
+  TilePlan const &p2 = *host_tile_plan(g.plan2);
+  for (int j2 = 0; j2 < g.n2; j2++) {
+    int const c = plan_slot(p2, j2);
+    for (int k1 = 0; k1 < g.n1; k1++) {
+      long double const ang = -2.0L * M_PIl * (long double)((long)k1 * j2) / (long double)points;
+      tw[(size_t)k1 * g.n2 + c] = make_float2((float)cosl(ang), (float)sinl(ang));
+    }
+  }
+  float2 *d_tw = nullptr;
+  if (cudaMalloc(&d_tw, sizeof(float2) * tw.size()) != cudaSuccess ||
+      cudaMemcpy(d_tw, tw.data(), sizeof(float2) * tw.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
+    cudaFree(d_tw);
+    fail("%d-point transform: twiddle upload failed", points);
+    return nullptr;
+  }
+  g.tw = d_tw;
+  return &(g_wide[points] = g);
 }
 }  // namespace kfft
 
@@ -936,20 +1022,26 @@ static int bank_commit(kgpu_bank *b, cudaStream_t st) {
     }
   }
   b->out_stride = (off + 3) / 4 * 4;
-  // one launch per distinct plan: order[] lists that plan's descriptors
+  // one launch per distinct plan: order[] lists that plan's descriptors.  Wide channels (chan_wide serves every
+  // variant) form one group per length; their plan is only their first factor's, so the length is part of the key.
   std::vector<int> order;
   b->groups.clear();
-  auto generic_only = [&](int i) { return (b->desc[(size_t)i].flags & (kChanRealOut | kChanBeam)) != 0; };
+  auto generic_only = [&](int i) {
+    return b->desc[(size_t)i].points <= kMaxChanPoints && (b->desc[(size_t)i].flags & (kChanRealOut | kChanBeam)) != 0;
+  };
+  auto same_group = [&](kgpu_bank::Group const &g, int k) {
+    return b->desc[(size_t)k].plan == g.plan && b->desc[(size_t)k].points == g.points && generic_only(k) == g.generic;
+  };
   for (int i = 0; i < b->nchan; i++) {
     if (b->desc[(size_t)i].plan < 0) continue;
     bool const gen = generic_only(i);
     bool found = false;
     for (auto &g : b->groups)
-      if (g.plan == b->desc[(size_t)i].plan && g.generic == gen) found = true;
+      if (same_group(g, i)) found = true;
     if (found) continue;
     kgpu_bank::Group g{b->desc[(size_t)i].plan, b->desc[(size_t)i].points, (int)order.size(), 0, gen};
     for (int k = i; k < b->nchan; k++)
-      if (b->desc[(size_t)k].plan == g.plan && generic_only(k) == gen) order.push_back(k);
+      if (same_group(g, k)) order.push_back(k);
     g.count = (int)order.size() - g.off;
     b->groups.push_back(g);
   }
@@ -1018,24 +1110,38 @@ extern "C" void kgpu_bank_destroy(kgpu_bank *b) {
 }
 static bool bad_idx(kgpu_bank const *b, int idx) { return !b || idx < 0 || idx >= b->capacity; }
 
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out);
-extern "C" int kgpu_bank_define(kgpu_bank *b, int idx, int olen) { return bank_define(b, idx, olen, false); }
+static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok);
+extern "C" int kgpu_bank_define(kgpu_bank *b, int idx, int olen) { return bank_define(b, idx, olen, false, false); }
 extern "C" int kgpu_bank_define_ex(kgpu_bank *b, int idx, int olen, int out_type) {
   if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_ex: out_type must be KGPU_COMPLEX or KGPU_REAL");
-  return bank_define(b, idx, olen, out_type == KGPU_REAL);
+  return bank_define(b, idx, olen, out_type == KGPU_REAL, false);
 }
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out) {
+extern "C" int kgpu_bank_define_wide(kgpu_bank *b, int idx, int olen, int out_type) {
+  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_wide: out_type must be KGPU_COMPLEX or KGPU_REAL");
+  return bank_define(b, idx, olen, out_type == KGPU_REAL, true);
+}
+static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok) {
   if (bad_idx(b, idx) || olen < 1) return fail("kgpu_bank_define: bad arguments");
   long const num = (long)olen * b->m->N;
   if (num % b->m->L) return fail("invalid output length %d for N=%d L=%d (filter.c:312-316)", olen, b->m->N, b->m->L);
   int const points = (int)(num / b->m->L);
   if (real_out && (points & 1)) return fail("kgpu_bank_define: REAL-output slaves need an even number of points (got %d)", points);
   // the channel kernel holds kChanWarps transforms of this length in shared memory; the bound also keeps the plan
-  // registry from filling (see kMaxPlans)
-  if (points > kMaxChanPoints)
+  // registry from filling (see kMaxPlans).  Longer channels (kgpu_bank_define_wide) run chan_wide, one CTA each, on
+  // a split into two registry lengths; their descriptor's plan is that of the first factor (>= 0: runnable).
+  int plan;
+  if (points <= kMaxChanPoints) {
+    plan = get_tile_plan(points);
+    if (plan < 0) return fail("kgpu_bank_define: %s", std::string(g_err).c_str());
+  } else if (!wide_ok) {
     return fail("kgpu_bank_define: %d-point inverse transform exceeds the %d-point maximum", points, kMaxChanPoints);
-  int const plan = get_tile_plan(points);
-  if (plan < 0) return fail("kgpu_bank_define: %s", std::string(g_err).c_str());
+  } else if (points > kMaxWideChanPoints) {
+    return fail("kgpu_bank_define_wide: %d-point inverse transform exceeds the %d-point maximum", points, kMaxWideChanPoints);
+  } else {
+    WideGeom const *g = get_wide_geom(points);
+    if (!g) return fail("kgpu_bank_define_wide: %s", std::string(g_err).c_str());
+    plan = g->plan1;
+  }
   ChanHost &c = b->ch[(size_t)idx];
   c.real_out = real_out;
   if (!(c.defined && c.points == points)) {
@@ -1080,7 +1186,15 @@ static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *ho
   if (on_stream) CUDA_OK(cudaStreamSynchronize(st));
   else CUDA_OK(cudaDeviceSynchronize());
   CUDA_OK(cudaMemcpyAsync(dst, host, sizeof(float2) * (size_t)c.points, cudaMemcpyHostToDevice, st));
-  if (transform) {
+  if (transform && c.points > kMaxChanPoints) {
+    WideGeom const *g = get_wide_geom(c.points);
+    if (!g) return -1;
+    size_t const sm = (size_t)wide_smem_bytes(g->n1, g->n2);
+    if (allow_smem((const void *)response_wide_kernel, sm)) return -1;
+    response_wide_kernel<<<1, kWideThreads, sm, st>>>(dst, *g);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+  } else if (transform) {
     size_t const sm = sizeof(float2) * (size_t)c.points;
     if (allow_smem((const void *)response_fft_kernel, sm)) return -1;
     response_fft_kernel<<<1, 32, sm, st>>>(dst, c.plan);
@@ -1250,6 +1364,14 @@ static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_ou
   a.power_stride = b->capacity;
   ProfScope ps(K_CHAN, st);
   g_launches++;
+  if (points > kMaxChanPoints) {  // wide channels: chan_wide whatever the static-kernel setting
+    WideGeom const *g = get_wide_geom(points);
+    if (!g) return -1;
+    size_t const sm = (size_t)wide_smem_bytes(g->n1, g->n2);
+    if (allow_smem((const void *)chan_wide, sm)) return -1;
+    chan_wide<<<dim3((unsigned)n, (unsigned)nblocks), kWideThreads, sm, st>>>(a, *g);
+    return 0;
+  }
   TilePlan const *tp = host_tile_plan(plan);
   if (g_static_on.load() && !generic) {
     if (plan_is<S600>(tp)) return launch_chan_v2<S600>(a, n, nblocks, st, b->any_osc);
