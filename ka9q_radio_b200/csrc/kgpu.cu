@@ -520,7 +520,8 @@ struct kgpu_master {
   Split2 sp;
   int plan1, plan2, pitch1, pitch2;
   long spec_stride;
-  int n_item_ctas = 0;             // row-pass CTAs per block of the generic and v2 kernels (row_item(): 4 pairs or 8 rows)
+  int n_item_ctas = 0;             // CTAs per block of fwd_rows_kernel (row_item(): 4 pairs or 8 rows)
+  int n_rows_ctas = 0;             // CTAs per block of the master's own row kernel (fwd_rows_v2 REAL: 8 pairs)
   ColsKernel cols = COLS_GENERIC;
   RowsKernel rows = ROWS_GENERIC;
   bool halved = false;             // the 1/2 of the real split is folded into the column pass
@@ -558,6 +559,10 @@ static RowsV2Fn rows_v2_kernel(kgpu_master const *m) {
   if (m->in_type == KGPU_REAL) return m->halved ? fwd_rows_v2<true, 1296, true> : fwd_rows_v2<true, 0, false>;
   return m->n1c ? fwd_rows_v2<false, 1296, false> : fwd_rows_v2<false, 0, false>;
 }
+static int rows_v2_threads(kgpu_master const *m) { return m->in_type == KGPU_REAL ? RowsV2Shape<true>::T : RowsV2Shape<false>::T; }
+static size_t rows_v2_smem(kgpu_master const *m) {
+  return m->in_type == KGPU_REAL ? RowsV2Shape<true>::smem : RowsV2Shape<false>::smem;
+}
 
 static int upload(float2 **d, std::vector<float2> const &v) {
   CUDA_OK(cudaMalloc(d, sizeof(float2) * v.size()));
@@ -580,6 +585,8 @@ static int master_setup(kgpu_master *m) {
   bool const padded = m->cols == COLS_2S || (m->cols == COLS_R36 && m->rows == ROWS_V2);  // both kernels know the pitch
   m->mid_ld = padded ? (n2 + 15) / 16 * 16 : n2;
   m->n_item_ctas = real ? (n1 / 2 + 1 + 3) / 4 : (n1 + 7) / 8;
+  int const ipc = m->rows == ROWS_V2 ? (real ? RowsV2Shape<true>::IPC : RowsV2Shape<false>::IPC) : 0;
+  m->n_rows_ctas = ipc ? ((real ? n1 / 2 + 1 : n1) + ipc - 1) / ipc : m->rows == ROWS_2S ? (n1 + 7) / 8 : m->n_item_ctas;
 
   auto root = [](long e, long n) {
     long double const ang = -2.0L * M_PIl * (long double)(e % n) / (long double)n;
@@ -628,7 +635,7 @@ static int master_setup(kgpu_master *m) {
       if (allow_smem((const void *)cols_2s_kernel(f), Cols2s::smem)) return -1;
     if (allow_smem((const void *)fwd_rows_2s<25, 25>, Rows2s::smem)) return -1;
   }
-  if (m->rows == ROWS_V2 && allow_smem((const void *)rows_v2_kernel(m), RowsV2Shape::smem)) return -1;
+  if (m->rows == ROWS_V2 && allow_smem((const void *)rows_v2_kernel(m), rows_v2_smem(m))) return -1;
   // the generic pair can run for every master (kgpu_use_static_kernels(0)); a master it does not fit is rejected here
   if (allow_smem((const void *)fwd_cols_kernel<0>, m->smem1) || allow_smem((const void *)fwd_cols_kernel<1>, m->smem1) ||
       allow_smem((const void *)fwd_rows_kernel, m->smem2))
@@ -705,12 +712,12 @@ extern "C" int kgpu_master_describe(kgpu_master const *m, char *buf, int buflen)
   std::string const rc = m->cols == COLS_2S ? "25,32" : m->cols == COLS_R36 ? "36,36" : radices(host_tile_plan(m->plan1));
   std::string const rr = m->rows == ROWS_2S ? "25,25" : m->rows == ROWS_V2 ? "10,25,5" : radices(host_tile_plan(m->plan2));
   size_t const s1 = m->cols == COLS_2S ? Cols2s::smem : m->cols == COLS_R36 ? ColsR36Shape::smem : m->smem1;
-  size_t const s2 = m->rows == ROWS_2S ? Rows2s::smem : m->rows == ROWS_V2 ? RowsV2Shape::smem : m->smem2;
+  size_t const s2 = m->rows == ROWS_2S ? Rows2s::smem : m->rows == ROWS_V2 ? rows_v2_smem(m) : m->smem2;
   char const *kc = m->cols == COLS_2S ? "fwd_cols_2s" : m->cols == COLS_R36 ? "fwd_cols_r36" : "fwd_cols_kernel";
   char const *kr = m->rows == ROWS_2S ? "fwd_rows_2s" : m->rows == ROWS_V2 ? "fwd_rows_v2" : "fwd_rows_kernel";
   snprintf(buf, (size_t)buflen, "N=%d %s, %ld-point complex two-pass %d x %d; cols radices [%s] rows radices [%s]; smem %zu/%zu B; "
            "grids %d/%d CTAs per block; kernels %s + %s", m->N, m->in_type == KGPU_REAL ? "real" : "complex", m->nc, m->sp.n1,
-           m->sp.n2, rc.c_str(), rr.c_str(), s1, s2, (m->sp.n2 + kTile - 1) / kTile, m->n_item_ctas, kc, kr);
+           m->sp.n2, rc.c_str(), rr.c_str(), s1, s2, (m->sp.n2 + kTile - 1) / kTile, m->n_rows_ctas, kc, kr);
   return 0;
 }
 
@@ -766,15 +773,15 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
   a2.spec = (float2 *)d_spec;
   a2.spec_stride = m->spec_stride;
   a2.mid_ld = a1.mid_ld;
-  dim3 const g2((unsigned)m->n_item_ctas, (unsigned)nblocks);
+  dim3 const g2((unsigned)(rows == ROWS_GENERIC ? m->n_item_ctas : m->n_rows_ctas), (unsigned)nblocks);
   {
     ProfScope ps(K_FWD_ROWS, st);
     switch (rows) {
       case ROWS_2S:
-        fwd_rows_2s<25, 25><<<dim3((unsigned)((m->sp.n1 + 7) / 8), (unsigned)nblocks), Rows2s::T, Rows2s::smem, st>>>(a2, m->d_rtw0);
+        fwd_rows_2s<25, 25><<<g2, Rows2s::T, Rows2s::smem, st>>>(a2, m->d_rtw0);
         break;
       case ROWS_V2:
-        rows_v2_kernel(m)<<<g2, RowsV2Shape::T, RowsV2Shape::smem, st>>>(a2, FwdTables{m->d_rootC});
+        rows_v2_kernel(m)<<<g2, rows_v2_threads(m), rows_v2_smem(m), st>>>(a2, FwdTables{m->d_rootC});
         break;
       case ROWS_GENERIC:
         fwd_rows_kernel<<<g2, kFwdThreads, m->smem2, st>>>(a2);

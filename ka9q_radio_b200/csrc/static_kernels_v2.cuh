@@ -38,11 +38,28 @@ __device__ __forceinline__ float i32_to_f32(int v) {
 // The row pass of every master with 1250 columns, REAL and COMPLEX.  On H100 it beat a two-stage 50 x 25 row kernel
 // (DESIGN.md section 4).  Blocks are taken last-to-first: the column pass wrote the last ones most recently, so their
 // rows are the likeliest to be still in L2.
+// Tiling: a group of 256 threads runs stages 0 and 1 on 8 tile columns.  COMPLEX: one group, 8 rows per CTA.  REAL: two
+// groups, 16 columns = 8 mirrored pairs per CTA (pair i in columns 2i, 2i+1; group g holds pairs 4g..4g+3), so that a
+// warp's split stores cover 8 consecutive k1: 64-byte runs X[k1 + n1 k2] and their mirrors, instead of 32-byte runs
+// from 4 pairs.  One 512-thread CTA per SM holds about as many rows and warps as two 4-pair CTAs did.
+// Shared-memory banks, in float2 slots (bank pair = offset mod 16), PITCH = 1250 = 2 mod 16:
+//  * stages 0 and 1 touch only their group's 8 columns, at 2c mod 16: conflict-free as in the one-group form.
+//  * stage 2 reads slot col_off(2i) + 5u + m (forward row) and col_off(2i+1) - 5u + m (mirror), lane = 8 (u - u0) + i.
+//    A half-warp holds i = 0..7 at two consecutive u.  Without a skew, 2i*PITCH = 4i mod 16 puts pairs i and i+4 on the
+//    same slots (2-way).  The second group's columns start SKEW = 2 slots later: pairs 0..3 take the slots
+//    {4a + 5b} = {0,1,4,5,8,9,12,13}, pairs 4..7 the slots {2,3,6,7,10,11,14,15}, and the mirror reads
+//    {4a + 2 - 5b} likewise split into two disjoint halves: every stage-2 read is conflict-free.  SKEW = 2 float2s
+//    = 16 bytes keeps every TMA destination 16-byte aligned (PITCH * 8 = 10000 bytes is a multiple of 16).
+template <bool REAL_SPLIT>
 struct RowsV2Shape {
   using P = SPlan<1250, 10, 25, 5>;  // what choose_radices(1250) picks: the kernel reads that registry plan's stage twiddles
-  static constexpr int N2 = 1250, PITCH = 1250, T = 256;
+  static constexpr int N2 = 1250, PITCH = 1250, GT = 256, SKEW = 2;
+  static constexpr int NG = REAL_SPLIT ? 2 : 1, T = GT * NG, COLS = 8 * NG;
+  static constexpr int IPC = REAL_SPLIT ? COLS / 2 : COLS;  // work items (row pairs or rows) per CTA
   static constexpr int TW = (static_tw_count<P>() + 1) & ~1;  // stage twiddles, even (bulk copies move 16-byte multiples)
-  static constexpr size_t smem = sizeof(float2) * (size_t)(8 * PITCH + TW);
+  static constexpr int TILE = COLS * PITCH + (NG - 1) * SKEW;
+  static constexpr size_t smem = sizeof(float2) * (size_t)(TILE + TW);
+  static __host__ __device__ constexpr int col_off(int c) { return c * PITCH + (c >> 3) * SKEW; }
 };
 
 // W_1250^{32 it t} literals for stage 0 of the row pass
@@ -54,22 +71,22 @@ __device__ constexpr float kRowsTw0[3][4][2] = {
 
 // Stage-0 twiddles W^{j t}, j = ul + 32 it, are (4 values loaded once per thread) x (literal W^{32 it t}) instead of 4 loads per
 // butterfly.  Variants tried and removed again: warp-per-column stages 0/1, stage-0 butterflies in groups of 2 / 4,
-// stage-1 twiddles by products, a persistent double-buffered form, an L2 prefetch of a later CTA's rows, blocks first-to-last.
+// stage-1 twiddles by products, a persistent double-buffered form, an L2 prefetch of a later CTA's rows, blocks first-to-last,
+// REAL with 4 row pairs per 256-thread CTA (32-byte store runs; 18.2 against 13.5 us per cfg-2 block, DESIGN.md section 4).
 template <bool REAL_SPLIT, int N1C = 0, bool HALVED = false>
-__global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const a, FwdTables const tb) {
-  using S = RowsV2Shape;
-  using P = S::P;
-  constexpr int N2 = S::N2, PITCH = S::PITCH, T = S::T;
+__global__ void __launch_bounds__(RowsV2Shape<REAL_SPLIT>::T, REAL_SPLIT ? 1 : 2) fwd_rows_v2(Pass2Args const a, FwdTables const tb) {
+  using S = RowsV2Shape<REAL_SPLIT>;
+  using P = typename S::P;
+  constexpr int N2 = S::N2, T = S::T, GT = S::GT, COLS = S::COLS, IPC = S::IPC;
   constexpr int R0 = 10, S0 = 125, R1 = 25, NSUB1 = 125, S1 = 5, R2 = 5;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // [8][PITCH]
-  float2 *s_tw = tile + 8 * PITCH;
-  __shared__ __align__(8) uint64_t bars[8];
+  float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // COLS columns at S::col_off(c)
+  float2 *s_tw = tile + S::TILE;
+  __shared__ __align__(8) uint64_t bars[COLS];
   __shared__ __align__(8) uint64_t tbar;
   TilePlan const &pl = c_plans[a.plan];
   int const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int const blk = gridDim.y - 1 - blockIdx.y;
-  constexpr int IPC = REAL_SPLIT ? 4 : 8;
   int const n1 = N1C ? N1C : a.n1;
   int const item0 = blockIdx.x * IPC;
   // which global row sits in which tile column
@@ -88,7 +105,7 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
     mbar_fence_init();
     if (row >= 0) {
       mbar_expect_tx(&bars[warp], N2 * 8);
-      bulk_g2s(tile + warp * PITCH, a.mid + ((long)blk * n1 + row) * a.mid_ld, N2 * 8, &bars[warp]);
+      bulk_g2s(tile + S::col_off(warp), a.mid + ((long)blk * n1 + row) * a.mid_ld, N2 * 8, &bars[warp]);
     }
     if (warp == 0) {
       constexpr uint32_t TWB = (uint32_t)S::TW * 8u;
@@ -97,11 +114,17 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
     }
   }
   __syncthreads();
-  int const c = tid & 7, ul = tid >> 3;  // column, butterfly lane 0..31
+  int const g = tid / GT;                                  // group
+  int const c = (tid & 7) + 8 * g, ul = (tid % GT) >> 3;  // column, butterfly lane 0..31
+  // stages 0 and 1 of a group touch only its own columns: the groups meet only before stage 2
+  auto group_sync = [&] {
+    if (S::NG == 1) __syncthreads();
+    else asm volatile("bar.sync %0, %1;" ::"r"(1 + g), "n"(GT) : "memory");
+  };
   bool const col_ok = row_of(c) >= 0;
   mbar_wait(&tbar, 0);
   if (col_ok) mbar_wait(&bars[c], 0);
-  float2 *mycol = tile + c * PITCH;
+  float2 *mycol = tile + S::col_off(c);
 
   // ---- stage 0: radix 10, stride 125 (125 butterflies per column) ------------------------------
   if (col_ok) {
@@ -110,7 +133,7 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
     for (int q = 0; q < 4; q++) base[q] = s_tw[((1 << q) - 1) * S0 + ul];  // W^{ul t}, t = 1, 2, 4, 8
 #pragma unroll
     for (int it = 0; it < 4; it++) {
-      int const j = ul + (T / 8) * it;
+      int const j = ul + (GT / 8) * it;
       if (it < 3 || j < S0) {
         float2 *p = mycol + j;
         float2 x[R0], w[R0];
@@ -131,12 +154,12 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
       }
     }
   }
-  __syncthreads();
+  group_sync();
   // ---- stage 1: radix 25, 10 blocks of 125, stride 5 (50 butterflies per column) ---------------
   if (col_ok) {
     float2 const *tw1 = s_tw + P::tw_off(1);
 #pragma unroll 1
-    for (int u = ul; u < N2 / R1; u += T / 8) {
+    for (int u = ul; u < N2 / R1; u += GT / 8) {
       int const b = u / S1, j = u - b * S1;
       float2 *p = mycol + b * NSUB1 + j;
       float2 x[R1];
@@ -150,7 +173,8 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
     }
   }
   // REAL: table factors of this thread's four split butterflies, requested before the barrier
-  int const i = tid & 3, uq = tid >> 2;  // item (row pair) 0..3, butterfly lane 0..63
+  constexpr int UQ = T / IPC;               // REAL: 64 butterfly lanes per row pair
+  int const i = tid % IPC, uq = tid / IPC;  // item (row pair) 0..7, butterfly lane 0..63
   RowItem const it = row_item(item0 + i, n1, REAL_SPLIT);
   float2 rootC = make_float2(1.f, 0.f), rd[4];
   bool self_item = false;
@@ -159,7 +183,7 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
     if (it.kind == kRowPair) rootC = __ldg(tb.rootC + it.row_a);
 #pragma unroll
     for (int q = 0; q < 4; q++) {
-      int const u = uq + (T / 4) * q;
+      int const u = uq + UQ * q;
       int const t0 = u / 25, t1 = u - t0 * 25;
       rd[q] = (it.kind == kRowPair && u < N2 / R2) ? __ldg(a.rootD + t0 + 10 * t1) : make_float2(1.f, 0.f);
     }
@@ -173,7 +197,7 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
     if (col_ok) {
       float2 *dst = spec + row_of(c);
 #pragma unroll 1
-      for (int u = ul; u < N2 / R2; u += T / 8) {
+      for (int u = ul; u < N2 / R2; u += GT / 8) {
         int const t0 = u / 25, t1 = u - t0 * 25;
         int const kb = t0 + 10 * t1;
         float2 const *p = mycol + u * R2;
@@ -192,10 +216,10 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
   // W_N^{n1*k2} = exp(-i*pi*k2/1250); k2 = kb + 250 t2 -> D[kb] * exp(-i*pi*t2/5)
   int const nc = N1C ? N1C * N2 : (int)a.nc;
   if (it.kind == kRowPair) {
-    float2 const *ca = tile + (2 * i) * PITCH, *cb = tile + (2 * i + 1) * PITCH;
+    float2 const *ca = tile + S::col_off(2 * i), *cb = tile + S::col_off(2 * i + 1);
 #pragma unroll
     for (int q = 0; q < 4; q++) {
-      int const u = uq + (T / 4) * q;
+      int const u = uq + UQ * q;
       if (u >= N2 / R2) break;
       int const t0 = u / 25, t1 = u - t0 * 25;
       int const kb = t0 + 10 * t1;
@@ -224,10 +248,10 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
   }
   // rows that pair with themselves (k1 = 0 and k1 = n1/2): last stage in place, then the v1 epilogue
   if (!has_self) return;  // CTA-uniform
-  for (int s = 0; s < 4; s++) {
+  for (int s = 0; s < IPC; s++) {
     RowItem const its = row_item(item0 + s, n1, true);
     if (its.kind != kRowSelf0 && its.kind != kRowSelfMid) continue;
-    float2 *col = tile + (2 * s) * PITCH;
+    float2 *col = tile + S::col_off(2 * s);
     for (int u = tid; u < N2 / R2; u += T) {
       float2 x[R2];
 #pragma unroll
@@ -238,10 +262,10 @@ __global__ void __launch_bounds__(RowsV2Shape::T, 2) fwd_rows_v2(Pass2Args const
     }
   }
   __syncthreads();
-  for (int s = 0; s < 4; s++) {
+  for (int s = 0; s < IPC; s++) {
     RowItem const its = row_item(item0 + s, n1, true);
     if (its.kind != kRowSelf0 && its.kind != kRowSelfMid) continue;
-    float2 const *col = tile + (2 * s) * PITCH;
+    float2 const *col = tile + S::col_off(2 * s);
     float2 const rC = __ldg(tb.rootC + its.row_a);
     bool const self0 = its.kind == kRowSelf0;
     int const kend = self0 ? N2 / 2 + 1 : (N2 + 1) / 2;
