@@ -1428,6 +1428,7 @@ extern "C" int kgpu_bank_run_one_ex(kgpu_bank *b, int idx, const void *d_spec, v
   return 0;
 }
 // Noise density per channel and block from the device-resident spectrum (estimate_noise, radio.c:1783-1866).
+static_assert(sizeof(unsigned) * kMaxWideChanPoints + 4096 <= 227 * 1024, "the widest channel's noise window must fit shared memory");
 extern "C" int kgpu_bank_noise(kgpu_bank *b, const void *d_spec, int nblocks, double samprate, double *d_n0, void *stream) {
   if (!b || !d_spec || !d_n0 || nblocks < 1 || !(samprate > 0)) return fail("kgpu_bank_noise: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1447,9 +1448,14 @@ extern "C" int kgpu_bank_noise(kgpu_bank *b, const void *d_spec, int nblocks, do
   a.scale = correction / ((double)b->m->bins * samprate);
   a.n0 = d_n0;
   a.n0_stride = b->capacity;
+  int window = 0;  // every runnable channel's window lives in shared memory whole
+  for (int i = 0; i < b->nchan; i++)
+    if (b->desc[(size_t)i].plan >= 0 && b->desc[(size_t)i].points > 0) window = std::max(window, noise_window(b->desc[(size_t)i]));
+  size_t const sm = sizeof(unsigned) * (size_t)window;
+  if (allow_smem((const void *)noise_kernel, sm)) return -1;
   {
     ProfScope ps(K_NOISE, st);
-    noise_kernel<<<dim3((unsigned)b->nchan, (unsigned)nblocks), kNoiseThreads, 0, st>>>(a);
+    noise_kernel<<<dim3((unsigned)b->nchan, (unsigned)nblocks), kNoiseThreads, sm, st>>>(a);
   }
   g_launches++;
   CUDA_OK(cudaGetLastError());

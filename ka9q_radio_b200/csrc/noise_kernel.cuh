@@ -5,15 +5,21 @@
 // which forces a 13 MB device->host copy of every block's spectrum; here one double per channel and block leaves the GPU.
 //
 // One CTA per (channel, block).  Order statistics by an exact 4 x 8-bit radix select on the float bit patterns
-// (energies are >= 0, so the unsigned order is the numeric order): no sort, O(n) per pass.
+// (energies are >= 0, so the unsigned order is the numeric order): no sort, O(n) per pass.  The window's energies sit in
+// dynamic shared memory of noise_window() words of the bank's widest runnable channel (at most kMaxWideChanPoints).
 #pragma once
 #include "chan_kernels.cuh"
 
 namespace kfft {
 
 constexpr int kNoiseThreads = 128;
-constexpr int kNoiseMaxBins = 4096;   // slave bins above this are estimated from the first 4096 (the reference has no limit)
 constexpr int kMinNoiseBins = 1000;   // radio.c:76
+
+// bins estimate_noise takes around a runnable channel: max(slave->bins, Min_noise_bins) (radio.c:1794-1797)
+__host__ __device__ inline int noise_window(ChanDesc const &d) {
+  int const s_bins = (d.flags & kChanRealOut) ? d.points / 2 + 1 : d.points;  // slave->bins (filter.c:347,374)
+  return s_bins < kMinNoiseBins ? kMinNoiseBins : s_bins;
+}
 
 struct NoiseArgs {
   float2 const *spec;
@@ -61,7 +67,7 @@ __device__ inline unsigned radix_select(unsigned const *e, int n, int k, unsigne
 }
 
 __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a) {
-  __shared__ unsigned e[kNoiseMaxBins];
+  extern __shared__ unsigned e[];  // [noise_window(d)]
   __shared__ unsigned hist[256];
   __shared__ int sh[4];
   __shared__ double red_s[kNoiseThreads / 32];
@@ -74,9 +80,7 @@ __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a)
     if (tid == 0) *out = 0.0;
     return;
   }
-  int const s_bins = (d.flags & kChanRealOut) ? d.points / 2 + 1 : d.points;  // slave->bins (filter.c:347,374)
-  int nbins = s_bins < kMinNoiseBins ? kMinNoiseBins : s_bins;
-  if (nbins > kNoiseMaxBins) nbins = kNoiseMaxBins;
+  int const nbins = noise_window(d);
   int const shift = a.shift[ci], m = a.m_bins;
   float2 const *X = a.spec + (long)blk * a.spec_stride;
   int filled = nbins;
@@ -84,7 +88,7 @@ __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a)
     int mbin = abs(shift) - nbins / 2;
     if (mbin < 0) mbin = 0;
     else if (mbin + nbins > m) mbin = m - nbins;
-    if (mbin < 0) {  // master smaller than the window: the reference would read out of bounds; use what exists
+    if (nbins > m) {  // master smaller than the window: the reference would read out of bounds; use what exists
       mbin = 0;
       filled = m;
     }
@@ -208,7 +212,11 @@ __global__ void __launch_bounds__(kFmThreads) fm_front_kernel(FmArgs const a) {
   __shared__ double mean_sh;
   int const ci = blockIdx.x, blk = blockIdx.y, tid = threadIdx.x;
   ChanDesc const d = a.desc[ci];
-  if (d.plan < 0 || (d.flags & kChanRealOut) || d.olen <= 0) return;
+  if (d.plan < 0 || (d.flags & kChanRealOut) || d.olen <= 0) {
+    // the memory buffers alternate per launch: a skipped channel carries its y[-1] to the one the next launch reads
+    if (tid == 0 && blk == a.nblocks - 1) a.mem_out[ci] = a.mem_in[ci];
+    return;
+  }
   float2 const *y = a.out + (long)blk * a.out_pitch + d.out_off;
   float2 const first_prev = blk > 0 ? a.out[(long)(blk - 1) * a.out_pitch + d.out_off + d.olen - 1] : a.mem_in[ci];
   float *bb = a.baseband + (long)blk * a.bb_pitch + 2 * d.out_off;
