@@ -58,6 +58,14 @@ int kgpu_set_device(int device);
 /* ---- master: replaces create_filter_input's planning (filter.c:186-269) ------------------- */
 /* L new samples per block, impulse length M, N = L+M-1 (radio.c:582-587).  REAL needs even N. */
 kgpu_master *kgpu_master_create(int L, int M, int in_type);
+/* Same, for complex transform lengths Nc (N for COMPLEX, N/2 for REAL) whose prime factors are 2, 3, 5, 7, 11, 13,
+ * 17, 19 and 23, e.g. the AirspyHF+ at 912 kS/s (N = 22800 = 2^4 3 5^2 19); the reference transforms any N
+ * (filter.c:201).  Where Nc has factors 2, 3, 5, 7 only it is kgpu_master_create: the same kernels, plans and
+ * kgpu_master_describe string.  Otherwise the master runs the extended generic pair fwd_cols_ext + fwd_rows_ext on two
+ * column plans of its own (radices 2 .. 25 and the five primes), freed by kgpu_master_destroy; kgpu_use_static_kernels
+ * has no effect on it.  Fails for a prime factor >= 29, or when Nc has no split n1 x n2 into plannable factors of at
+ * most 4096 points, or when that split does not fit shared memory. */
+kgpu_master *kgpu_master_create_ex(int L, int M, int in_type);
 void kgpu_master_destroy(kgpu_master *m);
 int kgpu_master_points(kgpu_master const *m);       /* N */
 int kgpu_master_bins(kgpu_master const *m);         /* REAL: N/2+1, COMPLEX: N (filter.c:197) */
@@ -161,6 +169,7 @@ int kgpu_bank_fm_front(kgpu_bank *b, const void *d_out, long out_pitch, int nblo
 int kgpu_bank_commit(kgpu_bank *b, void *stream);
 /* Testing aid: 0 forces the generic runtime-plan kernels even where a compile-time specialised
  * kernel exists (both are parity-tested); it takes effect at the next launch, also for existing masters. Default 1.
+ * Masters running the extended pair (kgpu_master_create_ex) have no specialised kernels and ignore it.
  * A master's forward kernel pair (specialised where its split has one, generic otherwise) is chosen when it is created;
  * kgpu_master_describe prints it.  Kernel variants that lost on H100 are not in the library. */
 int kgpu_use_static_kernels(int on);
@@ -170,6 +179,10 @@ int kgpu_use_static_kernels(int on);
  * n = n1*n2 of a long transform. */
 int kgpu_plan_radices(int len, int *radices, int max);
 int kgpu_plan_split(long n, int *n1, int *n2);
+/* The same for the plans of kgpu_master_create_ex: the radix search also takes 11, 13, 17, 19, 23, and the split
+ * accepts factors so planned.  Where len (n) has factors 2, 3, 5, 7 only they return what the two calls above return. */
+int kgpu_plan_radices_ex(int len, int *radices, int max);
+int kgpu_plan_split_ex(long n, int *n1, int *n2);
 
 /* Multi-GPU hand-off of the block spectra (SURVEY.md 8e; replaces the per-block multicast the
  * reference leaves to the network, multicast.c): copy `bytes` (multiple of 16) from this GPU's

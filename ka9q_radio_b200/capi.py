@@ -48,6 +48,8 @@ def load() -> C.CDLL:
     L.kgpu_set_device.argtypes = [i]
     L.kgpu_master_create.restype = vp
     L.kgpu_master_create.argtypes = [i, i, i]
+    L.kgpu_master_create_ex.restype = vp
+    L.kgpu_master_create_ex.argtypes = [i, i, i]
     L.kgpu_master_destroy.argtypes = [vp]
     L.kgpu_master_points.argtypes = [vp]
     L.kgpu_master_bins.argtypes = [vp]
@@ -96,6 +98,8 @@ def load() -> C.CDLL:
     L.kgpu_profile_get.argtypes = [i, vp, vp]
     L.kgpu_plan_radices.argtypes = [i, vp, i]
     L.kgpu_plan_split.argtypes = [l, vp, vp]
+    L.kgpu_plan_radices_ex.argtypes = [i, vp, i]
+    L.kgpu_plan_split_ex.argtypes = [l, vp, vp]
     L.kgpu_multicast_copy.argtypes = [vp, vp, C.c_ulonglong, i, vp]
     L.kgpu_algorithmic_bytes.argtypes = [vp, vp, i]
     L.kgpu_algorithmic_bytes.restype = d
@@ -123,17 +127,20 @@ def profile_snapshot() -> dict[str, tuple[float, int]]:
     return out
 
 
-def plan_radices(length: int) -> list[int]:
+def plan_radices(length: int, extended: bool = False) -> list[int]:
+    """extended: the radix set of kgpu_master_create_ex (also 11, 13, 17, 19, 23)"""
     out = (C.c_int * 16)()
-    n = load().kgpu_plan_radices(length, C.cast(out, C.c_void_p), 16)
+    fn = load().kgpu_plan_radices_ex if extended else load().kgpu_plan_radices
+    n = fn(length, C.cast(out, C.c_void_p), 16)
     if n < 0:
         raise KgpuError(f"length {length} cannot be planned")
     return [out[k] for k in range(n)]
 
 
-def plan_split(n: int) -> tuple[int, int]:
+def plan_split(n: int, extended: bool = False) -> tuple[int, int]:
     a, b = C.c_int(0), C.c_int(0)
-    if load().kgpu_plan_split(n, C.cast(C.pointer(a), C.c_void_p), C.cast(C.pointer(b), C.c_void_p)) != 0:
+    fn = load().kgpu_plan_split_ex if extended else load().kgpu_plan_split
+    if fn(n, C.cast(C.pointer(a), C.c_void_p), C.cast(C.pointer(b), C.c_void_p)) != 0:
         raise KgpuError(f"{n} points cannot be split")
     return a.value, b.value
 
@@ -147,11 +154,15 @@ def check(rc: int, what: str = "") -> int:
 class Master:
     """create_filter_input's device half (reference filter.c:186-269)."""
 
-    def __init__(self, L: int, M: int, in_type: int):
+    def __init__(self, L: int, M: int, in_type: int, extended: bool = False):
+        """extended: create with kgpu_master_create_ex, which also serves transform lengths with prime factors 11, 13,
+        17, 19 and 23 (and is kgpu_master_create for every other length)"""
         self.lib = load()
-        self.h = self.lib.kgpu_master_create(L, M, in_type)
+        create = self.lib.kgpu_master_create_ex if extended else self.lib.kgpu_master_create
+        self.h = create(L, M, in_type)
         if not self.h:
-            raise KgpuError("kgpu_master_create: " + self.lib.kgpu_last_error().decode())
+            what = "kgpu_master_create_ex" if extended else "kgpu_master_create"
+            raise KgpuError(f"{what}: " + self.lib.kgpu_last_error().decode())
         self.L, self.M, self.in_type = L, M, in_type
         self.N = self.lib.kgpu_master_points(self.h)
         self.bins = self.lib.kgpu_master_bins(self.h)

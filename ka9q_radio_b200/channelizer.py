@@ -13,13 +13,15 @@ from . import capi
 
 
 class Channelizer:
-    def __init__(self, L: int, M: int, in_type: int, device: str | torch.device = "cuda:0", capacity: int = 1024):
+    def __init__(self, L: int, M: int, in_type: int, device: str | torch.device = "cuda:0", capacity: int = 1024,
+                 extended: bool = False):
+        """extended: also serve masters whose transform length has prime factors up to 23 (capi.Master)"""
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise capi.KgpuError("Channelizer needs a CUDA device; there is no CPU fallback")
         torch.cuda.set_device(self.device)
         capi.check(capi.load().kgpu_set_device(self.device.index or 0), "kgpu_set_device")
-        self.master = capi.Master(L, M, in_type)
+        self.master = capi.Master(L, M, in_type, extended)
         self.bank = capi.Bank(self.master, capacity)
         self.L, self.M, self.N, self.in_type = L, M, L + M - 1, in_type
         self.nchan = 0

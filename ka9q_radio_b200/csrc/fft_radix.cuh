@@ -1,7 +1,8 @@
 // fft_radix.cuh -- in-register DFT butterflies for the Stockham/DIF stages (sm_90a).
 //
 // Everything here works on a thread-private float2 x[R] that the compiler keeps in registers
-// (all indices are literals after unrolling).  Primitive radices 2,3,4,5,7 are written out;
+// (all indices are literals after unrolling).  Primitive radices 2,3,4,5,7 are written out, and
+// the primes 11, 13, 17, 19, 23 of the extended master kernels share one pair-form template;
 // a radix with two coprime factors (6, 10, 12, 15, 20, 24, 36 ...) is a Good-Thomas prime-factor
 // split R = R1*R2 -- index maps only, no twiddles between the two levels -- and a prime power
 // (8, 9, 16, 25 ...) a two-level Cooley-Tukey split with compile-time twiddles from wconst.cuh.  INV selects exp(+i..) (the reference's FFTW_BACKWARD, filter.c:359).
@@ -130,6 +131,42 @@ template <bool INV> struct Dft<7, INV> {
     x[4] = fms_rot<INV>(w3, 1.0f, u3);
   }
 };
+
+// Odd prime P >= 11 (the extended master kernels only): Dft<7>'s symmetric pair form written as loops.
+//   p_j = x_j + x_{P-j}, m_j = x_j - x_{P-j}  (j = 1 .. H, H = (P-1)/2)
+//   u_k = x_0 + sum_j p_j cos(2 pi jk/P),  w_k = sum_j m_j sin(2 pi jk/P),  X_k = u_k -/+ i w_k,  X_{P-k} = u_k +/- i w_k
+// The cosines and sines are wroot<P> entries (generated, correctly rounded); each sum is one fma chain in j order.
+template <int P, bool INV> struct DftPair {
+  static constexpr int H = (P - 1) / 2;
+  static KFFT_HD void run(float2 (&x)[P]) {
+    float2 const a = x[0];
+    float2 p[H], m[H];
+#pragma unroll
+    for (int j = 0; j < H; j++) {
+      p[j] = cadd(x[j + 1], x[P - 1 - j]);
+      m[j] = csub(x[j + 1], x[P - 1 - j]);
+    }
+    float2 s = p[H - 1];
+#pragma unroll
+    for (int j = H - 2; j >= 0; j--) s = cadd(p[j], s);
+    x[0] = cadd(a, s);
+#pragma unroll
+    for (int k = 1; k <= H; k++) {
+      float2 u = a, w = p_mul(m[0], bb(-wroot<P>(k).y));
+#pragma unroll
+      for (int j = 0; j < H; j++) u = p_fma(p[j], bb(wroot<P>((j + 1) * k % P).x), u);
+#pragma unroll
+      for (int j = 1; j < H; j++) w = p_fma(m[j], bb(-wroot<P>((j + 1) * k % P).y), w);
+      x[k] = fma_rot<INV>(w, 1.0f, u);
+      x[P - k] = fms_rot<INV>(w, 1.0f, u);
+    }
+  }
+};
+template <bool INV> struct Dft<11, INV> : DftPair<11, INV> {};
+template <bool INV> struct Dft<13, INV> : DftPair<13, INV> {};
+template <bool INV> struct Dft<17, INV> : DftPair<17, INV> {};
+template <bool INV> struct Dft<19, INV> : DftPair<19, INV> {};
+template <bool INV> struct Dft<23, INV> : DftPair<23, INV> {};
 
 // first factor of the two-level split for composite radices
 constexpr int split_first(int r) {

@@ -74,8 +74,23 @@ __device__ __forceinline__ void dif_stage(float2 *__restrict__ col, int len, int
   }
 }
 
-// All stages of a plan on one column.  SYNC() is the group barrier (e.g. __syncwarp).
-template <bool INV, typename Sync>
+// The stages of the extended radices (primes 11 .. 23), which only the extended master kernels compile in.
+template <bool INV>
+__device__ __forceinline__ void dif_stage_ext(int r, float2 *__restrict__ col, int len, int nsub, int s, uint32_t magic,
+                                              float2 const *__restrict__ tw, int lane, int nl) {
+  switch (r) {
+    case 11: dif_stage<11, INV>(col, len, nsub, s, magic, tw, lane, nl); break;
+    case 13: dif_stage<13, INV>(col, len, nsub, s, magic, tw, lane, nl); break;
+    case 17: dif_stage<17, INV>(col, len, nsub, s, magic, tw, lane, nl); break;
+    case 19: dif_stage<19, INV>(col, len, nsub, s, magic, tw, lane, nl); break;
+    case 23: dif_stage<23, INV>(col, len, nsub, s, magic, tw, lane, nl); break;
+    default: break;
+  }
+}
+
+// All stages of a plan on one column.  SYNC() is the group barrier (e.g. __syncwarp).  EXT also dispatches the
+// extended radices; without it the switch is exactly the one every registry-plan kernel inlines.
+template <bool INV, bool EXT = false, typename Sync>
 __device__ __forceinline__ void tile_fft(TilePlan const &pl, float2 *col, int lane, int nl, Sync sync) {
   for (int i = 0; i < pl.nstages; i++) {
     int const r = pl.radix[i], n = pl.sub[i], s = pl.stride[i];
@@ -101,7 +116,9 @@ __device__ __forceinline__ void tile_fft(TilePlan const &pl, float2 *col, int la
       KFFT_CASE(25)
       KFFT_CASE(36)
 #undef KFFT_CASE
-      default: break;
+      default:
+        if constexpr (EXT) dif_stage_ext<INV>(r, col, pl.len, n, s, mg, tw, lane, nl);
+        break;
     }
     sync();
   }

@@ -49,15 +49,18 @@ __device__ __forceinline__ float2 unit_root_f(long e, long n) {
   return make_float2((float)c, (float)-s);
 }
 
-template <int FMT /*0: float pairs, 1: int16 pairs*/>
-__global__ void __launch_bounds__(kFwdThreads, 2) fwd_cols_kernel(Pass1Args const a) {
+// The generic pair is written once: fwd_cols_body here, the row pass in fwd_rows_body.cuh.  fwd_cols_kernel /
+// fwd_rows_kernel run them on registry plans with the radix switch of every other kernel; the extended pair
+// (fwd_cols_ext / fwd_rows_ext) runs them on plans the master passes by value, with EXT adding the prime radices
+// 11 .. 23 to tile_fft.
+template <int FMT /*0: float pairs, 1: int16 pairs*/, bool EXT>
+__device__ __forceinline__ void fwd_cols_body(Pass1Args const &a, TilePlan const &pl) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float2 *tile = reinterpret_cast<float2 *>(smem_raw);             // [kTile][pitch]
   int const rows_per_it = kFwdThreads / kTile;                      // 32
   int const nit = (a.n1 + rows_per_it - 1) / rows_per_it;
   float2 *twA = tile + kTile * a.pitch;                             // [kTile][nit]
 
-  TilePlan const &pl = c_plans[a.plan];
   int const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int const c = tid % kTile, r = tid / kTile;
   int const c0 = blockIdx.x * kTile;
@@ -135,7 +138,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fwd_cols_kernel(Pass1Args cons
   __syncthreads();
 
   // ---- one warp per column: length-n1 transform in shared memory -------------------------
-  if (warp < ncols) tile_fft<false>(pl, tile + warp * a.pitch, lane, 32, [] { __syncwarp(); });
+  if (warp < ncols) tile_fft<false, EXT>(pl, tile + warp * a.pitch, lane, 32, [] { __syncwarp(); });
   __syncthreads();
 
   // ---- cooperative store with the inter-pass twiddle: mid[k1][n2] ------------------------
@@ -158,6 +161,15 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fwd_cols_kernel(Pass1Args cons
     for (; k1 < a.n1; k1 += rows_per_it, it++)
       dst[(long)k1 * a.n2] = cmul(colp[__ldg(pl.perm + k1)], cmul(twB, twc[it]));
   }
+}
+
+template <int FMT>
+__global__ void __launch_bounds__(kFwdThreads, 2) fwd_cols_kernel(Pass1Args const a) {
+  fwd_cols_body<FMT, false>(a, c_plans[a.plan]);
+}
+template <int FMT>
+__global__ void __launch_bounds__(kFwdThreads, 2) fwd_cols_ext(Pass1Args const a, __grid_constant__ TilePlan const pl) {
+  fwd_cols_body<FMT, true>(a, pl);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -201,107 +213,15 @@ struct Pass2Args {
 };
 
 __global__ void __launch_bounds__(kFwdThreads, 2) fwd_rows_kernel(Pass2Args const a) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // [kTile][pitch]
   TilePlan const &pl = c_plans[a.plan];
-  int const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  int const blk = blockIdx.y;
-  int const item0 = blockIdx.x * (a.real_split ? kTile / 2 : kTile);  // items per CTA: 4 row pairs or 8 plain rows
-
-  // ---- each warp streams its own row into its column (contiguous 8-byte loads) ------------
-  {
-    RowItem const it = row_item(item0 + (a.real_split ? warp >> 1 : warp), a.n1, a.real_split);
-    int row = -1;
-    if (a.real_split) {
-      if ((warp & 1) == 0 && it.kind != kRowEmpty) row = it.row_a;
-      if ((warp & 1) == 1 && it.kind == kRowPair) row = it.row_b;
-    } else if (it.kind == kRowPlain) {
-      row = it.row_a;
-    }
-    if (row >= 0) {
-      float2 const *src = a.mid + (long)blk * a.nc + (long)row * a.n2;
-      float2 *colp = tile + warp * a.pitch;
-      constexpr int U = 8;
-      int n2 = lane;
-      for (; n2 + (U - 1) * 32 < a.n2; n2 += U * 32) {
-        float2 w[U];
-#pragma unroll
-        for (int u = 0; u < U; u++) w[u] = __ldg(src + n2 + u * 32);
-#pragma unroll
-        for (int u = 0; u < U; u++) colp[n2 + u * 32] = w[u];
-      }
-      for (; n2 < a.n2; n2 += 32) colp[n2] = __ldg(src + n2);
-      __syncwarp();
-      tile_fft<false>(pl, colp, lane, 32, [] { __syncwarp(); });
-    }
-  }
-  __syncthreads();
-
-  float2 *spec = a.spec + (long)blk * a.spec_stride;
-  if (!a.real_split) {
-    // plain rows: X[k1 + n1*k2] = Z; 8 adjacent rows -> 64-byte segments
-    int const i = tid % kTile, q0 = tid / kTile;
-    RowItem const it = row_item(item0 + i, a.n1, false);
-    if (it.kind == kRowPlain) {
-      float2 const *colp = tile + i * a.pitch;
-      constexpr int V = 4, QS = kFwdThreads / kTile;
-      int k2 = q0;
-      for (; k2 + (V - 1) * QS < a.n2; k2 += V * QS) {
-        int slot[V];
-        float2 v[V];
-#pragma unroll
-        for (int u = 0; u < V; u++) slot[u] = __ldg(pl.perm + k2 + u * QS);
-#pragma unroll
-        for (int u = 0; u < V; u++) v[u] = colp[slot[u]];
-#pragma unroll
-        for (int u = 0; u < V; u++) spec[(long)it.row_a + (long)a.n1 * (k2 + u * QS)] = v[u];
-      }
-      for (; k2 < a.n2; k2 += QS) spec[(long)it.row_a + (long)a.n1 * k2] = colp[__ldg(pl.perm + k2)];
-    }
-    return;
-  }
-  // ---- REAL epilogue: split the packed transform, 4 adjacent rows -> 32-byte segments -----
-  int const i = tid % (kTile / 2), q0 = tid / (kTile / 2);
-  int const qstep = kFwdThreads / (kTile / 2);
-  RowItem const it = row_item(item0 + i, a.n1, true);
-  if (it.kind == kRowEmpty) return;
-  float2 const *ca = tile + (2 * i) * a.pitch;
-  float2 const *cb = (it.kind == kRowPair) ? tile + (2 * i + 1) * a.pitch : ca;
-  float2 const rootC = unit_root_f(it.row_a, 2 * a.nc);  // W_N^{k1}
-  int const kend = (it.kind == kRowPair) ? a.n2 : (it.kind == kRowSelf0 ? a.n2 / 2 + 1 : (a.n2 + 1) / 2);
-  constexpr int V = 4;
-  auto partner = [&](int k2) { return (it.kind == kRowSelf0) ? (k2 == 0 ? 0 : a.n2 - k2) : a.n2 - 1 - k2; };
-  auto emit = [&](int k2, float2 za, float2 zb, float2 rd) {
-    long const k = (long)it.row_a + (long)a.n1 * k2;
-    float2 const w = cmul(rootC, rd);  // W_N^k
-    float2 const E = make_float2(0.5f * (za.x + zb.x), 0.5f * (za.y - zb.y));
-    float2 const O = make_float2(0.5f * (za.x - zb.x), 0.5f * (za.y + zb.y));
-    float2 const P = cmul(w, O);
-    // X[k] = E - i*P ;  X[Nc-k] = conj(E + i*P)
-    spec[k] = make_float2(E.x + P.y, E.y - P.x);
-    long const km = a.nc - k;
-    if (km != k) spec[km] = make_float2(E.x - P.y, -(E.y + P.x));
-  };
-  int k2 = q0;
-  for (; k2 + (V - 1) * qstep < kend; k2 += V * qstep) {
-    int sa[V], sb[V];
-    float2 za[V], zb[V], rd[V];
-#pragma unroll
-    for (int u = 0; u < V; u++) {
-      sa[u] = __ldg(pl.perm + k2 + u * qstep);
-      sb[u] = __ldg(pl.perm + partner(k2 + u * qstep));
-      rd[u] = __ldg(a.rootD + k2 + u * qstep);
-    }
-#pragma unroll
-    for (int u = 0; u < V; u++) {
-      za[u] = ca[sa[u]];
-      zb[u] = cb[sb[u]];
-    }
-#pragma unroll
-    for (int u = 0; u < V; u++) emit(k2 + u * qstep, za[u], zb[u], rd[u]);
-  }
-  for (; k2 < kend; k2 += qstep)
-    emit(k2, ca[__ldg(pl.perm + k2)], cb[__ldg(pl.perm + partner(k2))], __ldg(a.rootD + k2));
+#define KFFT_ROWS_EXT false
+#include "fwd_rows_body.cuh"
+#undef KFFT_ROWS_EXT
+}
+__global__ void __launch_bounds__(kFwdThreads, 2) fwd_rows_ext(Pass2Args const a, __grid_constant__ TilePlan const pl) {
+#define KFFT_ROWS_EXT true
+#include "fwd_rows_body.cuh"
+#undef KFFT_ROWS_EXT
 }
 
 // ---------------------------------------------------------------------------------------------

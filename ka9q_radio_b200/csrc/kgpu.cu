@@ -263,6 +263,10 @@ extern "C" int kgpu_set_device(int device) {
 namespace kfft {
 
 static int const kRadixSet[] = {25, 24, 20, 16, 15, 12, 10, 9, 8, 7, 6, 5, 4, 3, 2};
+// The extended set of masters created with kgpu_master_create_ex: the same radices, then the five primes.  A prime
+// above 7 divides no radix of kRadixSet, so every factorisation carries each of them as its own stage, and on a length
+// with factors 2, 3, 5, 7 only the search visits exactly what it visits with kRadixSet.
+static int const kRadixSetExt[] = {25, 24, 20, 16, 15, 12, 10, 9, 8, 7, 6, 5, 4, 3, 2, 23, 19, 17, 13, 11};
 
 // Every length the registry accepts has prime factors 2, 3, 5, 7 only and is at most kMaxChanPoints: masters split into
 // lengths <= kMaxTileLen and kgpu_bank_define rejects channels whose transform the channel kernel cannot hold.  If all
@@ -281,9 +285,10 @@ constexpr int plannable_lengths(int max) {
 }
 static_assert(plannable_lengths(kMaxChanPoints) <= kMaxPlans, "the plan registry must hold every plannable length");
 
-// exhaustive search over multisets of supported radices (depth <= kMaxStages): fewest stages,
+// exhaustive search over multisets of the radices set[0 .. nset) (depth <= kMaxStages): fewest stages,
 // then smallest sum.
-static void search(int n, int start, std::vector<int> &cur, std::vector<int> &best, int &best_sum) {
+static void search(int const *set, int nset, int n, int start, std::vector<int> &cur, std::vector<int> &best,
+                   int &best_sum) {
   if (n == 1) {
     int sum = 0;
     for (int r : cur) sum += r;
@@ -295,20 +300,20 @@ static void search(int n, int start, std::vector<int> &cur, std::vector<int> &be
   }
   if ((int)cur.size() >= kMaxStages) return;
   if (!best.empty() && cur.size() + 1 > best.size()) return;
-  for (int i = start; i < (int)(sizeof kRadixSet / sizeof kRadixSet[0]); i++) {
-    int const r = kRadixSet[i];
+  for (int i = start; i < nset; i++) {
+    int const r = set[i];
     if (n % r) continue;
     cur.push_back(r);
-    search(n / r, i, cur, best, best_sum);
+    search(set, nset, n / r, i, cur, best, best_sum);
     cur.pop_back();
   }
 }
 
-std::vector<int> choose_radices(int n) {
+static std::vector<int> radices_from(int const *set, int nset, int n) {
   std::vector<int> cur, best;
   int best_sum = 0;
   if (n < 2) return best;
-  search(n, 0, cur, best, best_sum);
+  search(set, nset, n, 0, cur, best, best_sum);
   // even radices first (descending): power-of-two strides stay away from the unit-stride stages;
   // odd ones last, descending: the last (unit-stride) stage gets the smallest radix, which is the
   // one the v2 kernels fuse with the global store / real split (fewest registers per butterfly)
@@ -320,6 +325,11 @@ std::vector<int> choose_radices(int n) {
   return best;
 }
 
+std::vector<int> choose_radices(int n) { return radices_from(kRadixSet, (int)(sizeof kRadixSet / sizeof kRadixSet[0]), n); }
+std::vector<int> choose_radices_ext(int n) {
+  return radices_from(kRadixSetExt, (int)(sizeof kRadixSetExt / sizeof kRadixSetExt[0]), n);
+}
+
 struct PlanSlot {
   int len = 0;
   TilePlan host;  // device pointers inside
@@ -327,16 +337,8 @@ struct PlanSlot {
 static std::mutex g_plan_mu;
 static std::vector<PlanSlot> g_plans;
 
-int get_tile_plan(int len) {
-  std::lock_guard<std::mutex> lk(g_plan_mu);
-  for (size_t i = 0; i < g_plans.size(); i++)
-    if (g_plans[i].len == len) return (int)i;
-  std::vector<int> rad;
-  if (len > 1) rad = choose_radices(len);
-  if (len < 1 || len > kMaxChanPoints || (len > 1 && rad.empty()))
-    return fail("%d-point transform cannot be planned (factors 2, 3, 5, 7; at most %d points)", len, kMaxChanPoints);
-  if ((int)g_plans.size() >= kMaxPlans) return fail("plan registry full (%d plans)", kMaxPlans);
-  TilePlan p;
+// Builds the column plan of `len` with stages `rad` and uploads its twiddle and perm tables (freed with free_tile_plan).
+static int make_tile_plan(int len, std::vector<int> const &rad, TilePlan &p) {
   memset(&p, 0, sizeof p);
   p.len = len;
   p.nstages = (int)rad.size();
@@ -373,21 +375,45 @@ int get_tile_plan(int len) {
   tw.push_back(make_float2(0.f, 0.f));
   p.tw = nullptr;
   p.perm = nullptr;
-  int const idx = (int)g_plans.size();
   auto upload = [&]() -> int {
     CUDA_OK(cudaMalloc(&d_tw, sizeof(float2) * tw.size()));
     CUDA_OK(cudaMalloc(&d_perm, sizeof(uint16_t) * (size_t)len));
     CUDA_OK(cudaMemcpy(d_tw, tw.data(), sizeof(float2) * tw.size(), cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(d_perm, perm.data(), sizeof(uint16_t) * (size_t)len, cudaMemcpyHostToDevice));
-    p.tw = d_tw;
-    p.perm = d_perm;
-    CUDA_OK(cudaMemcpyToSymbol(c_plans, &p, sizeof p, sizeof(TilePlan) * (size_t)idx));
     return 0;
   };
   if (upload()) {  // the CUDA error is in kgpu_last_error()
     cudaFree(d_tw);
     cudaFree(d_perm);
     return -1;
+  }
+  p.tw = d_tw;
+  p.perm = d_perm;
+  return 0;
+}
+static void free_tile_plan(TilePlan &p) {
+  cudaFree((void *)p.tw);
+  cudaFree((void *)p.perm);
+  p.tw = nullptr;
+  p.perm = nullptr;
+}
+
+int get_tile_plan(int len) {
+  std::lock_guard<std::mutex> lk(g_plan_mu);
+  for (size_t i = 0; i < g_plans.size(); i++)
+    if (g_plans[i].len == len) return (int)i;
+  std::vector<int> rad;
+  if (len > 1) rad = choose_radices(len);
+  if (len < 1 || len > kMaxChanPoints || (len > 1 && rad.empty()))
+    return fail("%d-point transform cannot be planned (factors 2, 3, 5, 7; at most %d points)", len, kMaxChanPoints);
+  if ((int)g_plans.size() >= kMaxPlans) return fail("plan registry full (%d plans)", kMaxPlans);
+  TilePlan p;
+  if (make_tile_plan(len, rad, p)) return -1;
+  int const idx = (int)g_plans.size();
+  cudaError_t const e = cudaMemcpyToSymbol(c_plans, &p, sizeof p, sizeof(TilePlan) * (size_t)idx);
+  if (e != cudaSuccess) {
+    free_tile_plan(p);
+    return fail("cudaMemcpyToSymbol(c_plans): %s", cudaGetErrorString(e));
   }
   PlanSlot sl;
   sl.len = len;
@@ -398,14 +424,16 @@ int get_tile_plan(int len) {
 TilePlan const *host_tile_plan(int idx) { return &g_plans[(size_t)idx].host; }
 
 static bool plannable(int len) { return len == 1 || (len <= kMaxTileLen && !choose_radices(len).empty()); }
+static bool plannable_ext(int len) { return len == 1 || (len <= kMaxTileLen && !choose_radices_ext(len).empty()); }
 
-bool choose_split(long n, Split2 *out) {
+// the largest d <= sqrt(n) with n = (n / d) * d, n / d <= kMaxTileLen and both factors plannable
+template <bool (*Plannable)(int)> static bool split_with(long n, Split2 *out) {
   long best = -1;
   for (long d = (long)floor(sqrt((double)n) + 1e-9); d >= 1; d--) {
     if (n % d) continue;
     long const a = n / d;  // a >= d
     if (a > kMaxTileLen) break;
-    if (plannable((int)a) && plannable((int)d)) {
+    if (Plannable((int)a) && Plannable((int)d)) {
       best = d;
       break;
     }
@@ -415,6 +443,8 @@ bool choose_split(long n, Split2 *out) {
   out->n2 = (int)best;
   return true;
 }
+bool choose_split(long n, Split2 *out) { return split_with<plannable>(n, out); }
+bool choose_split_ext(long n, Split2 *out) { return split_with<plannable_ext>(n, out); }
 
 // choose_split restated at compile time (a length <= kMaxTileLen is plannable iff its factors are 2, 3, 5, 7), to pin
 // kMaxWideChanPoints: every such length above kMaxChanPoints up to it fits chan_wide's shared memory, the next does not.
@@ -534,6 +564,10 @@ struct kgpu_master {
   float2 *d_mid = nullptr;
   int mid_blocks = 0;
   size_t smem1 = 0, smem2 = 0;     // generic kernels
+  // kgpu_master_create_ex with a prime factor 11 .. 23: the master owns its two plans (plan1 / plan2 stay -1) and runs
+  // the extended pair fwd_cols_ext / fwd_rows_ext, which take them by value
+  bool ext = false;
+  TilePlan xplan1{}, xplan2{};
   // notches
   NotchDev *d_notch = nullptr;
   int n_notch = 0;
@@ -686,8 +720,89 @@ extern "C" kgpu_master *kgpu_master_create(int L, int M, int in_type) {
   return m;
 }
 
+// kgpu_master_create for transform lengths whose prime factors go up to 23.  A length with factors 2, 3, 5, 7 only is
+// kgpu_master_create itself.  Any other gets the extended generic pair on two plans of its own, so the registry, which
+// keeps room for every length a 7-smooth master or channel can ask for, never sees them.
+#define KGPU_EXT_FACTORS "2, 3, 5, 7, 11, 13, 17, 19, 23"
+extern "C" kgpu_master *kgpu_master_create_ex(int L, int M, int in_type) {
+  if (L < 1 || M < 1 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX)) {
+    fail("kgpu_master_create_ex: bad arguments L=%d M=%d type=%d", L, M, in_type);
+    return nullptr;
+  }
+  int const N = L + M - 1;
+  if (in_type == KGPU_REAL && ((N & 1) || (L & 1))) {
+    fail("kgpu_master_create_ex: REAL input needs even L and even N=L+M-1 (got L=%d N=%d)", L, N);
+    return nullptr;
+  }
+  long const nc = (in_type == KGPU_COMPLEX) ? N : N / 2;
+  if (smooth7(nc)) return kgpu_master_create(L, M, in_type);
+  long rest = nc;
+  for (long p : {2, 3, 5, 7, 11, 13, 17, 19, 23})
+    while (rest % p == 0) rest /= p;
+  if (rest != 1) {
+    long q = 29;  // the smallest prime factor left
+    while (q * q <= rest && rest % q) q++;
+    if (rest % q) q = rest;
+    fail("kgpu_master_create_ex: %ld points have the prime factor %ld (accepted factors " KGPU_EXT_FACTORS ")", nc, q);
+    return nullptr;
+  }
+  Split2 sp;
+  if (!choose_split_ext(nc, &sp)) {
+    fail("kgpu_master_create_ex: %ld points cannot be split into two plannable lengths (factors " KGPU_EXT_FACTORS
+         "; <= %d)", nc, kMaxTileLen);
+    return nullptr;
+  }
+  size_t const smem1 = sizeof(float2) * ((size_t)kTile * column_pitch(sp.n1) + (size_t)kTile * ((sp.n1 + 31) / 32));
+  size_t const smem2 = sizeof(float2) * ((size_t)kTile * column_pitch(sp.n2));
+  if (smem1 > (size_t)kChanSmemLimit || smem2 > (size_t)kChanSmemLimit) {
+    fail("kgpu_master_create_ex: %ld points split as %d x %d, which needs %zu / %zu B of shared memory (at most %d; "
+         "factors " KGPU_EXT_FACTORS ")", nc, sp.n1, sp.n2, smem1, smem2, kChanSmemLimit);
+    return nullptr;
+  }
+  kgpu_master *m = new kgpu_master;
+  m->L = L;
+  m->M = M;
+  m->N = N;
+  m->in_type = in_type;
+  m->bins = (in_type == KGPU_COMPLEX) ? N : N / 2 + 1;
+  m->nc = nc;
+  m->sp = sp;
+  m->ext = true;
+  m->plan1 = m->plan2 = -1;
+  m->pitch1 = column_pitch(sp.n1);
+  m->pitch2 = column_pitch(sp.n2);
+  m->smem1 = smem1;
+  m->smem2 = smem2;
+  m->spec_stride = ((long)m->bins + 3) / 4 * 4;
+  bool const real = in_type == KGPU_REAL;
+  m->mid_ld = sp.n2;
+  m->n_item_ctas = m->n_rows_ctas = real ? (sp.n1 / 2 + 1 + 3) / 4 : (sp.n1 + 7) / 8;
+  bool ok = make_tile_plan(sp.n1, choose_radices_ext(sp.n1), m->xplan1) == 0 &&
+            make_tile_plan(sp.n2, choose_radices_ext(sp.n2), m->xplan2) == 0;
+  if (ok && real) {
+    std::vector<float2> rootD((size_t)sp.n2);
+    for (int k2 = 0; k2 < sp.n2; k2++) {
+      long double const ang = -M_PIl * (long double)k2 / (long double)sp.n2;
+      rootD[(size_t)k2] = make_float2((float)cosl(ang), (float)sinl(ang));
+    }
+    ok = upload(&m->d_rootD, rootD) == 0;
+  }
+  ok = ok && !allow_smem((const void *)fwd_cols_ext<0>, smem1) && !allow_smem((const void *)fwd_cols_ext<1>, smem1) &&
+       !allow_smem((const void *)fwd_rows_ext, smem2);
+  if (!ok) {
+    fail("kgpu_master_create_ex: %s", std::string(g_err).c_str());
+    kgpu_master_destroy(m);
+    return nullptr;
+  }
+  return m;
+}
+
 extern "C" void kgpu_master_destroy(kgpu_master *m) {
   if (!m) return;
+  if (m->ext) {
+    free_tile_plan(m->xplan1);
+    free_tile_plan(m->xplan2);
+  }
   cudaFree(m->d_rootD);
   cudaFree(m->d_rootC);
   cudaFree(m->d_tw0);
@@ -709,12 +824,13 @@ extern "C" int kgpu_master_describe(kgpu_master const *m, char *buf, int buflen)
     return r;
   };
   // the tile plans are what the generic kernels run
-  std::string const rc = m->cols == COLS_2S ? "25,32" : m->cols == COLS_R36 ? "36,36" : radices(host_tile_plan(m->plan1));
-  std::string const rr = m->rows == ROWS_2S ? "25,25" : m->rows == ROWS_V2 ? "10,25,5" : radices(host_tile_plan(m->plan2));
+  TilePlan const *p1 = m->ext ? &m->xplan1 : host_tile_plan(m->plan1), *p2 = m->ext ? &m->xplan2 : host_tile_plan(m->plan2);
+  std::string const rc = m->cols == COLS_2S ? "25,32" : m->cols == COLS_R36 ? "36,36" : radices(p1);
+  std::string const rr = m->rows == ROWS_2S ? "25,25" : m->rows == ROWS_V2 ? "10,25,5" : radices(p2);
   size_t const s1 = m->cols == COLS_2S ? Cols2s::smem : m->cols == COLS_R36 ? ColsR36Shape::smem : m->smem1;
   size_t const s2 = m->rows == ROWS_2S ? Rows2s::smem : m->rows == ROWS_V2 ? rows_v2_smem(m) : m->smem2;
-  char const *kc = m->cols == COLS_2S ? "fwd_cols_2s" : m->cols == COLS_R36 ? "fwd_cols_r36" : "fwd_cols_kernel";
-  char const *kr = m->rows == ROWS_2S ? "fwd_rows_2s" : m->rows == ROWS_V2 ? "fwd_rows_v2" : "fwd_rows_kernel";
+  char const *kc = m->ext ? "fwd_cols_ext" : m->cols == COLS_2S ? "fwd_cols_2s" : m->cols == COLS_R36 ? "fwd_cols_r36" : "fwd_cols_kernel";
+  char const *kr = m->ext ? "fwd_rows_ext" : m->rows == ROWS_2S ? "fwd_rows_2s" : m->rows == ROWS_V2 ? "fwd_rows_v2" : "fwd_rows_kernel";
   snprintf(buf, (size_t)buflen, "N=%d %s, %ld-point complex two-pass %d x %d; cols radices [%s] rows radices [%s]; smem %zu/%zu B; "
            "grids %d/%d CTAs per block; kernels %s + %s", m->N, m->in_type == KGPU_REAL ? "real" : "complex", m->nc, m->sp.n1,
            m->sp.n2, rc.c_str(), rr.c_str(), s1, s2, (m->sp.n2 + kTile - 1) / kTile, m->n_rows_ctas, kc, kr);
@@ -755,7 +871,9 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
         cols_r36_kernel(m, f)<<<g1, ColsR36Shape::T, ColsR36Shape::smem, st>>>(a1, ColsR36Tables{m->d_tw0, m->d_twA, m->d_twB});
         break;
       case COLS_GENERIC:
-        if (f) fwd_cols_kernel<1><<<g1, kFwdThreads, m->smem1, st>>>(a1);
+        if (m->ext && f) fwd_cols_ext<1><<<g1, kFwdThreads, m->smem1, st>>>(a1, m->xplan1);
+        else if (m->ext) fwd_cols_ext<0><<<g1, kFwdThreads, m->smem1, st>>>(a1, m->xplan1);
+        else if (f) fwd_cols_kernel<1><<<g1, kFwdThreads, m->smem1, st>>>(a1);
         else fwd_cols_kernel<0><<<g1, kFwdThreads, m->smem1, st>>>(a1);
         break;
     }
@@ -784,7 +902,8 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
         rows_v2_kernel(m)<<<g2, rows_v2_threads(m), rows_v2_smem(m), st>>>(a2, FwdTables{m->d_rootC});
         break;
       case ROWS_GENERIC:
-        fwd_rows_kernel<<<g2, kFwdThreads, m->smem2, st>>>(a2);
+        if (m->ext) fwd_rows_ext<<<g2, kFwdThreads, m->smem2, st>>>(a2, m->xplan2);
+        else fwd_rows_kernel<<<g2, kFwdThreads, m->smem2, st>>>(a2);
         break;
     }
   }
@@ -1500,6 +1619,19 @@ extern "C" int kgpu_plan_radices(int len, int *radices, int max) {
   if (len != 1 && r.empty()) return -1;
   for (int i = 0; i < (int)r.size() && i < max; i++) radices[i] = r[(size_t)i];
   return (int)r.size();
+}
+extern "C" int kgpu_plan_radices_ex(int len, int *radices, int max) {
+  std::vector<int> r = choose_radices_ext(len);
+  if (len != 1 && r.empty()) return -1;
+  for (int i = 0; i < (int)r.size() && i < max; i++) radices[i] = r[(size_t)i];
+  return (int)r.size();
+}
+extern "C" int kgpu_plan_split_ex(long n, int *n1, int *n2) {
+  Split2 sp;
+  if (!choose_split_ext(n, &sp)) return -1;
+  *n1 = sp.n1;
+  *n2 = sp.n2;
+  return 0;
 }
 extern "C" int kgpu_plan_split(long n, int *n1, int *n2) {
   Split2 sp;

@@ -15,6 +15,9 @@ constexpr int kMaxTileLen = 4096;
 // Factor n into supported in-register radices: fewest stages, then smallest radix sum; even
 // radices first (large strides are bank-conflict free), odd ones last.  Empty result = unsupported.
 std::vector<int> choose_radices(int n);
+// The same search over the extended set (today's radices plus the primes 11, 13, 17, 19, 23) that masters created with
+// kgpu_master_create_ex use.  On a length with factors 2, 3, 5, 7 only it returns exactly choose_radices(n).
+std::vector<int> choose_radices_ext(int n);
 
 // Returns the registry index of the column plan for `len` (creating and uploading it on first
 // use), or -1 if len cannot be planned.  Thread-safe.
@@ -35,5 +38,8 @@ struct Split2 {
   int n1, n2;
 };
 bool choose_split(long n, Split2 *out);
+// choose_split with choose_radices_ext deciding what is plannable (equal to choose_split where n has factors 2, 3, 5, 7).
+// Its plans never enter the registry: an extended master builds and owns them.
+bool choose_split_ext(long n, Split2 *out);
 
 }  // namespace kfft
