@@ -112,6 +112,12 @@ int kgpu_bank_define_ex(kgpu_bank *b, int idx, int olen, int out_type);
  * points splits into two factors of at most 4096 with factors 2, 3, 5, 7 (every such length in range does).  Every
  * other bank call treats such a channel like any other. */
 int kgpu_bank_define_wide(kgpu_bank *b, int idx, int olen, int out_type);
+/* Same, up to 1048576 points (e.g. the 1.536 MS/s websdr channels of an RX888 at 64.8 MS/s: 38400 points at overlap 5,
+ * 368640 at 120 ms blocks): at most 28812 points it is kgpu_bank_define_wide; above that the channel runs a four-step
+ * inverse transform in two kernels through a scratch buffer in global memory that the bank owns (grown on demand, at
+ * most about 128 MB per stream), provided points has factors 2, 3, 5, 7 only (every such length in range then splits
+ * into two factors of at most 4096).  Every other bank call treats such a channel like any other. */
+int kgpu_bank_define_huge(kgpu_bank *b, int idx, int olen, int out_type);
 /* set_filter (filter.c:968-1045): Kaiser-windowed sinc designed on the host in double, forward
  * transformed on the device.  low/high are fractions of the output rate. */
 int kgpu_bank_set_filter(kgpu_bank *b, int idx, double low, double high, double kaiser_beta);

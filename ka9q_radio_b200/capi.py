@@ -81,6 +81,7 @@ def load() -> C.CDLL:
     L.kgpu_unpack_airspy12.argtypes = [vp, l, vp, vp, vp]
     L.kgpu_bank_define_ex.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_wide.argtypes = [vp, i, i, i]
+    L.kgpu_bank_define_huge.argtypes = [vp, i, i, i]
     L.kgpu_bank_set_weights.argtypes = [vp, i, d, d, d, d]
     L.kgpu_bank_set_osc.argtypes = [vp, i, i, d, d, d, d]
     L.kgpu_bank_get_osc_phase.argtypes = [vp, i, vp]
@@ -211,6 +212,11 @@ class Bank:
     def define_wide(self, idx, olen, out_type=KGPU_COMPLEX) -> int:
         """define() without its 7260-point limit: longer channels (up to 28812 points) run the four-step channel kernel."""
         return check(self.lib.kgpu_bank_define_wide(self.h, idx, olen, out_type), "kgpu_bank_define_wide")
+
+    def define_huge(self, idx, olen, out_type=KGPU_COMPLEX) -> int:
+        """define_wide() up to 1048576 points: channels longer than 28812 points run the two-kernel four-step channel
+        transform through the bank's global scratch."""
+        return check(self.lib.kgpu_bank_define_huge(self.h, idx, olen, out_type), "kgpu_bank_define_huge")
 
     def set_weights(self, idx, i_weight=1.0, q_weight=0.0):
         """set_filter_weights (filter.c:922-929)"""

@@ -16,6 +16,7 @@
 
 #include "../../include/ka9q_gpu.h"
 #include "chan_kernels.cuh"
+#include "chan_huge.cuh"
 #include "chan_wide.cuh"
 #include "fwd_kernels.cuh"
 #include "noise_kernel.cuh"
@@ -529,6 +530,58 @@ static WideGeom const *get_wide_geom(int points) {
   }
   g.tw = d_tw;
   return &(g_wide[points] = g);
+}
+
+// Pins kMaxHugeChanPoints: every length with factors 2, 3, 5, 7 in (kMaxWideChanPoints, kMaxHugeChanPoints] splits
+// into two plannable factors whose kTile-column tiles fit shared memory (the largest factor is 2401, for 823 543 =
+// 2401 x 343), and there are 806 of them.  The lengths are enumerated by their exponents to keep the evaluation short.
+constexpr bool huge_fits(long n) {
+  long d = 1;
+  while ((d + 1) * (d + 1) <= n) d++;
+  for (; d >= 1; d--) {
+    if (n % d) continue;
+    if (n / d > kMaxTileLen) return false;
+    if (smooth7(n / d) && smooth7(d)) return huge_smem_bytes((int)(n / d)) <= kChanSmemLimit && huge_smem_bytes((int)d) <= kChanSmemLimit;
+  }
+  return false;
+}
+constexpr long huge_lengths(long lo, long hi) {  // how many 7-smooth lengths in (lo, hi]; -1 if one does not fit
+  long count = 0;
+  for (long a = 1; a <= hi; a *= 2)
+    for (long b = a; b <= hi; b *= 3)
+      for (long c = b; c <= hi; c *= 5)
+        for (long e = c; e <= hi; e *= 7)
+          if (e > lo) {
+            if (!huge_fits(e)) return -1;
+            count++;
+          }
+  return count;
+}
+static_assert(huge_lengths(kMaxWideChanPoints, kMaxHugeChanPoints) == 806, "a huge length does not split or fit");
+
+// Four-step geometry of every huge length used so far (never freed; no tables: the kernels compute their twiddles).
+static std::mutex g_huge_mu;
+static std::map<int, HugeGeom> g_huge;
+
+static HugeGeom const *get_huge_geom(int points) {
+  std::lock_guard<std::mutex> lk(g_huge_mu);
+  auto it = g_huge.find(points);
+  if (it != g_huge.end()) return &it->second;
+  Split2 sp;
+  if (!choose_split(points, &sp)) {
+    fail("%d-point transform cannot be split into two plannable lengths (factors 2, 3, 5, 7; each at most %d)", points,
+         kMaxTileLen);
+    return nullptr;
+  }
+  HugeGeom g;
+  g.n1 = sp.n1;
+  g.n2 = sp.n2;
+  g.pitch1 = huge_pitch(sp.n1);
+  g.pitch2 = huge_pitch(sp.n2);
+  g.plan1 = get_tile_plan(sp.n1);
+  g.plan2 = get_tile_plan(sp.n2);
+  if (g.plan1 < 0 || g.plan2 < 0) return nullptr;
+  return &(g_huge[points] = g);
 }
 }  // namespace kfft
 
@@ -1070,7 +1123,36 @@ struct kgpu_bank {
   long block_counter = 0;     // index of the next block a run will process (oscillator epoch arithmetic)
   long last_rebase = 0;
   bool any_osc = false;
+  // global scratch of the huge channels (chan_huge.cuh) and of noise_kernel_gm, one buffer per stream so that launches
+  // on different streams (a batched run and a run_one) never share one; grown on demand, freed in kgpu_bank_destroy
+  std::mutex scratch_mu;
+  std::map<cudaStream_t, std::pair<void *, size_t>> scratch;
 };
+
+// Bound on one launch's huge-channel scratch: chan_huge loops over chunks of channels and blocks to stay below it.
+static constexpr long kHugeScratchCap = 128L << 20;
+
+// the scratch buffer of stream `st`, at least `bytes` long (nullptr and kgpu_last_error() on failure)
+static void *bank_scratch(kgpu_bank *b, cudaStream_t st, size_t bytes) {
+  std::lock_guard<std::mutex> lk(b->scratch_mu);
+  auto &s = b->scratch[st];
+  if (s.second >= bytes) return s.first;
+  if (cudaStreamSynchronize(st) != cudaSuccess) {  // earlier launches on this stream may still use the old buffer
+    fail("bank scratch: cudaStreamSynchronize: %s", cudaGetErrorString(cudaGetLastError()));
+    return nullptr;
+  }
+  cudaFree(s.first);
+  s.first = nullptr;
+  s.second = 0;
+  cudaError_t const e = cudaMalloc(&s.first, bytes);
+  if (e != cudaSuccess) {
+    s.first = nullptr;
+    fail("bank scratch: cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e));
+    return nullptr;
+  }
+  s.second = bytes;
+  return s.first;
+}
 
 static void resolve_walk(kgpu_master const *m, ChanHost const &c, ChanDesc &d) {
   int const ns = c.points, mb = m->bins, half = ns / 2;
@@ -1232,11 +1314,12 @@ extern "C" void kgpu_bank_destroy(kgpu_bank *b) {
   cudaFree(b->d_shift);
   cudaFree(b->d_fm_mem[0]);
   cudaFree(b->d_fm_mem[1]);
+  for (auto &s : b->scratch) cudaFree(s.second.first);
   delete b;
 }
 static bool bad_idx(kgpu_bank const *b, int idx) { return !b || idx < 0 || idx >= b->capacity; }
 
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok);
+static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok = false);
 extern "C" int kgpu_bank_define(kgpu_bank *b, int idx, int olen) { return bank_define(b, idx, olen, false, false); }
 extern "C" int kgpu_bank_define_ex(kgpu_bank *b, int idx, int olen, int out_type) {
   if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_ex: out_type must be KGPU_COMPLEX or KGPU_REAL");
@@ -1246,7 +1329,11 @@ extern "C" int kgpu_bank_define_wide(kgpu_bank *b, int idx, int olen, int out_ty
   if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_wide: out_type must be KGPU_COMPLEX or KGPU_REAL");
   return bank_define(b, idx, olen, out_type == KGPU_REAL, true);
 }
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok) {
+extern "C" int kgpu_bank_define_huge(kgpu_bank *b, int idx, int olen, int out_type) {
+  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_huge: out_type must be KGPU_COMPLEX or KGPU_REAL");
+  return bank_define(b, idx, olen, out_type == KGPU_REAL, true, true);
+}
+static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok) {
   if (bad_idx(b, idx) || olen < 1) return fail("kgpu_bank_define: bad arguments");
   long const num = (long)olen * b->m->N;
   if (num % b->m->L) return fail("invalid output length %d for N=%d L=%d (filter.c:312-316)", olen, b->m->N, b->m->L);
@@ -1254,15 +1341,22 @@ static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide
   if (real_out && (points & 1)) return fail("kgpu_bank_define: REAL-output slaves need an even number of points (got %d)", points);
   // the channel kernel holds kChanWarps transforms of this length in shared memory; the bound also keeps the plan
   // registry from filling (see kMaxPlans).  Longer channels (kgpu_bank_define_wide) run chan_wide, one CTA each, on
-  // a split into two registry lengths; their descriptor's plan is that of the first factor (>= 0: runnable).
+  // a split into two registry lengths; their descriptor's plan is that of the first factor (>= 0: runnable).  Beyond
+  // kMaxWideChanPoints (kgpu_bank_define_huge) the same holds for chan_huge's split.
   int plan;
   if (points <= kMaxChanPoints) {
     plan = get_tile_plan(points);
     if (plan < 0) return fail("kgpu_bank_define: %s", std::string(g_err).c_str());
   } else if (!wide_ok) {
     return fail("kgpu_bank_define: %d-point inverse transform exceeds the %d-point maximum", points, kMaxChanPoints);
-  } else if (points > kMaxWideChanPoints) {
+  } else if (points > kMaxWideChanPoints && !huge_ok) {
     return fail("kgpu_bank_define_wide: %d-point inverse transform exceeds the %d-point maximum", points, kMaxWideChanPoints);
+  } else if (points > kMaxHugeChanPoints) {
+    return fail("kgpu_bank_define_huge: %d-point inverse transform exceeds the %d-point maximum", points, kMaxHugeChanPoints);
+  } else if (points > kMaxWideChanPoints) {
+    HugeGeom const *g = get_huge_geom(points);
+    if (!g) return fail("kgpu_bank_define_huge: %s", std::string(g_err).c_str());
+    plan = g->plan1;
   } else {
     WideGeom const *g = get_wide_geom(points);
     if (!g) return fail("kgpu_bank_define_wide: %s", std::string(g_err).c_str());
@@ -1312,7 +1406,18 @@ static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *ho
   if (on_stream) CUDA_OK(cudaStreamSynchronize(st));
   else CUDA_OK(cudaDeviceSynchronize());
   CUDA_OK(cudaMemcpyAsync(dst, host, sizeof(float2) * (size_t)c.points, cudaMemcpyHostToDevice, st));
-  if (transform && c.points > kMaxChanPoints) {
+  if (transform && c.points > kMaxWideChanPoints) {
+    HugeGeom const *g = get_huge_geom(c.points);
+    if (!g) return -1;
+    float2 *scr = (float2 *)bank_scratch(b, st, sizeof(float2) * (size_t)c.points);
+    if (!scr) return -1;
+    size_t const sm1 = (size_t)huge_smem_bytes(g->n1), sm2 = (size_t)huge_smem_bytes(g->n2);
+    if (allow_smem((const void *)response_huge_cols, sm1) || allow_smem((const void *)response_huge_rows, sm2)) return -1;
+    response_huge_cols<<<(unsigned)((g->n2 + kTile - 1) / kTile), kHugeThreads, sm1, st>>>(dst, *g, scr);
+    response_huge_rows<<<(unsigned)((g->n1 + kTile - 1) / kTile), kHugeThreads, sm2, st>>>(dst, *g, scr);
+    g_launches += 2;
+    CUDA_OK(cudaGetLastError());
+  } else if (transform && c.points > kMaxChanPoints) {
     WideGeom const *g = get_wide_geom(c.points);
     if (!g) return -1;
     size_t const sm = (size_t)wide_smem_bytes(g->n1, g->n2);
@@ -1467,6 +1572,43 @@ template <class P> static int launch_chan_static(ChanArgs const &a, int n, int n
   return 0;
 }
 
+// The huge channels of one length (chan_huge.cuh): pass A, pass B and, with d_power, the power reduction, in chunks of
+// channels and blocks whose scratch stays within kHugeScratchCap.
+static int launch_huge(kgpu_bank *b, ChanArgs const &a, int points, int n, int nblocks, cudaStream_t st) {
+  HugeGeom const *g = get_huge_geom(points);
+  if (!g) return -1;
+  long const slot = (long)points * (long)sizeof(float2);
+  long const per = std::max(1L, kHugeScratchCap / slot);  // (channel, block) slots per chunk
+  int const cch = (int)std::min<long>(n, per), cbl = (int)std::max(1L, std::min<long>(nblocks, per / cch));
+  int const tiles_a = (g->n2 + kTile - 1) / kTile, tiles_b = (g->n1 + kTile - 1) / kTile;
+  size_t const slots = (size_t)cch * (size_t)cbl, data = slots * (size_t)slot;
+  char *scr = (char *)bank_scratch(b, st, data + slots * (size_t)tiles_b * sizeof(float));
+  if (!scr) return -1;
+  float *partial = a.power ? (float *)(scr + data) : nullptr;
+  size_t const sm1 = (size_t)huge_smem_bytes(g->n1), sm2 = (size_t)huge_smem_bytes(g->n2);
+  if (allow_smem((const void *)chan_huge_cols, sm1) || allow_smem((const void *)chan_huge_rows, sm2)) return -1;
+  for (int c0 = 0; c0 < n; c0 += cch)
+    for (int b0 = 0; b0 < nblocks; b0 += cbl) {
+      int const nc = std::min(cch, n - c0), nb = std::min(cbl, nblocks - b0);
+      ChanArgs x = a;
+      if (x.order) x.order += c0;
+      else x.chan_base += c0;
+      x.norder = nc;
+      x.spec += (long)b0 * x.spec_stride;
+      x.out += (long)b0 * x.out_stride;
+      x.block0 += b0;
+      if (x.power) x.power += (long)b0 * x.power_stride;
+      chan_huge_cols<<<dim3((unsigned)tiles_a, (unsigned)nc, (unsigned)nb), kHugeThreads, sm1, st>>>(x, *g, (float2 *)scr);
+      chan_huge_rows<<<dim3((unsigned)tiles_b, (unsigned)nc, (unsigned)nb), kHugeThreads, sm2, st>>>(x, *g, (float2 const *)scr, partial);
+      g_launches += 2;
+      if (partial) {
+        huge_power_kernel<<<dim3((unsigned)nc, (unsigned)nb), 32, 0, st>>>(x, partial, tiles_b);
+        g_launches++;
+      }
+    }
+  return 0;
+}
+
 // one (plan, descriptor list) launch
 static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_out, long out_stride, int plan,
                        int points, int const *d_order, int base, int n, cudaStream_t st, bool generic = false,
@@ -1489,6 +1631,7 @@ static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_ou
   a.power = d_power;
   a.power_stride = b->capacity;
   ProfScope ps(K_CHAN, st);
+  if (points > kMaxWideChanPoints) return launch_huge(b, a, points, n, nblocks, st);  // huge channels: chan_huge
   g_launches++;
   if (points > kMaxChanPoints) {  // wide channels: chan_wide whatever the static-kernel setting
     WideGeom const *g = get_wide_geom(points);
@@ -1547,7 +1690,7 @@ extern "C" int kgpu_bank_run_one_ex(kgpu_bank *b, int idx, const void *d_spec, v
   return 0;
 }
 // Noise density per channel and block from the device-resident spectrum (estimate_noise, radio.c:1783-1866).
-static_assert(sizeof(unsigned) * kMaxWideChanPoints + 4096 <= 227 * 1024, "the widest channel's noise window must fit shared memory");
+static_assert(kNoiseSmemBins >= kMaxWideChanPoints, "every wide channel's noise window must fit shared memory");
 extern "C" int kgpu_bank_noise(kgpu_bank *b, const void *d_spec, int nblocks, double samprate, double *d_n0, void *stream) {
   if (!b || !d_spec || !d_n0 || nblocks < 1 || !(samprate > 0)) return fail("kgpu_bank_noise: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1567,9 +1710,20 @@ extern "C" int kgpu_bank_noise(kgpu_bank *b, const void *d_spec, int nblocks, do
   a.scale = correction / ((double)b->m->bins * samprate);
   a.n0 = d_n0;
   a.n0_stride = b->capacity;
-  int window = 0;  // every runnable channel's window lives in shared memory whole
-  for (int i = 0; i < b->nchan; i++)
-    if (b->desc[(size_t)i].plan >= 0 && b->desc[(size_t)i].points > 0) window = std::max(window, noise_window(b->desc[(size_t)i]));
+  // windows of at most kNoiseSmemBins live in noise_kernel's shared memory whole, sized for the widest of them; the
+  // wider ones (huge channels) go to noise_kernel_gm, which keeps them in the bank's scratch
+  int window = 0, big_window = 0;
+  std::vector<int> big;
+  for (int i = 0; i < b->nchan; i++) {
+    if (b->desc[(size_t)i].plan < 0 || b->desc[(size_t)i].points <= 0) continue;
+    int const w = noise_window(b->desc[(size_t)i]);
+    if (w <= kNoiseSmemBins) {
+      window = std::max(window, w);
+    } else {
+      big.push_back(i);
+      big_window = std::max(big_window, w);
+    }
+  }
   size_t const sm = sizeof(unsigned) * (size_t)window;
   if (allow_smem((const void *)noise_kernel, sm)) return -1;
   {
@@ -1577,6 +1731,24 @@ extern "C" int kgpu_bank_noise(kgpu_bank *b, const void *d_spec, int nblocks, do
     noise_kernel<<<dim3((unsigned)b->nchan, (unsigned)nblocks), kNoiseThreads, sm, st>>>(a);
   }
   g_launches++;
+  if (!big.empty()) {
+    long const stride = ((long)big_window + 31) / 32 * 32, nbig = (long)big.size();
+    long const per = std::max(1L, kHugeScratchCap / (stride * (long)sizeof(unsigned)));  // (channel, block) slots per chunk
+    int const cbl = (int)std::max(1L, std::min<long>(nblocks, per / nbig));
+    size_t const list_off = (size_t)nbig * (size_t)cbl * (size_t)stride * sizeof(unsigned);
+    char *scr = (char *)bank_scratch(b, st, list_off + sizeof(int) * big.size());
+    if (!scr) return -1;
+    CUDA_OK(cudaMemcpyAsync(scr + list_off, big.data(), sizeof(int) * big.size(), cudaMemcpyHostToDevice, st));
+    ProfScope ps(K_NOISE, st);
+    for (int b0 = 0; b0 < nblocks; b0 += cbl) {
+      NoiseArgs x = a;
+      x.spec += (long)b0 * x.spec_stride;
+      x.n0 += (long)b0 * x.n0_stride;
+      noise_kernel_gm<<<dim3((unsigned)nbig, (unsigned)std::min(cbl, nblocks - b0)), kNoiseGmThreads, 0, st>>>(
+          x, (int const *)(scr + list_off), (unsigned *)scr, stride);
+      g_launches++;
+    }
+  }
   CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -5,15 +5,20 @@
 // which forces a 13 MB device->host copy of every block's spectrum; here one double per channel and block leaves the GPU.
 //
 // One CTA per (channel, block).  Order statistics by an exact 4 x 8-bit radix select on the float bit patterns
-// (energies are >= 0, so the unsigned order is the numeric order): no sort, O(n) per pass.  The window's energies sit in
-// dynamic shared memory of noise_window() words of the bank's widest runnable channel (at most kMaxWideChanPoints).
+// (energies are >= 0, so the unsigned order is the numeric order): no sort, O(n) per pass.  noise_kernel keeps the
+// window's energies in dynamic shared memory of noise_window() words of the bank's widest channel whose window has at
+// most kNoiseSmemBins; windows above that (huge channels from 57 088 bins, chan_huge.cuh) are estimated by
+// noise_kernel_gm, which runs the same body on kNoiseGmThreads threads over energies kept in a global scratch slot.
 #pragma once
 #include "chan_kernels.cuh"
 
 namespace kfft {
 
 constexpr int kNoiseThreads = 128;
+constexpr int kNoiseGmThreads = 512;
 constexpr int kMinNoiseBins = 1000;   // radio.c:76
+// the largest window noise_kernel holds in shared memory: 227 KB less 4 KB for its static arrays
+constexpr int kNoiseSmemBins = (227 * 1024 - 4096) / 4;
 
 // bins estimate_noise takes around a runnable channel: max(slave->bins, Min_noise_bins) (radio.c:1794-1797)
 __host__ __device__ inline int noise_window(ChanDesc const &d) {
@@ -35,14 +40,15 @@ struct NoiseArgs {
 };
 
 // k-th smallest (0-based) of e[0..n): returns its bit pattern; *n_le = number of elements <= that value
+template <int NT>
 __device__ inline unsigned radix_select(unsigned const *e, int n, int k, unsigned *hist /*256*/, int *sh /*4 ints*/) {
   unsigned prefix = 0, mask = 0;
   int kk = k;
   for (int pass = 3; pass >= 0; pass--) {
-    for (int i = threadIdx.x; i < 256; i += kNoiseThreads) hist[i] = 0;
+    for (int i = threadIdx.x; i < 256; i += NT) hist[i] = 0;
     __syncthreads();
     int const sft = 8 * pass;
-    for (int i = threadIdx.x; i < n; i += kNoiseThreads) {
+    for (int i = threadIdx.x; i < n; i += NT) {
       unsigned const v = e[i];
       if ((v & mask) == prefix) atomicAdd(&hist[(v >> sft) & 255u], 1u);
     }
@@ -66,14 +72,15 @@ __device__ inline unsigned radix_select(unsigned const *e, int n, int k, unsigne
   return prefix;
 }
 
-__global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a) {
-  extern __shared__ unsigned e[];  // [noise_window(d)]
+// The estimate of channel ci in block blk, with NT threads and the window's energies in e[noise_window(d)].
+template <int NT>
+__device__ __forceinline__ void noise_body(NoiseArgs const &a, unsigned *e, int ci, int blk) {
   __shared__ unsigned hist[256];
   __shared__ int sh[4];
-  __shared__ double red_s[kNoiseThreads / 32];
-  __shared__ int red_c[kNoiseThreads / 32];
-  __shared__ unsigned red_m[kNoiseThreads / 32];
-  int const ci = blockIdx.x, blk = blockIdx.y, tid = threadIdx.x;
+  __shared__ double red_s[NT / 32];
+  __shared__ int red_c[NT / 32];
+  __shared__ unsigned red_m[NT / 32];
+  int const tid = threadIdx.x;
   ChanDesc const d = a.desc[ci];
   double *out = a.n0 + (long)blk * a.n0_stride + ci;
   if (d.plan < 0 || d.points <= 0) {
@@ -92,7 +99,7 @@ __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a)
       mbin = 0;
       filled = m;
     }
-    for (int i = tid; i < nbins; i += kNoiseThreads) {
+    for (int i = tid; i < nbins; i += NT) {
       float v = 0.f;
       if (i < filled) {
         float2 const x = __ldg(X + mbin + i);
@@ -111,7 +118,7 @@ __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a)
     // the reference stops filling when the walk reaches the master's Nyquist bin; what it leaves is zero here
     int const to_nyq = ((m / 2 - mbin) % m + m) % m;  // steps until mbin == m/2 (0 -> a full turn)
     filled = (to_nyq == 0 || to_nyq > nbins) ? nbins : to_nyq;
-    for (int i = tid; i < nbins; i += kNoiseThreads) {
+    for (int i = tid; i < nbins; i += NT) {
       float v = 0.f;
       if (i < filled) {
         int q = mbin + i;
@@ -127,11 +134,11 @@ __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a)
   double const pos = 0.10 * (double)(nbins - 1);
   int const k = (int)floor(pos);
   double const frac = pos - (double)k;
-  unsigned const b1 = radix_select(e, nbins, k, hist, sh);
+  unsigned const b1 = radix_select<NT>(e, nbins, k, hist, sh);
   // the next order statistic: b1 again if enough duplicates, else the smallest element above it
   int cnt_le = 0;
   unsigned next = 0xffffffffu;
-  for (int i = tid; i < nbins; i += kNoiseThreads) {
+  for (int i = tid; i < nbins; i += NT) {
     unsigned const v = e[i];
     cnt_le += (v <= b1);
     if (v > b1 && v < next) next = v;
@@ -147,7 +154,7 @@ __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a)
   __syncthreads();
   cnt_le = 0;
   next = 0xffffffffu;
-  for (int w = 0; w < kNoiseThreads / 32; w++) {
+  for (int w = 0; w < NT / 32; w++) {
     cnt_le += red_c[w];
     next = min(next, red_m[w]);
   }
@@ -161,7 +168,7 @@ __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a)
   double const en = 1.5 * q;  // N_cutoff, radio.c:74
   double sum = 0.0;
   int nb = 0;
-  for (int i = tid; i < nbins; i += kNoiseThreads) {
+  for (int i = tid; i < nbins; i += NT) {
     double const v = (double)__uint_as_float(e[i]);
     if (v <= en) {
       sum += v;
@@ -180,7 +187,7 @@ __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a)
   if (tid == 0) {
     sum = 0.0;
     nb = 0;
-    for (int w = 0; w < kNoiseThreads / 32; w++) {
+    for (int w = 0; w < NT / 32; w++) {
       sum += red_s[w];
       nb += red_c[w];
     }
@@ -188,6 +195,19 @@ __global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a)
   }
 }
 
+__global__ void __launch_bounds__(kNoiseThreads) noise_kernel(NoiseArgs const a) {
+  extern __shared__ unsigned e[];  // [noise_window(d)]
+  int const ci = blockIdx.x;
+  ChanDesc const d = a.desc[ci];
+  if (d.plan >= 0 && d.points > 0 && noise_window(d) > kNoiseSmemBins) return;  // noise_kernel_gm's
+  noise_body<kNoiseThreads>(a, e, ci, blockIdx.y);
+}
+
+// grid (listed channels, blocks): channel list[blockIdx.x], its energies in scratch slot blockIdx.y * gridDim.x + blockIdx.x
+// of `stride` words
+__global__ void __launch_bounds__(kNoiseGmThreads) noise_kernel_gm(NoiseArgs const a, int const *list, unsigned *scratch, long stride) {
+  noise_body<kNoiseGmThreads>(a, scratch + ((long)blockIdx.y * gridDim.x + blockIdx.x) * stride, list[blockIdx.x], blockIdx.y);
+}
 
 // ------------------------------------------------------------------ FM discriminator front half -----------------------
 // Replaces the per-sample loops at the top of demod_fm (reference fm.c:104-131 and :205-231, plain discriminator): for every
