@@ -118,6 +118,13 @@ int kgpu_bank_define_wide(kgpu_bank *b, int idx, int olen, int out_type);
  * most about 128 MB per stream), provided points has factors 2, 3, 5, 7 only (every such length in range then splits
  * into two factors of at most 4096).  Every other bank call treats such a channel like any other. */
 int kgpu_bank_define_huge(kgpu_bank *b, int idx, int olen, int out_type);
+/* Same, also for lengths of at most 28812 points whose prime factors reach 11, 13, 17, 19 or 23 (e.g. the 220 kHz and
+ * 277.2 kHz channels of the HFDL bank: 5500 = 2^2 5^3 11 and 6930 = 2 3^2 5 7 11 points at 20 ms and overlap 5).  Where
+ * points has factors 2, 3, 5, 7 only it is kgpu_bank_define_huge: the same result, kernels and messages.  Otherwise
+ * the channel runs the generic channel kernel (up to 7260 points) or the four-step wide kernel on plans of its own,
+ * which never take a slot of the plan registry.  Fails for a prime factor >= 29, and for a factor 11 .. 23 above 28812
+ * points.  Every other bank call treats such a channel like any other. */
+int kgpu_bank_define_ext(kgpu_bank *b, int idx, int olen, int out_type);
 /* set_filter (filter.c:968-1045): Kaiser-windowed sinc designed on the host in double, forward
  * transformed on the device.  low/high are fractions of the output rate. */
 int kgpu_bank_set_filter(kgpu_bank *b, int idx, double low, double high, double kaiser_beta);

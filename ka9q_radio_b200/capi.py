@@ -82,6 +82,7 @@ def load() -> C.CDLL:
     L.kgpu_bank_define_ex.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_wide.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_huge.argtypes = [vp, i, i, i]
+    L.kgpu_bank_define_ext.argtypes = [vp, i, i, i]
     L.kgpu_bank_set_weights.argtypes = [vp, i, d, d, d, d]
     L.kgpu_bank_set_osc.argtypes = [vp, i, i, d, d, d, d]
     L.kgpu_bank_get_osc_phase.argtypes = [vp, i, vp]
@@ -217,6 +218,11 @@ class Bank:
         """define_wide() up to 1048576 points: channels longer than 28812 points run the two-kernel four-step channel
         transform through the bank's global scratch."""
         return check(self.lib.kgpu_bank_define_huge(self.h, idx, olen, out_type), "kgpu_bank_define_huge")
+
+    def define_ext(self, idx, olen, out_type=KGPU_COMPLEX) -> int:
+        """define_huge() that also serves lengths of at most 28812 points with prime factors 11, 13, 17, 19 and 23 (e.g.
+        the 220 kHz and 277.2 kHz HFDL channels); their plans never take a registry slot."""
+        return check(self.lib.kgpu_bank_define_ext(self.h, idx, olen, out_type), "kgpu_bank_define_ext")
 
     def set_weights(self, idx, i_weight=1.0, q_weight=0.0):
         """set_filter_weights (filter.c:922-929)"""

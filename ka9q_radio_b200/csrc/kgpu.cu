@@ -490,6 +490,28 @@ static int plan_slot(TilePlan const &p, int k) {  // slot holding X[k] after the
   return slot;
 }
 
+// Sets g.tw, the device table of W_Ns^{k1 j2}: pass 1 leaves output j2 in column plan_slot(p2, j2), so it is tabulated
+// in column order.  p2: the plan of length g.n2.
+static int wide_twiddles(WideGeom &g, TilePlan const &p2) {
+  long const points = (long)g.n1 * g.n2;
+  std::vector<float2> tw((size_t)points);
+  for (int j2 = 0; j2 < g.n2; j2++) {
+    int const c = plan_slot(p2, j2);
+    for (int k1 = 0; k1 < g.n1; k1++) {
+      long double const ang = -2.0L * M_PIl * (long double)((long)k1 * j2) / (long double)points;
+      tw[(size_t)k1 * g.n2 + c] = make_float2((float)cosl(ang), (float)sinl(ang));
+    }
+  }
+  float2 *d_tw = nullptr;
+  if (cudaMalloc(&d_tw, sizeof(float2) * tw.size()) != cudaSuccess ||
+      cudaMemcpy(d_tw, tw.data(), sizeof(float2) * tw.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
+    cudaFree(d_tw);
+    return fail("%ld-point transform: twiddle upload failed", points);
+  }
+  g.tw = d_tw;
+  return 0;
+}
+
 static WideGeom const *get_wide_geom(int points) {
   std::lock_guard<std::mutex> lk(g_wide_mu);
   auto it = g_wide.find(points);
@@ -511,24 +533,7 @@ static WideGeom const *get_wide_geom(int points) {
   g.plan1 = get_tile_plan(sp.n1);
   g.plan2 = get_tile_plan(sp.n2);
   if (g.plan1 < 0 || g.plan2 < 0) return nullptr;
-  // pass 1 leaves output j2 in column plan_slot(j2): tabulate W_Ns^{k1 j2} in column order
-  std::vector<float2> tw((size_t)points);
-  TilePlan const &p2 = *host_tile_plan(g.plan2);
-  for (int j2 = 0; j2 < g.n2; j2++) {
-    int const c = plan_slot(p2, j2);
-    for (int k1 = 0; k1 < g.n1; k1++) {
-      long double const ang = -2.0L * M_PIl * (long double)((long)k1 * j2) / (long double)points;
-      tw[(size_t)k1 * g.n2 + c] = make_float2((float)cosl(ang), (float)sinl(ang));
-    }
-  }
-  float2 *d_tw = nullptr;
-  if (cudaMalloc(&d_tw, sizeof(float2) * tw.size()) != cudaSuccess ||
-      cudaMemcpy(d_tw, tw.data(), sizeof(float2) * tw.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
-    cudaFree(d_tw);
-    fail("%d-point transform: twiddle upload failed", points);
-    return nullptr;
-  }
-  g.tw = d_tw;
+  if (wide_twiddles(g, *host_tile_plan(g.plan2))) return nullptr;
   return &(g_wide[points] = g);
 }
 
@@ -582,6 +587,108 @@ static HugeGeom const *get_huge_geom(int points) {
   g.plan2 = get_tile_plan(sp.n2);
   if (g.plan1 < 0 || g.plan2 < 0) return nullptr;
   return &(g_huge[points] = g);
+}
+
+// ---- channels whose length has a prime factor 11 .. 23 (kgpu_bank_define_ext) ----
+// They keep their plans out of the registry: c_plans holds exactly the 7-smooth lengths, whose count kMaxPlans is
+// sized for.  Their kernels, chan_kernel_ext and chan_wide_ext, take the plans by value instead.
+constexpr bool smooth23(long n) {
+  for (long p : {2, 3, 5, 7, 11, 13, 17, 19, 23})
+    while (n % p == 0) n /= p;
+  return n == 1;
+}
+constexpr bool extended(long n) { return smooth23(n) && !smooth7(n); }
+// choose_split_ext restated as wide_fits is (a length <= kMaxTileLen is plannable_ext iff its factors reach 23 at most)
+constexpr bool wide_fits_ext(long n) {
+  long d = 1;
+  while ((d + 1) * (d + 1) <= n) d++;
+  for (; d >= 1; d--) {
+    if (n % d) continue;
+    if (n / d > kMaxTileLen) return false;
+    if (smooth23(n / d) && smooth23(d)) return wide_smem_bytes((int)(n / d), (int)d) <= kChanSmemLimit;
+  }
+  return false;
+}
+constexpr long ext_lengths(long lo, long hi, bool wide) {  // extended lengths in [lo, hi]; -1 if a wide one does not fit
+  long count = 0;
+  for (long n = lo; n <= hi; n++)
+    if (extended(n)) {
+      if (wide && !wide_fits_ext(n)) return -1;
+      count++;
+    }
+  return count;
+}
+// 863 extended lengths run chan_kernel_ext (7260 = 2^2 3 5 11^2 is one of them), and 1032 more, up to 28798 =
+// 2 7 11^2 17, split into two factors of at most kMaxTileLen whose chan_wide_ext footprint fits shared memory.
+static_assert(ext_lengths(2, kMaxChanPoints, false) == 863, "extended channel lengths up to kMaxChanPoints");
+static_assert(ext_lengths(kMaxChanPoints + 1, kMaxWideChanPoints, true) == 1032, "an extended wide length does not split or fit");
+
+// Plans of every extended length used so far, by length (process-wide, never freed, like the registry).  The 863
+// lengths of at most kMaxChanPoints bound it; DESIGN.md section 4 states the device memory it can reach.
+static std::mutex g_ext_mu;
+static std::map<int, TilePlan> g_ext;
+
+// The plan of `len` by value: the registry's for a 7-smooth length (factors of an extended wide length can be), an
+// extended plan otherwise.
+static int get_ext_plan(int len, TilePlan *out) {
+  if (smooth7(len)) {
+    int const idx = get_tile_plan(len);
+    if (idx < 0) return -1;
+    std::lock_guard<std::mutex> lk(g_plan_mu);
+    *out = g_plans[(size_t)idx].host;
+    return 0;
+  }
+  std::lock_guard<std::mutex> lk(g_ext_mu);
+  auto it = g_ext.find(len);
+  if (it == g_ext.end()) {
+    std::vector<int> rad;
+    if (len <= kMaxChanPoints) rad = choose_radices_ext(len);
+    if (rad.empty()) return fail("%d-point transform cannot be planned (prime factors up to 23; at most %d points)", len, kMaxChanPoints);
+    TilePlan p;
+    if (make_tile_plan(len, rad, p)) return -1;
+    it = g_ext.emplace(len, p).first;
+  }
+  *out = it->second;
+  return 0;
+}
+
+// Four-step geometry of every extended wide length used so far (never freed): chan_wide's split and twiddle table,
+// with the two factor plans by value.
+static std::mutex g_wide_ext_mu;
+static std::map<int, WideGeomExt> g_wide_ext;
+
+static WideGeomExt const *get_wide_geom_ext(int points) {
+  std::lock_guard<std::mutex> lk(g_wide_ext_mu);
+  auto it = g_wide_ext.find(points);
+  if (it != g_wide_ext.end()) return &it->second;
+  Split2 sp;
+  if (!choose_split_ext(points, &sp)) {
+    fail("%d-point transform cannot be split into two plannable lengths (prime factors up to 23; each at most %d)", points,
+         kMaxTileLen);
+    return nullptr;
+  }
+  if (wide_smem_bytes(sp.n1, sp.n2) > kChanSmemLimit) {
+    fail("%d-point transform (%d x %d) does not fit in shared memory", points, sp.n1, sp.n2);
+    return nullptr;
+  }
+  WideGeomExt x;
+  x.g.n1 = sp.n1;
+  x.g.n2 = sp.n2;
+  x.g.pitch = wide_pitch(sp.n2);
+  x.g.plan1 = x.g.plan2 = -1;
+  if (get_ext_plan(sp.n1, &x.p1) || get_ext_plan(sp.n2, &x.p2) || wide_twiddles(x.g, x.p2)) return nullptr;
+  return &(g_wide_ext[points] = x);
+}
+
+// The largest prime factor of n above 7, or 1 if n has none.
+static long factor_above7(long n) {
+  long big = 1;
+  for (long p = 2; p * p <= n; p++)
+    while (n % p == 0) {
+      n /= p;
+      if (p > 7) big = p;
+    }
+  return n > 7 ? std::max(big, n) : big;
 }
 }  // namespace kfft
 
@@ -1232,6 +1339,7 @@ static int bank_commit(kgpu_bank *b, cudaStream_t st) {
   b->out_stride = (off + 3) / 4 * 4;
   // one launch per distinct plan: order[] lists that plan's descriptors.  Wide channels (chan_wide serves every
   // variant) form one group per length; their plan is only their first factor's, so the length is part of the key.
+  // Extended channels all have plan kPlanExt, so they too form one group per length (and generic-only flag).
   std::vector<int> order;
   b->groups.clear();
   auto generic_only = [&](int i) {
@@ -1319,7 +1427,7 @@ extern "C" void kgpu_bank_destroy(kgpu_bank *b) {
 }
 static bool bad_idx(kgpu_bank const *b, int idx) { return !b || idx < 0 || idx >= b->capacity; }
 
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok = false);
+static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok = false, bool ext_ok = false);
 extern "C" int kgpu_bank_define(kgpu_bank *b, int idx, int olen) { return bank_define(b, idx, olen, false, false); }
 extern "C" int kgpu_bank_define_ex(kgpu_bank *b, int idx, int olen, int out_type) {
   if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_ex: out_type must be KGPU_COMPLEX or KGPU_REAL");
@@ -1333,7 +1441,11 @@ extern "C" int kgpu_bank_define_huge(kgpu_bank *b, int idx, int olen, int out_ty
   if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_huge: out_type must be KGPU_COMPLEX or KGPU_REAL");
   return bank_define(b, idx, olen, out_type == KGPU_REAL, true, true);
 }
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok) {
+extern "C" int kgpu_bank_define_ext(kgpu_bank *b, int idx, int olen, int out_type) {
+  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_ext: out_type must be KGPU_COMPLEX or KGPU_REAL");
+  return bank_define(b, idx, olen, out_type == KGPU_REAL, true, true, true);
+}
+static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok, bool ext_ok) {
   if (bad_idx(b, idx) || olen < 1) return fail("kgpu_bank_define: bad arguments");
   long const num = (long)olen * b->m->N;
   if (num % b->m->L) return fail("invalid output length %d for N=%d L=%d (filter.c:312-316)", olen, b->m->N, b->m->L);
@@ -1342,9 +1454,24 @@ static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide
   // the channel kernel holds kChanWarps transforms of this length in shared memory; the bound also keeps the plan
   // registry from filling (see kMaxPlans).  Longer channels (kgpu_bank_define_wide) run chan_wide, one CTA each, on
   // a split into two registry lengths; their descriptor's plan is that of the first factor (>= 0: runnable).  Beyond
-  // kMaxWideChanPoints (kgpu_bank_define_huge) the same holds for chan_huge's split.
+  // kMaxWideChanPoints (kgpu_bank_define_huge) the same holds for chan_huge's split.  A length with a prime factor
+  // 11 .. 23 (kgpu_bank_define_ext) has plans of its own outside the registry; its descriptor's plan is kPlanExt.
+  long const big = ext_ok ? factor_above7(points) : 1;
   int plan;
-  if (points <= kMaxChanPoints) {
+  if (big > 23) {
+    return fail("kgpu_bank_define_ext: %d-point inverse transform has the prime factor %ld (prime factors up to 23 are served)",
+                points, big);
+  } else if (big > 1 && points > kMaxWideChanPoints) {
+    return fail("kgpu_bank_define_ext: %d-point inverse transform has the prime factor %ld, served up to %d points only",
+                points, big, kMaxWideChanPoints);
+  } else if (big > 1 && points > kMaxChanPoints) {
+    if (!get_wide_geom_ext(points)) return fail("kgpu_bank_define_ext: %s", std::string(g_err).c_str());
+    plan = kPlanExt;
+  } else if (big > 1) {
+    TilePlan p;
+    if (get_ext_plan(points, &p)) return fail("kgpu_bank_define_ext: %s", std::string(g_err).c_str());
+    plan = kPlanExt;
+  } else if (points <= kMaxChanPoints) {
     plan = get_tile_plan(points);
     if (plan < 0) return fail("kgpu_bank_define: %s", std::string(g_err).c_str());
   } else if (!wide_ok) {
@@ -1406,7 +1533,23 @@ static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *ho
   if (on_stream) CUDA_OK(cudaStreamSynchronize(st));
   else CUDA_OK(cudaDeviceSynchronize());
   CUDA_OK(cudaMemcpyAsync(dst, host, sizeof(float2) * (size_t)c.points, cudaMemcpyHostToDevice, st));
-  if (transform && c.points > kMaxWideChanPoints) {
+  if (transform && c.plan == kPlanExt && c.points > kMaxChanPoints) {
+    WideGeomExt const *x = get_wide_geom_ext(c.points);
+    if (!x) return -1;
+    size_t const sm = (size_t)wide_smem_bytes(x->g.n1, x->g.n2);
+    if (allow_smem((const void *)response_wide_ext, sm)) return -1;
+    response_wide_ext<<<1, kWideThreads, sm, st>>>(dst, *x);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+  } else if (transform && c.plan == kPlanExt) {
+    TilePlan p;
+    if (get_ext_plan(c.points, &p)) return -1;
+    size_t const sm = sizeof(float2) * (size_t)c.points;
+    if (allow_smem((const void *)response_fft_ext, sm)) return -1;
+    response_fft_ext<<<1, 32, sm, st>>>(dst, p);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+  } else if (transform && c.points > kMaxWideChanPoints) {
     HugeGeom const *g = get_huge_geom(c.points);
     if (!g) return -1;
     float2 *scr = (float2 *)bank_scratch(b, st, sizeof(float2) * (size_t)c.points);
@@ -1609,6 +1752,26 @@ static int launch_huge(kgpu_bank *b, ChanArgs const &a, int points, int n, int n
   return 0;
 }
 
+// The channels of one extended length: chan_kernel_ext, or chan_wide_ext above kMaxChanPoints, whatever the
+// static-kernel setting (every variant runs the same kernel).
+static int launch_chan_ext(ChanArgs const &a, int points, int n, int nblocks, cudaStream_t st) {
+  if (points > kMaxChanPoints) {
+    WideGeomExt const *x = get_wide_geom_ext(points);
+    if (!x) return -1;
+    size_t const sm = (size_t)wide_smem_bytes(x->g.n1, x->g.n2);
+    if (allow_smem((const void *)chan_wide_ext, sm)) return -1;
+    chan_wide_ext<<<dim3((unsigned)n, (unsigned)nblocks), kWideThreads, sm, st>>>(a, *x);
+    return 0;
+  }
+  TilePlan p;
+  if (get_ext_plan(points, &p)) return -1;
+  size_t const sm = sizeof(float2) * (size_t)a.pitch * kChanWarps;
+  if (allow_smem((const void *)chan_kernel_ext, sm)) return -1;
+  dim3 const g((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks);
+  chan_kernel_ext<<<g, kChanWarps * 32, sm, st>>>(a, p);
+  return 0;
+}
+
 // one (plan, descriptor list) launch
 static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_out, long out_stride, int plan,
                        int points, int const *d_order, int base, int n, cudaStream_t st, bool generic = false,
@@ -1633,6 +1796,7 @@ static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_ou
   ProfScope ps(K_CHAN, st);
   if (points > kMaxWideChanPoints) return launch_huge(b, a, points, n, nblocks, st);  // huge channels: chan_huge
   g_launches++;
+  if (plan == kPlanExt) return launch_chan_ext(a, points, n, nblocks, st);  // before host_tile_plan: not a registry plan
   if (points > kMaxChanPoints) {  // wide channels: chan_wide whatever the static-kernel setting
     WideGeom const *g = get_wide_geom(points);
     if (!g) return -1;
