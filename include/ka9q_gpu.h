@@ -205,6 +205,35 @@ int kgpu_plan_split_ex(long n, int *n1, int *n2);
  * co-resides with the forward kernels of the next step. */
 int kgpu_multicast_copy(const void *d_src, void *mc_dst, unsigned long long bytes, int nctas, void *stream);
 
+/* ---- wideband spectrum analyzer: replaces wideband_poll's fft_avg loops (spectrum.c:354-497) -------------------- */
+typedef struct kgpu_spectrum kgpu_spectrum;
+/* An analyzer of fft_n-point segments of a REAL or COMPLEX front end's raw samples into bin_count float bins.  The
+ * transform is chosen from fft_n alone: REAL with even fft_n and fft_n/2 23-smooth runs the r2c of a REAL master
+ * (L = fft_n, M = 1); COMPLEX 23-smooth, or REAL odd 23-smooth, a COMPLEX master of length fft_n; any other length a
+ * Bluestein transform through a COMPLEX master of the smallest 7-smooth length P >= 2 fft_n - 1 whose split the
+ * forward pair runs (both factors fit shared memory, so P <= 3500 x 3500 and fft_n <= 6 125 000); NULL and
+ * kgpu_last_error() otherwise. */
+kgpu_spectrum *kgpu_spectrum_create(int fft_n, int in_type, int bin_count);
+/* fft_n floats, as generate_window() leaves them (spectrum.c:548-606); the default is all ones. */
+int kgpu_spectrum_set_window(kgpu_spectrum *s, float const *window);
+/* One poll (spectrum.c:354-497): d_bins[0 .. bin_count) = sum over fft_avg segments of gain |X|^2 in the reference's bin
+ * mapping and order; bins the reference leaves 0 are 0, nothing past bin_count is written.
+ *   d_ring        device ring of ring_samples samples (>= fft_n): float / int16 (fmt) samples (REAL) or pairs (COMPLEX)
+ *   end           ring position just past the newest sample (taken modulo ring_samples); segments start at
+ *                 end - adjust + i*hop (REAL) or end - adjust - i*hop (COMPLEX), adjust and hop as spectrum.c:364,407
+ *   scale, derandomize  int16 samples are scale * (float)x after the randomizer flip (rx888.c:707-712,765)
+ *   shift         spectrum.c:347; fft_avg >= 1; 0 <= overlap < 1
+ * Enqueued on `stream`; the analyzer's scratch is reused by the next run, so runs of one analyzer go on one stream.
+ * A REAL walk index the reference would take below 0 (out of its array) contributes 0. */
+int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring_samples, long end, int fmt, float scale,
+                      int derandomize, int shift, int fft_avg, double overlap, float *d_bins, void *stream);
+/* "r2c|complex|bluestein fft_n=... real|complex P=...: <nc>-point complex two-pass n1 x n2" */
+int kgpu_spectrum_describe(kgpu_spectrum const *s, char *buf, int buflen);
+void kgpu_spectrum_destroy(kgpu_spectrum *s);
+/* Pure host code: the path kgpu_spectrum_create would take for fft_n (0 r2c, 1 complex, 2 Bluestein; -1 when it would
+ * fail) and, if buf is not NULL, the string kgpu_spectrum_describe would print. */
+int kgpu_spectrum_plan(int fft_n, int in_type, char *buf, int buflen);
+
 /* Algorithmic bytes per block of one forward + all enabled channels (SURVEY.md 8d). */
 double kgpu_algorithmic_bytes(kgpu_master const *m, kgpu_bank const *b, int fmt);
 

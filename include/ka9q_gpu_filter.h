@@ -143,6 +143,16 @@ int filter_output_untune(struct filter_out *slave); /* back to plain execute_fil
 int filter_input_enable_noise(struct filter_in *master, double samprate);
 double filter_noise_estimate(struct filter_out const *slave);
 
+/* EXTENSION (spectrum.c:308-522 on the device) for a SPECTRUM slave: wideband_poll's fft_avg loops read a device copy of
+ * the master's input ring (float or int16, as it is fed), created and seeded from the host ring by the first setup on
+ * that master and appended by every block from then on.  setup: where setup_wideband / generate_window run, with fft_n
+ * window floats; -1 for a length the device cannot serve (the caller keeps its CPU loop).  poll: bin_count floats as
+ * wideband_poll leaves them, for the segments ending at the end of the last issued block, whose sample index goes to
+ * *end_sample (the reference reads up to the live write pointer, up to one block newer).  One poller per slave. */
+int filter_spectrum_setup(struct filter_out *slave, int fft_n, int bin_count, float const *window);
+int filter_spectrum_poll(struct filter_out *slave, int shift, int fft_avg, double overlap, float *bin_data,
+                         uint64_t *end_sample);
+
 /* housekeeping the reference exports from filter.c */
 void *run_fft(void *);
 void suggest(int size, int dir, int clex);

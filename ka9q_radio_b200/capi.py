@@ -105,6 +105,13 @@ def load() -> C.CDLL:
     L.kgpu_multicast_copy.argtypes = [vp, vp, C.c_ulonglong, i, vp]
     L.kgpu_algorithmic_bytes.argtypes = [vp, vp, i]
     L.kgpu_algorithmic_bytes.restype = d
+    L.kgpu_spectrum_create.restype = vp
+    L.kgpu_spectrum_create.argtypes = [i, i, i]
+    L.kgpu_spectrum_set_window.argtypes = [vp, vp]
+    L.kgpu_spectrum_run.argtypes = [vp, vp, l, l, i, f, i, i, i, d, vp, vp]
+    L.kgpu_spectrum_describe.argtypes = [vp, C.c_char_p, i]
+    L.kgpu_spectrum_destroy.argtypes = [vp]
+    L.kgpu_spectrum_plan.argtypes = [i, i, C.c_char_p, i]
     _lib = L
     return L
 
@@ -296,4 +303,63 @@ class Bank:
     def close(self):
         if self.h:
             self.lib.kgpu_bank_destroy(self.h)
+            self.h = None
+
+
+SPECTRUM_R2C, SPECTRUM_COMPLEX, SPECTRUM_BLUESTEIN = 0, 1, 2
+
+
+def spectrum_plan(fft_n: int, in_type: int) -> tuple[int, str]:
+    """(path, description) kgpu_spectrum_create would choose for fft_n; pure host code.  Raises when it would fail."""
+    buf = C.create_string_buffer(256)
+    return check(load().kgpu_spectrum_plan(fft_n, in_type, buf, 256), "kgpu_spectrum_plan"), buf.value.decode()
+
+
+class Spectrum:
+    """wideband_poll's analysis (reference spectrum.c:354-497) on a device ring of raw samples."""
+
+    def __init__(self, fft_n: int, in_type: int, bin_count: int):
+        self.lib = load()
+        self.h = self.lib.kgpu_spectrum_create(fft_n, in_type, bin_count)
+        if not self.h:
+            raise KgpuError("kgpu_spectrum_create: " + self.lib.kgpu_last_error().decode())
+        self.fft_n, self.in_type, self.bin_count = fft_n, in_type, bin_count
+
+    def describe(self) -> str:
+        buf = C.create_string_buffer(256)
+        self.lib.kgpu_spectrum_describe(self.h, buf, 256)
+        return buf.value.decode()
+
+    def set_window(self, window) -> None:
+        import numpy as np
+
+        w = np.ascontiguousarray(window, np.float32)
+        if w.shape != (self.fft_n,):
+            raise ValueError(f"window needs {self.fft_n} floats")
+        check(self.lib.kgpu_spectrum_set_window(self.h, w.ctypes.data), "kgpu_spectrum_set_window")
+
+    def run(self, ring, end: int, shift: int, fft_avg: int, overlap: float, bins, scale: float = 1.0,
+            derandomize: bool = False, stream: int = 0) -> None:
+        """ring: a CUDA tensor of float32 / int16 samples (REAL) or of (re, im) pairs as its last dimension of 2
+        (COMPLEX), any length >= fft_n; bins: a float32 CUDA tensor of at least bin_count elements."""
+        import torch
+
+        if not (ring.is_cuda and ring.is_contiguous() and bins.is_cuda and bins.dtype == torch.float32):
+            raise ValueError("ring and bins must be contiguous CUDA tensors, bins float32")
+        if ring.dtype == torch.float32:
+            fmt = KGPU_FMT_F32
+        elif ring.dtype == torch.int16:
+            fmt = KGPU_FMT_I16
+        else:
+            raise ValueError("ring must be float32 or int16")
+        samples = ring.numel() // (2 if self.in_type == KGPU_COMPLEX else 1)
+        if bins.numel() < self.bin_count:
+            raise ValueError(f"bins holds fewer than {self.bin_count} floats")
+        check(self.lib.kgpu_spectrum_run(self.h, ring.data_ptr(), samples, int(end), fmt, float(scale), int(derandomize),
+                                         int(shift), int(fft_avg), float(overlap), bins.data_ptr(), stream or None),
+              "kgpu_spectrum_run")
+
+    def close(self):
+        if self.h:
+            self.lib.kgpu_spectrum_destroy(self.h)
             self.h = None

@@ -64,6 +64,16 @@ struct snap { /* what the batched launch of one ring slot used for one slave */
   double complex alpha, beta;
 };
 
+/* a SPECTRUM slave served by filter_spectrum_setup / filter_spectrum_poll (extension) */
+struct spec_slave {
+  struct filter_out *slave;
+  kgpu_spectrum *ks;
+  int bin_count;
+  float *d_bins, *h_bins;
+  cudaEvent_t ev;
+  struct spec_slave *next;
+};
+
 struct master_ctx {
   kgpu_master *km;
   kgpu_bank *bank;
@@ -107,6 +117,14 @@ struct master_ctx {
   char *i16_wp, *i16_rp;
   float i16_scale;
   bool i16_derand;
+  unsigned long long issued; /* blocks issued to the device so far */
+  /* wideband spectrum analyzer (extension): a device copy of the input ring, in the ingest format, with the host float
+   * ring's capacity and positions; created by the first filter_spectrum_setup, then appended by every launch */
+  struct spec_slave *specs;
+  void *d_sring;
+  long sring_cap; /* samples */
+  long sring_pos; /* just past the newest issued sample */
+  bool sring_i16;
 };
 
 /* ---------------------------------------------------------------- mirrored ring ------------- */
@@ -174,6 +192,26 @@ static void *cache_aligned(size_t bytes) {
   return posix_memalign(&p, 64, bytes ? bytes : 64) == 0 ? p : NULL;
 }
 
+static void spec_slave_free(struct spec_slave *sp) {
+  kgpu_spectrum_destroy(sp->ks);
+  cudaFree(sp->d_bins);
+  cudaFreeHost(sp->h_bins);
+  if (sp->ev)
+    cudaEventDestroy(sp->ev);
+  free(sp);
+}
+/* unlink and free the analyzer of `slave` on master context c, if any (caller holds c->mu) */
+static void spec_slave_drop(struct master_ctx *c, struct filter_out const *slave) {
+  for (struct spec_slave **pp = &c->specs; *pp; pp = &(*pp)->next)
+    if ((*pp)->slave == slave) {
+      struct spec_slave *sp = *pp;
+      *pp = sp->next;
+      cudaStreamSynchronize(c->st);
+      spec_slave_free(sp);
+      return;
+    }
+}
+
 static void master_teardown(struct filter_in *master) {
   struct master_ctx *c = (struct master_ctx *)master->fwd_plan;
   if (c) {
@@ -203,6 +241,12 @@ static void master_teardown(struct filter_in *master) {
     cudaStreamDestroy(c->st_d2h);
     cudaEventDestroy(c->kev);
     ring_free(c->i16_ring, c->i16_ring_size);
+    while (c->specs) {
+      struct spec_slave *sp = c->specs;
+      c->specs = sp->next;
+      spec_slave_free(sp);
+    }
+    cudaFree(c->d_sring);
     pthread_mutex_destroy(&c->mu);
     free(c);
     master->fwd_plan = NULL;
@@ -341,6 +385,12 @@ int create_filter_output(struct filter_out *slave, struct filter_in *master, int
     pthread_mutex_init(&slave->response_mutex, NULL);
     slave->init = true;
   } else {
+    if (slave->out_type == SPECTRUM && slave->master && slave->master->fwd_plan) {
+      struct master_ctx *old = (struct master_ctx *)slave->master->fwd_plan;
+      pthread_mutex_lock(&old->mu);
+      spec_slave_drop(old, slave);
+      pthread_mutex_unlock(&old->mu);
+    }
     pthread_mutex_lock(&slave->response_mutex);
     free(slave->response);
     slave->response = NULL;
@@ -529,6 +579,77 @@ static void rebuild_ranges(struct filter_in *f, struct master_ctx *c) {
   }
 }
 
+/* ---------------------------------------------------------------- spectrum device ring ------ */
+/* n samples of esz bytes from a ring (src_cap samples, position src) to the device ring at position dst, both modular */
+static int sring_copy(struct master_ctx *c, char const *src_base, long src_cap, long src, long dst, long n, size_t esz,
+                      enum cudaMemcpyKind kind) {
+  while (n > 0) {
+    long len = n;
+    if (len > src_cap - src)
+      len = src_cap - src;
+    if (len > c->sring_cap - dst)
+      len = c->sring_cap - dst;
+    if (cudaMemcpyAsync((char *)c->d_sring + (size_t)dst * esz, src_base + (size_t)src * esz, (size_t)len * esz, kind,
+                        c->st) != cudaSuccess)
+      return -1;
+    n -= len;
+    src = (src + len) % src_cap;
+    dst = (dst + len) % c->sring_cap;
+  }
+  return 0;
+}
+/* (Re)create the device ring in the master's current ingest format and seed it from the host ring: the sring_cap samples
+ * up to the end of the last issued block.  Caller holds c->mu. */
+static int sring_seed(struct filter_in *f, struct master_ctx *c) {
+  cudaStreamSynchronize(c->st);
+  cudaFree(c->d_sring);
+  c->d_sring = NULL;
+  c->sring_i16 = c->i16_mode;
+  c->sring_cap = (long)(f->input_buffer_size / c->esz);
+  size_t const esz = c->sring_i16 ? c->i16_esz : c->esz;
+  if (cudaMalloc(&c->d_sring, (size_t)c->sring_cap * esz) != cudaSuccess) {
+    c->d_sring = NULL;
+    return kgf_fail("filter_spectrum_setup: device ring");
+  }
+  long const M1 = f->impulse_length - 1;
+  c->sring_pos = (long)((M1 + (unsigned long long)f->ilen * c->issued) % (unsigned long long)c->sring_cap);
+  char const *base;
+  long src_cap, src_end;
+  if (c->sring_i16) {
+    base = c->i16_ring;
+    src_cap = (long)(c->i16_ring_size / c->i16_esz);
+    src_end = (long)((c->i16_rp - (char *)c->i16_ring) / (long)c->i16_esz) + M1;
+  } else {
+    base = f->input_buffer;
+    src_cap = c->sring_cap;
+    src_end = (long)(((char *)(f->in_type == COMPLEX ? (void *)f->input_read_pointer.c : (void *)f->input_read_pointer.r) -
+                      (char *)f->input_buffer) / (long)c->esz) + M1;
+  }
+  long const n = c->sring_cap; /* the i16 ring holds at least as many samples as the float ring */
+  long const src = ((src_end - n) % src_cap + src_cap) % src_cap;
+  long const dst = ((c->sring_pos - n) % c->sring_cap + c->sring_cap) % c->sring_cap;
+  if (sring_copy(c, base, src_cap, src, dst, n, esz, cudaMemcpyHostToDevice) != 0 || cudaStreamSynchronize(c->st) != cudaSuccess)
+    return kgf_fail("filter_spectrum_setup: seeding the device ring");
+  return 0;
+}
+/* the k*L new samples of the launch just issued from d_win[slot] (after its M-1 history samples), on the pipeline stream */
+static int sring_append(struct filter_in *f, struct master_ctx *c, int k) {
+  if (c->sring_i16 != c->i16_mode) { /* the ingest format changed: the next poll seeds a new ring */
+    cudaStreamSynchronize(c->st);
+    cudaFree(c->d_sring);
+    c->d_sring = NULL;
+    return 0;
+  }
+  size_t const esz = c->sring_i16 ? c->i16_esz : c->esz;
+  long const n = (long)k * f->ilen;
+  void const *win = c->d_win[f->next_jobnum % ND];
+  if (sring_copy(c, (char const *)win + (size_t)(f->impulse_length - 1) * esz, LONG_MAX, 0, c->sring_pos, n, esz,
+                 cudaMemcpyDeviceToDevice) != 0)
+    return kgf_fail("execute_filter_input: spectrum ring append");
+  c->sring_pos = (c->sring_pos + n) % c->sring_cap;
+  return 0;
+}
+
 /* k consecutive blocks (jobs next_jobnum .. +k-1, ring slots without wrap) as one device launch sequence.
  * filter.c:558-651 (+ run_fft :485-555) */
 static int execute_filter_input_n(struct filter_in *const f, int const k) {
@@ -589,6 +710,9 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     rc = kgf_fail("execute_filter_input: H2D of the window");
   if (rc == 0 && kgpu_forward(c->km, c->d_win[slot], fmt, scale, c->i16_derand, k, spec, NULL, c->st) != 0)
     rc = kgf_fail("execute_filter_input: kgpu_forward");
+  if (rc == 0 && c->d_sring)
+    rc = sring_append(f, c, k);
+  c->issued += (unsigned long long)k;
   if (rc == 0 && f->notches && kgpu_apply_notches(c->km, spec, k, c->st) != 0)
     rc = kgf_fail("execute_filter_input: kgpu_apply_notches");
   /* every slave, batched, with the shift it used last (radio.c:1491: shifts move only on retune) */
@@ -1020,11 +1144,93 @@ int set_filter_weights(struct filter_out *out, double complex i_weight, double c
   return 0;
 }
 
+/* ---------------------------------------------------------------- wideband spectrum -------- */
+/* EXTENSION: wideband_poll (spectrum.c:308-522) on the device for a SPECTRUM slave.  fft_n floats of window, as
+ * generate_window() leaves them.  -1 (and the CPU loop stays with the caller) for lengths the analyzer cannot serve. */
+int filter_spectrum_setup(struct filter_out *slave, int fft_n, int bin_count, float const *window) {
+  if (slave == NULL || slave->out_type != SPECTRUM || slave->master == NULL || slave->master->fwd_plan == NULL ||
+      window == NULL || bin_count < 1)
+    return -1;
+  struct filter_in *f = slave->master;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  struct spec_slave *sp = calloc(1, sizeof *sp);
+  if (!sp)
+    return -1;
+  sp->slave = slave;
+  sp->bin_count = bin_count;
+  sp->ks = kgpu_spectrum_create(fft_n, f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL, bin_count);
+  if (!sp->ks) {
+    fprintf(stderr, "filter_spectrum_setup(fft_n=%d): %s\n", fft_n, kgpu_last_error());
+    free(sp);
+    return -1;
+  }
+  bool ok = kgpu_spectrum_set_window(sp->ks, window) == 0;
+  ok = ok && cudaMalloc((void **)&sp->d_bins, sizeof(float) * (size_t)bin_count) == cudaSuccess;
+  ok = ok && cudaHostAlloc((void **)&sp->h_bins, sizeof(float) * (size_t)bin_count, cudaHostAllocPortable) == cudaSuccess;
+  ok = ok && cudaEventCreateWithFlags(&sp->ev, cudaEventDisableTiming) == cudaSuccess;
+  if (!ok) {
+    spec_slave_free(sp);
+    return kgf_fail("filter_spectrum_setup");
+  }
+  pthread_mutex_lock(&c->mu);
+  spec_slave_drop(c, slave);
+  int rc = c->d_sring ? 0 : sring_seed(f, c);
+  if (rc == 0) {
+    sp->next = c->specs;
+    c->specs = sp;
+  }
+  pthread_mutex_unlock(&c->mu);
+  if (rc != 0)
+    spec_slave_free(sp);
+  return rc;
+}
+
+/* EXTENSION: one poll of the fft_avg segments ending at the end of the last block issued to the device (the reference
+ * reads up to the live write pointer, which may be up to one block newer); *end_sample = that sample index
+ * (frontend->samples at spectrum.c:365 / :425).  bin_data: bin_count floats, as wideband_poll leaves them. */
+int filter_spectrum_poll(struct filter_out *slave, int shift, int fft_avg, double overlap, float *bin_data,
+                         uint64_t *end_sample) {
+  if (slave == NULL || slave->master == NULL || slave->master->fwd_plan == NULL || bin_data == NULL)
+    return -1;
+  struct filter_in *f = slave->master;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  pthread_mutex_lock(&c->mu);
+  struct spec_slave *sp = c->specs;
+  while (sp && sp->slave != slave)
+    sp = sp->next;
+  int rc = sp ? 0 : -1;
+  if (rc == 0 && (c->d_sring == NULL || c->sring_i16 != c->i16_mode))
+    rc = sring_seed(f, c);
+  uint64_t const end = (uint64_t)f->ilen * c->issued;
+  if (rc == 0 && kgpu_spectrum_run(sp->ks, c->d_sring, c->sring_cap, c->sring_pos, c->sring_i16 ? KGPU_FMT_I16 : KGPU_FMT_F32,
+                                   c->i16_scale, c->i16_derand, shift, fft_avg, overlap, sp->d_bins, c->st) != 0)
+    rc = kgf_fail("filter_spectrum_poll: kgpu_spectrum_run");
+  if (rc == 0 && (cudaMemcpyAsync(sp->h_bins, sp->d_bins, sizeof(float) * (size_t)sp->bin_count, cudaMemcpyDeviceToHost,
+                                  c->st) != cudaSuccess ||
+                  cudaEventRecord(sp->ev, c->st) != cudaSuccess))
+    rc = kgf_fail("filter_spectrum_poll: D2H of the bins");
+  pthread_mutex_unlock(&c->mu);
+  if (rc == 0 && cudaEventSynchronize(sp->ev) != cudaSuccess)
+    rc = kgf_fail("filter_spectrum_poll: wait");
+  if (rc != 0)
+    return -1;
+  memcpy(bin_data, sp->h_bins, sizeof(float) * (size_t)sp->bin_count);
+  if (end_sample)
+    *end_sample = end;
+  return 0;
+}
+
 /* ---------------------------------------------------------------- delete -------------------- */
 int delete_filter_output(struct filter_out *slave) { /* filter.c:943-957 */
   if (slave == NULL)
     return -1;
   struct slave_ctx *sc = (struct slave_ctx *)slave->rev_plan;
+  if (slave->out_type == SPECTRUM && slave->master && slave->master->fwd_plan) {
+    struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
+    pthread_mutex_lock(&c->mu);
+    spec_slave_drop(c, slave);
+    pthread_mutex_unlock(&c->mu);
+  }
   if (sc && slave->master && slave->master->fwd_plan) {
     struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
     pthread_mutex_lock(&c->mu);

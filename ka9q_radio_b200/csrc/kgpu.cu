@@ -8,6 +8,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <complex>
 #include <atomic>
 #include <map>
 #include <mutex>
@@ -25,6 +26,7 @@
 #include "static_kernels_v2.cuh"
 #include "fwd_cols_r36.cuh"
 #include "fwd_2s.cuh"
+#include "spectrum_kernels.cuh"
 
 using namespace kfft;
 
@@ -1974,6 +1976,245 @@ extern "C" int kgpu_plan_split(long n, int *n1, int *n2) {
   if (!choose_split(n, &sp)) return -1;
   *n1 = sp.n1;
   *n2 = sp.n2;
+  return 0;
+}
+
+// ------------------------------------------------------------------ wideband spectrum analyzer ----------
+// wideband_poll (spectrum.c:308-522) on the device: spectrum_kernels.cuh around a forward master of its own.  The path
+// is a function of fft_n and the input type alone:
+//   SP_R2C        REAL, even fft_n, fft_n/2 23-smooth: the r2c pair of a REAL master L = fft_n, M = 1
+//   SP_C2C        COMPLEX 23-smooth fft_n, or REAL odd 23-smooth fft_n: a COMPLEX master of length fft_n
+//   SP_BLUESTEIN  anything else: two passes of a COMPLEX master of the smallest 7-smooth length P >= 2 fft_n - 1
+enum SpecPath { SP_R2C, SP_C2C, SP_BLUESTEIN };
+struct SpecPlan {
+  SpecPath path;
+  long nc;  // complex points of the forward master (fft_n/2, fft_n or P)
+  long P;   // transform length of the master (fft_n or P)
+  Split2 sp;
+};
+
+// Bound on the scratch of one poll (per buffer): longer polls run in chunks of segments.
+static constexpr long kSpectrumScratchCap = 64L << 20;
+
+// the split kgpu_master_create(_ex) would run for nc complex points, if its kernels fit shared memory
+static bool forward_split(long nc, bool ext, Split2 *sp) {
+  if (!(ext ? choose_split_ext(nc, sp) : choose_split(nc, sp))) return false;
+  size_t const smem1 = sizeof(float2) * ((size_t)kTile * column_pitch(sp->n1) + (size_t)kTile * ((sp->n1 + 31) / 32));
+  size_t const smem2 = sizeof(float2) * ((size_t)kTile * column_pitch(sp->n2));
+  return smem1 <= (size_t)kChanSmemLimit && smem2 <= (size_t)kChanSmemLimit;
+}
+static int spectrum_plan(int fft_n, int in_type, SpecPlan *pl) {
+  if (fft_n < 2 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX))
+    return fail("kgpu_spectrum: bad arguments fft_n=%d type=%d", fft_n, in_type);
+  bool const real = in_type == KGPU_REAL;
+  if (real && !(fft_n & 1) && smooth23(fft_n / 2) && forward_split(fft_n / 2, true, &pl->sp)) {
+    pl->path = SP_R2C;
+    pl->nc = fft_n / 2;
+    pl->P = fft_n;
+    return 0;
+  }
+  if ((!real || (fft_n & 1)) && smooth23(fft_n) && forward_split(fft_n, true, &pl->sp)) {
+    pl->path = SP_C2C;
+    pl->nc = pl->P = fft_n;
+    return 0;
+  }
+  long const limit = (long)kMaxTileLen * kMaxTileLen;
+  for (long P = 2L * fft_n - 1; P <= limit; P++)
+    if (smooth7(P) && forward_split(P, false, &pl->sp)) {
+      pl->path = SP_BLUESTEIN;
+      pl->nc = pl->P = P;
+      return 0;
+    }
+  return fail("kgpu_spectrum: %d points have a prime factor >= 29 and need a Bluestein transform of at least %ld points, "
+              "more than the forward pair splits", fft_n, 2L * fft_n - 1);
+}
+static void spectrum_plan_text(int fft_n, int in_type, SpecPlan const &pl, char *buf, int buflen) {
+  char const *path = pl.path == SP_R2C ? "r2c" : pl.path == SP_C2C ? "complex" : "bluestein";
+  snprintf(buf, (size_t)buflen, "%s fft_n=%d %s P=%ld: %ld-point complex two-pass %d x %d", path, fft_n,
+           in_type == KGPU_REAL ? "real" : "complex", pl.P, pl.nc, pl.sp.n1, pl.sp.n2);
+}
+
+// Forward DFT of n points (factors 2, 3, 5, 7) in place, in double: decimation in time, radix = smallest factor.
+// tw[e * d] = exp(-2 pi i e / n) (d: the stride of this sub-transform in the top-level table).
+static void host_dft(std::complex<double> *x, long n, std::complex<double> const *tw, long d) {
+  if (n == 1) return;
+  int const r = n % 2 == 0 ? 2 : n % 3 == 0 ? 3 : n % 5 == 0 ? 5 : 7;
+  long const m = n / r;
+  std::vector<std::complex<double>> t((size_t)n);
+  for (long j = 0; j < m; j++)
+    for (int q = 0; q < r; q++) t[(size_t)(q * m + j)] = x[j * r + q];
+  for (int q = 0; q < r; q++) host_dft(t.data() + q * m, m, tw, d * r);
+  for (long k = 0; k < m; k++)
+    for (int s = 0; s < r; s++) {
+      long const kk = k + s * m;
+      std::complex<double> acc = t[(size_t)k];
+      for (int q = 1; q < r; q++) acc += t[(size_t)(q * m + k)] * tw[(size_t)(((long)q * kk) % n * d)];
+      x[kk] = acc;
+    }
+}
+
+struct kgpu_spectrum {
+  int fft_n, in_type, bin_count;
+  SpecPlan pl;
+  kgpu_master *m = nullptr;
+  float *d_window = nullptr;
+  float2 *d_bspec = nullptr;  // Bluestein: DFT_P of the conjugate chirp
+  void *d_in = nullptr;       // chunk windowed segments (float fft_n for the r2c, float2 P otherwise)
+  float2 *d_spec = nullptr;   // chunk spectra, master spec_stride apart
+  long in_len = 0;            // elements per segment of d_in
+  long spec_stride = 0;
+  int chunk = 0;              // segments per chunk
+};
+
+extern "C" int kgpu_spectrum_plan(int fft_n, int in_type, char *buf, int buflen) {
+  SpecPlan pl;
+  if (spectrum_plan(fft_n, in_type, &pl)) return -1;
+  if (buf && buflen > 0) spectrum_plan_text(fft_n, in_type, pl, buf, buflen);
+  return (int)pl.path;
+}
+
+extern "C" void kgpu_spectrum_destroy(kgpu_spectrum *s) {
+  if (!s) return;
+  kgpu_master_destroy(s->m);
+  cudaFree(s->d_window);
+  cudaFree(s->d_bspec);
+  cudaFree(s->d_in);
+  cudaFree(s->d_spec);
+  delete s;
+}
+
+extern "C" kgpu_spectrum *kgpu_spectrum_create(int fft_n, int in_type, int bin_count) {
+  SpecPlan pl;
+  if (bin_count < 1) {
+    fail("kgpu_spectrum_create: bad bin_count %d", bin_count);
+    return nullptr;
+  }
+  if (spectrum_plan(fft_n, in_type, &pl)) return nullptr;
+  kgpu_spectrum *s = new kgpu_spectrum;
+  s->fft_n = fft_n;
+  s->in_type = in_type;
+  s->bin_count = bin_count;
+  s->pl = pl;
+  bool const r2c = pl.path == SP_R2C;
+  s->m = r2c ? kgpu_master_create_ex(fft_n, 1, KGPU_REAL)
+             : pl.path == SP_C2C ? kgpu_master_create_ex(fft_n, 1, KGPU_COMPLEX) : kgpu_master_create((int)pl.P, 1, KGPU_COMPLEX);
+  if (!s->m) {
+    fail("kgpu_spectrum_create: %s", std::string(g_err).c_str());
+    kgpu_spectrum_destroy(s);
+    return nullptr;
+  }
+  s->spec_stride = s->m->spec_stride;
+  s->in_len = r2c ? fft_n : pl.P;
+  size_t const in_bytes = r2c ? sizeof(float) * (size_t)fft_n : sizeof(float2) * (size_t)pl.P;
+  size_t const spec_bytes = sizeof(float2) * (size_t)s->spec_stride;
+  size_t const mid_bytes = sizeof(float2) * (size_t)s->m->sp.n1 * (size_t)((s->m->sp.n2 + 15) / 16 * 16);
+  s->chunk = (int)std::min(32768L, std::max(1L, kSpectrumScratchCap / (long)std::max(in_bytes, std::max(spec_bytes, mid_bytes))));
+  std::vector<float> ones((size_t)fft_n, 1.0f);
+  cudaError_t e = cudaMalloc(&s->d_window, sizeof(float) * (size_t)fft_n);
+  if (e == cudaSuccess) e = cudaMemcpy(s->d_window, ones.data(), sizeof(float) * (size_t)fft_n, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMalloc(&s->d_in, in_bytes * (size_t)s->chunk);
+  if (e == cudaSuccess) e = cudaMalloc(&s->d_spec, spec_bytes * (size_t)s->chunk);
+  if (e == cudaSuccess && pl.path == SP_BLUESTEIN) {
+    // b_m = conj(w_m) on -(fft_n-1) .. fft_n-1, wrapped modulo P, and its transform B = DFT_P(b)
+    long const P = pl.P, n = fft_n;
+    // transformed in double on the host and rounded once: a float transform here would add a third float transform's
+    // error to every poll
+    std::vector<std::complex<double>> bd((size_t)P), tw((size_t)P);
+    for (long m = 0; m < n; m++) {
+      long double const ang = M_PIl * (long double)((m * m) % (2 * n)) / (long double)n;
+      std::complex<double> const v((double)cosl(ang), (double)sinl(ang));  // conj(exp(-i ang))
+      bd[(size_t)m] = v;
+      if (m) bd[(size_t)(P - m)] = v;
+    }
+    for (long e2 = 0; e2 < P; e2++) {
+      long double const ang = -2.0L * M_PIl * (long double)e2 / (long double)P;
+      tw[(size_t)e2] = std::complex<double>((double)cosl(ang), (double)sinl(ang));
+    }
+    host_dft(bd.data(), P, tw.data(), 1);
+    std::vector<float2> b((size_t)P);
+    for (long k = 0; k < P; k++) b[(size_t)k] = make_float2((float)bd[(size_t)k].real(), (float)bd[(size_t)k].imag());
+    e = cudaMalloc(&s->d_bspec, sizeof(float2) * (size_t)P);
+    if (e == cudaSuccess) e = cudaMemcpy(s->d_bspec, b.data(), sizeof(float2) * (size_t)P, cudaMemcpyHostToDevice);
+  }
+  if (e != cudaSuccess) {
+    fail("kgpu_spectrum_create(%d): %s", fft_n, cudaGetErrorString(e));
+    kgpu_spectrum_destroy(s);
+    return nullptr;
+  }
+  return s;
+}
+
+extern "C" int kgpu_spectrum_set_window(kgpu_spectrum *s, float const *window) {
+  if (!s || !window) return fail("kgpu_spectrum_set_window: bad arguments");
+  CUDA_OK(cudaMemcpy(s->d_window, window, sizeof(float) * (size_t)s->fft_n, cudaMemcpyHostToDevice));
+  return 0;
+}
+
+extern "C" int kgpu_spectrum_describe(kgpu_spectrum const *s, char *buf, int buflen) {
+  if (!s || !buf || buflen < 1) return -1;
+  spectrum_plan_text(s->fft_n, s->in_type, s->pl, buf, buflen);
+  return 0;
+}
+
+extern "C" int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring_samples, long end, int fmt, float scale,
+                                 int derandomize, int shift, int fft_avg, double overlap, float *d_bins, void *stream) {
+  if (!s || !d_ring || !d_bins || fft_avg < 1 || !(overlap >= 0.0 && overlap < 1.0) ||
+      (fmt != KGPU_FMT_F32 && fmt != KGPU_FMT_I16))
+    return fail("kgpu_spectrum_run: bad arguments");
+  int const fft_n = s->fft_n;
+  if (ring_samples < fft_n) return fail("kgpu_spectrum_run: a ring of %ld samples is shorter than fft_n=%d", ring_samples, fft_n);
+  cudaStream_t st = (cudaStream_t)stream;
+  bool const real = s->in_type == KGPU_REAL;
+  // spectrum.c:364,407 (REAL) and :422,491 (COMPLEX), in double as there
+  long const adjust = lrint(fft_n * (1 + (fft_avg - 1) * (1 - overlap)));
+  long const hop = lrint(fft_n * (1. - overlap));
+  long start0 = (end - adjust) % ring_samples;
+  if (start0 < 0) start0 += ring_samples;
+  SpecWindowArgs w;
+  w.ring = d_ring;
+  w.cap = ring_samples;
+  w.start0 = start0;
+  w.step = real ? hop : -hop;
+  w.fft_n = fft_n;
+  w.out_len = (int)s->in_len;
+  w.complex_in = !real;
+  w.i16 = fmt == KGPU_FMT_I16;
+  w.derandomize = derandomize != 0;
+  w.flip = real && shift < 0;
+  w.complex_out = s->pl.path != SP_R2C;
+  w.chirp = s->pl.path == SP_BLUESTEIN;
+  w.scale = scale;
+  w.window = s->d_window;
+  w.out = s->d_in;
+  SpecPowerArgs p;
+  p.spec = s->d_spec;
+  p.spec_stride = s->spec_stride;
+  p.real_walk = real;
+  p.fft_n = fft_n;
+  p.shift = shift;
+  p.bin_count = s->bin_count;
+  p.norm = s->pl.path == SP_BLUESTEIN ? 1.0 / ((double)s->pl.P * (double)s->pl.P) : 1.0;
+  p.gain = (real ? 2. : 1.) / (double)((int64_t)fft_avg * fft_n * fft_n);  // spectrum.c:373, :431
+  p.bins = d_bins;
+  for (int seg0 = 0; seg0 < fft_avg; seg0 += s->chunk) {
+    int const nseg = std::min(s->chunk, fft_avg - seg0);
+    w.seg0 = seg0;
+    spectrum_window_kernel<<<dim3((unsigned)((s->in_len + kSpecThreads - 1) / kSpecThreads), (unsigned)nseg), kSpecThreads, 0,
+                             st>>>(w);
+    g_launches++;
+    if (kgpu_forward(s->m, s->d_in, KGPU_FMT_F32, 1.0f, 0, nseg, s->d_spec, nullptr, st) != 0) return -1;
+    if (s->pl.path == SP_BLUESTEIN) {
+      bluestein_mul_kernel<<<dim3((unsigned)((s->pl.P + kSpecThreads - 1) / kSpecThreads), (unsigned)nseg), kSpecThreads, 0,
+                             st>>>(s->d_spec, s->spec_stride, s->d_bspec, (int)s->pl.P, (float2 *)s->d_in);
+      g_launches++;
+      if (kgpu_forward(s->m, s->d_in, KGPU_FMT_F32, 1.0f, 0, nseg, s->d_spec, nullptr, st) != 0) return -1;
+    }
+    p.nseg = nseg;
+    p.first = seg0 == 0;
+    spectrum_power_kernel<<<(unsigned)((s->bin_count + kSpecThreads - 1) / kSpecThreads), kSpecThreads, 0, st>>>(p);
+    g_launches++;
+  }
+  CUDA_OK(cudaGetLastError());
   return 0;
 }
 
