@@ -66,11 +66,26 @@ kgpu_master *kgpu_master_create(int L, int M, int in_type);
  * has no effect on it.  Fails for a prime factor >= 29, or when Nc has no split n1 x n2 into plannable factors of at
  * most 4096 points, or when that split does not fit shared memory. */
 kgpu_master *kgpu_master_create_ex(int L, int M, int in_type);
+/* Same, for any transform length, as the reference plans (filter.c:201), e.g. an RX888 at 62 MS/s (REAL, N = 1550000,
+ * Nc = 775000 = 2^3 5^5 31) or a COMPLEX front end at 2.9 MS/s (N = 72500 = 2^2 5^4 29).  Where kgpu_master_create_ex
+ * succeeds it returns exactly that master.  Otherwise it builds a Bluestein transform: the window times the chirp
+ * exp(-i pi n^2 / Nc), zero-padded to the smallest P >= 2 Nc - 1 with factors 2, 3, 5, 7 whose split the forward pair
+ * runs, two forward passes of an internal COMPLEX master of length P around the product with the chirp's transform
+ * (computed in double on the host), then the output chirp and, for REAL masters, the real split.  The spectrum layout,
+ * int16 ingest, statistics and every other master call are those of any master.  The master owns scratch of at most
+ * about 128 MB per buffer; launches of more blocks run in chunks.  Fails for REAL input with odd L or odd N, and when
+ * P would exceed 3500 x 3500 (Nc > 6125000). */
+kgpu_master *kgpu_master_create_any(int L, int M, int in_type);
+/* Pure host code: the master kgpu_master_create_any would build (0 kgpu_master_create's, 1 kgpu_master_create_ex's
+ * extended pair, 2 Bluestein; -1 when it would fail) and, if buf is not NULL, the string kgpu_master_describe would
+ * print for it. */
+int kgpu_master_plan(int L, int M, int in_type, char *buf, int buflen);
 void kgpu_master_destroy(kgpu_master *m);
 int kgpu_master_points(kgpu_master const *m);       /* N */
 int kgpu_master_bins(kgpu_master const *m);         /* REAL: N/2+1, COMPLEX: N (filter.c:197) */
 long kgpu_master_spec_stride(kgpu_master const *m); /* float2 elements between consecutive block spectra */
-/* Plan description for logs/DESIGN.md: "n1 x n2, radices ..." */
+/* Plan description for logs/DESIGN.md: "n1 x n2, radices ..."; a Bluestein master of kgpu_master_create_any:
+ * "N=... real|complex, bluestein P=...: <the internal master's transform and kernels> around bluestein_in_kernel, ..." */
 int kgpu_master_describe(kgpu_master const *m, char *buf, int buflen);
 
 /* Forward transform of `nblocks` consecutive overlap-save windows (replaces run_fft's

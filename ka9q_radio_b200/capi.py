@@ -50,6 +50,9 @@ def load() -> C.CDLL:
     L.kgpu_master_create.argtypes = [i, i, i]
     L.kgpu_master_create_ex.restype = vp
     L.kgpu_master_create_ex.argtypes = [i, i, i]
+    L.kgpu_master_create_any.restype = vp
+    L.kgpu_master_create_any.argtypes = [i, i, i]
+    L.kgpu_master_plan.argtypes = [i, i, i, C.c_char_p, i]
     L.kgpu_master_destroy.argtypes = [vp]
     L.kgpu_master_points.argtypes = [vp]
     L.kgpu_master_bins.argtypes = [vp]
@@ -160,17 +163,31 @@ def check(rc: int, what: str = "") -> int:
     return rc
 
 
+MASTER_DIRECT, MASTER_EXTENDED, MASTER_BLUESTEIN = 0, 1, 2
+
+
+def plan_master(L: int, M: int, in_type: int) -> tuple[int, str]:
+    """(path, description) of the master kgpu_master_create_any would build; pure host code.  Raises when it would
+    fail."""
+    buf = C.create_string_buffer(512)
+    return check(load().kgpu_master_plan(L, M, in_type, buf, 512), "kgpu_master_plan"), buf.value.decode()
+
+
 class Master:
     """create_filter_input's device half (reference filter.c:186-269)."""
 
-    def __init__(self, L: int, M: int, in_type: int, extended: bool = False):
+    def __init__(self, L: int, M: int, in_type: int, extended: bool = False, any_length: bool = False):
         """extended: create with kgpu_master_create_ex, which also serves transform lengths with prime factors 11, 13,
-        17, 19 and 23 (and is kgpu_master_create for every other length)"""
+        17, 19 and 23 (and is kgpu_master_create for every other length).  any_length: create with
+        kgpu_master_create_any, which is kgpu_master_create_ex wherever that succeeds and a Bluestein transform
+        elsewhere."""
         self.lib = load()
-        create = self.lib.kgpu_master_create_ex if extended else self.lib.kgpu_master_create
-        self.h = create(L, M, in_type)
-        if not self.h:
+        if any_length:
+            what = "kgpu_master_create_any"
+        else:
             what = "kgpu_master_create_ex" if extended else "kgpu_master_create"
+        self.h = getattr(self.lib, what)(L, M, in_type)
+        if not self.h:
             raise KgpuError(f"{what}: " + self.lib.kgpu_last_error().decode())
         self.L, self.M, self.in_type = L, M, in_type
         self.N = self.lib.kgpu_master_points(self.h)

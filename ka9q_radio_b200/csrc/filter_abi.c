@@ -279,8 +279,9 @@ int create_filter_input(struct filter_in *master, int const L, int const M, enum
   struct master_ctx *c = calloc(1, sizeof *c);
   if (!c)
     return -1;
-  /* prime factors up to 23 (filter.c:201 plans any N): a 7-smooth N gets exactly kgpu_master_create's master */
-  c->km = kgpu_master_create_ex(L, M, in_type == REAL ? KGPU_REAL : KGPU_COMPLEX);
+  /* any N, as filter.c:201 plans: where kgpu_master_create_ex serves N this is exactly its master (and a 7-smooth N
+   * gets kgpu_master_create's); other lengths run a Bluestein transform with the same spectrum layout */
+  c->km = kgpu_master_create_any(L, M, in_type == REAL ? KGPU_REAL : KGPU_COMPLEX);
   if (!c->km) {
     fprintf(stderr, "create_filter_input(L=%d M=%d): %s\n", L, M, kgpu_last_error());
     free(c);

@@ -27,6 +27,7 @@
 #include "fwd_cols_r36.cuh"
 #include "fwd_2s.cuh"
 #include "spectrum_kernels.cuh"
+#include "bluestein_master.cuh"
 
 using namespace kfft;
 
@@ -692,6 +693,65 @@ static long factor_above7(long n) {
     }
   return n > 7 ? std::max(big, n) : big;
 }
+
+// the split kgpu_master_create(_ex) would run for nc complex points, if its kernels fit shared memory
+static bool forward_split(long nc, bool ext, Split2 *sp) {
+  if (!(ext ? choose_split_ext(nc, sp) : choose_split(nc, sp))) return false;
+  size_t const smem1 = sizeof(float2) * ((size_t)kTile * column_pitch(sp->n1) + (size_t)kTile * ((sp->n1 + 31) / 32));
+  size_t const smem2 = sizeof(float2) * ((size_t)kTile * column_pitch(sp->n2));
+  return smem1 <= (size_t)kChanSmemLimit && smem2 <= (size_t)kChanSmemLimit;
+}
+
+// The Bluestein length of a transform of n points, shared by the spectrum analyzer and kgpu_master_create_any: the
+// smallest P >= 2n - 1 with factors 2, 3, 5, 7 whose split the forward pair runs.  The largest such P is 3500 x 3500.
+static bool bluestein_length(long n, long *P, Split2 *sp) {
+  long const limit = (long)kMaxTileLen * kMaxTileLen;
+  for (long p = 2 * n - 1; p <= limit; p++)
+    if (smooth7(p) && forward_split(p, false, sp)) {
+      *P = p;
+      return true;
+    }
+  return false;
+}
+
+// Forward DFT of n points (factors 2, 3, 5, 7) in place, in double: decimation in time, radix = smallest factor.
+// tw[e * d] = exp(-2 pi i e / n) (d: the stride of this sub-transform in the top-level table).
+static void host_dft(std::complex<double> *x, long n, std::complex<double> const *tw, long d) {
+  if (n == 1) return;
+  int const r = n % 2 == 0 ? 2 : n % 3 == 0 ? 3 : n % 5 == 0 ? 5 : 7;
+  long const m = n / r;
+  std::vector<std::complex<double>> t((size_t)n);
+  for (long j = 0; j < m; j++)
+    for (int q = 0; q < r; q++) t[(size_t)(q * m + j)] = x[j * r + q];
+  for (int q = 0; q < r; q++) host_dft(t.data() + q * m, m, tw, d * r);
+  for (long k = 0; k < m; k++)
+    for (int s = 0; s < r; s++) {
+      long const kk = k + s * m;
+      std::complex<double> acc = t[(size_t)k];
+      for (int q = 1; q < r; q++) acc += t[(size_t)(q * m + k)] * tw[(size_t)(((long)q * kk) % n * d)];
+      x[kk] = acc;
+    }
+}
+
+// B = DFT_P(b), b_m = conj(w_m) on -(n-1) .. n-1 wrapped modulo P, w_m = exp(-i pi m^2 / n): transformed in double on
+// the host and rounded once, since a float transform here would add a third float transform's error to every result.
+static std::vector<float2> bluestein_bspec(long n, long P) {
+  std::vector<std::complex<double>> bd((size_t)P), tw((size_t)P);
+  for (long m = 0; m < n; m++) {
+    long double const ang = M_PIl * (long double)((m * m) % (2 * n)) / (long double)n;
+    std::complex<double> const v((double)cosl(ang), (double)sinl(ang));  // conj(exp(-i ang))
+    bd[(size_t)m] = v;
+    if (m) bd[(size_t)(P - m)] = v;
+  }
+  for (long e2 = 0; e2 < P; e2++) {
+    long double const ang = -2.0L * M_PIl * (long double)e2 / (long double)P;
+    tw[(size_t)e2] = std::complex<double>((double)cosl(ang), (double)sinl(ang));
+  }
+  host_dft(bd.data(), P, tw.data(), 1);
+  std::vector<float2> b((size_t)P);
+  for (long k = 0; k < P; k++) b[(size_t)k] = make_float2((float)bd[(size_t)k].real(), (float)bd[(size_t)k].imag());
+  return b;
+}
 }  // namespace kfft
 
 // ------------------------------------------------------------------ master ------------------
@@ -730,6 +790,12 @@ struct kgpu_master {
   // the extended pair fwd_cols_ext / fwd_rows_ext, which take them by value
   bool ext = false;
   TilePlan xplan1{}, xplan2{};
+  // kgpu_master_create_any with a Bluestein transform (bluestein_master.cuh): the internal COMPLEX master of length bp,
+  // the device copy of DFT_P of the conjugate chirp, and scratch for b_blocks blocks of at most b_chunk per launch
+  kgpu_master *bs = nullptr;
+  long bp = 0;
+  float2 *d_bspec = nullptr, *d_bin = nullptr, *d_bout = nullptr;
+  int b_chunk = 0, b_blocks = 0;
   // notches
   NotchDev *d_notch = nullptr;
   int n_notch = 0;
@@ -766,10 +832,30 @@ static int upload(float2 **d, std::vector<float2> const &v) {
   return 0;
 }
 
-// kernel choice, tables and shared-memory limits of a master whose split and plans are set
-static int master_setup(kgpu_master *m) {
-  int const n1 = m->sp.n1, n2 = m->sp.n2;
-  bool const real = m->in_type == KGPU_REAL;
+// The part of a master that needs no device: geometry, shared-memory sizes, the kernel pair and its launch shape.
+// kgpu_master_create(_ex) and the host-only kgpu_master_plan share it, so the plan describes what creation builds.
+static void master_shape(kgpu_master *m, int L, int M, int in_type, Split2 const &sp, bool ext) {
+  m->L = L;
+  m->M = M;
+  m->N = L + M - 1;
+  m->in_type = in_type;
+  m->bins = (in_type == KGPU_COMPLEX) ? m->N : m->N / 2 + 1;
+  m->nc = (in_type == KGPU_COMPLEX) ? m->N : m->N / 2;
+  m->sp = sp;
+  m->ext = ext;
+  m->pitch1 = column_pitch(sp.n1);
+  m->pitch2 = column_pitch(sp.n2);
+  int const nit = (sp.n1 + 31) / 32;
+  m->smem1 = sizeof(float2) * ((size_t)kTile * m->pitch1 + (size_t)kTile * nit);
+  m->smem2 = sizeof(float2) * ((size_t)kTile * m->pitch2);
+  m->spec_stride = ((long)m->bins + 3) / 4 * 4;
+  int const n1 = sp.n1, n2 = sp.n2;
+  bool const real = in_type == KGPU_REAL;
+  if (ext) {  // the extended generic pair only
+    m->mid_ld = n2;
+    m->n_item_ctas = m->n_rows_ctas = real ? (n1 / 2 + 1 + 3) / 4 : (n1 + 7) / 8;
+    return;
+  }
   if (!real && n1 == 800 && n2 == 625) {
     m->cols = COLS_2S;
     m->rows = ROWS_2S;
@@ -783,7 +869,12 @@ static int master_setup(kgpu_master *m) {
   m->n_item_ctas = real ? (n1 / 2 + 1 + 3) / 4 : (n1 + 7) / 8;
   int const ipc = m->rows == ROWS_V2 ? (real ? RowsV2Shape<true>::IPC : RowsV2Shape<false>::IPC) : 0;
   m->n_rows_ctas = ipc ? ((real ? n1 / 2 + 1 : n1) + ipc - 1) / ipc : m->rows == ROWS_2S ? (n1 + 7) / 8 : m->n_item_ctas;
+}
 
+// tables and shared-memory limits of a master whose shape and plans are set
+static int master_setup(kgpu_master *m) {
+  int const n1 = m->sp.n1, n2 = m->sp.n2;
+  bool const real = m->in_type == KGPU_REAL;
   auto root = [](long e, long n) {
     long double const ang = -2.0L * M_PIl * (long double)(e % n) / (long double)n;
     return make_float2((float)cosl(ang), (float)sinl(ang));
@@ -849,19 +940,15 @@ extern "C" kgpu_master *kgpu_master_create(int L, int M, int in_type) {
     fail("kgpu_master_create: REAL input needs even L and even N=L+M-1 (got L=%d N=%d)", L, N);
     return nullptr;
   }
-  kgpu_master *m = new kgpu_master;
-  m->L = L;
-  m->M = M;
-  m->N = N;
-  m->in_type = in_type;
-  m->bins = (in_type == KGPU_COMPLEX) ? N : N / 2 + 1;
-  m->nc = (in_type == KGPU_COMPLEX) ? N : N / 2;
-  if (!choose_split(m->nc, &m->sp)) {
-    fail("kgpu_master_create: %ld points cannot be split into two plannable lengths (factors 2,3,5,7; <= %d)",
-         m->nc, kMaxTileLen);
-    delete m;
+  long const nc = (in_type == KGPU_COMPLEX) ? N : N / 2;
+  Split2 sp;
+  if (!choose_split(nc, &sp)) {
+    fail("kgpu_master_create: %ld points cannot be split into two plannable lengths (factors 2,3,5,7; <= %d)", nc,
+         kMaxTileLen);
     return nullptr;
   }
+  kgpu_master *m = new kgpu_master;
+  master_shape(m, L, M, in_type, sp, false);
   m->plan1 = get_tile_plan(m->sp.n1);
   m->plan2 = get_tile_plan(m->sp.n2);
   if (m->plan1 < 0 || m->plan2 < 0) {
@@ -869,12 +956,6 @@ extern "C" kgpu_master *kgpu_master_create(int L, int M, int in_type) {
     delete m;
     return nullptr;
   }
-  m->pitch1 = column_pitch(m->sp.n1);
-  m->pitch2 = column_pitch(m->sp.n2);
-  int const nit = (m->sp.n1 + 31) / 32;
-  m->smem1 = sizeof(float2) * ((size_t)kTile * m->pitch1 + (size_t)kTile * nit);
-  m->smem2 = sizeof(float2) * ((size_t)kTile * m->pitch2);
-  m->spec_stride = ((long)m->bins + 3) / 4 * 4;
   if (master_setup(m)) {
     kgpu_master_destroy(m);
     return nullptr;
@@ -922,23 +1003,9 @@ extern "C" kgpu_master *kgpu_master_create_ex(int L, int M, int in_type) {
     return nullptr;
   }
   kgpu_master *m = new kgpu_master;
-  m->L = L;
-  m->M = M;
-  m->N = N;
-  m->in_type = in_type;
-  m->bins = (in_type == KGPU_COMPLEX) ? N : N / 2 + 1;
-  m->nc = nc;
-  m->sp = sp;
-  m->ext = true;
+  master_shape(m, L, M, in_type, sp, true);
   m->plan1 = m->plan2 = -1;
-  m->pitch1 = column_pitch(sp.n1);
-  m->pitch2 = column_pitch(sp.n2);
-  m->smem1 = smem1;
-  m->smem2 = smem2;
-  m->spec_stride = ((long)m->bins + 3) / 4 * 4;
   bool const real = in_type == KGPU_REAL;
-  m->mid_ld = sp.n2;
-  m->n_item_ctas = m->n_rows_ctas = real ? (sp.n1 / 2 + 1 + 3) / 4 : (sp.n1 + 7) / 8;
   bool ok = make_tile_plan(sp.n1, choose_radices_ext(sp.n1), m->xplan1) == 0 &&
             make_tile_plan(sp.n2, choose_radices_ext(sp.n2), m->xplan2) == 0;
   if (ok && real) {
@@ -973,30 +1040,134 @@ extern "C" void kgpu_master_destroy(kgpu_master *m) {
   cudaFree(m->d_rtw0);
   cudaFree(m->d_mid);
   cudaFree(m->d_notch);
+  kgpu_master_destroy(m->bs);
+  cudaFree(m->d_bspec);
+  cudaFree(m->d_bin);
+  cudaFree(m->d_bout);
   delete m;
 }
 extern "C" int kgpu_master_points(kgpu_master const *m) { return m ? m->N : -1; }
 extern "C" int kgpu_master_bins(kgpu_master const *m) { return m ? m->bins : -1; }
 extern "C" long kgpu_master_spec_stride(kgpu_master const *m) { return m ? m->spec_stride : -1; }
-extern "C" int kgpu_master_describe(kgpu_master const *m, char *buf, int buflen) {
-  if (!m || !buf) return -1;
-  auto radices = [](TilePlan const *p) {
+
+// What kgpu_master_describe prints for a master of this shape (master_shape: no device state is read).  The radices
+// are the planner's, which are what the tile plans of the generic kernels hold.
+static std::string describe_text(kgpu_master const *m) {
+  auto radices = [](std::vector<int> const &v) {
     std::string r;
-    for (int i = 0; i < p->nstages; i++) r += std::to_string(p->radix[i]) + (i + 1 < p->nstages ? "," : "");
+    for (size_t i = 0; i < v.size(); i++) r += std::to_string(v[i]) + (i + 1 < v.size() ? "," : "");
     return r;
   };
-  // the tile plans are what the generic kernels run
-  TilePlan const *p1 = m->ext ? &m->xplan1 : host_tile_plan(m->plan1), *p2 = m->ext ? &m->xplan2 : host_tile_plan(m->plan2);
-  std::string const rc = m->cols == COLS_2S ? "25,32" : m->cols == COLS_R36 ? "36,36" : radices(p1);
-  std::string const rr = m->rows == ROWS_2S ? "25,25" : m->rows == ROWS_V2 ? "10,25,5" : radices(p2);
+  auto plan_of = [m](int len) { return m->ext ? choose_radices_ext(len) : choose_radices(len); };
+  std::string const rc = m->cols == COLS_2S ? "25,32" : m->cols == COLS_R36 ? "36,36" : radices(plan_of(m->sp.n1));
+  std::string const rr = m->rows == ROWS_2S ? "25,25" : m->rows == ROWS_V2 ? "10,25,5" : radices(plan_of(m->sp.n2));
   size_t const s1 = m->cols == COLS_2S ? Cols2s::smem : m->cols == COLS_R36 ? ColsR36Shape::smem : m->smem1;
   size_t const s2 = m->rows == ROWS_2S ? Rows2s::smem : m->rows == ROWS_V2 ? rows_v2_smem(m) : m->smem2;
   char const *kc = m->ext ? "fwd_cols_ext" : m->cols == COLS_2S ? "fwd_cols_2s" : m->cols == COLS_R36 ? "fwd_cols_r36" : "fwd_cols_kernel";
   char const *kr = m->ext ? "fwd_rows_ext" : m->rows == ROWS_2S ? "fwd_rows_2s" : m->rows == ROWS_V2 ? "fwd_rows_v2" : "fwd_rows_kernel";
-  snprintf(buf, (size_t)buflen, "N=%d %s, %ld-point complex two-pass %d x %d; cols radices [%s] rows radices [%s]; smem %zu/%zu B; "
+  char buf[512];
+  snprintf(buf, sizeof buf, "N=%d %s, %ld-point complex two-pass %d x %d; cols radices [%s] rows radices [%s]; smem %zu/%zu B; "
            "grids %d/%d CTAs per block; kernels %s + %s", m->N, m->in_type == KGPU_REAL ? "real" : "complex", m->nc, m->sp.n1,
            m->sp.n2, rc.c_str(), rr.c_str(), s1, s2, (m->sp.n2 + kTile - 1) / kTile, m->n_rows_ctas, kc, kr);
+  return buf;
+}
+// A Bluestein master: its own length, then the internal master's description from its transform on.
+static std::string describe_bluestein(int N, int in_type, kgpu_master const *inner) {
+  std::string const t = describe_text(inner);
+  return "N=" + std::to_string(N) + (in_type == KGPU_REAL ? " real" : " complex") + ", bluestein P=" + std::to_string(inner->N) +
+         ": " + t.substr(t.find(", ") + 2) + " around bluestein_in_kernel, bluestein_mul_kernel, bluestein_out_kernel";
+}
+
+extern "C" int kgpu_master_describe(kgpu_master const *m, char *buf, int buflen) {
+  if (!m || !buf) return -1;
+  std::string const t = m->bs ? describe_bluestein(m->N, m->in_type, m->bs) : describe_text(m);
+  snprintf(buf, (size_t)buflen, "%s", t.c_str());
   return 0;
+}
+
+// ---- kgpu_master_create_any: the path chosen from L, M and the input type alone ----
+// Bound on each of a Bluestein master's scratch buffers (the chirped input, the passes' spectra, and the internal
+// master's inter-pass buffer), as the bank bounds its huge-channel scratch: longer launches run in chunks of blocks.
+static constexpr long kBluesteinScratchCap = 128L << 20;
+enum MasterPath { MP_DIRECT = 0, MP_EXTENDED = 1, MP_BLUESTEIN = 2 };
+struct MasterPlan {
+  MasterPath path;
+  long nc;
+  long P;     // Bluestein: the internal master's length
+  Split2 sp;  // the split of nc (direct, extended) or of P (Bluestein)
+};
+// The master kgpu_master_create_any builds: kgpu_master_create_ex's wherever that succeeds (its host-side checks,
+// restated), a Bluestein transform otherwise.
+static int master_plan(int L, int M, int in_type, char const *who, MasterPlan *pl) {
+  if (L < 1 || M < 1 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX))
+    return fail("%s: bad arguments L=%d M=%d type=%d", who, L, M, in_type);
+  long const N = (long)L + M - 1;
+  if (N > INT32_MAX) return fail("%s: N=L+M-1 is too large (L=%d M=%d)", who, L, M);
+  if (in_type == KGPU_REAL && ((N & 1) || (L & 1)))
+    return fail("%s: REAL input needs even L and even N=L+M-1 (got L=%d N=%ld)", who, L, N);
+  long const nc = (in_type == KGPU_COMPLEX) ? N : N / 2;
+  pl->nc = nc;
+  pl->P = 0;
+  if (smooth7(nc) && forward_split(nc, false, &pl->sp)) {
+    pl->path = MP_DIRECT;
+    return 0;
+  }
+  if (smooth23(nc) && forward_split(nc, true, &pl->sp)) {
+    pl->path = MP_EXTENDED;
+    return 0;
+  }
+  if (bluestein_length(nc, &pl->P, &pl->sp)) {
+    pl->path = MP_BLUESTEIN;
+    return 0;
+  }
+  return fail("%s: %ld points need a Bluestein transform of at least %ld points, more than the forward pair splits (at "
+              "most 3500 x 3500)", who, nc, 2 * nc - 1);
+}
+
+extern "C" int kgpu_master_plan(int L, int M, int in_type, char *buf, int buflen) {
+  MasterPlan pl;
+  if (master_plan(L, M, in_type, "kgpu_master_plan", &pl)) return -1;
+  if (buf && buflen > 0) {
+    kgpu_master m, inner;
+    std::string t;
+    if (pl.path == MP_BLUESTEIN) {
+      master_shape(&inner, (int)pl.P, 1, KGPU_COMPLEX, pl.sp, false);
+      t = describe_bluestein(L + M - 1, in_type, &inner);
+    } else {
+      master_shape(&m, L, M, in_type, pl.sp, pl.path == MP_EXTENDED);
+      t = describe_text(&m);
+    }
+    snprintf(buf, (size_t)buflen, "%s", t.c_str());
+  }
+  return (int)pl.path;
+}
+
+extern "C" kgpu_master *kgpu_master_create_any(int L, int M, int in_type) {
+  MasterPlan pl;
+  if (master_plan(L, M, in_type, "kgpu_master_create_any", &pl)) return nullptr;
+  if (pl.path != MP_BLUESTEIN) return kgpu_master_create_ex(L, M, in_type);
+  kgpu_master *m = new kgpu_master;
+  m->L = L;
+  m->M = M;
+  m->N = L + M - 1;
+  m->in_type = in_type;
+  m->bins = (in_type == KGPU_COMPLEX) ? m->N : m->N / 2 + 1;
+  m->nc = pl.nc;
+  m->spec_stride = ((long)m->bins + 3) / 4 * 4;
+  m->bp = pl.P;
+  m->b_chunk = (int)std::max(1L, kBluesteinScratchCap / (long)(sizeof(float2) * (size_t)(pl.P + 3)));
+  m->bs = kgpu_master_create((int)pl.P, 1, KGPU_COMPLEX);
+  bool ok = m->bs != nullptr;
+  if (ok) {
+    std::vector<float2> const b = bluestein_bspec(pl.nc, pl.P);
+    ok = upload(&m->d_bspec, b) == 0;
+  }
+  if (!ok) {
+    fail("kgpu_master_create_any: %ld-point Bluestein transform of %ld points: %s", pl.nc, pl.P, std::string(g_err).c_str());
+    kgpu_master_destroy(m);
+    return nullptr;
+  }
+  return m;
 }
 
 // One launch pair (column pass, row pass) over `nblocks` consecutive blocks on stream `st`, inter-pass data in `mid`.
@@ -1074,10 +1245,76 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
   return 0;
 }
 
+// kgpu_forward of a Bluestein master (bluestein_master.cuh), in chunks of at most b_chunk blocks.
+static int bluestein_forward(kgpu_master *m, const void *d_in, int fmt, float scale, int derandomize, int nblocks, void *d_spec,
+                             void *d_stats, cudaStream_t st) {
+  kgpu_master *bs = m->bs;
+  int const chunk = std::min(nblocks, m->b_chunk);
+  if (m->b_blocks < chunk) {  // earlier launches on this stream may still use the old buffers
+    CUDA_OK(cudaStreamSynchronize(st));
+    cudaFree(m->d_bin);
+    cudaFree(m->d_bout);
+    m->d_bin = m->d_bout = nullptr;
+    m->b_blocks = 0;
+    CUDA_OK(cudaMalloc(&m->d_bin, sizeof(float2) * (size_t)m->bp * (size_t)chunk));
+    CUDA_OK(cudaMalloc(&m->d_bout, sizeof(float2) * (size_t)bs->spec_stride * (size_t)chunk));
+    m->b_blocks = chunk;
+  }
+  bool const i16 = fmt == KGPU_FMT_I16;
+  if (i16 && d_stats) CUDA_OK(cudaMemsetAsync(d_stats, 0, sizeof(IngestStats) * (size_t)nblocks, st));
+  bool const real = m->in_type == KGPU_REAL;
+  BluesteinInArgs a;
+  a.hop = real ? m->L / 2 : m->L;
+  a.nc = m->nc;
+  a.P = m->bp;
+  a.first_new = real ? (m->M - 1) / 2 : (m->M - 1);
+  a.i16 = i16;
+  a.derandomize = i16 && derandomize;
+  a.scale = scale;
+  a.out = m->d_bin;
+  BluesteinOutArgs o;
+  o.y = m->d_bout;
+  o.y_stride = bs->spec_stride;
+  o.nc = m->nc;
+  o.inv_p = 1.0 / (double)m->bp;
+  o.real_split = real;
+  o.spec_stride = m->spec_stride;
+  size_t const pair = i16 ? sizeof(short2) : sizeof(float2);
+  for (int b0 = 0; b0 < nblocks; b0 += chunk) {
+    int const nb = std::min(chunk, nblocks - b0);
+    a.in = (char const *)d_in + pair * (size_t)a.hop * (size_t)b0;
+    a.nblocks = nb;
+    a.stats = (i16 && d_stats) ? (IngestStats *)d_stats + b0 : nullptr;
+    {
+      ProfScope ps(K_FWD_COLS, st);
+      bluestein_in_kernel<<<(unsigned)((m->bp + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(a);
+    }
+    g_launches++;
+    if (kgpu_forward(bs, m->d_bin, KGPU_FMT_F32, 1.0f, 0, nb, m->d_bout, nullptr, st) != 0) return -1;
+    {
+      ProfScope ps(K_FWD_COLS, st);
+      bluestein_mul_kernel<<<dim3((unsigned)((m->bp + kSpecThreads - 1) / kSpecThreads), (unsigned)nb), kSpecThreads, 0, st>>>(
+          m->d_bout, bs->spec_stride, m->d_bspec, (int)m->bp, m->d_bin);
+    }
+    g_launches++;
+    if (kgpu_forward(bs, m->d_bin, KGPU_FMT_F32, 1.0f, 0, nb, m->d_bout, nullptr, st) != 0) return -1;
+    o.nblocks = nb;
+    o.spec = (float2 *)d_spec + (size_t)m->spec_stride * (size_t)b0;
+    {
+      ProfScope ps(K_FWD_ROWS, st);
+      bluestein_out_kernel<<<(unsigned)((m->bins + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(o);
+    }
+    g_launches++;
+  }
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 extern "C" int kgpu_forward(kgpu_master *m, const void *d_in, int fmt, float scale, int derandomize, int nblocks,
                             void *d_spec, void *d_stats, void *stream) {
   if (!m || !d_in || !d_spec || nblocks < 1) return fail("kgpu_forward: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
+  if (m->bs) return bluestein_forward(m, d_in, fmt, scale, derandomize, nblocks, d_spec, d_stats, st);
   if (m->mid_blocks < nblocks) {
     CUDA_OK(cudaStreamSynchronize(st));
     cudaFree(m->d_mid);
@@ -1996,13 +2233,6 @@ struct SpecPlan {
 // Bound on the scratch of one poll (per buffer): longer polls run in chunks of segments.
 static constexpr long kSpectrumScratchCap = 64L << 20;
 
-// the split kgpu_master_create(_ex) would run for nc complex points, if its kernels fit shared memory
-static bool forward_split(long nc, bool ext, Split2 *sp) {
-  if (!(ext ? choose_split_ext(nc, sp) : choose_split(nc, sp))) return false;
-  size_t const smem1 = sizeof(float2) * ((size_t)kTile * column_pitch(sp->n1) + (size_t)kTile * ((sp->n1 + 31) / 32));
-  size_t const smem2 = sizeof(float2) * ((size_t)kTile * column_pitch(sp->n2));
-  return smem1 <= (size_t)kChanSmemLimit && smem2 <= (size_t)kChanSmemLimit;
-}
 static int spectrum_plan(int fft_n, int in_type, SpecPlan *pl) {
   if (fft_n < 2 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX))
     return fail("kgpu_spectrum: bad arguments fft_n=%d type=%d", fft_n, in_type);
@@ -2018,13 +2248,11 @@ static int spectrum_plan(int fft_n, int in_type, SpecPlan *pl) {
     pl->nc = pl->P = fft_n;
     return 0;
   }
-  long const limit = (long)kMaxTileLen * kMaxTileLen;
-  for (long P = 2L * fft_n - 1; P <= limit; P++)
-    if (smooth7(P) && forward_split(P, false, &pl->sp)) {
-      pl->path = SP_BLUESTEIN;
-      pl->nc = pl->P = P;
-      return 0;
-    }
+  if (bluestein_length(fft_n, &pl->P, &pl->sp)) {
+    pl->path = SP_BLUESTEIN;
+    pl->nc = pl->P;
+    return 0;
+  }
   return fail("kgpu_spectrum: %d points have a prime factor >= 29 and need a Bluestein transform of at least %ld points, "
               "more than the forward pair splits", fft_n, 2L * fft_n - 1);
 }
@@ -2032,25 +2260,6 @@ static void spectrum_plan_text(int fft_n, int in_type, SpecPlan const &pl, char 
   char const *path = pl.path == SP_R2C ? "r2c" : pl.path == SP_C2C ? "complex" : "bluestein";
   snprintf(buf, (size_t)buflen, "%s fft_n=%d %s P=%ld: %ld-point complex two-pass %d x %d", path, fft_n,
            in_type == KGPU_REAL ? "real" : "complex", pl.P, pl.nc, pl.sp.n1, pl.sp.n2);
-}
-
-// Forward DFT of n points (factors 2, 3, 5, 7) in place, in double: decimation in time, radix = smallest factor.
-// tw[e * d] = exp(-2 pi i e / n) (d: the stride of this sub-transform in the top-level table).
-static void host_dft(std::complex<double> *x, long n, std::complex<double> const *tw, long d) {
-  if (n == 1) return;
-  int const r = n % 2 == 0 ? 2 : n % 3 == 0 ? 3 : n % 5 == 0 ? 5 : 7;
-  long const m = n / r;
-  std::vector<std::complex<double>> t((size_t)n);
-  for (long j = 0; j < m; j++)
-    for (int q = 0; q < r; q++) t[(size_t)(q * m + j)] = x[j * r + q];
-  for (int q = 0; q < r; q++) host_dft(t.data() + q * m, m, tw, d * r);
-  for (long k = 0; k < m; k++)
-    for (int s = 0; s < r; s++) {
-      long const kk = k + s * m;
-      std::complex<double> acc = t[(size_t)k];
-      for (int q = 1; q < r; q++) acc += t[(size_t)(q * m + k)] * tw[(size_t)(((long)q * kk) % n * d)];
-      x[kk] = acc;
-    }
 }
 
 struct kgpu_spectrum {
@@ -2115,24 +2324,8 @@ extern "C" kgpu_spectrum *kgpu_spectrum_create(int fft_n, int in_type, int bin_c
   if (e == cudaSuccess) e = cudaMalloc(&s->d_in, in_bytes * (size_t)s->chunk);
   if (e == cudaSuccess) e = cudaMalloc(&s->d_spec, spec_bytes * (size_t)s->chunk);
   if (e == cudaSuccess && pl.path == SP_BLUESTEIN) {
-    // b_m = conj(w_m) on -(fft_n-1) .. fft_n-1, wrapped modulo P, and its transform B = DFT_P(b)
-    long const P = pl.P, n = fft_n;
-    // transformed in double on the host and rounded once: a float transform here would add a third float transform's
-    // error to every poll
-    std::vector<std::complex<double>> bd((size_t)P), tw((size_t)P);
-    for (long m = 0; m < n; m++) {
-      long double const ang = M_PIl * (long double)((m * m) % (2 * n)) / (long double)n;
-      std::complex<double> const v((double)cosl(ang), (double)sinl(ang));  // conj(exp(-i ang))
-      bd[(size_t)m] = v;
-      if (m) bd[(size_t)(P - m)] = v;
-    }
-    for (long e2 = 0; e2 < P; e2++) {
-      long double const ang = -2.0L * M_PIl * (long double)e2 / (long double)P;
-      tw[(size_t)e2] = std::complex<double>((double)cosl(ang), (double)sinl(ang));
-    }
-    host_dft(bd.data(), P, tw.data(), 1);
-    std::vector<float2> b((size_t)P);
-    for (long k = 0; k < P; k++) b[(size_t)k] = make_float2((float)bd[(size_t)k].real(), (float)bd[(size_t)k].imag());
+    long const P = pl.P;
+    std::vector<float2> const b = bluestein_bspec(fft_n, P);
     e = cudaMalloc(&s->d_bspec, sizeof(float2) * (size_t)P);
     if (e == cudaSuccess) e = cudaMemcpy(s->d_bspec, b.data(), sizeof(float2) * (size_t)P, cudaMemcpyHostToDevice);
   }
