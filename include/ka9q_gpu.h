@@ -140,6 +140,21 @@ int kgpu_bank_define_huge(kgpu_bank *b, int idx, int olen, int out_type);
  * which never take a slot of the plan registry.  Fails for a prime factor >= 29, and for a factor 11 .. 23 above 28812
  * points.  Every other bank call treats such a channel like any other. */
 int kgpu_bank_define_ext(kgpu_bank *b, int idx, int olen, int out_type);
+/* Same, for any point count up to 1048576, as the reference plans (filter.c:298-415), e.g. a 29 kHz (725 = 5^2 29
+ * points), 62 kHz (1550 = 2 5^2 31) or 1.76 MS/s (44000 = 2^5 5^3 11) channel at 20 ms and overlap 5.  Where
+ * kgpu_bank_define_ext succeeds it is that call: the same result, kernels and messages.  Otherwise (a prime factor >= 29,
+ * or a factor 11 .. 23 above 28812 points) the channel runs a Bluestein transform: the conjugate slice x response times
+ * the chirp exp(-i pi n^2 / points), zero-padded to the smallest P >= 2 points - 1 with factors 2, 3, 5, 7 whose split the
+ * forward pair runs, two forward passes of an internal COMPLEX master of length P (one per bank and stream) around the
+ * product with the chirp's transform (computed in double on the host once per length and process), then the output
+ * chirp and 1/P.  The scratch is the bank's, at most about 128 MB per buffer and stream; launches of more channels and
+ * blocks run in chunks.  Every other bank call treats such a channel like any other.  Fails above 1048576 points, and
+ * for an odd point count with KGPU_REAL output. */
+int kgpu_bank_define_any(kgpu_bank *b, int idx, int olen, int out_type);
+/* Pure host code: the path kgpu_bank_define_any takes for a channel of `points` points (0 direct, 1 wide, 2 huge,
+ * 3 extended, 4 Bluestein; -1 when it would fail) and, if buf is not NULL, a description: the radices or the split, the
+ * kernels and, for Bluestein, P and the internal master's split. */
+int kgpu_chan_plan(int points, int out_type, char *buf, int buflen);
 /* set_filter (filter.c:968-1045): Kaiser-windowed sinc designed on the host in double, forward
  * transformed on the device.  low/high are fractions of the output rate. */
 int kgpu_bank_set_filter(kgpu_bank *b, int idx, double low, double high, double kaiser_beta);

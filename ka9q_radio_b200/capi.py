@@ -86,6 +86,8 @@ def load() -> C.CDLL:
     L.kgpu_bank_define_wide.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_huge.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_ext.argtypes = [vp, i, i, i]
+    L.kgpu_bank_define_any.argtypes = [vp, i, i, i]
+    L.kgpu_chan_plan.argtypes = [i, i, C.c_char_p, i]
     L.kgpu_bank_set_weights.argtypes = [vp, i, d, d, d, d]
     L.kgpu_bank_set_osc.argtypes = [vp, i, i, d, d, d, d]
     L.kgpu_bank_get_osc_phase.argtypes = [vp, i, vp]
@@ -173,6 +175,16 @@ def plan_master(L: int, M: int, in_type: int) -> tuple[int, str]:
     return check(load().kgpu_master_plan(L, M, in_type, buf, 512), "kgpu_master_plan"), buf.value.decode()
 
 
+CHAN_DIRECT, CHAN_WIDE, CHAN_HUGE, CHAN_EXTENDED, CHAN_BLUESTEIN = 0, 1, 2, 3, 4
+
+
+def chan_plan(points: int, out_type: int = KGPU_COMPLEX) -> tuple[int, str]:
+    """(path, description) of the channel kgpu_bank_define_any would define for `points` points; pure host code.  Raises
+    when it would fail."""
+    buf = C.create_string_buffer(512)
+    return check(load().kgpu_chan_plan(points, out_type, buf, 512), "kgpu_chan_plan"), buf.value.decode()
+
+
 class Master:
     """create_filter_input's device half (reference filter.c:186-269)."""
 
@@ -247,6 +259,11 @@ class Bank:
         """define_huge() that also serves lengths of at most 28812 points with prime factors 11, 13, 17, 19 and 23 (e.g.
         the 220 kHz and 277.2 kHz HFDL channels); their plans never take a registry slot."""
         return check(self.lib.kgpu_bank_define_ext(self.h, idx, olen, out_type), "kgpu_bank_define_ext")
+
+    def define_any(self, idx, olen, out_type=KGPU_COMPLEX) -> int:
+        """define_ext() for any point count up to 1048576: where define_ext refuses a length for its prime factors, the
+        channel runs a Bluestein transform."""
+        return check(self.lib.kgpu_bank_define_any(self.h, idx, olen, out_type), "kgpu_bank_define_any")
 
     def set_weights(self, idx, i_weight=1.0, q_weight=0.0):
         """set_filter_weights (filter.c:922-929)"""

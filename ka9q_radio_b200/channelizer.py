@@ -35,7 +35,7 @@ class Channelizer:
                     beam=None) -> int:
         """out_type KGPU_REAL: REAL-output slave (olen floats per block); beam=(i_weight, q_weight): beam synthesis."""
         idx = self.nchan
-        pts = self.bank.define_ext(idx, olen, out_type)
+        pts = self.bank.define_any(idx, olen, out_type)
         if response is not None:
             self.bank.set_response(idx, response)
         else:

@@ -24,7 +24,7 @@ constexpr int kMaxChanPoints = (kChanSmemLimit / (8 * kChanWarps) - 2) / 4 * 4;
 // most negative output bin) maps onto the master spectrum.  Covers filter.c:810-893 (REAL
 // master, upright or inverted) and :728-793 (COMPLEX master with circular wrap).
 struct ChanDesc {
-  int plan;        // registry index of the length-`points` inverse plan (kPlanExt: none), < 0: channel disabled
+  int plan;        // registry index of the length-`points` inverse plan (kPlanExt, kPlanBluestein: none), < 0: disabled
   int points;      // Ns
   int olen;        // Ls
   int zlead;       // walk positions t < zlead are zero
@@ -40,6 +40,9 @@ struct ChanDesc {
 // registry index, so it must never reach a kernel that reads c_plans[d.plan]; its plan reaches chan_kernel_ext or
 // chan_wide_ext by value.
 constexpr int kPlanExt = kMaxPlans;
+// ChanDesc::plan of a channel served by a Bluestein transform (kgpu_bank_define_any, bluestein_chan.cuh): runnable for
+// the noise estimator and huge_power_kernel, and never a registry index either.
+constexpr int kPlanBluestein = kMaxPlans + 1;
 
 enum : int {
   kChanIsb = 1,      // filter_out.isb (filter.c:895-909)

@@ -436,7 +436,7 @@ int create_filter_output(struct filter_out *slave, struct filter_in *master, int
       slave->rev_plan = (fftwf_plan)sc;
     }
     cudaStreamSynchronize(c->st);
-    int const pts = kgpu_bank_define_ext(c->bank, sc->idx, len, out_type == REAL ? KGPU_REAL : KGPU_COMPLEX);
+    int const pts = kgpu_bank_define_any(c->bank, sc->idx, len, out_type == REAL ? KGPU_REAL : KGPU_COMPLEX);
     c->ver[sc->idx]++;
     pthread_mutex_unlock(&c->mu);
     if (pts != slave->points) {

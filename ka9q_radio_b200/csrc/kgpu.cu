@@ -28,6 +28,7 @@
 #include "fwd_2s.cuh"
 #include "spectrum_kernels.cuh"
 #include "bluestein_master.cuh"
+#include "bluestein_chan.cuh"
 
 using namespace kfft;
 
@@ -1435,6 +1436,47 @@ int design_taps(int points, int olen, int master_points, bool master_real, doubl
 }  // namespace
 
 // ------------------------------------------------------------------ bank --------------------
+// ---- channels served by a Bluestein transform (kgpu_bank_define_any, bluestein_chan.cuh) ----
+// Exactly the lengths kgpu_bank_define_ext refuses for their factors: a prime factor >= 29, or one of 11 .. 23 above
+// kMaxWideChanPoints.
+static bool chan_needs_bluestein(long points) {
+  long const big = factor_above7(points);
+  return big > 23 || (big > 1 && points > kMaxWideChanPoints);
+}
+
+// P, its split and the device copy of B = DFT_P of the conjugate chirp, for every Bluestein channel length used so far,
+// per device (never freed, like the extended plans).  B is read-only and its host transform takes about 1 s at P = 1.5 M,
+// so it is computed once per length, not per channel or bank.
+struct BluesteinChan {
+  long P;
+  Split2 sp;
+  float2 *d_b;
+};
+static std::mutex g_bchan_mu;
+static std::map<std::pair<int, int>, BluesteinChan> g_bchan;
+
+static BluesteinChan const *get_bluestein_chan(int points) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) {
+    fail("cudaGetDevice: %s", cudaGetErrorString(cudaGetLastError()));
+    return nullptr;
+  }
+  std::lock_guard<std::mutex> lk(g_bchan_mu);
+  auto it = g_bchan.find({dev, points});
+  if (it != g_bchan.end()) return &it->second;
+  BluesteinChan c{0, {0, 0}, nullptr};
+  if (!bluestein_length(points, &c.P, &c.sp)) {
+    fail("%d-point inverse transform needs a Bluestein transform of at least %d points, more than the forward pair splits",
+         points, 2 * points - 1);
+    return nullptr;
+  }
+  if (upload(&c.d_b, bluestein_bspec(points, c.P))) {
+    cudaFree(c.d_b);
+    return nullptr;
+  }
+  return &(g_bchan[{dev, points}] = c);
+}
+
 struct ChanHost {
   bool defined = false, enabled = false, has_response = false;
   bool real_out = false;  // REAL-output slave (filter.c:370-390): olen floats per block
@@ -1473,10 +1515,23 @@ struct kgpu_bank {
   // on different streams (a batched run and a run_one) never share one; grown on demand, freed in kgpu_bank_destroy
   std::mutex scratch_mu;
   std::map<cudaStream_t, std::pair<void *, size_t>> scratch;
+  // the internal COMPLEX masters of the Bluestein channels, by (stream, P): kgpu_forward keeps its inter-pass buffer in
+  // the master, so launches on two streams must never share one; created on first use, freed in kgpu_bank_destroy
+  std::map<std::pair<cudaStream_t, long>, kgpu_master *> bmaster;
 };
 
 // Bound on one launch's huge-channel scratch: chan_huge loops over chunks of channels and blocks to stay below it.
 static constexpr long kHugeScratchCap = 128L << 20;
+// Bound on the (channel, block) rows of one Bluestein chunk: they are the blocks (grid.y) of one kgpu_forward.
+static constexpr long kMaxBluesteinRows = 65535;
+
+// the internal master of length P for the Bluestein channels launched on stream `st` (nullptr and kgpu_last_error())
+static kgpu_master *bank_bluestein_master(kgpu_bank *b, cudaStream_t st, long P) {
+  std::lock_guard<std::mutex> lk(b->scratch_mu);
+  kgpu_master *&m = b->bmaster[{st, P}];
+  if (!m) m = kgpu_master_create((int)P, 1, KGPU_COMPLEX);
+  return m;
+}
 
 // the scratch buffer of stream `st`, at least `bytes` long (nullptr and kgpu_last_error() on failure)
 static void *bank_scratch(kgpu_bank *b, cudaStream_t st, size_t bytes) {
@@ -1662,11 +1717,13 @@ extern "C" void kgpu_bank_destroy(kgpu_bank *b) {
   cudaFree(b->d_fm_mem[0]);
   cudaFree(b->d_fm_mem[1]);
   for (auto &s : b->scratch) cudaFree(s.second.first);
+  for (auto &m : b->bmaster) kgpu_master_destroy(m.second);
   delete b;
 }
 static bool bad_idx(kgpu_bank const *b, int idx) { return !b || idx < 0 || idx >= b->capacity; }
 
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok = false, bool ext_ok = false);
+static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok = false, bool ext_ok = false,
+                       bool any_ok = false);
 extern "C" int kgpu_bank_define(kgpu_bank *b, int idx, int olen) { return bank_define(b, idx, olen, false, false); }
 extern "C" int kgpu_bank_define_ex(kgpu_bank *b, int idx, int olen, int out_type) {
   if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_ex: out_type must be KGPU_COMPLEX or KGPU_REAL");
@@ -1684,7 +1741,11 @@ extern "C" int kgpu_bank_define_ext(kgpu_bank *b, int idx, int olen, int out_typ
   if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_ext: out_type must be KGPU_COMPLEX or KGPU_REAL");
   return bank_define(b, idx, olen, out_type == KGPU_REAL, true, true, true);
 }
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok, bool ext_ok) {
+extern "C" int kgpu_bank_define_any(kgpu_bank *b, int idx, int olen, int out_type) {
+  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_any: out_type must be KGPU_COMPLEX or KGPU_REAL");
+  return bank_define(b, idx, olen, out_type == KGPU_REAL, true, true, true, true);
+}
+static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok, bool ext_ok, bool any_ok) {
   if (bad_idx(b, idx) || olen < 1) return fail("kgpu_bank_define: bad arguments");
   long const num = (long)olen * b->m->N;
   if (num % b->m->L) return fail("invalid output length %d for N=%d L=%d (filter.c:312-316)", olen, b->m->N, b->m->L);
@@ -1694,10 +1755,16 @@ static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide
   // registry from filling (see kMaxPlans).  Longer channels (kgpu_bank_define_wide) run chan_wide, one CTA each, on
   // a split into two registry lengths; their descriptor's plan is that of the first factor (>= 0: runnable).  Beyond
   // kMaxWideChanPoints (kgpu_bank_define_huge) the same holds for chan_huge's split.  A length with a prime factor
-  // 11 .. 23 (kgpu_bank_define_ext) has plans of its own outside the registry; its descriptor's plan is kPlanExt.
+  // 11 .. 23 (kgpu_bank_define_ext) has plans of its own outside the registry; its descriptor's plan is kPlanExt.  A
+  // length that refuses for its factors (kgpu_bank_define_any) runs a Bluestein transform; its plan is kPlanBluestein.
   long const big = ext_ok ? factor_above7(points) : 1;
   int plan;
-  if (big > 23) {
+  if (any_ok && points > kMaxHugeChanPoints) {
+    return fail("kgpu_bank_define_any: %d-point inverse transform exceeds the %d-point maximum", points, kMaxHugeChanPoints);
+  } else if (any_ok && chan_needs_bluestein(points)) {
+    if (!get_bluestein_chan(points)) return fail("kgpu_bank_define_any: %s", std::string(g_err).c_str());
+    plan = kPlanBluestein;
+  } else if (big > 23) {
     return fail("kgpu_bank_define_ext: %d-point inverse transform has the prime factor %ld (prime factors up to 23 are served)",
                 points, big);
   } else if (big > 1 && points > kMaxWideChanPoints) {
@@ -1762,6 +1829,47 @@ static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide
   return points;
 }
 
+// Forward transform in place of a Bluestein channel's response (set_filter's fftwf_execute, filter.c:1030): one block of
+// bluestein_master.cuh's chain for a COMPLEX transform of `points`, through the scratch and internal master of stream st.
+static int bluestein_response(kgpu_bank *b, float2 *resp, int points, cudaStream_t st) {
+  BluesteinChan const *bc = get_bluestein_chan(points);
+  if (!bc) return -1;
+  kgpu_master *im = bank_bluestein_master(b, st, bc->P);
+  if (!im) return -1;
+  long const P = bc->P, ld = im->spec_stride, in_len = (P + 31) / 32 * 32;
+  float2 *bin = (float2 *)bank_scratch(b, st, sizeof(float2) * (size_t)(in_len + ld));
+  if (!bin) return -1;
+  float2 *bout = bin + in_len;
+  BluesteinInArgs a;
+  a.in = resp;
+  a.hop = 0;
+  a.nc = points;
+  a.P = P;
+  a.first_new = 0;
+  a.nblocks = 1;
+  a.i16 = a.derandomize = 0;
+  a.scale = 1.0f;
+  a.stats = nullptr;
+  a.out = bin;
+  BluesteinOutArgs o;
+  o.y = bout;
+  o.y_stride = ld;
+  o.nc = points;
+  o.inv_p = 1.0 / (double)P;
+  o.real_split = 0;
+  o.nblocks = 1;
+  o.spec = resp;
+  o.spec_stride = ld;
+  bluestein_in_kernel<<<(unsigned)((P + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(a);
+  if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, 1, bout, nullptr, st) != 0) return -1;
+  bluestein_mul_kernel<<<(unsigned)((P + kSpecThreads - 1) / kSpecThreads), kSpecThreads, 0, st>>>(bout, ld, bc->d_b, (int)P, bin);
+  if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, 1, bout, nullptr, st) != 0) return -1;
+  bluestein_out_kernel<<<(unsigned)((points + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(o);
+  g_launches += 3;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 // st == nullptr: legacy entry points, whole-device synchronisation (any stream may be using the response);
 // otherwise only `st` is synchronised: the caller guarantees that every launch reading this bank is ordered on it
 static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *host, bool transform, cudaStream_t st = nullptr,
@@ -1772,7 +1880,9 @@ static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *ho
   if (on_stream) CUDA_OK(cudaStreamSynchronize(st));
   else CUDA_OK(cudaDeviceSynchronize());
   CUDA_OK(cudaMemcpyAsync(dst, host, sizeof(float2) * (size_t)c.points, cudaMemcpyHostToDevice, st));
-  if (transform && c.plan == kPlanExt && c.points > kMaxChanPoints) {
+  if (transform && c.plan == kPlanBluestein) {
+    if (bluestein_response(b, dst, c.points, st)) return -1;
+  } else if (transform && c.plan == kPlanExt && c.points > kMaxChanPoints) {
     WideGeomExt const *x = get_wide_geom_ext(c.points);
     if (!x) return -1;
     size_t const sm = (size_t)wide_smem_bytes(x->g.n1, x->g.n2);
@@ -1991,6 +2101,52 @@ static int launch_huge(kgpu_bank *b, ChanArgs const &a, int points, int n, int n
   return 0;
 }
 
+// The Bluestein channels of one length (bluestein_chan.cuh): bluestein_chan_in, two passes of the stream's internal
+// master around bluestein_mul_kernel, bluestein_chan_out and, with d_power, the power reduction, in chunks of channels
+// and blocks whose two scratch buffers stay within kHugeScratchCap each.
+static int launch_bluestein(kgpu_bank *b, ChanArgs const &a, int points, int n, int nblocks, cudaStream_t st) {
+  BluesteinChan const *bc = get_bluestein_chan(points);
+  if (!bc) return -1;
+  kgpu_master *im = bank_bluestein_master(b, st, bc->P);
+  if (!im) return -1;
+  long const P = bc->P, ld = im->spec_stride;  // rows of P points in, rows of ld between the passes' spectra
+  int const olen = (int)((long)points * b->m->L / b->m->N);
+  long const per = std::min(kMaxBluesteinRows, std::max(1L, kHugeScratchCap / (ld * (long)sizeof(float2))));  // rows per chunk
+  int const cch = (int)std::min<long>(n, per), cbl = (int)std::max(1L, std::min<long>(nblocks, per / cch));
+  int const tiles_in = (int)((P + kBluesteinThreads - 1) / kBluesteinThreads), tiles_out = (olen + kBluesteinThreads - 1) / kBluesteinThreads;
+  size_t const rows = (size_t)cch * (size_t)cbl;
+  size_t const in_bytes = (rows * (size_t)P * sizeof(float2) + 255) / 256 * 256, out_bytes = rows * (size_t)ld * sizeof(float2);
+  char *scr = (char *)bank_scratch(b, st, in_bytes + out_bytes + rows * (size_t)tiles_out * sizeof(float));
+  if (!scr) return -1;
+  float2 *bin = (float2 *)scr, *bout = (float2 *)(scr + in_bytes);
+  float *partial = a.power ? (float *)(scr + in_bytes + out_bytes) : nullptr;
+  for (int c0 = 0; c0 < n; c0 += cch)
+    for (int b0 = 0; b0 < nblocks; b0 += cbl) {
+      int const nc = std::min(cch, n - c0), nb = std::min(cbl, nblocks - b0);
+      ChanArgs x = a;
+      if (x.order) x.order += c0;
+      else x.chan_base += c0;
+      x.norder = nc;
+      x.spec += (long)b0 * x.spec_stride;
+      x.out += (long)b0 * x.out_stride;
+      x.block0 += b0;
+      if (x.power) x.power += (long)b0 * x.power_stride;
+      bluestein_chan_in<<<dim3((unsigned)tiles_in, (unsigned)nc, (unsigned)nb), kBluesteinThreads, 0, st>>>(x, P, bin);
+      if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, nc * nb, bout, nullptr, st) != 0) return -1;
+      bluestein_mul_kernel<<<dim3((unsigned)((P + kSpecThreads - 1) / kSpecThreads), (unsigned)(nc * nb)), kSpecThreads, 0, st>>>(
+          bout, ld, bc->d_b, (int)P, bin);
+      if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, nc * nb, bout, nullptr, st) != 0) return -1;
+      bluestein_chan_out<<<dim3((unsigned)tiles_out, (unsigned)nc, (unsigned)nb), kBluesteinThreads, 0, st>>>(x, 1.0 / (double)P, bout,
+                                                                                                            ld, partial);
+      g_launches += 3;
+      if (partial) {
+        huge_power_kernel<<<dim3((unsigned)nc, (unsigned)nb), 32, 0, st>>>(x, partial, tiles_out);
+        g_launches++;
+      }
+    }
+  return 0;
+}
+
 // The channels of one extended length: chan_kernel_ext, or chan_wide_ext above kMaxChanPoints, whatever the
 // static-kernel setting (every variant runs the same kernel).
 static int launch_chan_ext(ChanArgs const &a, int points, int n, int nblocks, cudaStream_t st) {
@@ -2033,6 +2189,7 @@ static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_ou
   a.power = d_power;
   a.power_stride = b->capacity;
   ProfScope ps(K_CHAN, st);
+  if (plan == kPlanBluestein) return launch_bluestein(b, a, points, n, nblocks, st);  // before the length tests: any length
   if (points > kMaxWideChanPoints) return launch_huge(b, a, points, n, nblocks, st);  // huge channels: chan_huge
   g_launches++;
   if (plan == kPlanExt) return launch_chan_ext(a, points, n, nblocks, st);  // before host_tile_plan: not a registry plan
@@ -2214,6 +2371,50 @@ extern "C" int kgpu_plan_split(long n, int *n1, int *n2) {
   *n1 = sp.n1;
   *n2 = sp.n2;
   return 0;
+}
+
+// The path kgpu_bank_define_any takes for a channel of `points` points, from the same tests, without a device.
+enum ChanPath { CP_DIRECT = 0, CP_WIDE = 1, CP_HUGE = 2, CP_EXTENDED = 3, CP_BLUESTEIN = 4 };
+extern "C" int kgpu_chan_plan(int points, int out_type, char *buf, int buflen) {
+  if (points < 1 || (out_type != KGPU_COMPLEX && out_type != KGPU_REAL)) return fail("kgpu_chan_plan: bad arguments");
+  if (out_type == KGPU_REAL && (points & 1))
+    return fail("kgpu_bank_define: REAL-output slaves need an even number of points (got %d)", points);
+  if (points > kMaxHugeChanPoints)
+    return fail("kgpu_chan_plan: %d-point inverse transform exceeds the %d-point maximum", points, kMaxHugeChanPoints);
+  auto list = [](std::vector<int> const &v) {
+    std::string r;
+    for (size_t i = 0; i < v.size(); i++) r += std::to_string(v[i]) + (i + 1 < v.size() ? "," : "");
+    return r;
+  };
+  bool const ext = factor_above7(points) > 1;
+  ChanPath path;
+  Split2 sp{0, 0};
+  char text[512];
+  if (chan_needs_bluestein(points)) {
+    long P = 0;
+    if (!bluestein_length(points, &P, &sp)) return fail("kgpu_chan_plan: %d points have no Bluestein length", points);
+    kgpu_master inner;
+    master_shape(&inner, (int)P, 1, KGPU_COMPLEX, sp, false);
+    std::string const t = describe_text(&inner);
+    snprintf(text, sizeof text, "bluestein: %d points, P=%ld: %s around bluestein_chan_in, bluestein_mul_kernel, bluestein_chan_out",
+             points, P, t.substr(t.find(", ") + 2).c_str());
+    path = CP_BLUESTEIN;
+  } else if (points <= kMaxChanPoints) {
+    std::vector<int> const r = ext ? choose_radices_ext(points) : choose_radices(points);
+    if (points > 1 && r.empty()) return fail("kgpu_chan_plan: %d-point transform cannot be planned", points);
+    snprintf(text, sizeof text, "%s: %d points, radices [%s]; kernel %s", ext ? "extended" : "direct", points, list(r).c_str(),
+             ext ? "chan_kernel_ext" : "chan_kernel");
+    path = ext ? CP_EXTENDED : CP_DIRECT;
+  } else {
+    if (!(ext ? choose_split_ext(points, &sp) : choose_split(points, &sp)))
+      return fail("kgpu_chan_plan: %d-point transform cannot be split into two plannable lengths", points);
+    bool const huge = points > kMaxWideChanPoints;
+    snprintf(text, sizeof text, "%s: %d points, four-step %d x %d; kernels %s", ext ? "extended" : huge ? "huge" : "wide", points,
+             sp.n1, sp.n2, ext ? "chan_wide_ext" : huge ? "chan_huge_cols + chan_huge_rows" : "chan_wide");
+    path = ext ? CP_EXTENDED : huge ? CP_HUGE : CP_WIDE;
+  }
+  if (buf && buflen > 0) snprintf(buf, (size_t)buflen, "%s", text);
+  return (int)path;
 }
 
 // ------------------------------------------------------------------ wideband spectrum analyzer ----------
