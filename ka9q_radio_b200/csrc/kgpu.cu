@@ -480,11 +480,6 @@ constexpr long next_smooth7(long n) {
 static_assert(all_wide_fit(kMaxChanPoints + 1, kMaxWideChanPoints), "a wide length up to the maximum does not fit");
 static_assert(!wide_fits(next_smooth7(kMaxWideChanPoints + 1)), "kMaxWideChanPoints is below what shared memory holds");
 
-// Four-step geometry of every wide length used so far (never freed, like the plan registry).  Its two plans are
-// registry plans of at most kMaxTileLen points, so wide channels add no registry entries.
-static std::mutex g_wide_mu;
-static std::map<int, WideGeom> g_wide;
-
 static int plan_slot(TilePlan const &p, int k) {  // slot holding X[k] after the plan's last stage (its perm[k])
   int slot = 0;
   for (int i = 0; i < p.nstages; i++) {
@@ -516,31 +511,6 @@ static int wide_twiddles(WideGeom &g, TilePlan const &p2) {
   return 0;
 }
 
-static WideGeom const *get_wide_geom(int points) {
-  std::lock_guard<std::mutex> lk(g_wide_mu);
-  auto it = g_wide.find(points);
-  if (it != g_wide.end()) return &it->second;
-  Split2 sp;
-  if (!choose_split(points, &sp)) {
-    fail("%d-point transform cannot be split into two plannable lengths (factors 2, 3, 5, 7; each at most %d)", points,
-         kMaxTileLen);
-    return nullptr;
-  }
-  if (wide_smem_bytes(sp.n1, sp.n2) > kChanSmemLimit) {
-    fail("%d-point transform (%d x %d) does not fit in shared memory", points, sp.n1, sp.n2);
-    return nullptr;
-  }
-  WideGeom g;
-  g.n1 = sp.n1;
-  g.n2 = sp.n2;
-  g.pitch = wide_pitch(sp.n2);
-  g.plan1 = get_tile_plan(sp.n1);
-  g.plan2 = get_tile_plan(sp.n2);
-  if (g.plan1 < 0 || g.plan2 < 0) return nullptr;
-  if (wide_twiddles(g, *host_tile_plan(g.plan2))) return nullptr;
-  return &(g_wide[points] = g);
-}
-
 // Pins kMaxHugeChanPoints: every length with factors 2, 3, 5, 7 in (kMaxWideChanPoints, kMaxHugeChanPoints] splits
 // into two plannable factors whose kTile-column tiles fit shared memory (the largest factor is 2401, for 823 543 =
 // 2401 x 343), and there are 806 of them.  The lengths are enumerated by their exponents to keep the evaluation short.
@@ -567,31 +537,6 @@ constexpr long huge_lengths(long lo, long hi) {  // how many 7-smooth lengths in
   return count;
 }
 static_assert(huge_lengths(kMaxWideChanPoints, kMaxHugeChanPoints) == 806, "a huge length does not split or fit");
-
-// Four-step geometry of every huge length used so far (never freed; no tables: the kernels compute their twiddles).
-static std::mutex g_huge_mu;
-static std::map<int, HugeGeom> g_huge;
-
-static HugeGeom const *get_huge_geom(int points) {
-  std::lock_guard<std::mutex> lk(g_huge_mu);
-  auto it = g_huge.find(points);
-  if (it != g_huge.end()) return &it->second;
-  Split2 sp;
-  if (!choose_split(points, &sp)) {
-    fail("%d-point transform cannot be split into two plannable lengths (factors 2, 3, 5, 7; each at most %d)", points,
-         kMaxTileLen);
-    return nullptr;
-  }
-  HugeGeom g;
-  g.n1 = sp.n1;
-  g.n2 = sp.n2;
-  g.pitch1 = huge_pitch(sp.n1);
-  g.pitch2 = huge_pitch(sp.n2);
-  g.plan1 = get_tile_plan(sp.n1);
-  g.plan2 = get_tile_plan(sp.n2);
-  if (g.plan1 < 0 || g.plan2 < 0) return nullptr;
-  return &(g_huge[points] = g);
-}
 
 // ---- channels whose length has a prime factor 11 .. 23 (kgpu_bank_define_ext) ----
 // They keep their plans out of the registry: c_plans holds exactly the 7-smooth lengths, whose count kMaxPlans is
@@ -626,63 +571,6 @@ constexpr long ext_lengths(long lo, long hi, bool wide) {  // extended lengths i
 // 2 7 11^2 17, split into two factors of at most kMaxTileLen whose chan_wide_ext footprint fits shared memory.
 static_assert(ext_lengths(2, kMaxChanPoints, false) == 863, "extended channel lengths up to kMaxChanPoints");
 static_assert(ext_lengths(kMaxChanPoints + 1, kMaxWideChanPoints, true) == 1032, "an extended wide length does not split or fit");
-
-// Plans of every extended length used so far, by length (process-wide, never freed, like the registry).  The 863
-// lengths of at most kMaxChanPoints bound it; DESIGN.md section 4 states the device memory it can reach.
-static std::mutex g_ext_mu;
-static std::map<int, TilePlan> g_ext;
-
-// The plan of `len` by value: the registry's for a 7-smooth length (factors of an extended wide length can be), an
-// extended plan otherwise.
-static int get_ext_plan(int len, TilePlan *out) {
-  if (smooth7(len)) {
-    int const idx = get_tile_plan(len);
-    if (idx < 0) return -1;
-    std::lock_guard<std::mutex> lk(g_plan_mu);
-    *out = g_plans[(size_t)idx].host;
-    return 0;
-  }
-  std::lock_guard<std::mutex> lk(g_ext_mu);
-  auto it = g_ext.find(len);
-  if (it == g_ext.end()) {
-    std::vector<int> rad;
-    if (len <= kMaxChanPoints) rad = choose_radices_ext(len);
-    if (rad.empty()) return fail("%d-point transform cannot be planned (prime factors up to 23; at most %d points)", len, kMaxChanPoints);
-    TilePlan p;
-    if (make_tile_plan(len, rad, p)) return -1;
-    it = g_ext.emplace(len, p).first;
-  }
-  *out = it->second;
-  return 0;
-}
-
-// Four-step geometry of every extended wide length used so far (never freed): chan_wide's split and twiddle table,
-// with the two factor plans by value.
-static std::mutex g_wide_ext_mu;
-static std::map<int, WideGeomExt> g_wide_ext;
-
-static WideGeomExt const *get_wide_geom_ext(int points) {
-  std::lock_guard<std::mutex> lk(g_wide_ext_mu);
-  auto it = g_wide_ext.find(points);
-  if (it != g_wide_ext.end()) return &it->second;
-  Split2 sp;
-  if (!choose_split_ext(points, &sp)) {
-    fail("%d-point transform cannot be split into two plannable lengths (prime factors up to 23; each at most %d)", points,
-         kMaxTileLen);
-    return nullptr;
-  }
-  if (wide_smem_bytes(sp.n1, sp.n2) > kChanSmemLimit) {
-    fail("%d-point transform (%d x %d) does not fit in shared memory", points, sp.n1, sp.n2);
-    return nullptr;
-  }
-  WideGeomExt x;
-  x.g.n1 = sp.n1;
-  x.g.n2 = sp.n2;
-  x.g.pitch = wide_pitch(sp.n2);
-  x.g.plan1 = x.g.plan2 = -1;
-  if (get_ext_plan(sp.n1, &x.p1) || get_ext_plan(sp.n2, &x.p2) || wide_twiddles(x.g, x.p2)) return nullptr;
-  return &(g_wide_ext[points] = x);
-}
 
 // The largest prime factor of n above 7, or 1 if n has none.
 static long factor_above7(long n) {
@@ -924,107 +812,16 @@ static int master_setup(kgpu_master *m) {
     if (allow_smem((const void *)fwd_rows_2s<25, 25>, Rows2s::smem)) return -1;
   }
   if (m->rows == ROWS_V2 && allow_smem((const void *)rows_v2_kernel(m), rows_v2_smem(m))) return -1;
-  // the generic pair can run for every master (kgpu_use_static_kernels(0)); a master it does not fit is rejected here
-  if (allow_smem((const void *)fwd_cols_kernel<0>, m->smem1) || allow_smem((const void *)fwd_cols_kernel<1>, m->smem1) ||
-      allow_smem((const void *)fwd_rows_kernel, m->smem2))
+  // an extended master runs the extended pair; the generic pair can run for every other one (kgpu_use_static_kernels(0))
+  if (m->ext) {
+    if (allow_smem((const void *)fwd_cols_ext<0>, m->smem1) || allow_smem((const void *)fwd_cols_ext<1>, m->smem1) ||
+        allow_smem((const void *)fwd_rows_ext, m->smem2))
+      return -1;
+  } else if (allow_smem((const void *)fwd_cols_kernel<0>, m->smem1) || allow_smem((const void *)fwd_cols_kernel<1>, m->smem1) ||
+             allow_smem((const void *)fwd_rows_kernel, m->smem2)) {
     return -1;
+  }
   return 0;
-}
-
-extern "C" kgpu_master *kgpu_master_create(int L, int M, int in_type) {
-  if (L < 1 || M < 1 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX)) {
-    fail("kgpu_master_create: bad arguments L=%d M=%d type=%d", L, M, in_type);
-    return nullptr;
-  }
-  int const N = L + M - 1;
-  if (in_type == KGPU_REAL && ((N & 1) || (L & 1))) {
-    fail("kgpu_master_create: REAL input needs even L and even N=L+M-1 (got L=%d N=%d)", L, N);
-    return nullptr;
-  }
-  long const nc = (in_type == KGPU_COMPLEX) ? N : N / 2;
-  Split2 sp;
-  if (!choose_split(nc, &sp)) {
-    fail("kgpu_master_create: %ld points cannot be split into two plannable lengths (factors 2,3,5,7; <= %d)", nc,
-         kMaxTileLen);
-    return nullptr;
-  }
-  kgpu_master *m = new kgpu_master;
-  master_shape(m, L, M, in_type, sp, false);
-  m->plan1 = get_tile_plan(m->sp.n1);
-  m->plan2 = get_tile_plan(m->sp.n2);
-  if (m->plan1 < 0 || m->plan2 < 0) {
-    fail("kgpu_master_create: %s", std::string(g_err).c_str());
-    delete m;
-    return nullptr;
-  }
-  if (master_setup(m)) {
-    kgpu_master_destroy(m);
-    return nullptr;
-  }
-  return m;
-}
-
-// kgpu_master_create for transform lengths whose prime factors go up to 23.  A length with factors 2, 3, 5, 7 only is
-// kgpu_master_create itself.  Any other gets the extended generic pair on two plans of its own, so the registry, which
-// keeps room for every length a 7-smooth master or channel can ask for, never sees them.
-#define KGPU_EXT_FACTORS "2, 3, 5, 7, 11, 13, 17, 19, 23"
-extern "C" kgpu_master *kgpu_master_create_ex(int L, int M, int in_type) {
-  if (L < 1 || M < 1 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX)) {
-    fail("kgpu_master_create_ex: bad arguments L=%d M=%d type=%d", L, M, in_type);
-    return nullptr;
-  }
-  int const N = L + M - 1;
-  if (in_type == KGPU_REAL && ((N & 1) || (L & 1))) {
-    fail("kgpu_master_create_ex: REAL input needs even L and even N=L+M-1 (got L=%d N=%d)", L, N);
-    return nullptr;
-  }
-  long const nc = (in_type == KGPU_COMPLEX) ? N : N / 2;
-  if (smooth7(nc)) return kgpu_master_create(L, M, in_type);
-  long rest = nc;
-  for (long p : {2, 3, 5, 7, 11, 13, 17, 19, 23})
-    while (rest % p == 0) rest /= p;
-  if (rest != 1) {
-    long q = 29;  // the smallest prime factor left
-    while (q * q <= rest && rest % q) q++;
-    if (rest % q) q = rest;
-    fail("kgpu_master_create_ex: %ld points have the prime factor %ld (accepted factors " KGPU_EXT_FACTORS ")", nc, q);
-    return nullptr;
-  }
-  Split2 sp;
-  if (!choose_split_ext(nc, &sp)) {
-    fail("kgpu_master_create_ex: %ld points cannot be split into two plannable lengths (factors " KGPU_EXT_FACTORS
-         "; <= %d)", nc, kMaxTileLen);
-    return nullptr;
-  }
-  size_t const smem1 = sizeof(float2) * ((size_t)kTile * column_pitch(sp.n1) + (size_t)kTile * ((sp.n1 + 31) / 32));
-  size_t const smem2 = sizeof(float2) * ((size_t)kTile * column_pitch(sp.n2));
-  if (smem1 > (size_t)kChanSmemLimit || smem2 > (size_t)kChanSmemLimit) {
-    fail("kgpu_master_create_ex: %ld points split as %d x %d, which needs %zu / %zu B of shared memory (at most %d; "
-         "factors " KGPU_EXT_FACTORS ")", nc, sp.n1, sp.n2, smem1, smem2, kChanSmemLimit);
-    return nullptr;
-  }
-  kgpu_master *m = new kgpu_master;
-  master_shape(m, L, M, in_type, sp, true);
-  m->plan1 = m->plan2 = -1;
-  bool const real = in_type == KGPU_REAL;
-  bool ok = make_tile_plan(sp.n1, choose_radices_ext(sp.n1), m->xplan1) == 0 &&
-            make_tile_plan(sp.n2, choose_radices_ext(sp.n2), m->xplan2) == 0;
-  if (ok && real) {
-    std::vector<float2> rootD((size_t)sp.n2);
-    for (int k2 = 0; k2 < sp.n2; k2++) {
-      long double const ang = -M_PIl * (long double)k2 / (long double)sp.n2;
-      rootD[(size_t)k2] = make_float2((float)cosl(ang), (float)sinl(ang));
-    }
-    ok = upload(&m->d_rootD, rootD) == 0;
-  }
-  ok = ok && !allow_smem((const void *)fwd_cols_ext<0>, smem1) && !allow_smem((const void *)fwd_cols_ext<1>, smem1) &&
-       !allow_smem((const void *)fwd_rows_ext, smem2);
-  if (!ok) {
-    fail("kgpu_master_create_ex: %s", std::string(g_err).c_str());
-    kgpu_master_destroy(m);
-    return nullptr;
-  }
-  return m;
 }
 
 extern "C" void kgpu_master_destroy(kgpu_master *m) {
@@ -1086,7 +883,7 @@ extern "C" int kgpu_master_describe(kgpu_master const *m, char *buf, int buflen)
   return 0;
 }
 
-// ---- kgpu_master_create_any: the path chosen from L, M and the input type alone ----
+// ---- the path of a master, chosen from L, M and the input type alone ----
 // Bound on each of a Bluestein master's scratch buffers (the chirped input, the passes' spectra, and the internal
 // master's inter-pass buffer), as the bank bounds its huge-channel scratch: longer launches run in chunks of blocks.
 static constexpr long kBluesteinScratchCap = 128L << 20;
@@ -1097,9 +894,13 @@ struct MasterPlan {
   long P;     // Bluestein: the internal master's length
   Split2 sp;  // the split of nc (direct, extended) or of P (Bluestein)
 };
-// The master kgpu_master_create_any builds: kgpu_master_create_ex's wherever that succeeds (its host-side checks,
-// restated), a Bluestein transform otherwise.
-static int master_plan(int L, int M, int in_type, char const *who, MasterPlan *pl) {
+#define KGPU_EXT_FACTORS "2, 3, 5, 7, 11, 13, 17, 19, 23"
+// The one place a master's path is decided: the direct pair for a 7-smooth length whose split fits shared memory, else
+// the extended pair for a 23-smooth one, else a Bluestein transform; the first of them at or below `ceiling`, the highest
+// path the caller serves (kgpu_master_create: direct, _ex: extended, _any and kgpu_master_plan: Bluestein).  `who` names
+// the caller in its messages.  A length above the ceiling is refused as kgpu_master_create words it for a 7-smooth
+// length and as kgpu_master_create_ex words it for any other.
+static int master_plan(int L, int M, int in_type, MasterPath ceiling, char const *who, MasterPlan *pl) {
   if (L < 1 || M < 1 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX))
     return fail("%s: bad arguments L=%d M=%d type=%d", who, L, M, in_type);
   long const N = (long)L + M - 1;
@@ -1113,21 +914,97 @@ static int master_plan(int L, int M, int in_type, char const *who, MasterPlan *p
     pl->path = MP_DIRECT;
     return 0;
   }
-  if (smooth23(nc) && forward_split(nc, true, &pl->sp)) {
+  if (ceiling >= MP_EXTENDED && smooth23(nc) && forward_split(nc, true, &pl->sp)) {
     pl->path = MP_EXTENDED;
     return 0;
   }
-  if (bluestein_length(nc, &pl->P, &pl->sp)) {
-    pl->path = MP_BLUESTEIN;
-    return 0;
+  if (ceiling == MP_BLUESTEIN) {
+    if (bluestein_length(nc, &pl->P, &pl->sp)) {
+      pl->path = MP_BLUESTEIN;
+      return 0;
+    }
+    return fail("%s: %ld points need a Bluestein transform of at least %ld points, more than the forward pair splits (at "
+                "most 3500 x 3500)", who, nc, 2 * nc - 1);
   }
-  return fail("%s: %ld points need a Bluestein transform of at least %ld points, more than the forward pair splits (at "
-              "most 3500 x 3500)", who, nc, 2 * nc - 1);
+  bool const ext = ceiling == MP_EXTENDED && !smooth7(nc);
+  char const *const name = ext ? "kgpu_master_create_ex" : "kgpu_master_create";
+  char const *const factors = ext ? KGPU_EXT_FACTORS : "2,3,5,7";
+  if (ext) {
+    long rest = nc;
+    for (long p : {2, 3, 5, 7, 11, 13, 17, 19, 23})
+      while (rest % p == 0) rest /= p;
+    if (rest != 1) {
+      long q = 29;  // the smallest prime factor left
+      while (q * q <= rest && rest % q) q++;
+      if (rest % q) q = rest;
+      return fail("%s: %ld points have the prime factor %ld (accepted factors %s)", name, nc, q, factors);
+    }
+  }
+  Split2 sp;
+  if (!(ext ? choose_split_ext(nc, &sp) : choose_split(nc, &sp)))
+    return fail("%s: %ld points cannot be split into two plannable lengths (factors %s; <= %d)", name, nc, factors, kMaxTileLen);
+  kgpu_master m;
+  master_shape(&m, L, M, in_type, sp, ext);
+  return fail("%s: %ld points split as %d x %d, which needs %zu / %zu B of shared memory (at most %d; factors %s)", name, nc,
+              sp.n1, sp.n2, m.smem1, m.smem2, kChanSmemLimit, factors);
+}
+
+// The master master_plan chooses, built.  An extended master keeps its two plans out of the registry, which keeps room
+// for every length a 7-smooth master or channel can ask for.
+static kgpu_master *master_create(int L, int M, int in_type, MasterPath ceiling, char const *who) {
+  MasterPlan pl;
+  if (master_plan(L, M, in_type, ceiling, who, &pl)) return nullptr;
+  kgpu_master *m = new kgpu_master;
+  bool ok;
+  if (pl.path == MP_BLUESTEIN) {
+    m->L = L;
+    m->M = M;
+    m->N = L + M - 1;
+    m->in_type = in_type;
+    m->bins = (in_type == KGPU_COMPLEX) ? m->N : m->N / 2 + 1;
+    m->nc = pl.nc;
+    m->spec_stride = ((long)m->bins + 3) / 4 * 4;
+    m->bp = pl.P;
+    m->b_chunk = (int)std::max(1L, kBluesteinScratchCap / (long)(sizeof(float2) * (size_t)(pl.P + 3)));
+    m->bs = kgpu_master_create((int)pl.P, 1, KGPU_COMPLEX);
+    ok = m->bs && upload(&m->d_bspec, bluestein_bspec(pl.nc, pl.P)) == 0;
+  } else {
+    master_shape(m, L, M, in_type, pl.sp, pl.path == MP_EXTENDED);
+    if (m->ext) {
+      m->plan1 = m->plan2 = -1;
+      ok = make_tile_plan(pl.sp.n1, choose_radices_ext(pl.sp.n1), m->xplan1) == 0 &&
+           make_tile_plan(pl.sp.n2, choose_radices_ext(pl.sp.n2), m->xplan2) == 0;
+    } else {
+      m->plan1 = get_tile_plan(pl.sp.n1);
+      m->plan2 = get_tile_plan(pl.sp.n2);
+      ok = m->plan1 >= 0 && m->plan2 >= 0;
+    }
+    ok = ok && master_setup(m) == 0;
+  }
+  if (!ok) {
+    fail("%s: %s", who, std::string(g_err).c_str());
+    kgpu_master_destroy(m);
+    return nullptr;
+  }
+  return m;
+}
+
+extern "C" kgpu_master *kgpu_master_create(int L, int M, int in_type) {
+  return master_create(L, M, in_type, MP_DIRECT, "kgpu_master_create");
+}
+// kgpu_master_create for transform lengths whose prime factors go up to 23.  A length with factors 2, 3, 5, 7 only
+// gets exactly kgpu_master_create's master; any other the extended generic pair.
+extern "C" kgpu_master *kgpu_master_create_ex(int L, int M, int in_type) {
+  return master_create(L, M, in_type, MP_EXTENDED, "kgpu_master_create_ex");
+}
+// Any length: kgpu_master_create_ex's master wherever that succeeds, a Bluestein transform otherwise.
+extern "C" kgpu_master *kgpu_master_create_any(int L, int M, int in_type) {
+  return master_create(L, M, in_type, MP_BLUESTEIN, "kgpu_master_create_any");
 }
 
 extern "C" int kgpu_master_plan(int L, int M, int in_type, char *buf, int buflen) {
   MasterPlan pl;
-  if (master_plan(L, M, in_type, "kgpu_master_plan", &pl)) return -1;
+  if (master_plan(L, M, in_type, MP_BLUESTEIN, "kgpu_master_plan", &pl)) return -1;
   if (buf && buflen > 0) {
     kgpu_master m, inner;
     std::string t;
@@ -1141,34 +1018,6 @@ extern "C" int kgpu_master_plan(int L, int M, int in_type, char *buf, int buflen
     snprintf(buf, (size_t)buflen, "%s", t.c_str());
   }
   return (int)pl.path;
-}
-
-extern "C" kgpu_master *kgpu_master_create_any(int L, int M, int in_type) {
-  MasterPlan pl;
-  if (master_plan(L, M, in_type, "kgpu_master_create_any", &pl)) return nullptr;
-  if (pl.path != MP_BLUESTEIN) return kgpu_master_create_ex(L, M, in_type);
-  kgpu_master *m = new kgpu_master;
-  m->L = L;
-  m->M = M;
-  m->N = L + M - 1;
-  m->in_type = in_type;
-  m->bins = (in_type == KGPU_COMPLEX) ? m->N : m->N / 2 + 1;
-  m->nc = pl.nc;
-  m->spec_stride = ((long)m->bins + 3) / 4 * 4;
-  m->bp = pl.P;
-  m->b_chunk = (int)std::max(1L, kBluesteinScratchCap / (long)(sizeof(float2) * (size_t)(pl.P + 3)));
-  m->bs = kgpu_master_create((int)pl.P, 1, KGPU_COMPLEX);
-  bool ok = m->bs != nullptr;
-  if (ok) {
-    std::vector<float2> const b = bluestein_bspec(pl.nc, pl.P);
-    ok = upload(&m->d_bspec, b) == 0;
-  }
-  if (!ok) {
-    fail("kgpu_master_create_any: %ld-point Bluestein transform of %ld points: %s", pl.nc, pl.P, std::string(g_err).c_str());
-    kgpu_master_destroy(m);
-    return nullptr;
-  }
-  return m;
 }
 
 // One launch pair (column pass, row pass) over `nblocks` consecutive blocks on stream `st`, inter-pass data in `mid`.
@@ -1436,51 +1285,153 @@ int design_taps(int points, int olen, int master_points, bool master_real, doubl
 }  // namespace
 
 // ------------------------------------------------------------------ bank --------------------
-// ---- channels served by a Bluestein transform (kgpu_bank_define_any, bluestein_chan.cuh) ----
-// Exactly the lengths kgpu_bank_define_ext refuses for their factors: a prime factor >= 29, or one of 11 .. 23 above
-// kMaxWideChanPoints.
-static bool chan_needs_bluestein(long points) {
-  long const big = factor_above7(points);
-  return big > 23 || (big > 1 && points > kMaxWideChanPoints);
+// ---- the path of a channel's inverse transform, chosen from its point count alone ----
+//   CP_DIRECT     factors 2, 3, 5, 7, at most kMaxChanPoints: one warp per channel on a registry plan (chan_kernel, or
+//                 a specialised kernel of chan_v2 / chan_static)
+//   CP_WIDE       factors 2, 3, 5, 7, at most kMaxWideChanPoints: chan_wide, one CTA per channel on a four-step split
+//                 into two registry lengths
+//   CP_HUGE       factors 2, 3, 5, 7, at most kMaxHugeChanPoints: chan_huge's two passes through the bank's scratch
+//   CP_EXTENDED   a prime factor 11 .. 23, at most kMaxWideChanPoints: chan_kernel_ext, or chan_wide_ext above
+//                 kMaxChanPoints, on plans outside the registry
+//   CP_BLUESTEIN  every other length up to kMaxHugeChanPoints: a Bluestein transform (bluestein_chan.cuh)
+// The values are kgpu_chan_plan's.  Each kgpu_bank_define* entry point serves the paths up to its own (its ceiling), and
+// kDefineName[path] is the entry point that introduced a path, which names it in messages.
+enum ChanPath { CP_DIRECT = 0, CP_WIDE = 1, CP_HUGE = 2, CP_EXTENDED = 3, CP_BLUESTEIN = 4 };
+static char const *const kDefineName[] = {"kgpu_bank_define", "kgpu_bank_define_wide", "kgpu_bank_define_huge",
+                                          "kgpu_bank_define_ext", "kgpu_bank_define_any"};
+struct ChanRoute {
+  ChanPath path;
+  bool narrow;  // at most kMaxChanPoints: the transform fits one warp (direct, extended; Bluestein only for grouping)
+  Split2 sp;    // wide, huge, extended above kMaxChanPoints: the four-step split; Bluestein: the split of P
+  long P;       // Bluestein: the length of the internal 7-smooth master, the smallest that splits >= 2 points - 1
+};
+
+// The route of a channel of `points` points, without a device.  A length above `ceiling`, or above every path, is
+// refused with the message each entry point has always given; `who` names the caller when it is above every path.
+static int chan_route(int points, ChanPath ceiling, char const *who, ChanRoute *r) {
+  long const big = factor_above7(points);  // 1: factors 2, 3, 5, 7 only
+  // the path a 7-smooth length of this size takes
+  ChanPath const size = points <= kMaxChanPoints ? CP_DIRECT : points <= kMaxWideChanPoints ? CP_WIDE : CP_HUGE;
+  bool const too_long = points > kMaxHugeChanPoints;
+  *r = ChanRoute{};
+  r->path = big == 1 ? size : (big <= 23 && size != CP_HUGE) ? CP_EXTENDED : CP_BLUESTEIN;
+  r->narrow = size == CP_DIRECT;
+  if (too_long && ceiling == CP_BLUESTEIN)
+    return fail("%s: %d-point inverse transform exceeds the %d-point maximum", who, points, kMaxHugeChanPoints);
+  if (r->path == CP_BLUESTEIN && ceiling == CP_EXTENDED) {
+    if (big > 23)
+      return fail("kgpu_bank_define_ext: %d-point inverse transform has the prime factor %ld (prime factors up to 23 are served)",
+                  points, big);
+    return fail("kgpu_bank_define_ext: %d-point inverse transform has the prime factor %ld, served up to %d points only",
+                points, big, kMaxWideChanPoints);
+  }
+  if (r->path > ceiling || too_long) {  // a 7-smooth length too long for define_ext gets define_huge's message
+    static int const kMaxPoints[] = {kMaxChanPoints, kMaxWideChanPoints, kMaxHugeChanPoints};
+    ChanPath const c = std::min(ceiling, CP_HUGE);
+    if (size > c || too_long)
+      return fail("%s: %d-point inverse transform exceeds the %d-point maximum", kDefineName[c], points, kMaxPoints[c]);
+    if (size == CP_DIRECT)
+      return fail("kgpu_bank_define: %d-point transform cannot be planned (factors 2, 3, 5, 7; at most %d points)", points,
+                  kMaxChanPoints);
+    return fail("%s: %d-point transform cannot be split into two plannable lengths (factors 2, 3, 5, 7; each at most %d)",
+                kDefineName[size], points, kMaxTileLen);
+  }
+  // the static_asserts on wide_fits, huge_lengths and ext_lengths pin that every split below exists and fits
+  bool ok = true;
+  if (r->path == CP_BLUESTEIN) ok = bluestein_length(points, &r->P, &r->sp);
+  else if (!r->narrow) ok = r->path == CP_EXTENDED ? choose_split_ext(points, &r->sp) : choose_split(points, &r->sp);
+  if (!ok) return fail("%s: %d-point transform has no split", who, points);
+  return 0;
 }
 
-// P, its split and the device copy of B = DFT_P of the conjugate chirp, for every Bluestein channel length used so far,
-// per device (never freed, like the extended plans).  B is read-only and its host transform takes about 1 s at P = 1.5 M,
-// so it is computed once per length, not per channel or bank.
-struct BluesteinChan {
-  long P;
-  Split2 sp;
-  float2 *d_b;
+// A channel length's route and the device state its kernels read, per device and length: built by the first
+// kgpu_bank_define* of the length, never freed (like the plan registry).  Map nodes are stable, so channels keep a
+// pointer.  Bluestein's B is read-only and its host transform takes about 1 s at P = 1.5 M, so it is computed once per
+// length, not per channel or bank.  DESIGN.md section 4 states the device memory the extended plans can reach.
+struct ChanGeom {
+  ChanRoute r;
+  int points = 0;
+  int plan = -1;          // ChanDesc::plan: the registry plan of the length (direct) or of n1 (wide, huge); kPlanExt,
+                          // kPlanBluestein
+  WideGeom wide{};        // CP_WIDE
+  HugeGeom huge{};        // CP_HUGE (no tables: the kernels compute their twiddles)
+  TilePlan ext{};         // CP_EXTENDED, narrow
+  WideGeomExt wide_ext{}; // CP_EXTENDED above kMaxChanPoints: chan_wide's split and twiddles, the factor plans by value
+  float2 *d_b = nullptr;  // CP_BLUESTEIN: B = DFT_P of the conjugate chirp
 };
-static std::mutex g_bchan_mu;
-static std::map<std::pair<int, int>, BluesteinChan> g_bchan;
+static std::recursive_mutex g_geom_mu;  // recursive: an extended wide length builds the records of its factors
+static std::map<std::pair<int, int>, ChanGeom> g_geom;
 
-static BluesteinChan const *get_bluestein_chan(int points) {
+static ChanGeom const *chan_geom(int points, ChanRoute const &r);
+// The plan of a factor (<= kMaxTileLen) of an extended wide length by value: the registry's for a 7-smooth factor,
+// the factor's own extended plan otherwise.
+static int factor_plan(int len, TilePlan *out) {
+  ChanRoute r;
+  if (chan_route(len, CP_EXTENDED, "factor_plan", &r)) return -1;
+  ChanGeom const *g = chan_geom(len, r);
+  if (!g) return -1;
+  if (r.path == CP_EXTENDED) {
+    *out = g->ext;
+    return 0;
+  }
+  std::lock_guard<std::mutex> lk(g_plan_mu);
+  *out = g_plans[(size_t)g->plan].host;
+  return 0;
+}
+
+static ChanGeom const *chan_geom(int points, ChanRoute const &r) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) {
     fail("cudaGetDevice: %s", cudaGetErrorString(cudaGetLastError()));
     return nullptr;
   }
-  std::lock_guard<std::mutex> lk(g_bchan_mu);
-  auto it = g_bchan.find({dev, points});
-  if (it != g_bchan.end()) return &it->second;
-  BluesteinChan c{0, {0, 0}, nullptr};
-  if (!bluestein_length(points, &c.P, &c.sp)) {
-    fail("%d-point inverse transform needs a Bluestein transform of at least %d points, more than the forward pair splits",
-         points, 2 * points - 1);
-    return nullptr;
+  std::lock_guard<std::recursive_mutex> lk(g_geom_mu);
+  auto it = g_geom.find({dev, points});
+  if (it != g_geom.end()) return &it->second;
+  ChanGeom g;
+  g.r = r;
+  g.points = points;
+  int const n1 = r.sp.n1, n2 = r.sp.n2;
+  bool ok = true;
+  switch (r.path) {
+    case CP_DIRECT:
+      g.plan = get_tile_plan(points);
+      ok = g.plan >= 0;
+      break;
+    case CP_WIDE:
+      g.wide = WideGeom{n1, n2, wide_pitch(n2), get_tile_plan(n1), get_tile_plan(n2), nullptr};
+      ok = g.wide.plan1 >= 0 && g.wide.plan2 >= 0 && !wide_twiddles(g.wide, *host_tile_plan(g.wide.plan2));
+      g.plan = g.wide.plan1;
+      break;
+    case CP_HUGE:
+      g.huge = HugeGeom{n1, n2, huge_pitch(n1), huge_pitch(n2), get_tile_plan(n1), get_tile_plan(n2)};
+      ok = g.huge.plan1 >= 0 && g.huge.plan2 >= 0;
+      g.plan = g.huge.plan1;
+      break;
+    case CP_EXTENDED:
+      g.plan = kPlanExt;
+      if (r.narrow) {
+        ok = make_tile_plan(points, choose_radices_ext(points), g.ext) == 0;
+      } else {
+        g.wide_ext.g = WideGeom{n1, n2, wide_pitch(n2), -1, -1, nullptr};
+        ok = !factor_plan(n1, &g.wide_ext.p1) && !factor_plan(n2, &g.wide_ext.p2) && !wide_twiddles(g.wide_ext.g, g.wide_ext.p2);
+      }
+      break;
+    case CP_BLUESTEIN:
+      g.plan = kPlanBluestein;
+      ok = upload(&g.d_b, bluestein_bspec(points, r.P)) == 0;
+      if (!ok) cudaFree(g.d_b);
+      break;
   }
-  if (upload(&c.d_b, bluestein_bspec(points, c.P))) {
-    cudaFree(c.d_b);
-    return nullptr;
-  }
-  return &(g_bchan[{dev, points}] = c);
+  if (!ok) return nullptr;
+  return &(g_geom[{dev, points}] = g);
 }
 
 struct ChanHost {
   bool defined = false, enabled = false, has_response = false;
   bool real_out = false;  // REAL-output slave (filter.c:370-390): olen floats per block
-  int olen = 0, points = 0, plan = -1, shift = 0, flags = 0;
+  int olen = 0, points = 0, shift = 0, flags = 0;
+  ChanGeom const *geom = nullptr;  // the path and geometry of `points` (set by kgpu_bank_define*)
   long resp_off = 0, resp_cap = 0;  // region of the response arena owned by this slot
   ChanAux aux{};          // oscillator / beam parameters (zero = unused)
 };
@@ -1498,10 +1449,11 @@ struct kgpu_bank {
   bool dirty = true;
   int max_points = 0;
   struct Group {
-    int plan, points, off, count;
-    bool generic;  // REAL-output / beam channels: served by the runtime-plan kernel only
+    ChanGeom const *geom;
+    int off, count;
+    bool generic;  // runtime_plan_only
   };
-  std::vector<Group> groups;  // enabled channels grouped by inverse-transform plan
+  std::vector<Group> groups;  // enabled channels grouped by length
   int *d_order = nullptr;
   ChanAux *d_aux = nullptr;   // [capacity]
   int *d_shift = nullptr;     // [capacity] shifts, for the noise estimator
@@ -1603,6 +1555,12 @@ static void resolve_walk(kgpu_master const *m, ChanHost const &c, ChanDesc &d) {
   }
 }
 
+// REAL-output and beam channels of at most kMaxChanPoints: a direct one is served by the runtime-plan kernel only, and
+// the other narrow paths keep them in groups of their own as well.
+static bool runtime_plan_only(kgpu_bank const *b, int i) {
+  return b->ch[(size_t)i].geom->r.narrow && (b->desc[(size_t)i].flags & (kChanRealOut | kChanBeam)) != 0;
+}
+
 static int bank_commit(kgpu_bank *b, cudaStream_t st) {
   if (!b->dirty) return 0;
   b->desc.assign((size_t)std::max(b->nchan, 1), ChanDesc{});
@@ -1625,31 +1583,25 @@ static int bank_commit(kgpu_bank *b, cudaStream_t st) {
     d.out_off = off;
     off += c.real_out ? (c.olen + 1) / 2 : c.olen;
     if (c.enabled && c.has_response) {
-      d.plan = c.plan;
+      d.plan = c.geom->plan;
       resolve_walk(b->m, c, d);
       b->max_points = std::max(b->max_points, c.points);
     }
   }
   b->out_stride = (off + 3) / 4 * 4;
-  // one launch per distinct plan: order[] lists that plan's descriptors.  Wide channels (chan_wide serves every
-  // variant) form one group per length; their plan is only their first factor's, so the length is part of the key.
-  // Extended channels all have plan kPlanExt, so they too form one group per length (and generic-only flag).
+  // one launch per distinct length (and runtime_plan_only flag): order[] lists that group's descriptors
   std::vector<int> order;
   b->groups.clear();
-  auto generic_only = [&](int i) {
-    return b->desc[(size_t)i].points <= kMaxChanPoints && (b->desc[(size_t)i].flags & (kChanRealOut | kChanBeam)) != 0;
-  };
   auto same_group = [&](kgpu_bank::Group const &g, int k) {
-    return b->desc[(size_t)k].plan == g.plan && b->desc[(size_t)k].points == g.points && generic_only(k) == g.generic;
+    return b->desc[(size_t)k].plan >= 0 && b->ch[(size_t)k].geom == g.geom && runtime_plan_only(b, k) == g.generic;
   };
   for (int i = 0; i < b->nchan; i++) {
     if (b->desc[(size_t)i].plan < 0) continue;
-    bool const gen = generic_only(i);
     bool found = false;
     for (auto &g : b->groups)
       if (same_group(g, i)) found = true;
     if (found) continue;
-    kgpu_bank::Group g{b->desc[(size_t)i].plan, b->desc[(size_t)i].points, (int)order.size(), 0, gen};
+    kgpu_bank::Group g{b->ch[(size_t)i].geom, (int)order.size(), 0, runtime_plan_only(b, i)};
     for (int k = i; k < b->nchan; k++)
       if (same_group(g, k)) order.push_back(k);
     g.count = (int)order.size() - g.off;
@@ -1722,79 +1674,19 @@ extern "C" void kgpu_bank_destroy(kgpu_bank *b) {
 }
 static bool bad_idx(kgpu_bank const *b, int idx) { return !b || idx < 0 || idx >= b->capacity; }
 
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok = false, bool ext_ok = false,
-                       bool any_ok = false);
-extern "C" int kgpu_bank_define(kgpu_bank *b, int idx, int olen) { return bank_define(b, idx, olen, false, false); }
-extern "C" int kgpu_bank_define_ex(kgpu_bank *b, int idx, int olen, int out_type) {
-  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_ex: out_type must be KGPU_COMPLEX or KGPU_REAL");
-  return bank_define(b, idx, olen, out_type == KGPU_REAL, false);
-}
-extern "C" int kgpu_bank_define_wide(kgpu_bank *b, int idx, int olen, int out_type) {
-  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_wide: out_type must be KGPU_COMPLEX or KGPU_REAL");
-  return bank_define(b, idx, olen, out_type == KGPU_REAL, true);
-}
-extern "C" int kgpu_bank_define_huge(kgpu_bank *b, int idx, int olen, int out_type) {
-  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_huge: out_type must be KGPU_COMPLEX or KGPU_REAL");
-  return bank_define(b, idx, olen, out_type == KGPU_REAL, true, true);
-}
-extern "C" int kgpu_bank_define_ext(kgpu_bank *b, int idx, int olen, int out_type) {
-  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_ext: out_type must be KGPU_COMPLEX or KGPU_REAL");
-  return bank_define(b, idx, olen, out_type == KGPU_REAL, true, true, true);
-}
-extern "C" int kgpu_bank_define_any(kgpu_bank *b, int idx, int olen, int out_type) {
-  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("kgpu_bank_define_any: out_type must be KGPU_COMPLEX or KGPU_REAL");
-  return bank_define(b, idx, olen, out_type == KGPU_REAL, true, true, true, true);
-}
-static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide_ok, bool huge_ok, bool ext_ok, bool any_ok) {
+// Defines channel idx with the path chan_route chooses, if it lies at or below `ceiling`.  who: the entry point.
+static int bank_define(char const *who, kgpu_bank *b, int idx, int olen, int out_type, ChanPath ceiling) {
+  if (out_type != KGPU_COMPLEX && out_type != KGPU_REAL) return fail("%s: out_type must be KGPU_COMPLEX or KGPU_REAL", who);
   if (bad_idx(b, idx) || olen < 1) return fail("kgpu_bank_define: bad arguments");
+  bool const real_out = out_type == KGPU_REAL;
   long const num = (long)olen * b->m->N;
   if (num % b->m->L) return fail("invalid output length %d for N=%d L=%d (filter.c:312-316)", olen, b->m->N, b->m->L);
   int const points = (int)(num / b->m->L);
   if (real_out && (points & 1)) return fail("kgpu_bank_define: REAL-output slaves need an even number of points (got %d)", points);
-  // the channel kernel holds kChanWarps transforms of this length in shared memory; the bound also keeps the plan
-  // registry from filling (see kMaxPlans).  Longer channels (kgpu_bank_define_wide) run chan_wide, one CTA each, on
-  // a split into two registry lengths; their descriptor's plan is that of the first factor (>= 0: runnable).  Beyond
-  // kMaxWideChanPoints (kgpu_bank_define_huge) the same holds for chan_huge's split.  A length with a prime factor
-  // 11 .. 23 (kgpu_bank_define_ext) has plans of its own outside the registry; its descriptor's plan is kPlanExt.  A
-  // length that refuses for its factors (kgpu_bank_define_any) runs a Bluestein transform; its plan is kPlanBluestein.
-  long const big = ext_ok ? factor_above7(points) : 1;
-  int plan;
-  if (any_ok && points > kMaxHugeChanPoints) {
-    return fail("kgpu_bank_define_any: %d-point inverse transform exceeds the %d-point maximum", points, kMaxHugeChanPoints);
-  } else if (any_ok && chan_needs_bluestein(points)) {
-    if (!get_bluestein_chan(points)) return fail("kgpu_bank_define_any: %s", std::string(g_err).c_str());
-    plan = kPlanBluestein;
-  } else if (big > 23) {
-    return fail("kgpu_bank_define_ext: %d-point inverse transform has the prime factor %ld (prime factors up to 23 are served)",
-                points, big);
-  } else if (big > 1 && points > kMaxWideChanPoints) {
-    return fail("kgpu_bank_define_ext: %d-point inverse transform has the prime factor %ld, served up to %d points only",
-                points, big, kMaxWideChanPoints);
-  } else if (big > 1 && points > kMaxChanPoints) {
-    if (!get_wide_geom_ext(points)) return fail("kgpu_bank_define_ext: %s", std::string(g_err).c_str());
-    plan = kPlanExt;
-  } else if (big > 1) {
-    TilePlan p;
-    if (get_ext_plan(points, &p)) return fail("kgpu_bank_define_ext: %s", std::string(g_err).c_str());
-    plan = kPlanExt;
-  } else if (points <= kMaxChanPoints) {
-    plan = get_tile_plan(points);
-    if (plan < 0) return fail("kgpu_bank_define: %s", std::string(g_err).c_str());
-  } else if (!wide_ok) {
-    return fail("kgpu_bank_define: %d-point inverse transform exceeds the %d-point maximum", points, kMaxChanPoints);
-  } else if (points > kMaxWideChanPoints && !huge_ok) {
-    return fail("kgpu_bank_define_wide: %d-point inverse transform exceeds the %d-point maximum", points, kMaxWideChanPoints);
-  } else if (points > kMaxHugeChanPoints) {
-    return fail("kgpu_bank_define_huge: %d-point inverse transform exceeds the %d-point maximum", points, kMaxHugeChanPoints);
-  } else if (points > kMaxWideChanPoints) {
-    HugeGeom const *g = get_huge_geom(points);
-    if (!g) return fail("kgpu_bank_define_huge: %s", std::string(g_err).c_str());
-    plan = g->plan1;
-  } else {
-    WideGeom const *g = get_wide_geom(points);
-    if (!g) return fail("kgpu_bank_define_wide: %s", std::string(g_err).c_str());
-    plan = g->plan1;
-  }
+  ChanRoute r;
+  if (chan_route(points, ceiling, who, &r)) return -1;
+  ChanGeom const *geom = chan_geom(points, r);
+  if (!geom) return fail("%s: %s", kDefineName[r.path], std::string(g_err).c_str());
   ChanHost &c = b->ch[(size_t)idx];
   c.real_out = real_out;
   if (!(c.defined && c.points == points)) {
@@ -1823,20 +1715,38 @@ static int bank_define(kgpu_bank *b, int idx, int olen, bool real_out, bool wide
   c.enabled = true;
   c.olen = olen;
   c.points = points;
-  c.plan = plan;
+  c.geom = geom;
   b->nchan = std::max(b->nchan, idx + 1);
   b->dirty = true;
   return points;
 }
+extern "C" int kgpu_bank_define(kgpu_bank *b, int idx, int olen) {
+  return bank_define("kgpu_bank_define", b, idx, olen, KGPU_COMPLEX, CP_DIRECT);
+}
+extern "C" int kgpu_bank_define_ex(kgpu_bank *b, int idx, int olen, int out_type) {
+  return bank_define("kgpu_bank_define_ex", b, idx, olen, out_type, CP_DIRECT);
+}
+extern "C" int kgpu_bank_define_wide(kgpu_bank *b, int idx, int olen, int out_type) {
+  return bank_define("kgpu_bank_define_wide", b, idx, olen, out_type, CP_WIDE);
+}
+extern "C" int kgpu_bank_define_huge(kgpu_bank *b, int idx, int olen, int out_type) {
+  return bank_define("kgpu_bank_define_huge", b, idx, olen, out_type, CP_HUGE);
+}
+extern "C" int kgpu_bank_define_ext(kgpu_bank *b, int idx, int olen, int out_type) {
+  return bank_define("kgpu_bank_define_ext", b, idx, olen, out_type, CP_EXTENDED);
+}
+extern "C" int kgpu_bank_define_any(kgpu_bank *b, int idx, int olen, int out_type) {
+  return bank_define("kgpu_bank_define_any", b, idx, olen, out_type, CP_BLUESTEIN);
+}
 
 // Forward transform in place of a Bluestein channel's response (set_filter's fftwf_execute, filter.c:1030): one block of
 // bluestein_master.cuh's chain for a COMPLEX transform of `points`, through the scratch and internal master of stream st.
-static int bluestein_response(kgpu_bank *b, float2 *resp, int points, cudaStream_t st) {
-  BluesteinChan const *bc = get_bluestein_chan(points);
-  if (!bc) return -1;
-  kgpu_master *im = bank_bluestein_master(b, st, bc->P);
+static int bluestein_response(kgpu_bank *b, float2 *resp, ChanGeom const &g, cudaStream_t st) {
+  int const points = g.points;
+  long const P = g.r.P;
+  kgpu_master *im = bank_bluestein_master(b, st, P);
   if (!im) return -1;
-  long const P = bc->P, ld = im->spec_stride, in_len = (P + 31) / 32 * 32;
+  long const ld = im->spec_stride, in_len = (P + 31) / 32 * 32;
   float2 *bin = (float2 *)bank_scratch(b, st, sizeof(float2) * (size_t)(in_len + ld));
   if (!bin) return -1;
   float2 *bout = bin + in_len;
@@ -1862,11 +1772,10 @@ static int bluestein_response(kgpu_bank *b, float2 *resp, int points, cudaStream
   o.spec_stride = ld;
   bluestein_in_kernel<<<(unsigned)((P + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(a);
   if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, 1, bout, nullptr, st) != 0) return -1;
-  bluestein_mul_kernel<<<(unsigned)((P + kSpecThreads - 1) / kSpecThreads), kSpecThreads, 0, st>>>(bout, ld, bc->d_b, (int)P, bin);
+  bluestein_mul_kernel<<<(unsigned)((P + kSpecThreads - 1) / kSpecThreads), kSpecThreads, 0, st>>>(bout, ld, g.d_b, (int)P, bin);
   if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, 1, bout, nullptr, st) != 0) return -1;
   bluestein_out_kernel<<<(unsigned)((points + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(o);
   g_launches += 3;
-  CUDA_OK(cudaGetLastError());
   return 0;
 }
 
@@ -1880,48 +1789,47 @@ static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *ho
   if (on_stream) CUDA_OK(cudaStreamSynchronize(st));
   else CUDA_OK(cudaDeviceSynchronize());
   CUDA_OK(cudaMemcpyAsync(dst, host, sizeof(float2) * (size_t)c.points, cudaMemcpyHostToDevice, st));
-  if (transform && c.plan == kPlanBluestein) {
-    if (bluestein_response(b, dst, c.points, st)) return -1;
-  } else if (transform && c.plan == kPlanExt && c.points > kMaxChanPoints) {
-    WideGeomExt const *x = get_wide_geom_ext(c.points);
-    if (!x) return -1;
-    size_t const sm = (size_t)wide_smem_bytes(x->g.n1, x->g.n2);
-    if (allow_smem((const void *)response_wide_ext, sm)) return -1;
-    response_wide_ext<<<1, kWideThreads, sm, st>>>(dst, *x);
-    g_launches++;
-    CUDA_OK(cudaGetLastError());
-  } else if (transform && c.plan == kPlanExt) {
-    TilePlan p;
-    if (get_ext_plan(c.points, &p)) return -1;
-    size_t const sm = sizeof(float2) * (size_t)c.points;
-    if (allow_smem((const void *)response_fft_ext, sm)) return -1;
-    response_fft_ext<<<1, 32, sm, st>>>(dst, p);
-    g_launches++;
-    CUDA_OK(cudaGetLastError());
-  } else if (transform && c.points > kMaxWideChanPoints) {
-    HugeGeom const *g = get_huge_geom(c.points);
-    if (!g) return -1;
-    float2 *scr = (float2 *)bank_scratch(b, st, sizeof(float2) * (size_t)c.points);
-    if (!scr) return -1;
-    size_t const sm1 = (size_t)huge_smem_bytes(g->n1), sm2 = (size_t)huge_smem_bytes(g->n2);
-    if (allow_smem((const void *)response_huge_cols, sm1) || allow_smem((const void *)response_huge_rows, sm2)) return -1;
-    response_huge_cols<<<(unsigned)((g->n2 + kTile - 1) / kTile), kHugeThreads, sm1, st>>>(dst, *g, scr);
-    response_huge_rows<<<(unsigned)((g->n1 + kTile - 1) / kTile), kHugeThreads, sm2, st>>>(dst, *g, scr);
-    g_launches += 2;
-    CUDA_OK(cudaGetLastError());
-  } else if (transform && c.points > kMaxChanPoints) {
-    WideGeom const *g = get_wide_geom(c.points);
-    if (!g) return -1;
-    size_t const sm = (size_t)wide_smem_bytes(g->n1, g->n2);
-    if (allow_smem((const void *)response_wide_kernel, sm)) return -1;
-    response_wide_kernel<<<1, kWideThreads, sm, st>>>(dst, *g);
-    g_launches++;
-    CUDA_OK(cudaGetLastError());
-  } else if (transform) {
-    size_t const sm = sizeof(float2) * (size_t)c.points;
-    if (allow_smem((const void *)response_fft_kernel, sm)) return -1;
-    response_fft_kernel<<<1, 32, sm, st>>>(dst, c.plan);
-    g_launches++;
+  if (transform) {
+    ChanGeom const &g = *c.geom;
+    size_t const sm = sizeof(float2) * (size_t)c.points;  // the narrow paths' transform in shared memory
+    switch (g.r.path) {
+      case CP_DIRECT:
+        if (allow_smem((const void *)response_fft_kernel, sm)) return -1;
+        response_fft_kernel<<<1, 32, sm, st>>>(dst, g.plan);
+        g_launches++;
+        break;
+      case CP_WIDE: {
+        size_t const smw = (size_t)wide_smem_bytes(g.wide.n1, g.wide.n2);
+        if (allow_smem((const void *)response_wide_kernel, smw)) return -1;
+        response_wide_kernel<<<1, kWideThreads, smw, st>>>(dst, g.wide);
+        g_launches++;
+        break;
+      }
+      case CP_HUGE: {
+        float2 *scr = (float2 *)bank_scratch(b, st, sizeof(float2) * (size_t)c.points);
+        if (!scr) return -1;
+        size_t const sm1 = (size_t)huge_smem_bytes(g.huge.n1), sm2 = (size_t)huge_smem_bytes(g.huge.n2);
+        if (allow_smem((const void *)response_huge_cols, sm1) || allow_smem((const void *)response_huge_rows, sm2)) return -1;
+        response_huge_cols<<<(unsigned)((g.huge.n2 + kTile - 1) / kTile), kHugeThreads, sm1, st>>>(dst, g.huge, scr);
+        response_huge_rows<<<(unsigned)((g.huge.n1 + kTile - 1) / kTile), kHugeThreads, sm2, st>>>(dst, g.huge, scr);
+        g_launches += 2;
+        break;
+      }
+      case CP_EXTENDED:
+        if (g.r.narrow) {
+          if (allow_smem((const void *)response_fft_ext, sm)) return -1;
+          response_fft_ext<<<1, 32, sm, st>>>(dst, g.ext);
+        } else {
+          size_t const smw = (size_t)wide_smem_bytes(g.wide_ext.g.n1, g.wide_ext.g.n2);
+          if (allow_smem((const void *)response_wide_ext, smw)) return -1;
+          response_wide_ext<<<1, kWideThreads, smw, st>>>(dst, g.wide_ext);
+        }
+        g_launches++;
+        break;
+      case CP_BLUESTEIN:
+        if (bluestein_response(b, dst, g, st)) return -1;
+        break;
+    }
     CUDA_OK(cudaGetLastError());
   }
   if (on_stream) CUDA_OK(cudaStreamSynchronize(st));
@@ -2064,113 +1972,94 @@ template <class P> static int launch_chan_static(ChanArgs const &a, int n, int n
   return 0;
 }
 
+// The chunks of channels and blocks of the multi-kernel paths (huge, Bluestein): at most `per` (channel, block) rows
+// each, as many channels as fit, then as many blocks.  for_each runs launch(x, nc, nb) on each chunk of nc channels and
+// nb blocks, x being its ChanArgs.
+struct ChanChunks {
+  int n, nblocks, cch, cbl;  // channels and blocks in all, per chunk
+  ChanChunks(int n_, int nblocks_, long per)
+      : n(n_), nblocks(nblocks_), cch((int)std::min<long>(n_, per)), cbl((int)std::max(1L, std::min<long>(nblocks_, per / cch))) {}
+  size_t rows() const { return (size_t)cch * (size_t)cbl; }
+  template <class F> int for_each(ChanArgs const &a, F launch) const {
+    for (int c0 = 0; c0 < n; c0 += cch)
+      for (int b0 = 0; b0 < nblocks; b0 += cbl) {
+        ChanArgs x = a;
+        if (x.order) x.order += c0;
+        else x.chan_base += c0;
+        x.norder = std::min(cch, n - c0);
+        x.spec += (long)b0 * x.spec_stride;
+        x.out += (long)b0 * x.out_stride;
+        x.block0 += b0;
+        if (x.power) x.power += (long)b0 * x.power_stride;
+        if (launch(x, x.norder, std::min(cbl, nblocks - b0))) return -1;
+      }
+    return 0;
+  }
+};
+
 // The huge channels of one length (chan_huge.cuh): pass A, pass B and, with d_power, the power reduction, in chunks of
 // channels and blocks whose scratch stays within kHugeScratchCap.
-static int launch_huge(kgpu_bank *b, ChanArgs const &a, int points, int n, int nblocks, cudaStream_t st) {
-  HugeGeom const *g = get_huge_geom(points);
-  if (!g) return -1;
-  long const slot = (long)points * (long)sizeof(float2);
-  long const per = std::max(1L, kHugeScratchCap / slot);  // (channel, block) slots per chunk
-  int const cch = (int)std::min<long>(n, per), cbl = (int)std::max(1L, std::min<long>(nblocks, per / cch));
-  int const tiles_a = (g->n2 + kTile - 1) / kTile, tiles_b = (g->n1 + kTile - 1) / kTile;
-  size_t const slots = (size_t)cch * (size_t)cbl, data = slots * (size_t)slot;
-  char *scr = (char *)bank_scratch(b, st, data + slots * (size_t)tiles_b * sizeof(float));
+static int launch_huge(kgpu_bank *b, ChanArgs const &a, ChanGeom const &geom, int n, int nblocks, cudaStream_t st) {
+  HugeGeom const &g = geom.huge;
+  long const slot = (long)geom.points * (long)sizeof(float2);
+  ChanChunks const ch(n, nblocks, std::max(1L, kHugeScratchCap / slot));
+  int const tiles_a = (g.n2 + kTile - 1) / kTile, tiles_b = (g.n1 + kTile - 1) / kTile;
+  size_t const data = ch.rows() * (size_t)slot;
+  char *scr = (char *)bank_scratch(b, st, data + ch.rows() * (size_t)tiles_b * sizeof(float));
   if (!scr) return -1;
   float *partial = a.power ? (float *)(scr + data) : nullptr;
-  size_t const sm1 = (size_t)huge_smem_bytes(g->n1), sm2 = (size_t)huge_smem_bytes(g->n2);
+  size_t const sm1 = (size_t)huge_smem_bytes(g.n1), sm2 = (size_t)huge_smem_bytes(g.n2);
   if (allow_smem((const void *)chan_huge_cols, sm1) || allow_smem((const void *)chan_huge_rows, sm2)) return -1;
-  for (int c0 = 0; c0 < n; c0 += cch)
-    for (int b0 = 0; b0 < nblocks; b0 += cbl) {
-      int const nc = std::min(cch, n - c0), nb = std::min(cbl, nblocks - b0);
-      ChanArgs x = a;
-      if (x.order) x.order += c0;
-      else x.chan_base += c0;
-      x.norder = nc;
-      x.spec += (long)b0 * x.spec_stride;
-      x.out += (long)b0 * x.out_stride;
-      x.block0 += b0;
-      if (x.power) x.power += (long)b0 * x.power_stride;
-      chan_huge_cols<<<dim3((unsigned)tiles_a, (unsigned)nc, (unsigned)nb), kHugeThreads, sm1, st>>>(x, *g, (float2 *)scr);
-      chan_huge_rows<<<dim3((unsigned)tiles_b, (unsigned)nc, (unsigned)nb), kHugeThreads, sm2, st>>>(x, *g, (float2 const *)scr, partial);
-      g_launches += 2;
-      if (partial) {
-        huge_power_kernel<<<dim3((unsigned)nc, (unsigned)nb), 32, 0, st>>>(x, partial, tiles_b);
-        g_launches++;
-      }
+  return ch.for_each(a, [&](ChanArgs const &x, int nc, int nb) {
+    chan_huge_cols<<<dim3((unsigned)tiles_a, (unsigned)nc, (unsigned)nb), kHugeThreads, sm1, st>>>(x, g, (float2 *)scr);
+    chan_huge_rows<<<dim3((unsigned)tiles_b, (unsigned)nc, (unsigned)nb), kHugeThreads, sm2, st>>>(x, g, (float2 const *)scr, partial);
+    g_launches += 2;
+    if (partial) {
+      huge_power_kernel<<<dim3((unsigned)nc, (unsigned)nb), 32, 0, st>>>(x, partial, tiles_b);
+      g_launches++;
     }
-  return 0;
+    return 0;
+  });
 }
 
 // The Bluestein channels of one length (bluestein_chan.cuh): bluestein_chan_in, two passes of the stream's internal
 // master around bluestein_mul_kernel, bluestein_chan_out and, with d_power, the power reduction, in chunks of channels
 // and blocks whose two scratch buffers stay within kHugeScratchCap each.
-static int launch_bluestein(kgpu_bank *b, ChanArgs const &a, int points, int n, int nblocks, cudaStream_t st) {
-  BluesteinChan const *bc = get_bluestein_chan(points);
-  if (!bc) return -1;
-  kgpu_master *im = bank_bluestein_master(b, st, bc->P);
+static int launch_bluestein(kgpu_bank *b, ChanArgs const &a, ChanGeom const &geom, int n, int nblocks, cudaStream_t st) {
+  long const P = geom.r.P;
+  kgpu_master *im = bank_bluestein_master(b, st, P);
   if (!im) return -1;
-  long const P = bc->P, ld = im->spec_stride;  // rows of P points in, rows of ld between the passes' spectra
-  int const olen = (int)((long)points * b->m->L / b->m->N);
-  long const per = std::min(kMaxBluesteinRows, std::max(1L, kHugeScratchCap / (ld * (long)sizeof(float2))));  // rows per chunk
-  int const cch = (int)std::min<long>(n, per), cbl = (int)std::max(1L, std::min<long>(nblocks, per / cch));
+  long const ld = im->spec_stride;  // rows of P points in, rows of ld between the passes' spectra
+  int const olen = (int)((long)geom.points * b->m->L / b->m->N);
+  ChanChunks const ch(n, nblocks, std::min(kMaxBluesteinRows, std::max(1L, kHugeScratchCap / (ld * (long)sizeof(float2)))));
   int const tiles_in = (int)((P + kBluesteinThreads - 1) / kBluesteinThreads), tiles_out = (olen + kBluesteinThreads - 1) / kBluesteinThreads;
-  size_t const rows = (size_t)cch * (size_t)cbl;
+  size_t const rows = ch.rows();
   size_t const in_bytes = (rows * (size_t)P * sizeof(float2) + 255) / 256 * 256, out_bytes = rows * (size_t)ld * sizeof(float2);
   char *scr = (char *)bank_scratch(b, st, in_bytes + out_bytes + rows * (size_t)tiles_out * sizeof(float));
   if (!scr) return -1;
   float2 *bin = (float2 *)scr, *bout = (float2 *)(scr + in_bytes);
   float *partial = a.power ? (float *)(scr + in_bytes + out_bytes) : nullptr;
-  for (int c0 = 0; c0 < n; c0 += cch)
-    for (int b0 = 0; b0 < nblocks; b0 += cbl) {
-      int const nc = std::min(cch, n - c0), nb = std::min(cbl, nblocks - b0);
-      ChanArgs x = a;
-      if (x.order) x.order += c0;
-      else x.chan_base += c0;
-      x.norder = nc;
-      x.spec += (long)b0 * x.spec_stride;
-      x.out += (long)b0 * x.out_stride;
-      x.block0 += b0;
-      if (x.power) x.power += (long)b0 * x.power_stride;
-      bluestein_chan_in<<<dim3((unsigned)tiles_in, (unsigned)nc, (unsigned)nb), kBluesteinThreads, 0, st>>>(x, P, bin);
-      if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, nc * nb, bout, nullptr, st) != 0) return -1;
-      bluestein_mul_kernel<<<dim3((unsigned)((P + kSpecThreads - 1) / kSpecThreads), (unsigned)(nc * nb)), kSpecThreads, 0, st>>>(
-          bout, ld, bc->d_b, (int)P, bin);
-      if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, nc * nb, bout, nullptr, st) != 0) return -1;
-      bluestein_chan_out<<<dim3((unsigned)tiles_out, (unsigned)nc, (unsigned)nb), kBluesteinThreads, 0, st>>>(x, 1.0 / (double)P, bout,
-                                                                                                            ld, partial);
-      g_launches += 3;
-      if (partial) {
-        huge_power_kernel<<<dim3((unsigned)nc, (unsigned)nb), 32, 0, st>>>(x, partial, tiles_out);
-        g_launches++;
-      }
+  return ch.for_each(a, [&](ChanArgs const &x, int nc, int nb) {
+    bluestein_chan_in<<<dim3((unsigned)tiles_in, (unsigned)nc, (unsigned)nb), kBluesteinThreads, 0, st>>>(x, P, bin);
+    if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, nc * nb, bout, nullptr, st) != 0) return -1;
+    bluestein_mul_kernel<<<dim3((unsigned)((P + kSpecThreads - 1) / kSpecThreads), (unsigned)(nc * nb)), kSpecThreads, 0, st>>>(
+        bout, ld, geom.d_b, (int)P, bin);
+    if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, nc * nb, bout, nullptr, st) != 0) return -1;
+    bluestein_chan_out<<<dim3((unsigned)tiles_out, (unsigned)nc, (unsigned)nb), kBluesteinThreads, 0, st>>>(x, 1.0 / (double)P, bout,
+                                                                                                          ld, partial);
+    g_launches += 3;
+    if (partial) {
+      huge_power_kernel<<<dim3((unsigned)nc, (unsigned)nb), 32, 0, st>>>(x, partial, tiles_out);
+      g_launches++;
     }
-  return 0;
-}
-
-// The channels of one extended length: chan_kernel_ext, or chan_wide_ext above kMaxChanPoints, whatever the
-// static-kernel setting (every variant runs the same kernel).
-static int launch_chan_ext(ChanArgs const &a, int points, int n, int nblocks, cudaStream_t st) {
-  if (points > kMaxChanPoints) {
-    WideGeomExt const *x = get_wide_geom_ext(points);
-    if (!x) return -1;
-    size_t const sm = (size_t)wide_smem_bytes(x->g.n1, x->g.n2);
-    if (allow_smem((const void *)chan_wide_ext, sm)) return -1;
-    chan_wide_ext<<<dim3((unsigned)n, (unsigned)nblocks), kWideThreads, sm, st>>>(a, *x);
     return 0;
-  }
-  TilePlan p;
-  if (get_ext_plan(points, &p)) return -1;
-  size_t const sm = sizeof(float2) * (size_t)a.pitch * kChanWarps;
-  if (allow_smem((const void *)chan_kernel_ext, sm)) return -1;
-  dim3 const g((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks);
-  chan_kernel_ext<<<g, kChanWarps * 32, sm, st>>>(a, p);
-  return 0;
+  });
 }
 
-// one (plan, descriptor list) launch
-static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_out, long out_stride, int plan,
-                       int points, int const *d_order, int base, int n, cudaStream_t st, bool generic = false,
-                       float *d_power = nullptr) {
+// one launch of the channels of one group
+static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_out, long out_stride, ChanGeom const &g,
+                       int const *d_order, int base, int n, cudaStream_t st, bool generic = false, float *d_power = nullptr) {
+  int const points = g.points;
   ChanArgs a;
   a.spec = (float2 const *)d_spec;
   a.spec_stride = b->m->spec_stride;
@@ -2189,28 +2078,46 @@ static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_ou
   a.power = d_power;
   a.power_stride = b->capacity;
   ProfScope ps(K_CHAN, st);
-  if (plan == kPlanBluestein) return launch_bluestein(b, a, points, n, nblocks, st);  // before the length tests: any length
-  if (points > kMaxWideChanPoints) return launch_huge(b, a, points, n, nblocks, st);  // huge channels: chan_huge
-  g_launches++;
-  if (plan == kPlanExt) return launch_chan_ext(a, points, n, nblocks, st);  // before host_tile_plan: not a registry plan
-  if (points > kMaxChanPoints) {  // wide channels: chan_wide whatever the static-kernel setting
-    WideGeom const *g = get_wide_geom(points);
-    if (!g) return -1;
-    size_t const sm = (size_t)wide_smem_bytes(g->n1, g->n2);
-    if (allow_smem((const void *)chan_wide, sm)) return -1;
-    chan_wide<<<dim3((unsigned)n, (unsigned)nblocks), kWideThreads, sm, st>>>(a, *g);
-    return 0;
+  dim3 const ctas((unsigned)n, (unsigned)nblocks);  // chan_wide(_ext): one CTA per channel and block
+  dim3 const warps((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks);  // chan_kernel(_ext): one warp each
+  size_t const warp_smem = sizeof(float2) * (size_t)a.pitch * kChanWarps;
+  // the paths other than direct run the same kernels whatever the static-kernel setting (they serve every variant)
+  switch (g.r.path) {
+    case CP_BLUESTEIN:
+      return launch_bluestein(b, a, g, n, nblocks, st);
+    case CP_HUGE:
+      return launch_huge(b, a, g, n, nblocks, st);
+    case CP_WIDE: {
+      g_launches++;
+      size_t const sm = (size_t)wide_smem_bytes(g.wide.n1, g.wide.n2);
+      if (allow_smem((const void *)chan_wide, sm)) return -1;
+      chan_wide<<<ctas, kWideThreads, sm, st>>>(a, g.wide);
+      return 0;
+    }
+    case CP_EXTENDED: {
+      g_launches++;
+      if (!g.r.narrow) {
+        size_t const sm = (size_t)wide_smem_bytes(g.wide_ext.g.n1, g.wide_ext.g.n2);
+        if (allow_smem((const void *)chan_wide_ext, sm)) return -1;
+        chan_wide_ext<<<ctas, kWideThreads, sm, st>>>(a, g.wide_ext);
+        return 0;
+      }
+      if (allow_smem((const void *)chan_kernel_ext, warp_smem)) return -1;
+      chan_kernel_ext<<<warps, kChanWarps * 32, warp_smem, st>>>(a, g.ext);
+      return 0;
+    }
+    case CP_DIRECT:
+      break;
   }
-  TilePlan const *tp = host_tile_plan(plan);
+  g_launches++;
+  TilePlan const *tp = host_tile_plan(g.plan);
   if (g_static_on.load() && !generic) {
     if (plan_is<S600>(tp)) return launch_chan_v2<S600>(a, n, nblocks, st, b->any_osc);
     if (plan_is<S300>(tp)) return launch_chan_v2<S300>(a, n, nblocks, st, b->any_osc);
     if (plan_is<S1200>(tp)) return launch_chan_static<S1200>(a, n, nblocks, st);
   }
-  size_t const sm = sizeof(float2) * (size_t)a.pitch * kChanWarps;
-  if (allow_smem((const void *)chan_kernel, sm)) return -1;
-  dim3 const g((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks);
-  chan_kernel<<<g, kChanWarps * 32, sm, st>>>(a);
+  if (allow_smem((const void *)chan_kernel, warp_smem)) return -1;
+  chan_kernel<<<warps, kChanWarps * 32, warp_smem, st>>>(a);
   return 0;
 }
 
@@ -2221,8 +2128,8 @@ extern "C" int kgpu_bank_run_ex(kgpu_bank *b, const void *d_spec, int nblocks, v
   if (bank_commit(b, st)) return -1;
   if (out_pitch && out_pitch < b->out_stride) return fail("kgpu_bank_run_ex: out_pitch %ld < packed row %ld", out_pitch, b->out_stride);
   for (auto const &g : b->groups)
-    if (launch_chan(b, d_spec, nblocks, d_out, out_pitch ? out_pitch : b->out_stride, g.plan, g.points, b->d_order + g.off, 0, g.count,
-                    st, g.generic, d_power))
+    if (launch_chan(b, d_spec, nblocks, d_out, out_pitch ? out_pitch : b->out_stride, *g.geom, b->d_order + g.off, 0, g.count, st,
+                    g.generic, d_power))
       return -1;
   b->block_counter += nblocks;
   CUDA_OK(cudaGetLastError());
@@ -2244,8 +2151,8 @@ extern "C" int kgpu_bank_run_one_ex(kgpu_bank *b, int idx, const void *d_spec, v
   if (!c.defined || !c.has_response || !c.enabled) return fail("kgpu_bank_run_one: channel %d not runnable", idx);
   // write this channel's olen samples at d_out[0..olen): shift the row origin back by out_off
   float2 *origin = (float2 *)d_out - b->out_off[(size_t)idx];
-  bool const gen = (b->desc[(size_t)idx].flags & (kChanRealOut | kChanBeam)) != 0;
-  if (launch_chan(b, d_spec, 1, origin, 0, c.plan, c.points, nullptr, idx, 1, st, gen, d_power ? d_power - idx : nullptr)) return -1;
+  if (launch_chan(b, d_spec, 1, origin, 0, *c.geom, nullptr, idx, 1, st, runtime_plan_only(b, idx), d_power ? d_power - idx : nullptr))
+    return -1;
   CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -2373,48 +2280,37 @@ extern "C" int kgpu_plan_split(long n, int *n1, int *n2) {
   return 0;
 }
 
-// The path kgpu_bank_define_any takes for a channel of `points` points, from the same tests, without a device.
-enum ChanPath { CP_DIRECT = 0, CP_WIDE = 1, CP_HUGE = 2, CP_EXTENDED = 3, CP_BLUESTEIN = 4 };
+// The path kgpu_bank_define_any takes for a channel of `points` points (chan_route), described without a device.
 extern "C" int kgpu_chan_plan(int points, int out_type, char *buf, int buflen) {
   if (points < 1 || (out_type != KGPU_COMPLEX && out_type != KGPU_REAL)) return fail("kgpu_chan_plan: bad arguments");
   if (out_type == KGPU_REAL && (points & 1))
     return fail("kgpu_bank_define: REAL-output slaves need an even number of points (got %d)", points);
-  if (points > kMaxHugeChanPoints)
-    return fail("kgpu_chan_plan: %d-point inverse transform exceeds the %d-point maximum", points, kMaxHugeChanPoints);
+  ChanRoute r;
+  if (chan_route(points, CP_BLUESTEIN, "kgpu_chan_plan", &r)) return -1;
   auto list = [](std::vector<int> const &v) {
-    std::string r;
-    for (size_t i = 0; i < v.size(); i++) r += std::to_string(v[i]) + (i + 1 < v.size() ? "," : "");
-    return r;
+    std::string s;
+    for (size_t i = 0; i < v.size(); i++) s += std::to_string(v[i]) + (i + 1 < v.size() ? "," : "");
+    return s;
   };
-  bool const ext = factor_above7(points) > 1;
-  ChanPath path;
-  Split2 sp{0, 0};
+  bool const ext = r.path == CP_EXTENDED;
   char text[512];
-  if (chan_needs_bluestein(points)) {
-    long P = 0;
-    if (!bluestein_length(points, &P, &sp)) return fail("kgpu_chan_plan: %d points have no Bluestein length", points);
+  if (r.path == CP_BLUESTEIN) {
     kgpu_master inner;
-    master_shape(&inner, (int)P, 1, KGPU_COMPLEX, sp, false);
+    master_shape(&inner, (int)r.P, 1, KGPU_COMPLEX, r.sp, false);
     std::string const t = describe_text(&inner);
     snprintf(text, sizeof text, "bluestein: %d points, P=%ld: %s around bluestein_chan_in, bluestein_mul_kernel, bluestein_chan_out",
-             points, P, t.substr(t.find(", ") + 2).c_str());
-    path = CP_BLUESTEIN;
-  } else if (points <= kMaxChanPoints) {
-    std::vector<int> const r = ext ? choose_radices_ext(points) : choose_radices(points);
-    if (points > 1 && r.empty()) return fail("kgpu_chan_plan: %d-point transform cannot be planned", points);
-    snprintf(text, sizeof text, "%s: %d points, radices [%s]; kernel %s", ext ? "extended" : "direct", points, list(r).c_str(),
+             points, r.P, t.substr(t.find(", ") + 2).c_str());
+  } else if (r.narrow) {
+    std::vector<int> const rad = ext ? choose_radices_ext(points) : choose_radices(points);
+    snprintf(text, sizeof text, "%s: %d points, radices [%s]; kernel %s", ext ? "extended" : "direct", points, list(rad).c_str(),
              ext ? "chan_kernel_ext" : "chan_kernel");
-    path = ext ? CP_EXTENDED : CP_DIRECT;
   } else {
-    if (!(ext ? choose_split_ext(points, &sp) : choose_split(points, &sp)))
-      return fail("kgpu_chan_plan: %d-point transform cannot be split into two plannable lengths", points);
-    bool const huge = points > kMaxWideChanPoints;
+    bool const huge = r.path == CP_HUGE;
     snprintf(text, sizeof text, "%s: %d points, four-step %d x %d; kernels %s", ext ? "extended" : huge ? "huge" : "wide", points,
-             sp.n1, sp.n2, ext ? "chan_wide_ext" : huge ? "chan_huge_cols + chan_huge_rows" : "chan_wide");
-    path = ext ? CP_EXTENDED : huge ? CP_HUGE : CP_WIDE;
+             r.sp.n1, r.sp.n2, ext ? "chan_wide_ext" : huge ? "chan_huge_cols + chan_huge_rows" : "chan_wide");
   }
   if (buf && buflen > 0) snprintf(buf, (size_t)buflen, "%s", text);
-  return (int)path;
+  return (int)r.path;
 }
 
 // ------------------------------------------------------------------ wideband spectrum analyzer ----------
