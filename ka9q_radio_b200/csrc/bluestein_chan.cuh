@@ -4,7 +4,7 @@
 // and B = DFT_P of the conjugate chirp (bluestein_master.cuh) exactly.  Per chunk of (channel, block) rows:
 //   bluestein_chan_in      a_k = conj(S_k) w_k, S = slice x response (huge_slice: every variant), zero-padded to P
 //   kgpu_forward           A = DFT_P(a)                       (an internal 7-smooth COMPLEX master, L = P, M = 1)
-//   bluestein_mul_kernel   conj(A B)                          (spectrum_kernels.cuh)
+//   bluestein_mul_kernel   conj(A B)                          (bluestein_master.cuh)
 //   kgpu_forward           y = DFT_P(conj(A B))
 //   bluestein_chan_out     Z_n = w_n conj(y_n) / P; output conj(Z_n) for the last olen n, with the plain, oscillator
 //                          and REAL-output stores of chan_huge_rows

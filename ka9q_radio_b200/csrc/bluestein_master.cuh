@@ -3,7 +3,7 @@
 // kgpu_forward passes of an internal 7-smooth COMPLEX master of length P >= 2 nc - 1, per chunk of blocks:
 //   bluestein_in_kernel    window (float or int16 pairs, the master's hop) -> a = z w, zero-padded to P; int16 statistics
 //   kgpu_forward           A = DFT_P(a)
-//   bluestein_mul_kernel   conj(A B), B = DFT_P of the conjugate chirp (spectrum_kernels.cuh)
+//   bluestein_mul_kernel   conj(A B), B = DFT_P of the conjugate chirp
 //   kgpu_forward           y = DFT_P(conj(A B)) = P conj(a (*) conj w)
 //   bluestein_out_kernel   Z_k = w_k conj(y_k) / P, k < nc; REAL masters: the real split to bins 0 .. nc
 // w_n = exp(-i pi n^2 / nc), from n^2 mod 2 nc in 64-bit integers and one double sincospi, rounded once.
@@ -23,6 +23,18 @@ __device__ __forceinline__ float2 bluestein_chirp(long k, long nc, double mul) {
   double s, c;
   sincospi((double)r / (double)nc, &s, &c);
   return make_float2((float)(c * mul), (float)(-s * mul));
+}
+
+// out[s][k] = conj(spec[s][k] * B[k]) for k < P: the input of the second pass.  Every Bluestein transform (masters,
+// channels, the spectrum analyzer) runs it between its two passes.
+__global__ void __launch_bounds__(kBluesteinThreads) bluestein_mul_kernel(float2 const *__restrict__ spec, long spec_stride,
+                                                                          float2 const *__restrict__ B, int P,
+                                                                          float2 *__restrict__ out) {
+  long const k = (long)blockIdx.x * kBluesteinThreads + threadIdx.x;
+  if (k >= P) return;
+  int const seg = blockIdx.y;
+  float2 const a = spec[(long)seg * spec_stride + k], b = B[k];
+  out[(long)seg * P + k] = make_float2(a.x * b.x - a.y * b.y, -(a.x * b.y + a.y * b.x));
 }
 
 struct BluesteinInArgs {

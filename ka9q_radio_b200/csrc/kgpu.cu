@@ -82,6 +82,29 @@ static int allow_smem(const void *func, size_t bytes) {
   return 0;
 }
 
+// A device buffer used by the launches of one stream, grown on demand by grow(); its owner frees `p`.
+struct StreamBuf {
+  void *p = nullptr;
+  size_t bytes = 0;
+};
+// Makes `s` at least `bytes` long.  Earlier launches on `st` may still use the old buffer, so it waits for the stream
+// before freeing it.  `who` begins the messages.
+static int grow(StreamBuf &s, size_t bytes, cudaStream_t st, char const *who) {
+  if (s.bytes >= bytes) return 0;
+  if (cudaStreamSynchronize(st) != cudaSuccess)
+    return fail("%s: cudaStreamSynchronize: %s", who, cudaGetErrorString(cudaGetLastError()));
+  cudaFree(s.p);
+  s.p = nullptr;
+  s.bytes = 0;
+  cudaError_t const e = cudaMalloc(&s.p, bytes);
+  if (e != cudaSuccess) {
+    s.p = nullptr;
+    return fail("%s: cudaMalloc(%zu): %s", who, bytes, cudaGetErrorString(e));
+  }
+  s.bytes = bytes;
+  return 0;
+}
+
 // ------------------------------------------------------------------ per-launch profiling -----
 // When enabled, every kernel launch is bracketed by CUDA events on the launching stream; bench.py
 // reads the per-kernel totals for its roofline line (events are markers, they do not serialise).
@@ -591,13 +614,22 @@ static bool forward_split(long nc, bool ext, Split2 *sp) {
   return smem1 <= (size_t)kChanSmemLimit && smem2 <= (size_t)kChanSmemLimit;
 }
 
-// The Bluestein length of a transform of n points, shared by the spectrum analyzer and kgpu_master_create_any: the
-// smallest P >= 2n - 1 with factors 2, 3, 5, 7 whose split the forward pair runs.  The largest such P is 3500 x 3500.
-static bool bluestein_length(long n, long *P, Split2 *sp) {
+// A Bluestein transform of n points (bluestein_master.cuh), as masters, channels and the spectrum analyzer run it: two
+// passes of an internal 7-smooth COMPLEX master of length P around bluestein_mul_kernel.  bluestein_shape fills n, P and
+// the split without a device; bluestein_upload computes B and puts it on the device, where its owner frees it.
+struct Bluestein {
+  long n = 0;
+  long P = 0;             // the smallest length >= 2n - 1 with factors 2, 3, 5, 7 whose split the forward pair runs
+  Split2 sp{};            // the split of P
+  float2 *d_b = nullptr;  // B = DFT_P of the conjugate chirp
+};
+// The largest P is 3500 x 3500; false if n needs more.
+static bool bluestein_shape(long n, Bluestein *b) {
   long const limit = (long)kMaxTileLen * kMaxTileLen;
   for (long p = 2 * n - 1; p <= limit; p++)
-    if (smooth7(p) && forward_split(p, false, sp)) {
-      *P = p;
+    if (smooth7(p) && forward_split(p, false, &b->sp)) {
+      b->n = n;
+      b->P = p;
       return true;
     }
   return false;
@@ -672,19 +704,18 @@ struct kgpu_master {
   float2 *d_rootC = nullptr;       // REAL with fwd_rows_v2: W_{2nc}^{k1}
   float2 *d_tw0 = nullptr, *d_twA = nullptr, *d_twB = nullptr;  // tables of fwd_cols_r36 / fwd_cols_2s
   float2 *d_rtw0 = nullptr;        // stage-0 powers of fwd_rows_2s
-  float2 *d_mid = nullptr;
-  int mid_blocks = 0;
+  StreamBuf mid;                   // the inter-pass buffer
   size_t smem1 = 0, smem2 = 0;     // generic kernels
   // kgpu_master_create_ex with a prime factor 11 .. 23: the master owns its two plans (plan1 / plan2 stay -1) and runs
   // the extended pair fwd_cols_ext / fwd_rows_ext, which take them by value
   bool ext = false;
   TilePlan xplan1{}, xplan2{};
-  // kgpu_master_create_any with a Bluestein transform (bluestein_master.cuh): the internal COMPLEX master of length bp,
-  // the device copy of DFT_P of the conjugate chirp, and scratch for b_blocks blocks of at most b_chunk per launch
+  // kgpu_master_create_any with a Bluestein transform of nc points: the internal COMPLEX master of length blue.P, and
+  // the chirped input and the passes' spectra of chunks of at most b_chunk blocks
   kgpu_master *bs = nullptr;
-  long bp = 0;
-  float2 *d_bspec = nullptr, *d_bin = nullptr, *d_bout = nullptr;
-  int b_chunk = 0, b_blocks = 0;
+  Bluestein blue;
+  StreamBuf b_in, b_out;
+  int b_chunk = 0;
   // notches
   NotchDev *d_notch = nullptr;
   int n_notch = 0;
@@ -721,15 +752,30 @@ static int upload(float2 **d, std::vector<float2> const &v) {
   return 0;
 }
 
-// The part of a master that needs no device: geometry, shared-memory sizes, the kernel pair and its launch shape.
-// kgpu_master_create(_ex) and the host-only kgpu_master_plan share it, so the plan describes what creation builds.
-static void master_shape(kgpu_master *m, int L, int M, int in_type, Split2 const &sp, bool ext) {
+// The device step of a Bluestein record: B = DFT_P of the conjugate chirp, computed on the host and uploaded to b->d_b
+// (nothing stays allocated on failure).
+static int bluestein_upload(Bluestein *b) {
+  if (upload(&b->d_b, bluestein_bspec(b->n, b->P)) == 0) return 0;
+  cudaFree(b->d_b);
+  b->d_b = nullptr;
+  return -1;
+}
+
+// A master's outer geometry: what it takes in and the spectrum it writes, whichever transform computes it.
+static void master_geometry(kgpu_master *m, int L, int M, int in_type) {
   m->L = L;
   m->M = M;
   m->N = L + M - 1;
   m->in_type = in_type;
   m->bins = (in_type == KGPU_COMPLEX) ? m->N : m->N / 2 + 1;
   m->nc = (in_type == KGPU_COMPLEX) ? m->N : m->N / 2;
+  m->spec_stride = ((long)m->bins + 3) / 4 * 4;
+}
+
+// The part of a master that needs no device: geometry, shared-memory sizes, the kernel pair and its launch shape.
+// kgpu_master_create(_ex) and the host-only kgpu_master_plan share it, so the plan describes what creation builds.
+static void master_shape(kgpu_master *m, int L, int M, int in_type, Split2 const &sp, bool ext) {
+  master_geometry(m, L, M, in_type);
   m->sp = sp;
   m->ext = ext;
   m->pitch1 = column_pitch(sp.n1);
@@ -737,7 +783,6 @@ static void master_shape(kgpu_master *m, int L, int M, int in_type, Split2 const
   int const nit = (sp.n1 + 31) / 32;
   m->smem1 = sizeof(float2) * ((size_t)kTile * m->pitch1 + (size_t)kTile * nit);
   m->smem2 = sizeof(float2) * ((size_t)kTile * m->pitch2);
-  m->spec_stride = ((long)m->bins + 3) / 4 * 4;
   int const n1 = sp.n1, n2 = sp.n2;
   bool const real = in_type == KGPU_REAL;
   if (ext) {  // the extended generic pair only
@@ -836,12 +881,12 @@ extern "C" void kgpu_master_destroy(kgpu_master *m) {
   cudaFree(m->d_twA);
   cudaFree(m->d_twB);
   cudaFree(m->d_rtw0);
-  cudaFree(m->d_mid);
+  cudaFree(m->mid.p);
   cudaFree(m->d_notch);
   kgpu_master_destroy(m->bs);
-  cudaFree(m->d_bspec);
-  cudaFree(m->d_bin);
-  cudaFree(m->d_bout);
+  cudaFree(m->blue.d_b);
+  cudaFree(m->b_in.p);
+  cudaFree(m->b_out.p);
   delete m;
 }
 extern "C" int kgpu_master_points(kgpu_master const *m) { return m ? m->N : -1; }
@@ -869,16 +914,23 @@ static std::string describe_text(kgpu_master const *m) {
            m->sp.n2, rc.c_str(), rr.c_str(), s1, s2, (m->sp.n2 + kTile - 1) / kTile, m->n_rows_ctas, kc, kr);
   return buf;
 }
-// A Bluestein master: its own length, then the internal master's description from its transform on.
-static std::string describe_bluestein(int N, int in_type, kgpu_master const *inner) {
-  std::string const t = describe_text(inner);
-  return "N=" + std::to_string(N) + (in_type == KGPU_REAL ? " real" : " complex") + ", bluestein P=" + std::to_string(inner->N) +
-         ": " + t.substr(t.find(", ") + 2) + " around bluestein_in_kernel, bluestein_mul_kernel, bluestein_out_kernel";
+// A Bluestein transform: its internal master's description from the transform on, then the kernels around it (`in` and
+// `out`, the master's or the channels').
+static std::string bluestein_text(Bluestein const &b, char const *in, char const *out) {
+  kgpu_master inner;
+  master_shape(&inner, (int)b.P, 1, KGPU_COMPLEX, b.sp, false);
+  std::string const t = describe_text(&inner);
+  return t.substr(t.find(", ") + 2) + " around " + in + ", bluestein_mul_kernel, " + out;
+}
+// A Bluestein master: its own length, then bluestein_text.
+static std::string describe_bluestein(int N, int in_type, Bluestein const &b) {
+  return "N=" + std::to_string(N) + (in_type == KGPU_REAL ? " real" : " complex") + ", bluestein P=" + std::to_string(b.P) +
+         ": " + bluestein_text(b, "bluestein_in_kernel", "bluestein_out_kernel");
 }
 
 extern "C" int kgpu_master_describe(kgpu_master const *m, char *buf, int buflen) {
   if (!m || !buf) return -1;
-  std::string const t = m->bs ? describe_bluestein(m->N, m->in_type, m->bs) : describe_text(m);
+  std::string const t = m->bs ? describe_bluestein(m->N, m->in_type, m->blue) : describe_text(m);
   snprintf(buf, (size_t)buflen, "%s", t.c_str());
   return 0;
 }
@@ -891,8 +943,8 @@ enum MasterPath { MP_DIRECT = 0, MP_EXTENDED = 1, MP_BLUESTEIN = 2 };
 struct MasterPlan {
   MasterPath path;
   long nc;
-  long P;     // Bluestein: the internal master's length
-  Split2 sp;  // the split of nc (direct, extended) or of P (Bluestein)
+  Split2 sp;       // direct, extended: the split of nc
+  Bluestein blue;  // Bluestein: its shape
 };
 #define KGPU_EXT_FACTORS "2, 3, 5, 7, 11, 13, 17, 19, 23"
 // The one place a master's path is decided: the direct pair for a 7-smooth length whose split fits shared memory, else
@@ -909,7 +961,6 @@ static int master_plan(int L, int M, int in_type, MasterPath ceiling, char const
     return fail("%s: REAL input needs even L and even N=L+M-1 (got L=%d N=%ld)", who, L, N);
   long const nc = (in_type == KGPU_COMPLEX) ? N : N / 2;
   pl->nc = nc;
-  pl->P = 0;
   if (smooth7(nc) && forward_split(nc, false, &pl->sp)) {
     pl->path = MP_DIRECT;
     return 0;
@@ -919,7 +970,7 @@ static int master_plan(int L, int M, int in_type, MasterPath ceiling, char const
     return 0;
   }
   if (ceiling == MP_BLUESTEIN) {
-    if (bluestein_length(nc, &pl->P, &pl->sp)) {
+    if (bluestein_shape(nc, &pl->blue)) {
       pl->path = MP_BLUESTEIN;
       return 0;
     }
@@ -957,17 +1008,11 @@ static kgpu_master *master_create(int L, int M, int in_type, MasterPath ceiling,
   kgpu_master *m = new kgpu_master;
   bool ok;
   if (pl.path == MP_BLUESTEIN) {
-    m->L = L;
-    m->M = M;
-    m->N = L + M - 1;
-    m->in_type = in_type;
-    m->bins = (in_type == KGPU_COMPLEX) ? m->N : m->N / 2 + 1;
-    m->nc = pl.nc;
-    m->spec_stride = ((long)m->bins + 3) / 4 * 4;
-    m->bp = pl.P;
-    m->b_chunk = (int)std::max(1L, kBluesteinScratchCap / (long)(sizeof(float2) * (size_t)(pl.P + 3)));
-    m->bs = kgpu_master_create((int)pl.P, 1, KGPU_COMPLEX);
-    ok = m->bs && upload(&m->d_bspec, bluestein_bspec(pl.nc, pl.P)) == 0;
+    master_geometry(m, L, M, in_type);
+    m->blue = pl.blue;
+    m->b_chunk = (int)std::max(1L, kBluesteinScratchCap / (long)(sizeof(float2) * (size_t)(pl.blue.P + 3)));
+    m->bs = kgpu_master_create((int)pl.blue.P, 1, KGPU_COMPLEX);
+    ok = m->bs && bluestein_upload(&m->blue) == 0;
   } else {
     master_shape(m, L, M, in_type, pl.sp, pl.path == MP_EXTENDED);
     if (m->ext) {
@@ -1006,12 +1051,11 @@ extern "C" int kgpu_master_plan(int L, int M, int in_type, char *buf, int buflen
   MasterPlan pl;
   if (master_plan(L, M, in_type, MP_BLUESTEIN, "kgpu_master_plan", &pl)) return -1;
   if (buf && buflen > 0) {
-    kgpu_master m, inner;
     std::string t;
     if (pl.path == MP_BLUESTEIN) {
-      master_shape(&inner, (int)pl.P, 1, KGPU_COMPLEX, pl.sp, false);
-      t = describe_bluestein(L + M - 1, in_type, &inner);
+      t = describe_bluestein(L + M - 1, in_type, pl.blue);
     } else {
+      kgpu_master m;
       master_shape(&m, L, M, in_type, pl.sp, pl.path == MP_EXTENDED);
       t = describe_text(&m);
     }
@@ -1095,66 +1139,73 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
   return 0;
 }
 
-// kgpu_forward of a Bluestein master (bluestein_master.cuh), in chunks of at most b_chunk blocks.
+// The convolution of every Bluestein transform, over `rows` rows on stream st: A = DFT_P(a) of the chirped input a
+// ([rows][P]) into y ([rows][im->spec_stride]), conj(A B) back into a, then y = DFT_P(conj(A B)).  im: the internal
+// master, a COMPLEX master of length b.P.
+static int bluestein_conv(kgpu_master *im, Bluestein const &b, float2 *a, int rows, float2 *y, cudaStream_t st) {
+  if (kgpu_forward(im, a, KGPU_FMT_F32, 1.0f, 0, rows, y, nullptr, st) != 0) return -1;
+  {
+    ProfScope ps(K_FWD_COLS, st);
+    bluestein_mul_kernel<<<dim3((unsigned)((b.P + kBluesteinThreads - 1) / kBluesteinThreads), (unsigned)rows), kBluesteinThreads, 0,
+                           st>>>(y, im->spec_stride, b.d_b, (int)b.P, a);
+  }
+  g_launches++;
+  return kgpu_forward(im, a, KGPU_FMT_F32, 1.0f, 0, rows, y, nullptr, st);
+}
+
+// A forward Bluestein transform of b.n points over a.nblocks blocks (bluestein_master.cuh): bluestein_in_kernel into
+// bin ([nblocks][P]), the convolution into bout ([nblocks][im->spec_stride]), bluestein_out_kernel.  The caller sets
+// a's input fields and o's output fields; the transform's own are set here.
+static int bluestein_chain(kgpu_master *im, Bluestein const &b, BluesteinInArgs a, BluesteinOutArgs o, float2 *bin, float2 *bout,
+                           cudaStream_t st) {
+  a.nc = o.nc = b.n;
+  a.P = b.P;
+  a.out = bin;
+  o.y = bout;
+  o.y_stride = im->spec_stride;
+  o.inv_p = 1.0 / (double)b.P;
+  o.nblocks = a.nblocks;
+  long const bins = o.real_split ? b.n + 1 : b.n;
+  {
+    ProfScope ps(K_FWD_COLS, st);
+    bluestein_in_kernel<<<(unsigned)((b.P + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(a);
+  }
+  g_launches++;
+  if (bluestein_conv(im, b, bin, a.nblocks, bout, st)) return -1;
+  {
+    ProfScope ps(K_FWD_ROWS, st);
+    bluestein_out_kernel<<<(unsigned)((bins + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(o);
+  }
+  g_launches++;
+  return 0;
+}
+
+// kgpu_forward of a Bluestein master, in chunks of at most b_chunk blocks.
 static int bluestein_forward(kgpu_master *m, const void *d_in, int fmt, float scale, int derandomize, int nblocks, void *d_spec,
                              void *d_stats, cudaStream_t st) {
-  kgpu_master *bs = m->bs;
   int const chunk = std::min(nblocks, m->b_chunk);
-  if (m->b_blocks < chunk) {  // earlier launches on this stream may still use the old buffers
-    CUDA_OK(cudaStreamSynchronize(st));
-    cudaFree(m->d_bin);
-    cudaFree(m->d_bout);
-    m->d_bin = m->d_bout = nullptr;
-    m->b_blocks = 0;
-    CUDA_OK(cudaMalloc(&m->d_bin, sizeof(float2) * (size_t)m->bp * (size_t)chunk));
-    CUDA_OK(cudaMalloc(&m->d_bout, sizeof(float2) * (size_t)bs->spec_stride * (size_t)chunk));
-    m->b_blocks = chunk;
-  }
+  if (grow(m->b_in, sizeof(float2) * (size_t)m->blue.P * (size_t)chunk, st, "kgpu_forward") ||
+      grow(m->b_out, sizeof(float2) * (size_t)m->bs->spec_stride * (size_t)chunk, st, "kgpu_forward"))
+    return -1;
   bool const i16 = fmt == KGPU_FMT_I16;
   if (i16 && d_stats) CUDA_OK(cudaMemsetAsync(d_stats, 0, sizeof(IngestStats) * (size_t)nblocks, st));
   bool const real = m->in_type == KGPU_REAL;
-  BluesteinInArgs a;
+  BluesteinInArgs a{};
   a.hop = real ? m->L / 2 : m->L;
-  a.nc = m->nc;
-  a.P = m->bp;
   a.first_new = real ? (m->M - 1) / 2 : (m->M - 1);
   a.i16 = i16;
   a.derandomize = i16 && derandomize;
   a.scale = scale;
-  a.out = m->d_bin;
-  BluesteinOutArgs o;
-  o.y = m->d_bout;
-  o.y_stride = bs->spec_stride;
-  o.nc = m->nc;
-  o.inv_p = 1.0 / (double)m->bp;
+  BluesteinOutArgs o{};
   o.real_split = real;
   o.spec_stride = m->spec_stride;
   size_t const pair = i16 ? sizeof(short2) : sizeof(float2);
   for (int b0 = 0; b0 < nblocks; b0 += chunk) {
-    int const nb = std::min(chunk, nblocks - b0);
     a.in = (char const *)d_in + pair * (size_t)a.hop * (size_t)b0;
-    a.nblocks = nb;
+    a.nblocks = std::min(chunk, nblocks - b0);
     a.stats = (i16 && d_stats) ? (IngestStats *)d_stats + b0 : nullptr;
-    {
-      ProfScope ps(K_FWD_COLS, st);
-      bluestein_in_kernel<<<(unsigned)((m->bp + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(a);
-    }
-    g_launches++;
-    if (kgpu_forward(bs, m->d_bin, KGPU_FMT_F32, 1.0f, 0, nb, m->d_bout, nullptr, st) != 0) return -1;
-    {
-      ProfScope ps(K_FWD_COLS, st);
-      bluestein_mul_kernel<<<dim3((unsigned)((m->bp + kSpecThreads - 1) / kSpecThreads), (unsigned)nb), kSpecThreads, 0, st>>>(
-          m->d_bout, bs->spec_stride, m->d_bspec, (int)m->bp, m->d_bin);
-    }
-    g_launches++;
-    if (kgpu_forward(bs, m->d_bin, KGPU_FMT_F32, 1.0f, 0, nb, m->d_bout, nullptr, st) != 0) return -1;
-    o.nblocks = nb;
     o.spec = (float2 *)d_spec + (size_t)m->spec_stride * (size_t)b0;
-    {
-      ProfScope ps(K_FWD_ROWS, st);
-      bluestein_out_kernel<<<(unsigned)((m->bins + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(o);
-    }
-    g_launches++;
+    if (bluestein_chain(m->bs, m->blue, a, o, (float2 *)m->b_in.p, (float2 *)m->b_out.p, st)) return -1;
   }
   CUDA_OK(cudaGetLastError());
   return 0;
@@ -1165,16 +1216,10 @@ extern "C" int kgpu_forward(kgpu_master *m, const void *d_in, int fmt, float sca
   if (!m || !d_in || !d_spec || nblocks < 1) return fail("kgpu_forward: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   if (m->bs) return bluestein_forward(m, d_in, fmt, scale, derandomize, nblocks, d_spec, d_stats, st);
-  if (m->mid_blocks < nblocks) {
-    CUDA_OK(cudaStreamSynchronize(st));
-    cudaFree(m->d_mid);
-    m->d_mid = nullptr;
-    m->mid_blocks = 0;
-    CUDA_OK(cudaMalloc(&m->d_mid, sizeof(float2) * (size_t)m->sp.n1 * (size_t)((m->sp.n2 + 15) / 16 * 16) * (size_t)nblocks));
-    m->mid_blocks = nblocks;
-  }
+  size_t const mid = sizeof(float2) * (size_t)m->sp.n1 * (size_t)((m->sp.n2 + 15) / 16 * 16);
+  if (grow(m->mid, mid * (size_t)nblocks, st, "kgpu_forward")) return -1;
   if (fmt == KGPU_FMT_I16 && d_stats) CUDA_OK(cudaMemsetAsync(d_stats, 0, sizeof(IngestStats) * (size_t)nblocks, st));
-  return forward_span(m, d_in, fmt, scale, derandomize, nblocks, d_spec, d_stats, st, m->d_mid);
+  return forward_span(m, d_in, fmt, scale, derandomize, nblocks, d_spec, d_stats, st, (float2 *)m->mid.p);
 }
 
 extern "C" int kgpu_master_set_notches(kgpu_master *m, int const *bins, double const *alpha, int n) {
@@ -1302,8 +1347,8 @@ static char const *const kDefineName[] = {"kgpu_bank_define", "kgpu_bank_define_
 struct ChanRoute {
   ChanPath path;
   bool narrow;  // at most kMaxChanPoints: the transform fits one warp (direct, extended; Bluestein only for grouping)
-  Split2 sp;    // wide, huge, extended above kMaxChanPoints: the four-step split; Bluestein: the split of P
-  long P;       // Bluestein: the length of the internal 7-smooth master, the smallest that splits >= 2 points - 1
+  Split2 sp;       // wide, huge, extended above kMaxChanPoints: the four-step split
+  Bluestein blue;  // Bluestein: its shape, and B once chan_geom has built the length's record
 };
 
 // The route of a channel of `points` points, without a device.  A length above `ceiling`, or above every path, is
@@ -1338,7 +1383,7 @@ static int chan_route(int points, ChanPath ceiling, char const *who, ChanRoute *
   }
   // the static_asserts on wide_fits, huge_lengths and ext_lengths pin that every split below exists and fits
   bool ok = true;
-  if (r->path == CP_BLUESTEIN) ok = bluestein_length(points, &r->P, &r->sp);
+  if (r->path == CP_BLUESTEIN) ok = bluestein_shape(points, &r->blue);
   else if (!r->narrow) ok = r->path == CP_EXTENDED ? choose_split_ext(points, &r->sp) : choose_split(points, &r->sp);
   if (!ok) return fail("%s: %d-point transform has no split", who, points);
   return 0;
@@ -1357,7 +1402,6 @@ struct ChanGeom {
   HugeGeom huge{};        // CP_HUGE (no tables: the kernels compute their twiddles)
   TilePlan ext{};         // CP_EXTENDED, narrow
   WideGeomExt wide_ext{}; // CP_EXTENDED above kMaxChanPoints: chan_wide's split and twiddles, the factor plans by value
-  float2 *d_b = nullptr;  // CP_BLUESTEIN: B = DFT_P of the conjugate chirp
 };
 static std::recursive_mutex g_geom_mu;  // recursive: an extended wide length builds the records of its factors
 static std::map<std::pair<int, int>, ChanGeom> g_geom;
@@ -1419,8 +1463,7 @@ static ChanGeom const *chan_geom(int points, ChanRoute const &r) {
       break;
     case CP_BLUESTEIN:
       g.plan = kPlanBluestein;
-      ok = upload(&g.d_b, bluestein_bspec(points, r.P)) == 0;
-      if (!ok) cudaFree(g.d_b);
+      ok = bluestein_upload(&g.r.blue) == 0;
       break;
   }
   if (!ok) return nullptr;
@@ -1466,7 +1509,7 @@ struct kgpu_bank {
   // global scratch of the huge channels (chan_huge.cuh) and of noise_kernel_gm, one buffer per stream so that launches
   // on different streams (a batched run and a run_one) never share one; grown on demand, freed in kgpu_bank_destroy
   std::mutex scratch_mu;
-  std::map<cudaStream_t, std::pair<void *, size_t>> scratch;
+  std::map<cudaStream_t, StreamBuf> scratch;
   // the internal COMPLEX masters of the Bluestein channels, by (stream, P): kgpu_forward keeps its inter-pass buffer in
   // the master, so launches on two streams must never share one; created on first use, freed in kgpu_bank_destroy
   std::map<std::pair<cudaStream_t, long>, kgpu_master *> bmaster;
@@ -1488,23 +1531,8 @@ static kgpu_master *bank_bluestein_master(kgpu_bank *b, cudaStream_t st, long P)
 // the scratch buffer of stream `st`, at least `bytes` long (nullptr and kgpu_last_error() on failure)
 static void *bank_scratch(kgpu_bank *b, cudaStream_t st, size_t bytes) {
   std::lock_guard<std::mutex> lk(b->scratch_mu);
-  auto &s = b->scratch[st];
-  if (s.second >= bytes) return s.first;
-  if (cudaStreamSynchronize(st) != cudaSuccess) {  // earlier launches on this stream may still use the old buffer
-    fail("bank scratch: cudaStreamSynchronize: %s", cudaGetErrorString(cudaGetLastError()));
-    return nullptr;
-  }
-  cudaFree(s.first);
-  s.first = nullptr;
-  s.second = 0;
-  cudaError_t const e = cudaMalloc(&s.first, bytes);
-  if (e != cudaSuccess) {
-    s.first = nullptr;
-    fail("bank scratch: cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e));
-    return nullptr;
-  }
-  s.second = bytes;
-  return s.first;
+  StreamBuf &s = b->scratch[st];
+  return grow(s, bytes, st, "bank scratch") ? nullptr : s.p;
 }
 
 static void resolve_walk(kgpu_master const *m, ChanHost const &c, ChanDesc &d) {
@@ -1668,7 +1696,7 @@ extern "C" void kgpu_bank_destroy(kgpu_bank *b) {
   cudaFree(b->d_shift);
   cudaFree(b->d_fm_mem[0]);
   cudaFree(b->d_fm_mem[1]);
-  for (auto &s : b->scratch) cudaFree(s.second.first);
+  for (auto &s : b->scratch) cudaFree(s.second.p);
   for (auto &m : b->bmaster) kgpu_master_destroy(m.second);
   delete b;
 }
@@ -1739,46 +1767,6 @@ extern "C" int kgpu_bank_define_any(kgpu_bank *b, int idx, int olen, int out_typ
   return bank_define("kgpu_bank_define_any", b, idx, olen, out_type, CP_BLUESTEIN);
 }
 
-// Forward transform in place of a Bluestein channel's response (set_filter's fftwf_execute, filter.c:1030): one block of
-// bluestein_master.cuh's chain for a COMPLEX transform of `points`, through the scratch and internal master of stream st.
-static int bluestein_response(kgpu_bank *b, float2 *resp, ChanGeom const &g, cudaStream_t st) {
-  int const points = g.points;
-  long const P = g.r.P;
-  kgpu_master *im = bank_bluestein_master(b, st, P);
-  if (!im) return -1;
-  long const ld = im->spec_stride, in_len = (P + 31) / 32 * 32;
-  float2 *bin = (float2 *)bank_scratch(b, st, sizeof(float2) * (size_t)(in_len + ld));
-  if (!bin) return -1;
-  float2 *bout = bin + in_len;
-  BluesteinInArgs a;
-  a.in = resp;
-  a.hop = 0;
-  a.nc = points;
-  a.P = P;
-  a.first_new = 0;
-  a.nblocks = 1;
-  a.i16 = a.derandomize = 0;
-  a.scale = 1.0f;
-  a.stats = nullptr;
-  a.out = bin;
-  BluesteinOutArgs o;
-  o.y = bout;
-  o.y_stride = ld;
-  o.nc = points;
-  o.inv_p = 1.0 / (double)P;
-  o.real_split = 0;
-  o.nblocks = 1;
-  o.spec = resp;
-  o.spec_stride = ld;
-  bluestein_in_kernel<<<(unsigned)((P + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(a);
-  if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, 1, bout, nullptr, st) != 0) return -1;
-  bluestein_mul_kernel<<<(unsigned)((P + kSpecThreads - 1) / kSpecThreads), kSpecThreads, 0, st>>>(bout, ld, g.d_b, (int)P, bin);
-  if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, 1, bout, nullptr, st) != 0) return -1;
-  bluestein_out_kernel<<<(unsigned)((points + kBluesteinThreads - 1) / kBluesteinThreads), kBluesteinThreads, 0, st>>>(o);
-  g_launches += 3;
-  return 0;
-}
-
 // st == nullptr: legacy entry points, whole-device synchronisation (any stream may be using the response);
 // otherwise only `st` is synchronised: the caller guarantees that every launch reading this bank is ordered on it
 static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *host, bool transform, cudaStream_t st = nullptr,
@@ -1826,9 +1814,21 @@ static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *ho
         }
         g_launches++;
         break;
-      case CP_BLUESTEIN:
-        if (bluestein_response(b, dst, g, st)) return -1;
+      case CP_BLUESTEIN: {  // one block of the masters' chain: a COMPLEX master of `points` with hop 0, in place
+        kgpu_master *im = bank_bluestein_master(b, st, g.r.blue.P);
+        if (!im) return -1;
+        long const in_len = (g.r.blue.P + 31) / 32 * 32;
+        float2 *bin = (float2 *)bank_scratch(b, st, sizeof(float2) * (size_t)(in_len + im->spec_stride));
+        if (!bin) return -1;
+        BluesteinInArgs a{};
+        a.in = dst;
+        a.nblocks = 1;
+        a.scale = 1.0f;
+        BluesteinOutArgs o{};
+        o.spec = dst;
+        if (bluestein_chain(im, g.r.blue, a, o, bin, bin + in_len, st)) return -1;
         break;
+      }
     }
     CUDA_OK(cudaGetLastError());
   }
@@ -2022,11 +2022,11 @@ static int launch_huge(kgpu_bank *b, ChanArgs const &a, ChanGeom const &geom, in
   });
 }
 
-// The Bluestein channels of one length (bluestein_chan.cuh): bluestein_chan_in, two passes of the stream's internal
-// master around bluestein_mul_kernel, bluestein_chan_out and, with d_power, the power reduction, in chunks of channels
+// The Bluestein channels of one length (bluestein_chan.cuh): bluestein_chan_in, bluestein_conv on the stream's internal
+// master, bluestein_chan_out and, with d_power, the power reduction, in chunks of channels
 // and blocks whose two scratch buffers stay within kHugeScratchCap each.
 static int launch_bluestein(kgpu_bank *b, ChanArgs const &a, ChanGeom const &geom, int n, int nblocks, cudaStream_t st) {
-  long const P = geom.r.P;
+  long const P = geom.r.blue.P;
   kgpu_master *im = bank_bluestein_master(b, st, P);
   if (!im) return -1;
   long const ld = im->spec_stride;  // rows of P points in, rows of ld between the passes' spectra
@@ -2041,13 +2041,10 @@ static int launch_bluestein(kgpu_bank *b, ChanArgs const &a, ChanGeom const &geo
   float *partial = a.power ? (float *)(scr + in_bytes + out_bytes) : nullptr;
   return ch.for_each(a, [&](ChanArgs const &x, int nc, int nb) {
     bluestein_chan_in<<<dim3((unsigned)tiles_in, (unsigned)nc, (unsigned)nb), kBluesteinThreads, 0, st>>>(x, P, bin);
-    if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, nc * nb, bout, nullptr, st) != 0) return -1;
-    bluestein_mul_kernel<<<dim3((unsigned)((P + kSpecThreads - 1) / kSpecThreads), (unsigned)(nc * nb)), kSpecThreads, 0, st>>>(
-        bout, ld, geom.d_b, (int)P, bin);
-    if (kgpu_forward(im, bin, KGPU_FMT_F32, 1.0f, 0, nc * nb, bout, nullptr, st) != 0) return -1;
+    if (bluestein_conv(im, geom.r.blue, bin, nc * nb, bout, st)) return -1;
     bluestein_chan_out<<<dim3((unsigned)tiles_out, (unsigned)nc, (unsigned)nb), kBluesteinThreads, 0, st>>>(x, 1.0 / (double)P, bout,
                                                                                                           ld, partial);
-    g_launches += 3;
+    g_launches += 2;
     if (partial) {
       huge_power_kernel<<<dim3((unsigned)nc, (unsigned)nb), 32, 0, st>>>(x, partial, tiles_out);
       g_launches++;
@@ -2295,11 +2292,8 @@ extern "C" int kgpu_chan_plan(int points, int out_type, char *buf, int buflen) {
   bool const ext = r.path == CP_EXTENDED;
   char text[512];
   if (r.path == CP_BLUESTEIN) {
-    kgpu_master inner;
-    master_shape(&inner, (int)r.P, 1, KGPU_COMPLEX, r.sp, false);
-    std::string const t = describe_text(&inner);
-    snprintf(text, sizeof text, "bluestein: %d points, P=%ld: %s around bluestein_chan_in, bluestein_mul_kernel, bluestein_chan_out",
-             points, r.P, t.substr(t.find(", ") + 2).c_str());
+    snprintf(text, sizeof text, "bluestein: %d points, P=%ld: %s", points, r.blue.P,
+             bluestein_text(r.blue, "bluestein_chan_in", "bluestein_chan_out").c_str());
   } else if (r.narrow) {
     std::vector<int> const rad = ext ? choose_radices_ext(points) : choose_radices(points);
     snprintf(text, sizeof text, "%s: %d points, radices [%s]; kernel %s", ext ? "extended" : "direct", points, list(rad).c_str(),
@@ -2325,6 +2319,7 @@ struct SpecPlan {
   long nc;  // complex points of the forward master (fft_n/2, fft_n or P)
   long P;   // transform length of the master (fft_n or P)
   Split2 sp;
+  Bluestein blue;  // SP_BLUESTEIN: its shape, and B once kgpu_spectrum_create has uploaded it
 };
 
 // Bound on the scratch of one poll (per buffer): longer polls run in chunks of segments.
@@ -2345,9 +2340,10 @@ static int spectrum_plan(int fft_n, int in_type, SpecPlan *pl) {
     pl->nc = pl->P = fft_n;
     return 0;
   }
-  if (bluestein_length(fft_n, &pl->P, &pl->sp)) {
+  if (bluestein_shape(fft_n, &pl->blue)) {
     pl->path = SP_BLUESTEIN;
-    pl->nc = pl->P;
+    pl->nc = pl->P = pl->blue.P;
+    pl->sp = pl->blue.sp;
     return 0;
   }
   return fail("kgpu_spectrum: %d points have a prime factor >= 29 and need a Bluestein transform of at least %ld points, "
@@ -2364,7 +2360,6 @@ struct kgpu_spectrum {
   SpecPlan pl;
   kgpu_master *m = nullptr;
   float *d_window = nullptr;
-  float2 *d_bspec = nullptr;  // Bluestein: DFT_P of the conjugate chirp
   void *d_in = nullptr;       // chunk windowed segments (float fft_n for the r2c, float2 P otherwise)
   float2 *d_spec = nullptr;   // chunk spectra, master spec_stride apart
   long in_len = 0;            // elements per segment of d_in
@@ -2383,7 +2378,7 @@ extern "C" void kgpu_spectrum_destroy(kgpu_spectrum *s) {
   if (!s) return;
   kgpu_master_destroy(s->m);
   cudaFree(s->d_window);
-  cudaFree(s->d_bspec);
+  cudaFree(s->pl.blue.d_b);
   cudaFree(s->d_in);
   cudaFree(s->d_spec);
   delete s;
@@ -2420,18 +2415,14 @@ extern "C" kgpu_spectrum *kgpu_spectrum_create(int fft_n, int in_type, int bin_c
   if (e == cudaSuccess) e = cudaMemcpy(s->d_window, ones.data(), sizeof(float) * (size_t)fft_n, cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMalloc(&s->d_in, in_bytes * (size_t)s->chunk);
   if (e == cudaSuccess) e = cudaMalloc(&s->d_spec, spec_bytes * (size_t)s->chunk);
-  if (e == cudaSuccess && pl.path == SP_BLUESTEIN) {
-    long const P = pl.P;
-    std::vector<float2> const b = bluestein_bspec(fft_n, P);
-    e = cudaMalloc(&s->d_bspec, sizeof(float2) * (size_t)P);
-    if (e == cudaSuccess) e = cudaMemcpy(s->d_bspec, b.data(), sizeof(float2) * (size_t)P, cudaMemcpyHostToDevice);
-  }
-  if (e != cudaSuccess) {
+  if (e != cudaSuccess)
     fail("kgpu_spectrum_create(%d): %s", fft_n, cudaGetErrorString(e));
-    kgpu_spectrum_destroy(s);
-    return nullptr;
-  }
-  return s;
+  else if (pl.path == SP_BLUESTEIN && bluestein_upload(&s->pl.blue))
+    fail("kgpu_spectrum_create(%d): %s", fft_n, std::string(g_err).c_str());
+  else
+    return s;
+  kgpu_spectrum_destroy(s);
+  return nullptr;
 }
 
 extern "C" int kgpu_spectrum_set_window(kgpu_spectrum *s, float const *window) {
@@ -2483,7 +2474,7 @@ extern "C" int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring
   p.fft_n = fft_n;
   p.shift = shift;
   p.bin_count = s->bin_count;
-  p.norm = s->pl.path == SP_BLUESTEIN ? 1.0 / ((double)s->pl.P * (double)s->pl.P) : 1.0;
+  p.norm = s->pl.path == SP_BLUESTEIN ? 1.0 / ((double)s->pl.blue.P * (double)s->pl.blue.P) : 1.0;
   p.gain = (real ? 2. : 1.) / (double)((int64_t)fft_avg * fft_n * fft_n);  // spectrum.c:373, :431
   p.bins = d_bins;
   for (int seg0 = 0; seg0 < fft_avg; seg0 += s->chunk) {
@@ -2492,13 +2483,9 @@ extern "C" int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring
     spectrum_window_kernel<<<dim3((unsigned)((s->in_len + kSpecThreads - 1) / kSpecThreads), (unsigned)nseg), kSpecThreads, 0,
                              st>>>(w);
     g_launches++;
-    if (kgpu_forward(s->m, s->d_in, KGPU_FMT_F32, 1.0f, 0, nseg, s->d_spec, nullptr, st) != 0) return -1;
-    if (s->pl.path == SP_BLUESTEIN) {
-      bluestein_mul_kernel<<<dim3((unsigned)((s->pl.P + kSpecThreads - 1) / kSpecThreads), (unsigned)nseg), kSpecThreads, 0,
-                             st>>>(s->d_spec, s->spec_stride, s->d_bspec, (int)s->pl.P, (float2 *)s->d_in);
-      g_launches++;
-      if (kgpu_forward(s->m, s->d_in, KGPU_FMT_F32, 1.0f, 0, nseg, s->d_spec, nullptr, st) != 0) return -1;
-    }
+    if (s->pl.path == SP_BLUESTEIN ? bluestein_conv(s->m, s->pl.blue, (float2 *)s->d_in, nseg, s->d_spec, st)
+                                   : kgpu_forward(s->m, s->d_in, KGPU_FMT_F32, 1.0f, 0, nseg, s->d_spec, nullptr, st))
+      return -1;
     p.nseg = nseg;
     p.first = seg0 == 0;
     spectrum_power_kernel<<<(unsigned)((s->bin_count + kSpecThreads - 1) / kSpecThreads), kSpecThreads, 0, st>>>(p);

@@ -3,11 +3,14 @@
 //   spectrum_window_kernel   ring (float or int16, REAL or COMPLEX, modular) -> windowed segments the forward pass reads
 //   kgpu_forward             r2c (REAL, even fft_n), c2c of length fft_n, or the first Bluestein pass of length P
 //   bluestein_mul_kernel     Bluestein only: conj(A * B), B the stored transform of the conjugate chirp; second pass
+//                            (bluestein_master.cuh)
 //   spectrum_power_kernel    one thread per output bin: index mapping, bin += gain * |X|^2 over the chunk's segments
 // Bluestein: X_k = w_k sum_n (x_n w_n) conj(w_{k-n}) with w_n = exp(-i pi n^2 / fft_n), so with a = x w zero-padded to P,
 // y = DFT_P(conj(DFT_P(a) B)) = P conj(conv(a, conj w)) and |X_k|^2 = |y_k|^2 / P^2 (|w_k| = 1: no post-chirp).
 #pragma once
 #include <cuda_runtime.h>
+
+#include "bluestein_master.cuh"
 
 namespace kfft {
 
@@ -69,12 +72,9 @@ __global__ void __launch_bounds__(kSpecThreads) spectrum_window_kernel(SpecWindo
         if ((a.fft_n & 1) && k == a.fft_n - 1) re = 0.f;
       }
     }
-    if (a.chirp) {  // n^2 mod 2 fft_n in 64-bit integers, then one double sincospi
-      long const r = (k * k) % (2L * a.fft_n);
-      double s, c;
-      sincospi((double)r / (double)a.fft_n, &s, &c);
-      float const cr = (float)c, ci = (float)-s;
-      float const pr = re * cr - im * ci, pi = re * ci + im * cr;
+    if (a.chirp) {
+      float2 const w = bluestein_chirp(k, a.fft_n, 1.0);
+      float const pr = re * w.x - im * w.y, pi = re * w.y + im * w.x;
       re = pr;
       im = pi;
     }
@@ -82,17 +82,6 @@ __global__ void __launch_bounds__(kSpecThreads) spectrum_window_kernel(SpecWindo
   long const o = (long)seg * a.out_len + k;
   if (a.complex_out) reinterpret_cast<float2 *>(a.out)[o] = make_float2(re, im);
   else reinterpret_cast<float *>(a.out)[o] = re;
-}
-
-// out[s][k] = conj(spec[s][k] * B[k]) for k < P: the input of the second Bluestein pass
-__global__ void __launch_bounds__(kSpecThreads) bluestein_mul_kernel(float2 const *__restrict__ spec, long spec_stride,
-                                                                     float2 const *__restrict__ B, int P,
-                                                                     float2 *__restrict__ out) {
-  long const k = (long)blockIdx.x * kSpecThreads + threadIdx.x;
-  if (k >= P) return;
-  int const seg = blockIdx.y;
-  float2 const a = spec[(long)seg * spec_stride + k], b = B[k];
-  out[(long)seg * P + k] = make_float2(a.x * b.x - a.y * b.y, -(a.x * b.y + a.y * b.x));
 }
 
 struct SpecPowerArgs {

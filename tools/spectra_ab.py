@@ -5,7 +5,10 @@ usage: spectra_ab.py --dump DIR       run the seeded cases below with the librar
        spectra_ab.py --compare A B    compare two such dumps bit by bit; exit status 1 on any difference
 
 Cases: cfg-2 (REAL int16, 32 blocks from block 3, the workload's 1024 channels), cfg-2 with float input, and REAL masters
-on fwd_rows_v2 with other row counts (odd n1 included), plus the COMPLEX 1296 x 1250 master."""
+on fwd_rows_v2 with other row counts (odd n1 included), plus the COMPLEX 1296 x 1250 master.  Then every Bluestein
+transform: REAL 62 MS/s and COMPLEX 2.9 MS/s masters (kgpu_master_create_any; int16 with statistics, float), a bank of
+725-, 1550- and 44 000-point channels on each (responses, outputs, oscillator channels with block power), and spectrum
+polls at the REAL and COMPLEX fft_n 104 400, short and long enough to run in chunks of segments."""
 import argparse, sys
 from pathlib import Path
 import numpy as np
@@ -20,6 +23,85 @@ CASES = [  # (name, L, M, real, int16 input, blocks, first block, channels of cf
     ("r1250x1250_f32", 2500000, 625001, True, False, 3, 1, False),
     ("c1296x1250_i16", 1296000, 324001, False, True, 3, 1, False),
 ]
+BLUESTEIN_MASTERS = [  # (name, L, M, real, int16 input, blocks); N / L = 5 / 4 for both
+    ("b62m_i16", 1240000, 310001, True, True, 3),
+    ("b62m_f32", 1240000, 310001, True, False, 2),
+    ("b2m9_c_i16", 58000, 14501, False, True, 3),
+    ("b2m9_c_f32", 58000, 14501, False, False, 3),
+]
+BLUESTEIN_POINTS = (725, 1550, 44000)  # channels with no transform of their own: 5^2 29, 2 5^2 31, 2^5 5^3 11
+BLUESTEIN_SPECTRA = [  # (name, fft_n, real, int16 ring, fft_avg); 100 segments run in chunks of 39
+    ("s104400_r_i16", 104400, True, True, 3),
+    ("s104400_r_i16_long", 104400, True, True, 100),
+    ("s104400_c_f32", 104400, False, False, 3),
+    ("s104400_c_f32_long", 104400, False, False, 100),
+]
+
+
+def _save(out: Path, name: str, v):
+    import torch
+    a = v.contiguous().cpu().numpy() if isinstance(v, torch.Tensor) else np.ascontiguousarray(v)
+    np.save(out / f"{name}.npy", a.view(np.int32))
+
+
+def dump_bluestein(out: Path, dev):
+    import torch
+    from ka9q_radio_b200 import capi
+
+    st = torch.cuda.current_stream(dev).cuda_stream
+    for name, L, M, real, i16, nb in BLUESTEIN_MASTERS:
+        rng = np.random.default_rng(L + M + nb + i16)
+        per = 1 if real else 2
+        n = (nb * L + M - 1) * per
+        host = rng.integers(-3000, 3000, n, dtype=np.int16) if i16 else rng.standard_normal(n, dtype=np.float32)
+        m = capi.Master(L, M, capi.KGPU_REAL if real else capi.KGPU_COMPLEX, any_length=True)
+        b = capi.Bank(m, 8)
+        try:
+            print(f"{name}: {m.describe()}")
+            x = torch.from_numpy(host).to(dev)
+            spec = torch.empty((nb, m.spec_stride), dtype=torch.complex64, device=dev)
+            stats = torch.zeros((nb, 2), dtype=torch.int64, device=dev)  # IngestStats: energy, clips
+            m.forward(x.data_ptr(), capi.KGPU_FMT_I16 if i16 else capi.KGPU_FMT_F32, 1 / 3000 if i16 else 1.0, nb, spec.data_ptr(),
+                      st, derandomize=i16, d_stats=stats.data_ptr() if i16 else 0)
+            res = {"spec": spec[:, :m.bins]}
+            if i16:
+                res["stats"] = stats
+            # channels 0-2 plain, 3-5 the same lengths with an oscillator
+            for i in range(6):
+                pts = BLUESTEIN_POINTS[i % 3]
+                assert b.define_any(i, pts * L // m.N) == pts
+                b.set_filter(i, -0.3 + 0.05 * i, 0.35 - 0.04 * i, 11.0)
+                b.set_shift(i, (m.bins // 7) * (i + 1) * (1 if real or i % 2 else -1))
+                if i >= 3:
+                    b.set_osc(i, True, 0.1 * i, 1e-3 * i, 1e-9 * i, 0.01 * i)
+                res[f"resp{i}"] = b.get_response(i, pts)
+            o = torch.empty((nb, b.out_stride), dtype=torch.complex64, device=dev)
+            b.run(spec.data_ptr(), nb, o.data_ptr(), st)
+            res["chan"] = o.clone()
+            power = torch.zeros((nb, 8), dtype=torch.float32, device=dev)
+            b.run(spec.data_ptr(), nb, o.data_ptr(), st, power.data_ptr())
+            res["chan_osc"], res["power"] = o, power
+            torch.cuda.synchronize()
+            for k, v in res.items():
+                _save(out, f"{name}.{k}", v)
+        finally:
+            b.close()
+            m.close()
+    for name, fft_n, real, i16, avg in BLUESTEIN_SPECTRA:
+        rng = np.random.default_rng(fft_n + avg + real)
+        samples = 1_000_003
+        n = samples * (1 if real else 2)
+        ring = torch.from_numpy(rng.integers(-3000, 3000, n, dtype=np.int16) if i16 else rng.standard_normal(n, dtype=np.float32))
+        s = capi.Spectrum(fft_n, capi.KGPU_REAL if real else capi.KGPU_COMPLEX, 4001)
+        try:
+            print(f"{name}: {s.describe()}")
+            s.set_window(np.hanning(fft_n).astype(np.float32))
+            bins = torch.zeros(4001, dtype=torch.float32, device=dev)
+            s.run(ring.to(dev), 987_654, -1234 if real else 777, avg, 0.5, bins, scale=1 / 3000 if i16 else 1.0, derandomize=i16)
+            torch.cuda.synchronize()
+            _save(out, f"{name}.bins", bins)
+        finally:
+            s.close()
 
 
 def dump(out: Path):
@@ -54,6 +136,7 @@ def dump(out: Path):
                 np.save(out / f"{name}.{k}.npy", v.contiguous().view(torch.int32).cpu().numpy())
         finally:
             cz.close()
+    dump_bluestein(out, dev)
 
 
 def compare(a: Path, b: Path) -> int:
