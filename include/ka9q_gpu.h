@@ -257,6 +257,20 @@ int kgpu_spectrum_set_window(kgpu_spectrum *s, float const *window);
  * A REAL walk index the reference would take below 0 (out of its array) contributes 0. */
 int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring_samples, long end, int fmt, float scale,
                       int derandomize, int shift, int fft_avg, double overlap, float *d_bins, void *stream);
+/* One narrowband poll (narrowband_poll, spectrum.c:206-306) on an analyzer created with in_type KGPU_COMPLEX:
+ *   d_ring        device ring of ring_size float2 samples (>= fft_n), the channel's delivered blocks as spectrum.c:147-151
+ *                 appends them (kgpu_spectrum_ring_append); ring_idx the position the next sample would take
+ *   fft_avg       clamped as spectrum.c:244-246 does; *fft_avg_used (if not NULL) receives the count the poll used
+ *   overlap       0 <= overlap < 1; segments start at ring_idx - lrint(fft_n (1 + (fft_avg-1)(1-overlap))) and step
+ *                 fft_n - lrint(fft_n overlap)
+ * d_bins[0 .. bin_count) = sum of |X|^2 / (fft_n^2 fft_avg) in narrowband_poll's mapping (bin i < bin_count/2 from X[i],
+ * the others from X[fft_n - 2 (bin_count/2) + i]) and order; with an odd bin_count the last bin, which the reference reads
+ * past its transform, is 0.  -1 if bin_count > fft_n or ring_size < fft_n.  Enqueued on `stream`, as kgpu_spectrum_run. */
+int kgpu_spectrum_run_narrow(kgpu_spectrum *s, const void *d_ring, long ring_size, long ring_idx, int fft_avg,
+                             double overlap, float *d_bins, int *fft_avg_used, void *stream);
+/* olen float2 samples from d_src (device), or zeros when d_src is NULL, into the device ring d_ring of ring_size samples
+ * starting at position ring_idx and wrapping (spectrum.c:147-151).  The new position is (ring_idx + olen) % ring_size. */
+int kgpu_spectrum_ring_append(void *d_ring, long ring_size, long ring_idx, const void *d_src, long olen, void *stream);
 /* "r2c|complex|bluestein fft_n=... real|complex P=...: <nc>-point complex two-pass n1 x n2" */
 int kgpu_spectrum_describe(kgpu_spectrum const *s, char *buf, int buflen);
 void kgpu_spectrum_destroy(kgpu_spectrum *s);

@@ -21,8 +21,8 @@
  * Semantics kept: return 0 / -1 (write_*: 1 if a block fired), ND-deep spectrum ring with
  * lap -> zeros + block_drops++ (filter.c:690-701), owner-thread shortcut (filter.c:681-683),
  * missing response -> 0 with stale output (filter.c:715-718), caller-owned structs zeroed by
- * delete_*.  Not supported on the GPU path (return -1): REAL output slaves (wfm/stereod only),
- * beam synthesis (filter.c:756-775).
+ * delete_*.  COMPLEX and REAL output slaves (filter.c:345-392), ISB and beam synthesis (filter.c:756-775) all run in
+ * the master's batched launch.
  */
 #ifndef KA9Q_GPU_FILTER_H
 #define KA9Q_GPU_FILTER_H 1
@@ -152,6 +152,22 @@ double filter_noise_estimate(struct filter_out const *slave);
 int filter_spectrum_setup(struct filter_out *slave, int fft_n, int bin_count, float const *window);
 int filter_spectrum_poll(struct filter_out *slave, int shift, int fft_avg, double overlap, float *bin_data,
                          uint64_t *end_sample);
+
+/* EXTENSION (spectrum.c:123-155 and narrowband_poll, :206-306, on the device) for a COMPLEX slave: its delivered blocks
+ * are appended to a device ring exactly as the slave receives them (batched, recomputed after a retune, or zeros after a
+ * lap), so with execute_filter_output_tuned the ring is spectrum.c's ring of chan->baseband; with plain
+ * execute_filter_output it holds the untuned samples.  Slaves without an analyzer append nothing.
+ *   setup    where setup_narrowband runs (after set_filter), with fft_n window floats as generate_window leaves them;
+ *            -1 when the device cannot serve the slave (the caller keeps its CPU loop)
+ *   reserve  spectrum.c:124-145, before downconvert() delivers the block: the first call creates ring_samples zeros
+ *            with the write index at 0, a larger size keeps [0, old) and zeroes the rest, a smaller one does nothing
+ *   poll     bin_count floats as narrowband_poll leaves them before its base / step scaling; one poller per slave
+ *   ring     host copy of up to cap ring samples and the write index; returns the ring size (0 before reserve)
+ * delete_filter_output frees the analyzer and its ring. */
+int filter_spectrum_narrow_setup(struct filter_out *slave, int fft_n, int bin_count, float const *window);
+int filter_spectrum_narrow_reserve(struct filter_out *slave, long ring_samples);
+int filter_spectrum_narrow_poll(struct filter_out *slave, int fft_avg, double overlap, float *bin_data);
+long filter_spectrum_narrow_ring(struct filter_out *slave, float complex *ring, long cap, long *ring_idx);
 
 /* housekeeping the reference exports from filter.c */
 void *run_fft(void *);

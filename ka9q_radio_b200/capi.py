@@ -114,6 +114,8 @@ def load() -> C.CDLL:
     L.kgpu_spectrum_create.argtypes = [i, i, i]
     L.kgpu_spectrum_set_window.argtypes = [vp, vp]
     L.kgpu_spectrum_run.argtypes = [vp, vp, l, l, i, f, i, i, i, d, vp, vp]
+    L.kgpu_spectrum_run_narrow.argtypes = [vp, vp, l, l, i, d, vp, vp, vp]
+    L.kgpu_spectrum_ring_append.argtypes = [vp, l, l, vp, l, vp]
     L.kgpu_spectrum_describe.argtypes = [vp, C.c_char_p, i]
     L.kgpu_spectrum_destroy.argtypes = [vp]
     L.kgpu_spectrum_plan.argtypes = [i, i, C.c_char_p, i]
@@ -349,8 +351,28 @@ def spectrum_plan(fft_n: int, in_type: int) -> tuple[int, str]:
     return check(load().kgpu_spectrum_plan(fft_n, in_type, buf, 256), "kgpu_spectrum_plan"), buf.value.decode()
 
 
+def spectrum_ring_append(ring, ring_idx: int, block, stream: int = 0) -> int:
+    """Append one delivered block (a float32 CUDA tensor of (re, im) pairs, or None for a block of zeros of `block`
+    samples when block is an int) to a device ring as spectrum.c:147-151 does; returns the new ring_idx."""
+    import torch
+
+    if not (ring.is_cuda and ring.is_contiguous() and ring.dtype == torch.float32 and ring.shape[-1] == 2):
+        raise ValueError("ring must be a contiguous float32 CUDA tensor of (re, im) pairs")
+    size = ring.numel() // 2
+    if isinstance(block, int):
+        src, n = None, block
+    else:
+        if not (block.is_cuda and block.is_contiguous() and block.dtype == torch.float32 and block.shape[-1] == 2):
+            raise ValueError("block must be a contiguous float32 CUDA tensor of (re, im) pairs")
+        src, n = block.data_ptr(), block.numel() // 2
+    check(load().kgpu_spectrum_ring_append(ring.data_ptr(), size, int(ring_idx), src, n, stream or None),
+          "kgpu_spectrum_ring_append")
+    return (int(ring_idx) + n) % size
+
+
 class Spectrum:
-    """wideband_poll's analysis (reference spectrum.c:354-497) on a device ring of raw samples."""
+    """wideband_poll's analysis (reference spectrum.c:354-497) on a device ring of raw samples; run_narrow is
+    narrowband_poll's (spectrum.c:206-306) on a ring of a COMPLEX channel's delivered blocks."""
 
     def __init__(self, fft_n: int, in_type: int, bin_count: int):
         self.lib = load()
@@ -392,6 +414,22 @@ class Spectrum:
         check(self.lib.kgpu_spectrum_run(self.h, ring.data_ptr(), samples, int(end), fmt, float(scale), int(derandomize),
                                          int(shift), int(fft_avg), float(overlap), bins.data_ptr(), stream or None),
               "kgpu_spectrum_run")
+
+    def run_narrow(self, ring, ring_idx: int, fft_avg: int, overlap: float, bins, stream: int = 0) -> int:
+        """narrowband_poll's analysis (reference spectrum.c:206-306) of a COMPLEX analyzer: ring is a contiguous float32
+        CUDA tensor of (re, im) pairs, the ring of delivered blocks; ring_idx the position its next sample would take.
+        Returns the fft_avg the poll used after the reference's clamp."""
+        import torch
+
+        if not (ring.is_cuda and ring.is_contiguous() and ring.dtype == torch.float32 and ring.shape[-1] == 2):
+            raise ValueError("ring must be a contiguous float32 CUDA tensor of (re, im) pairs")
+        if not (bins.is_cuda and bins.dtype == torch.float32 and bins.numel() >= self.bin_count):
+            raise ValueError(f"bins must be a float32 CUDA tensor of at least {self.bin_count} floats")
+        used = C.c_int(0)
+        check(self.lib.kgpu_spectrum_run_narrow(self.h, ring.data_ptr(), ring.numel() // 2, int(ring_idx), int(fft_avg),
+                                                float(overlap), bins.data_ptr(), C.byref(used), stream or None),
+              "kgpu_spectrum_run_narrow")
+        return used.value
 
     def close(self):
         if self.h:

@@ -54,6 +54,18 @@ struct slave_ctx {
   unsigned ft_ver; /* bumped whenever the oscillator parameters change */
   float last_power;
   double last_n0;
+  struct nb_spec *nb; /* narrowband analyzer (filter_spectrum_narrow_*), NULL for every other slave */
+};
+
+/* the narrowband analyzer of a COMPLEX slave (extension): a device ring of the blocks it was delivered, appended as
+ * spectrum.c:147-151 appends chan->baseband; every field is guarded by the master's c->mu */
+struct nb_spec {
+  kgpu_spectrum *ks;
+  int bin_count;
+  float complex *d_ring; /* NULL until the first filter_spectrum_narrow_reserve */
+  long ring_size, ring_idx;
+  float *d_bins, *h_bins;
+  cudaEvent_t ev;
 };
 
 struct snap { /* what the batched launch of one ring slot used for one slave */
@@ -210,6 +222,29 @@ static void spec_slave_drop(struct master_ctx *c, struct filter_out const *slave
       spec_slave_free(sp);
       return;
     }
+}
+
+static void nb_free(struct nb_spec *nb) {
+  if (!nb)
+    return;
+  kgpu_spectrum_destroy(nb->ks);
+  cudaFree(nb->d_ring);
+  cudaFree(nb->d_bins);
+  cudaFreeHost(nb->h_bins);
+  if (nb->ev)
+    cudaEventDestroy(nb->ev);
+  free(nb);
+}
+/* the block a slave with a narrowband analyzer was just delivered (device samples, or NULL for a lap's zeros) onto its
+ * ring, on stream st (caller holds c->mu) */
+static int nb_append(struct slave_ctx *sc, void const *d_src, int olen, cudaStream_t st) {
+  struct nb_spec *nb = sc->nb;
+  if (!nb || !nb->d_ring)
+    return 0;
+  if (kgpu_spectrum_ring_append(nb->d_ring, nb->ring_size, nb->ring_idx, d_src, olen, st) != 0)
+    return kgf_fail("narrowband spectrum ring append");
+  nb->ring_idx = (nb->ring_idx + olen) % nb->ring_size;
+  return 0;
 }
 
 static void master_teardown(struct filter_in *master) {
@@ -874,6 +909,14 @@ static int take_job(struct filter_out *slave, struct filter_in *master, unsigned
         own_output(slave, sc);
         memset(sc->own, 0, (slave->out_type == REAL ? sizeof(float) : sizeof(float complex)) * (size_t)slave->points);
       }
+      if (sc && sc->nb) {
+        struct master_ctx *c = (struct master_ctx *)master->fwd_plan;
+        pthread_mutex_lock(&c->mu);
+        int const rc = nb_append(sc, NULL, slave->olen, c->st);
+        pthread_mutex_unlock(&c->mu);
+        if (rc != 0)
+          return -1;
+      }
       return 1;
     }
   }
@@ -912,7 +955,12 @@ static int deliver(struct filter_out *slave, struct master_ctx *c, unsigned job,
     void const *src = c->h_out + (size_t)slot * (size_t)c->out_pitch + s->off;
     sc->last_power = c->h_pw[(size_t)slot * KGF_MAX_SLAVES + i];
     sc->last_n0 = c->h_n0[(size_t)slot * KGF_MAX_SLAVES + i];
+    /* the device row of h_out's copy, enqueued before the producer can issue job + ND into it (it issues under c->mu) */
+    if (sc->nb)
+      rc = nb_append(sc, c->d_out + (size_t)slot * (size_t)c->out_pitch + s->off, slave->olen, c->st);
     pthread_mutex_unlock(&c->mu);
+    if (rc != 0)
+      return rc;
     if (c->zero_copy) { /* the pinned row stays untouched until job + ND is issued */
       if (slave->out_type == REAL)
         slave->output.r = (float *)src;
@@ -935,6 +983,8 @@ static int deliver(struct filter_out *slave, struct master_ctx *c, unsigned job,
     rc = kgf_fail("execute_filter_output: scratch allocation");
   else if (kgpu_bank_run_one_ex(c->bank, i, spec, c->d_one, c->d_one_pw, c->st_one) != 0)
     rc = kgf_fail("execute_filter_output: kgpu_bank_run_one");
+  else if (nb_append(sc, c->d_one, slave->olen, c->st_one) != 0) /* d_one is reused by the next recompute */
+    rc = -1;
   else if (cudaMemcpyAsync(c->h_one, c->d_one, obytes, cudaMemcpyDeviceToHost, c->st_one) != cudaSuccess ||
            cudaMemcpyAsync(c->h_one_pw, c->d_one_pw, sizeof(float), cudaMemcpyDeviceToHost, c->st_one) != cudaSuccess ||
            cudaStreamSynchronize(c->st_one) != cudaSuccess)
@@ -1221,6 +1271,130 @@ int filter_spectrum_poll(struct filter_out *slave, int shift, int fft_avg, doubl
   return 0;
 }
 
+/* ---------------------------------------------------------------- narrowband spectrum ------ */
+/* EXTENSION: narrowband_poll (spectrum.c:206-306) on the device for a COMPLEX slave.  fft_n floats of window, as
+ * generate_window() leaves them.  -1 (and the CPU loop stays with the caller) when the device cannot serve the slave. */
+int filter_spectrum_narrow_setup(struct filter_out *slave, int fft_n, int bin_count, float const *window) {
+  if (slave == NULL || slave->out_type != COMPLEX || slave->rev_plan == NULL || slave->master == NULL ||
+      slave->master->fwd_plan == NULL || window == NULL || bin_count < 1 || bin_count > fft_n)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
+  struct slave_ctx *sc = (struct slave_ctx *)slave->rev_plan;
+  struct nb_spec *nb = calloc(1, sizeof *nb);
+  if (!nb)
+    return -1;
+  nb->bin_count = bin_count;
+  nb->ks = kgpu_spectrum_create(fft_n, KGPU_COMPLEX, bin_count);
+  if (!nb->ks) {
+    fprintf(stderr, "filter_spectrum_narrow_setup(fft_n=%d): %s\n", fft_n, kgpu_last_error());
+    free(nb);
+    return -1;
+  }
+  bool ok = kgpu_spectrum_set_window(nb->ks, window) == 0;
+  ok = ok && cudaMalloc((void **)&nb->d_bins, sizeof(float) * (size_t)bin_count) == cudaSuccess;
+  ok = ok && cudaHostAlloc((void **)&nb->h_bins, sizeof(float) * (size_t)bin_count, cudaHostAllocPortable) == cudaSuccess;
+  ok = ok && cudaEventCreateWithFlags(&nb->ev, cudaEventDisableTiming) == cudaSuccess;
+  if (!ok) {
+    nb_free(nb);
+    return kgf_fail("filter_spectrum_narrow_setup");
+  }
+  pthread_mutex_lock(&c->mu);
+  struct nb_spec *old = sc->nb;
+  if (old) {
+    cudaStreamSynchronize(c->st);
+    nb_free(old);
+  }
+  sc->nb = nb;
+  pthread_mutex_unlock(&c->mu);
+  return 0;
+}
+
+/* EXTENSION: the ring of spectrum.c:124-145 before a block is appended: the first call creates ring_samples zeros with
+ * the write index at 0; a larger size keeps [0, old size), zeroes the rest and leaves the index; a smaller one does
+ * nothing.  Call it where demod_spectrum would grow its ring, before downconvert() delivers the block. */
+int filter_spectrum_narrow_reserve(struct filter_out *slave, long ring_samples) {
+  if (slave == NULL || slave->rev_plan == NULL || slave->master == NULL || slave->master->fwd_plan == NULL ||
+      ring_samples < 1)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
+  struct nb_spec *nb = ((struct slave_ctx *)slave->rev_plan)->nb;
+  if (nb == NULL)
+    return -1;
+  int rc = 0;
+  pthread_mutex_lock(&c->mu);
+  if (nb->d_ring == NULL || ring_samples > nb->ring_size) {
+    float complex *ring = NULL;
+    size_t const old = nb->d_ring ? sizeof(float complex) * (size_t)nb->ring_size : 0;
+    cudaStreamSynchronize(c->st); /* pending appends and polls read the old ring */
+    if (cudaMalloc((void **)&ring, sizeof(float complex) * (size_t)ring_samples) != cudaSuccess ||
+        cudaMemsetAsync((char *)ring + old, 0, sizeof(float complex) * (size_t)ring_samples - old, c->st) != cudaSuccess ||
+        (old && cudaMemcpyAsync(ring, nb->d_ring, old, cudaMemcpyDeviceToDevice, c->st) != cudaSuccess) ||
+        cudaStreamSynchronize(c->st) != cudaSuccess) {
+      cudaFree(ring);
+      rc = kgf_fail("filter_spectrum_narrow_reserve");
+    } else {
+      cudaFree(nb->d_ring);
+      nb->d_ring = ring;
+      nb->ring_size = ring_samples;
+    }
+  }
+  pthread_mutex_unlock(&c->mu);
+  return rc;
+}
+
+/* EXTENSION: one narrowband_poll of the slave's ring as its delivered blocks have left it: bin_count floats into
+ * bin_data, as narrowband_poll leaves them before its base / step scaling (spectrum.c:284-305), which stays with the
+ * caller.  -1 before the first reserve.  One poller per slave. */
+int filter_spectrum_narrow_poll(struct filter_out *slave, int fft_avg, double overlap, float *bin_data) {
+  if (slave == NULL || slave->rev_plan == NULL || slave->master == NULL || slave->master->fwd_plan == NULL ||
+      bin_data == NULL)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
+  struct slave_ctx *sc = (struct slave_ctx *)slave->rev_plan;
+  pthread_mutex_lock(&c->mu);
+  struct nb_spec *nb = sc->nb;
+  int rc = nb && nb->d_ring ? 0 : -1;
+  if (rc == 0 && kgpu_spectrum_run_narrow(nb->ks, nb->d_ring, nb->ring_size, nb->ring_idx, fft_avg, overlap, nb->d_bins,
+                                          NULL, c->st) != 0)
+    rc = kgf_fail("filter_spectrum_narrow_poll: kgpu_spectrum_run_narrow");
+  if (rc == 0 && (cudaMemcpyAsync(nb->h_bins, nb->d_bins, sizeof(float) * (size_t)nb->bin_count, cudaMemcpyDeviceToHost,
+                                  c->st) != cudaSuccess ||
+                  cudaEventRecord(nb->ev, c->st) != cudaSuccess))
+    rc = kgf_fail("filter_spectrum_narrow_poll: D2H of the bins");
+  pthread_mutex_unlock(&c->mu);
+  if (rc == 0 && cudaEventSynchronize(nb->ev) != cudaSuccess)
+    rc = kgf_fail("filter_spectrum_narrow_poll: wait");
+  if (rc != 0)
+    return -1;
+  memcpy(bin_data, nb->h_bins, sizeof(float) * (size_t)nb->bin_count);
+  return 0;
+}
+
+/* EXTENSION: a host copy of the slave's ring (up to cap samples) with its size and write index, e.g. for a caller that
+ * hands the analysis back to its CPU loop.  Returns the ring size, 0 before the first reserve, -1 on error. */
+long filter_spectrum_narrow_ring(struct filter_out *slave, float complex *ring, long cap, long *ring_idx) {
+  if (slave == NULL || slave->rev_plan == NULL || slave->master == NULL || slave->master->fwd_plan == NULL)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
+  struct nb_spec *nb = ((struct slave_ctx *)slave->rev_plan)->nb;
+  if (nb == NULL)
+    return -1;
+  long rc = 0;
+  pthread_mutex_lock(&c->mu);
+  if (nb->d_ring) {
+    rc = nb->ring_size;
+    if (ring_idx)
+      *ring_idx = nb->ring_idx;
+    long const n = cap < nb->ring_size ? cap : nb->ring_size;
+    if (ring && n > 0 &&
+        (cudaMemcpyAsync(ring, nb->d_ring, sizeof(float complex) * (size_t)n, cudaMemcpyDeviceToHost, c->st) != cudaSuccess ||
+         cudaStreamSynchronize(c->st) != cudaSuccess))
+      rc = kgf_fail("filter_spectrum_narrow_ring");
+  }
+  pthread_mutex_unlock(&c->mu);
+  return rc;
+}
+
 /* ---------------------------------------------------------------- delete -------------------- */
 int delete_filter_output(struct filter_out *slave) { /* filter.c:943-957 */
   if (slave == NULL)
@@ -1242,10 +1416,14 @@ int delete_filter_output(struct filter_out *slave) { /* filter.c:943-957 */
     c->ranges_dirty = true;
     for (int s = 0; s < ND; s++)
       c->snap[s][sc->idx].ok = false;
+    nb_free(sc->nb); /* after the synchronise above: no append or poll still reads it */
+    sc->nb = NULL;
     pthread_mutex_unlock(&c->mu);
   }
-  if (sc)
+  if (sc) {
+    nb_free(sc->nb); /* the master was deleted first */
     free(sc->own);
+  }
   free(sc);
   if (slave->init)
     pthread_mutex_destroy(&slave->response_mutex);

@@ -2437,6 +2437,31 @@ extern "C" int kgpu_spectrum_describe(kgpu_spectrum const *s, char *buf, int buf
   return 0;
 }
 
+// One poll in chunks of at most s->chunk segments: window, transform, then the wideband or narrowband bin mapping.  The
+// bins carry over from chunk to chunk, so they accumulate in the reference's segment order.
+static int spectrum_chunks(kgpu_spectrum *s, SpecWindowArgs w, SpecPowerArgs p, int fft_avg, bool narrow, cudaStream_t st) {
+  for (int seg0 = 0; seg0 < fft_avg; seg0 += s->chunk) {
+    int const nseg = std::min(s->chunk, fft_avg - seg0);
+    w.seg0 = seg0;
+    spectrum_window_kernel<<<dim3((unsigned)((s->in_len + kSpecThreads - 1) / kSpecThreads), (unsigned)nseg), kSpecThreads, 0,
+                             st>>>(w);
+    g_launches++;
+    if (s->pl.path == SP_BLUESTEIN ? bluestein_conv(s->m, s->pl.blue, (float2 *)s->d_in, nseg, s->d_spec, st)
+                                   : kgpu_forward(s->m, s->d_in, KGPU_FMT_F32, 1.0f, 0, nseg, s->d_spec, nullptr, st))
+      return -1;
+    p.nseg = nseg;
+    p.first = seg0 == 0;
+    unsigned const grid = (unsigned)((s->bin_count + kSpecThreads - 1) / kSpecThreads);
+    if (narrow)
+      narrowband_power_kernel<<<grid, kSpecThreads, 0, st>>>(p);
+    else
+      spectrum_power_kernel<<<grid, kSpecThreads, 0, st>>>(p);
+    g_launches++;
+  }
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 extern "C" int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring_samples, long end, int fmt, float scale,
                                  int derandomize, int shift, int fft_avg, double overlap, float *d_bins, void *stream) {
   if (!s || !d_ring || !d_bins || fft_avg < 1 || !(overlap >= 0.0 && overlap < 1.0) ||
@@ -2477,20 +2502,62 @@ extern "C" int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring
   p.norm = s->pl.path == SP_BLUESTEIN ? 1.0 / ((double)s->pl.blue.P * (double)s->pl.blue.P) : 1.0;
   p.gain = (real ? 2. : 1.) / (double)((int64_t)fft_avg * fft_n * fft_n);  // spectrum.c:373, :431
   p.bins = d_bins;
-  for (int seg0 = 0; seg0 < fft_avg; seg0 += s->chunk) {
-    int const nseg = std::min(s->chunk, fft_avg - seg0);
-    w.seg0 = seg0;
-    spectrum_window_kernel<<<dim3((unsigned)((s->in_len + kSpecThreads - 1) / kSpecThreads), (unsigned)nseg), kSpecThreads, 0,
-                             st>>>(w);
-    g_launches++;
-    if (s->pl.path == SP_BLUESTEIN ? bluestein_conv(s->m, s->pl.blue, (float2 *)s->d_in, nseg, s->d_spec, st)
-                                   : kgpu_forward(s->m, s->d_in, KGPU_FMT_F32, 1.0f, 0, nseg, s->d_spec, nullptr, st))
-      return -1;
-    p.nseg = nseg;
-    p.first = seg0 == 0;
-    spectrum_power_kernel<<<(unsigned)((s->bin_count + kSpecThreads - 1) / kSpecThreads), kSpecThreads, 0, st>>>(p);
-    g_launches++;
-  }
+  return spectrum_chunks(s, w, p, fft_avg, false, st);
+}
+
+extern "C" int kgpu_spectrum_run_narrow(kgpu_spectrum *s, const void *d_ring, long ring_size, long ring_idx, int fft_avg,
+                                        double overlap, float *d_bins, int *fft_avg_used, void *stream) {
+  if (!s || s->in_type != KGPU_COMPLEX || !d_ring || !d_bins || fft_avg < 1 || !(overlap >= 0.0 && overlap < 1.0))
+    return fail("kgpu_spectrum_run_narrow: bad arguments");
+  int const fft_n = s->fft_n;
+  if (s->bin_count > fft_n) return fail("kgpu_spectrum_run_narrow: bin_count %d > fft_n %d", s->bin_count, fft_n);
+  if (ring_size < fft_n) return fail("kgpu_spectrum_run_narrow: a ring of %ld samples is shorter than fft_n=%d", ring_size, fft_n);
+  if (ring_idx < 0 || ring_idx >= ring_size) return fail("kgpu_spectrum_run_narrow: ring_idx %ld outside the ring", ring_idx);
+  // spectrum.c:244-249, :278: the clamp with an integer ring_size / fft_n, the start, and the hop as the walk takes it
+  // (fft_n forward, then lrint(fft_n overlap) back)
+  double const avg_limit = floor(1 + ((ring_size / fft_n) - 1) / (1 - overlap));
+  int const avg = fft_avg > avg_limit ? (int)lrint(avg_limit) : fft_avg;
+  long rp = ring_idx - lrint(fft_n * (1 + (avg - 1) * (1 - overlap)));
+  if (rp < 0) rp += ring_size;
+  if (fft_avg_used) *fft_avg_used = avg;
+  SpecWindowArgs w;
+  w.ring = d_ring;
+  w.cap = ring_size;
+  w.start0 = ((rp % ring_size) + ring_size) % ring_size;
+  w.step = fft_n - lrint(fft_n * overlap);
+  w.fft_n = fft_n;
+  w.out_len = (int)s->in_len;
+  w.complex_in = 1;
+  w.i16 = 0;
+  w.derandomize = 0;
+  w.flip = 0;
+  w.complex_out = 1;
+  w.chirp = s->pl.path == SP_BLUESTEIN;
+  w.scale = 1.0f;
+  w.window = s->d_window;
+  w.out = s->d_in;
+  SpecPowerArgs p;
+  p.spec = s->d_spec;
+  p.spec_stride = s->spec_stride;
+  p.real_walk = 0;
+  p.fft_n = fft_n;
+  p.shift = 0;
+  p.bin_count = s->bin_count;
+  p.norm = s->pl.path == SP_BLUESTEIN ? 1.0 / ((double)s->pl.blue.P * (double)s->pl.blue.P) : 1.0;
+  p.gain = 1.0 / ((double)fft_n * fft_n * avg);  // spectrum.c:255
+  p.bins = d_bins;
+  return spectrum_chunks(s, w, p, avg, true, (cudaStream_t)stream);
+}
+
+extern "C" int kgpu_spectrum_ring_append(void *d_ring, long ring_size, long ring_idx, const void *d_src, long olen,
+                                         void *stream) {
+  if (!d_ring || ring_size < 1 || ring_idx < 0 || ring_idx >= ring_size || olen < 0)
+    return fail("kgpu_spectrum_ring_append: bad arguments");
+  long const n = std::min(olen, ring_size);
+  if (n == 0) return 0;
+  nb_ring_append_kernel<<<(unsigned)((n + kSpecThreads - 1) / kSpecThreads), kSpecThreads, 0, (cudaStream_t)stream>>>(
+      (float2 *)d_ring, ring_size, ring_idx, (float2 const *)d_src, olen);
+  g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
 }

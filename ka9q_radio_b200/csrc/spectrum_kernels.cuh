@@ -5,6 +5,8 @@
 //   bluestein_mul_kernel     Bluestein only: conj(A * B), B the stored transform of the conjugate chirp; second pass
 //                            (bluestein_master.cuh)
 //   spectrum_power_kernel    one thread per output bin: index mapping, bin += gain * |X|^2 over the chunk's segments
+// The narrowband analyzer (narrowband_poll, spectrum.c:206-306) runs the same chain on a ring of a COMPLEX slave's
+// delivered blocks (nb_ring_append_kernel), with narrowband_power_kernel's bin mapping in place of the last step.
 // Bluestein: X_k = w_k sum_n (x_n w_n) conj(w_{k-n}) with w_n = exp(-i pi n^2 / fft_n), so with a = x w zero-padded to P,
 // y = DFT_P(conj(DFT_P(a) B)) = P conj(conv(a, conj w)) and |X_k|^2 = |y_k|^2 / P^2 (|w_k| = 1: no post-chirp).
 #pragma once
@@ -114,11 +116,12 @@ __device__ __forceinline__ long spec_source(SpecPowerArgs const &a, int i) {
   return b >= 0 ? b : b + a.fft_n;
 }
 
-__global__ void __launch_bounds__(kSpecThreads) spectrum_power_kernel(SpecPowerArgs a) {
-  int const i = blockIdx.x * kSpecThreads + threadIdx.x;
-  if (i >= a.bin_count) return;
+// bins[i] += gain * |X[src]|^2 over the chunk's segments in order, in double and stored as float after every segment;
+// src = Source(a, i), -1 for a bin that gets nothing
+template <long (*Source)(SpecPowerArgs const &, int)>
+__device__ __forceinline__ void spec_accumulate(SpecPowerArgs const &a, int i) {
   float acc = a.first ? 0.f : a.bins[i];
-  long const src = spec_source(a, i);
+  long const src = Source(a, i);
   if (src >= 0)
     for (int s = 0; s < a.nseg; s++) {
       float2 const v = a.spec[(long)s * a.spec_stride + src];
@@ -126,6 +129,40 @@ __global__ void __launch_bounds__(kSpecThreads) spectrum_power_kernel(SpecPowerA
       if (isfinite(p)) acc = (float)__dadd_rn((double)acc, __dmul_rn(a.gain, p));
     }
   a.bins[i] = acc;
+}
+
+__global__ void __launch_bounds__(kSpecThreads) spectrum_power_kernel(SpecPowerArgs a) {
+  int const i = blockIdx.x * kSpecThreads + threadIdx.x;
+  if (i >= a.bin_count) return;
+  spec_accumulate<spec_source>(a, i);
+}
+
+// ---- the narrowband analyzer (narrowband_poll, reference spectrum.c:206-306) ------------------------------------------
+// Its segments are spectrum_window_kernel's COMPLEX float walk with a forward step; only the bin mapping differs.
+// narrowband_poll's bin mapping (spectrum.c:267-271): bin i < bin_count/2 reads X[i], bin i >= bin_count/2 reads
+// X[fft_n - 2 (bin_count/2) + i].  With an odd bin_count the last bin would read X[fft_n], past the transform: 0 here.
+// shift and real_walk of the arguments are unused.
+__device__ __forceinline__ long nb_source(SpecPowerArgs const &a, int i) {
+  int const half = a.bin_count / 2;
+  long const src = i < half ? (long)i : (long)a.fft_n - 2L * half + i;
+  return src < a.fft_n ? src : -1;
+}
+
+__global__ void __launch_bounds__(kSpecThreads) narrowband_power_kernel(SpecPowerArgs a) {
+  int const i = blockIdx.x * kSpecThreads + threadIdx.x;
+  if (i >= a.bin_count) return;
+  spec_accumulate<nb_source>(a, i);
+}
+
+// One delivered block of olen samples (src, or zeros when src is NULL: a lapped slave's block) into a ring of ring_size
+// samples from position ring_idx on, wrapping (spectrum.c:147-151).  When the block is longer than the ring only its last
+// ring_size samples survive the sample-by-sample loop, so only they are written.
+__global__ void __launch_bounds__(kSpecThreads) nb_ring_append_kernel(float2 *ring, long ring_size, long ring_idx,
+                                                                      float2 const *src, long olen) {
+  long const first = olen > ring_size ? olen - ring_size : 0;
+  long const i = first + (long)blockIdx.x * kSpecThreads + threadIdx.x;
+  if (i >= olen) return;
+  ring[(ring_idx + i) % ring_size] = src ? src[i] : make_float2(0.f, 0.f);
 }
 
 }  // namespace kfft
