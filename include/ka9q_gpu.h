@@ -106,6 +106,32 @@ int kgpu_forward(kgpu_master *m, const void *d_in, int fmt, float scale, int der
  * d_stats: NULL or ONE kgpu_ingest_stats receiving the energy and the clip count (x == 2047 || x <= -2047). */
 int kgpu_unpack_airspy12(const void *d_packed, long sampcount, void *d_i16, void *d_stats, void *stream);
 
+/* 8-bit sample words of kgpu_unpack8.  Kept apart from kgpu_format: kgpu_forward does not read them. */
+enum kgpu_raw8 {
+  KGPU_RAW_U8 = 1, /* excess-128 bytes: RTL-SDR (rtlsdr.c:316-343), HydraSDR UINT8_REAL / UINT8_IQ (hydrasdr.c:759-775, :793-811) */
+  KGPU_RAW_S8 = 2  /* signed bytes: HydraSDR INT8_REAL / INT8_IQ (hydrasdr.c:776-791, :812-830) */
+};
+/* A/D statistics of one block's L new samples (never its M-1 history samples).  A sample is one value (REAL) or one I/Q
+ * pair (COMPLEX). */
+struct kgpu_block_stats {
+  unsigned long long energy; /* sum of x*x over every component */
+  unsigned int overs;        /* components at the format's limits */
+  unsigned int over_samples; /* samples with at least one component at the limits */
+};
+/* 8-bit ingest (replaces the conversion loops cited at kgpu_raw8): the bytes of an overlap-save launch -- `history`
+ * samples, then nblocks blocks of L new samples, laid out as kgpu_forward's d_in -- to floats at d_out (4-byte aligned),
+ * each (float)(scale * (double)x) with x = byte - 128 (U8) or the signed byte (S8), bitwise what the drivers' loops
+ * store; then kgpu_forward(..., KGPU_FMT_F32, ...) reads d_out.  d_stats: NULL or nblocks kgpu_block_stats, zeroed by the
+ * call; at the limits: x >= 127 or x <= -128.  nblocks may be 0 (conversion only: history samples). */
+int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, int nblocks, double scale, void *d_out,
+                 void *d_stats, void *stream);
+/* Per-block statistics of int16 words on the device, laid out as kgpu_forward's KGPU_FMT_I16 d_in (history samples, then
+ * nblocks blocks of L): the RX888's words after the optional derandomization (rx888.c:707-712, 759-762; limit 32767, i.e.
+ * x > 32766 or x < -32766), or kgpu_unpack_airspy12's output (airspy-unpack.c:121-124; limit 2047).  A component is at the
+ * limits when |x| >= limit.  d_stats: nblocks kgpu_block_stats, zeroed by the call. */
+int kgpu_block_stats_i16(const void *d_in, int in_type, long history, long L, int nblocks, int derandomize, int limit,
+                         void *d_stats, void *stream);
+
 /* Notch EWMA on listed bins (apply_notch_filters, filter.c:464-474); list ends with bin 0. The state
  * lives in the master; blocks are processed in order. */
 int kgpu_master_set_notches(kgpu_master *m, int const *bins, double const *alpha, int n);

@@ -17,6 +17,9 @@
  *   delete_filter_input/output    filter.c:930-957
  *   write_i16filter               (EXTENSION, not in the reference) raw int16 ingest: fuses
  *                                 rx888.c:753-767 convert() into the first FFT pass
+ *   write_rawfilter               (EXTENSION) raw 8-bit and packed 12-bit ingest: the conversion loops of rtlsdr.c,
+ *                                 hydrasdr.c and airspy-unpack.c on the device
+ *   filter_ingest_stats           (EXTENSION) the A/D energy and overranges those loops return, per drained block
  *
  * Semantics kept: return 0 / -1 (write_*: 1 if a block fired), ND-deep spectrum ring with
  * lap -> zeros + block_drops++ (filter.c:690-701), owner-thread shortcut (filter.c:681-683),
@@ -127,6 +130,35 @@ int write_i16filter(struct filter_in *master, int16_t const *samples, int n, flo
 /* Where a driver may deposit the next raw samples itself (pinned, mirrored ring: a block's worth stays contiguous),
  * e.g. as the libusb transfer buffer of rx888.c:797-826; publish with write_i16filter(master, NULL, n, scale, derand). */
 int16_t *filter_i16_write_pointer(struct filter_in *master);
+/* EXTENSION: raw 8-bit and packed 12-bit ADC words, unpacked on the device (airspy-unpack.c:105-129 for Airspy R2 and
+ * HydraSDR RAW; rtlsdr.c:316-343 and hydrasdr.c:759-830 for the 8-bit formats).  n samples (REAL master) or I/Q pairs
+ * (COMPLEX master) are copied into a pinned, mirrored ring of their own and fire blocks as write_i16filter does; each
+ * launch sends the raw bytes of its windows to the device, unpacks them there, then runs the usual forward, notch,
+ * channel and noise work.  U8 and S8 give floats bitwise equal to the drivers' (float)(scale * x) with a double scale;
+ * PACKED12 (REAL masters only) gives (float)scale * (float)x, the drivers' float scale.  scale applies from the next
+ * launch on, to that launch's whole window.  PACKED12 needs n a multiple of 8 (whole groups of three 32-bit words), and
+ * L and M - 1 multiples of 8 so every window starts on a group boundary (Airspy R2: L = 400000 / 200000, M - 1 = L/4);
+ * other geometries are rejected with -1 and a message at the first write.  A master fed one format (raw, int16 or
+ * float) rejects writes in another with -1.  Returns -1 on error, 1 if a block fired, else 0. */
+enum filter_raw_format { FILTER_RAW_PACKED12 = 1, FILTER_RAW_U8 = 2, FILTER_RAW_S8 = 3 };
+int write_rawfilter(struct filter_in *master, void const *samples, int n, int format, double scale);
+/* Pure host code: the byte size of the raw ring write_rawfilter allocates for a master of this geometry and format (a
+ * whole number of pages, and for PACKED12 of 12-byte groups, holding at least the master's float ring of samples), or -1
+ * where write_rawfilter would reject the geometry. */
+long filter_raw_ring_bytes(int L, int M, enum filtertype in_type, int format);
+/* EXTENSION: the A/D statistics the drivers' conversion loops return (in_energy, overranges, samp_since_over), for masters
+ * fed through write_rawfilter or write_i16filter.  Never blocks: sums over the blocks whose device work completed since
+ * the previous call, each block counted once however rarely the caller asks.  Collection starts with the first call on
+ * a master, which returns zeros; a master never asked launches nothing extra.  -1 for a master fed floats. */
+struct filter_ingest_stats {
+  uint64_t blocks;            /* blocks summed by this call */
+  uint64_t samples;           /* their new samples (blocks * L): samples (REAL) or I/Q pairs (COMPLEX) */
+  uint64_t energy;            /* sum of x * x over every component of those samples */
+  uint64_t overranges;        /* components at the format's limits */
+  uint64_t overrange_samples; /* samples with at least one component at the limits */
+  uint64_t since_over;        /* samples after the last summed block that had an overrange (over all calls) */
+};
+int filter_ingest_stats(struct filter_in *master, struct filter_ingest_stats *stats);
 /* EXTENSION: serve many slaves with one call (what 1024 channel threads would each do): one wait per block. */
 int execute_filter_output_batch(struct filter_out *const *slaves, int const *shifts, int n);
 /* EXTENSION (downconvert()'s per-sample work, radio.c:1476-1501 and :1515-1520, on the device): execute_filter_output

@@ -16,6 +16,7 @@ LIB_PATH = PKG / "libka9qgpu.so"
 
 KGPU_COMPLEX, KGPU_REAL = 1, 2
 KGPU_FMT_F32, KGPU_FMT_I16 = 0, 1
+KGPU_RAW_U8, KGPU_RAW_S8 = 1, 2   # kgpu_unpack8's formats, apart from kgpu_format
 KGPU_CHAN_ISB = 1
 KGPU_CHAN_BEAM = 4
 
@@ -82,6 +83,8 @@ def load() -> C.CDLL:
     L.kgpu_bank_run_one.argtypes = [vp, i, vp, vp, vp]
     L.kgpu_bank_commit.argtypes = [vp, vp]
     L.kgpu_unpack_airspy12.argtypes = [vp, l, vp, vp, vp]
+    L.kgpu_unpack8.argtypes = [vp, i, i, l, l, i, d, vp, vp, vp]
+    L.kgpu_block_stats_i16.argtypes = [vp, i, l, l, i, i, i, vp, vp]
     L.kgpu_bank_define_ex.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_wide.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_huge.argtypes = [vp, i, i, i]
@@ -165,6 +168,23 @@ def check(rc: int, what: str = "") -> int:
     if rc < 0:
         raise KgpuError(f"{what}: {load().kgpu_last_error().decode()}")
     return rc
+
+
+def unpack8(d_raw: int, fmt: int, in_type: int, history: int, L: int, nblocks: int, scale: float, d_out: int,
+            d_stats: int = 0, stream: int = 0) -> None:
+    """8-bit ingest (kgpu_unpack8): the u8 / s8 bytes of `history` samples then nblocks blocks of L to float32 at d_out,
+    each (float)(scale * (double)x); d_stats: 0 or nblocks kgpu_block_stats (uint64 energy, uint32 overs, uint32
+    over_samples)."""
+    check(load().kgpu_unpack8(d_raw, fmt, in_type, history, L, nblocks, scale, d_out, d_stats or None, stream or None),
+          "kgpu_unpack8")
+
+
+def block_stats_i16(d_in: int, in_type: int, history: int, L: int, nblocks: int, d_stats: int, derandomize: bool = False,
+                    limit: int = 32767, stream: int = 0) -> None:
+    """Per-block statistics of int16 words on the device (kgpu_block_stats_i16): limit 32767 for the RX888's words,
+    2047 for unpacked packed-12 values."""
+    check(load().kgpu_block_stats_i16(d_in, in_type, history, L, nblocks, int(derandomize), limit, d_stats, stream or None),
+          "kgpu_block_stats_i16")
 
 
 MASTER_DIRECT, MASTER_EXTENDED, MASTER_BLUESTEIN = 0, 1, 2

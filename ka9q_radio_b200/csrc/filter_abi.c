@@ -129,6 +129,19 @@ struct master_ctx {
   char *i16_wp, *i16_rp;
   float i16_scale;
   bool i16_derand;
+  /* raw 8-bit / packed 12-bit ingest (extension): the bytes in a mirrored ring of their own, unpacked on the device from
+   * d_raw into d_win[slot] */
+  int raw_fmt; /* 0, or the enum filter_raw_format the master is fed */
+  void *raw_ring;
+  size_t raw_ring_size;
+  char *raw_wp, *raw_rp;
+  double raw_scale;
+  void *d_raw;
+  /* A/D statistics (filter_ingest_stats): one kgpu_block_stats per ring slot, folded in job order into `acc` */
+  bool stats_on;
+  struct kgpu_block_stats *d_bstats, *h_bstats;
+  unsigned long long folded; /* blocks folded (or, before stats_on, skipped) so far */
+  struct filter_ingest_stats acc;
   unsigned long long issued; /* blocks issued to the device so far */
   /* wideband spectrum analyzer (extension): a device copy of the input ring, in the ingest format, with the host float
    * ring's capacity and positions; created by the first filter_spectrum_setup, then appended by every launch */
@@ -276,6 +289,10 @@ static void master_teardown(struct filter_in *master) {
     cudaStreamDestroy(c->st_d2h);
     cudaEventDestroy(c->kev);
     ring_free(c->i16_ring, c->i16_ring_size);
+    ring_free(c->raw_ring, c->raw_ring_size);
+    cudaFree(c->d_raw);
+    cudaFree(c->d_bstats);
+    cudaFreeHost(c->h_bstats);
     while (c->specs) {
       struct spec_slave *sp = c->specs;
       c->specs = sp->next;
@@ -615,6 +632,95 @@ static void rebuild_ranges(struct filter_in *f, struct master_ctx *c) {
   }
 }
 
+/* ---------------------------------------------------------------- raw ingest ---------------- */
+/* bytes of n samples (REAL) or I/Q pairs (COMPLEX) in a raw format; a packed-12 n is a multiple of 8 (three words) */
+static size_t raw_bytes(int fmt, bool cplx, size_t n) { return fmt == FILTER_RAW_PACKED12 ? n / 8 * 12 : n * (cplx ? 2 : 1); }
+static long raw_samples(int fmt, bool cplx, size_t bytes) {
+  return (long)(fmt == FILTER_RAW_PACKED12 ? bytes / 12 * 8 : bytes / (cplx ? 2 : 1));
+}
+/* the device window holds int16 words (int16 ingest, or packed-12 after the unpack) rather than floats */
+static bool ingest_i16(struct master_ctx const *c) { return c->i16_mode || c->raw_fmt == FILTER_RAW_PACKED12; }
+
+long filter_raw_ring_bytes(int L, int M, enum filtertype in_type, int format) {
+  if (L <= 0 || M <= 0 || (in_type != REAL && in_type != COMPLEX))
+    return -1;
+  bool const cplx = in_type == COMPLEX;
+  size_t unit = page_round(1);
+  if (format == FILTER_RAW_PACKED12) { /* whole groups, so a group never straddles the end of the ring */
+    if (cplx || L % 8 != 0 || (M - 1) % 8 != 0)
+      return -1;
+    unit = unit / (size_t)gcd((long)unit, 12) * 12;
+  } else if (format != FILTER_RAW_U8 && format != FILTER_RAW_S8)
+    return -1;
+  size_t const fsz = cplx ? sizeof(float complex) : sizeof(float);
+  size_t const samples = page_round((size_t)ND * (size_t)(L + M - 1) * fsz) / fsz; /* the float ring's capacity */
+  size_t const need = raw_bytes(format, cplx, (samples + 7) / 8 * 8);
+  return (long)((need + unit - 1) / unit * unit);
+}
+
+/* the first write_rawfilter on a master: its ring, prefilled with the format's zero so the M-1 history samples (and
+ * whatever the wideband analyzer's seeding reads before the stream reaches it) are 0.0 as in the float ring */
+static int raw_start(struct filter_in *f, struct master_ctx *c, int format) {
+  long const size = filter_raw_ring_bytes(f->ilen, f->impulse_length, f->in_type, format);
+  if (size < 0) {
+    fprintf(stderr, "write_rawfilter(L=%d M=%d): format %d cannot feed this master%s\n", f->ilen, f->impulse_length, format,
+            format == FILTER_RAW_PACKED12 ? " (packed 12-bit needs a REAL master with L and M-1 multiples of 8)" : "");
+    return -1;
+  }
+  if (c->i16_mode || f->wcnt != 0 || c->issued != 0) {
+    fprintf(stderr, "write_rawfilter: the master is already fed int16 or float samples\n");
+    return -1;
+  }
+  bool const cplx = f->in_type == COMPLEX;
+  c->raw_ring = ring_alloc((size_t)size);
+  if (!c->raw_ring)
+    return -1;
+  c->raw_ring_size = (size_t)size;
+  if (format == FILTER_RAW_U8)
+    memset(c->raw_ring, 128, c->raw_ring_size);
+  else if (format == FILTER_RAW_PACKED12) { /* eight offset-binary 2048s per three words (airspy-unpack.c:110-117) */
+    uint32_t const g[3] = {0x80080080u, 0x08008008u, 0x00800800u};
+    for (size_t o = 0; o < c->raw_ring_size; o += sizeof g)
+      memcpy((char *)c->raw_ring + o, g, sizeof g);
+  }
+  size_t const span = (size_t)(ND - 2) * (size_t)f->ilen + (size_t)f->points;
+  if (cudaMalloc(&c->d_raw, raw_bytes(format, cplx, span)) != cudaSuccess) {
+    c->d_raw = NULL;
+    ring_free(c->raw_ring, c->raw_ring_size);
+    c->raw_ring = NULL;
+    return kgf_fail("write_rawfilter: device buffer");
+  }
+  c->raw_rp = c->raw_ring;
+  c->raw_wp = c->raw_rp + raw_bytes(format, cplx, (size_t)(f->impulse_length - 1));
+  c->raw_fmt = format;
+  return 0;
+}
+
+/* raw bytes on the device (history samples, then nblocks blocks of L) -> the master's device samples at d_dst: floats for
+ * the 8-bit formats, int16 for packed-12, which kgpu_forward then scales.  d_stats: NULL or nblocks block statistics. */
+static int raw_unpack(struct filter_in const *f, struct master_ctx const *c, void const *d_src, long history, int nblocks,
+                      void *d_dst, void *d_stats, cudaStream_t st) {
+  int const type = f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL;
+  if (c->raw_fmt != FILTER_RAW_PACKED12)
+    return kgpu_unpack8(d_src, c->raw_fmt == FILTER_RAW_U8 ? KGPU_RAW_U8 : KGPU_RAW_S8, type, history, f->ilen, nblocks,
+                        c->raw_scale, d_dst, d_stats, st);
+  if (kgpu_unpack_airspy12(d_src, history + (long)nblocks * f->ilen, d_dst, NULL, st) != 0)
+    return -1;
+  return d_stats ? kgpu_block_stats_i16(d_dst, type, history, f->ilen, nblocks, 0, 2047, d_stats, st) : 0;
+}
+
+/* the block statistics of job c->folded into c->acc (its slot's device work has completed) */
+static void fold_one(struct filter_in const *f, struct master_ctx *c) {
+  struct kgpu_block_stats const *s = &c->h_bstats[c->folded % ND];
+  c->acc.blocks++;
+  c->acc.samples += (uint64_t)f->ilen;
+  c->acc.energy += s->energy;
+  c->acc.overranges += s->overs;
+  c->acc.overrange_samples += s->over_samples;
+  c->acc.since_over = s->over_samples ? 0 : c->acc.since_over + (uint64_t)f->ilen;
+  c->folded++;
+}
+
 /* ---------------------------------------------------------------- spectrum device ring ------ */
 /* n samples of esz bytes from a ring (src_cap samples, position src) to the device ring at position dst, both modular */
 static int sring_copy(struct master_ctx *c, char const *src_base, long src_cap, long src, long dst, long n, size_t esz,
@@ -640,15 +746,35 @@ static int sring_seed(struct filter_in *f, struct master_ctx *c) {
   cudaStreamSynchronize(c->st);
   cudaFree(c->d_sring);
   c->d_sring = NULL;
-  c->sring_i16 = c->i16_mode;
+  c->sring_i16 = ingest_i16(c);
   c->sring_cap = (long)(f->input_buffer_size / c->esz);
-  size_t const esz = c->sring_i16 ? c->i16_esz : c->esz;
+  size_t const esz = c->sring_i16 ? (f->in_type == COMPLEX ? 2 * sizeof(int16_t) : sizeof(int16_t)) : c->esz;
   if (cudaMalloc(&c->d_sring, (size_t)c->sring_cap * esz) != cudaSuccess) {
     c->d_sring = NULL;
     return kgf_fail("filter_spectrum_setup: device ring");
   }
   long const M1 = f->impulse_length - 1;
   c->sring_pos = (long)((M1 + (unsigned long long)f->ilen * c->issued) % (unsigned long long)c->sring_cap);
+  if (c->raw_fmt) { /* the host ring holds raw bytes: send the last sring_cap samples' bytes over and unpack them there */
+    bool const cplx = f->in_type == COMPLEX;
+    long const n = c->sring_cap, cap = raw_samples(c->raw_fmt, cplx, c->raw_ring_size);
+    long const end = raw_samples(c->raw_fmt, cplx, (size_t)(c->raw_rp - (char *)c->raw_ring)) + M1;
+    long const src = ((end - n) % cap + cap) % cap;
+    long const dst = c->sring_pos; /* (sring_pos - n) modulo sring_cap, n being sring_cap */
+    long const first = n - dst;
+    void *tmp = NULL;
+    int rc = cudaMalloc(&tmp, raw_bytes(c->raw_fmt, cplx, (size_t)n)) == cudaSuccess ? 0 : -1;
+    rc = rc ? rc
+            : window_h2d(tmp, (char *)c->raw_ring + raw_bytes(c->raw_fmt, cplx, (size_t)src), raw_bytes(c->raw_fmt, cplx, (size_t)n),
+                         c->raw_ring, c->raw_ring_size, c->st);
+    rc = rc ? rc : raw_unpack(f, c, tmp, first, 0, (char *)c->d_sring + (size_t)dst * esz, NULL, c->st);
+    if (rc == 0 && dst > 0)
+      rc = raw_unpack(f, c, (char *)tmp + raw_bytes(c->raw_fmt, cplx, (size_t)first), dst, 0, c->d_sring, NULL, c->st);
+    if (cudaStreamSynchronize(c->st) != cudaSuccess)
+      rc = -1;
+    cudaFree(tmp);
+    return rc ? kgf_fail("filter_spectrum_setup: seeding the device ring from the raw ring") : 0;
+  }
   char const *base;
   long src_cap, src_end;
   if (c->sring_i16) {
@@ -670,13 +796,13 @@ static int sring_seed(struct filter_in *f, struct master_ctx *c) {
 }
 /* the k*L new samples of the launch just issued from d_win[slot] (after its M-1 history samples), on the pipeline stream */
 static int sring_append(struct filter_in *f, struct master_ctx *c, int k) {
-  if (c->sring_i16 != c->i16_mode) { /* the ingest format changed: the next poll seeds a new ring */
+  if (c->sring_i16 != ingest_i16(c)) { /* the ingest format changed: the next poll seeds a new ring */
     cudaStreamSynchronize(c->st);
     cudaFree(c->d_sring);
     c->d_sring = NULL;
     return 0;
   }
-  size_t const esz = c->sring_i16 ? c->i16_esz : c->esz;
+  size_t const esz = c->sring_i16 ? (f->in_type == COMPLEX ? 2 * sizeof(int16_t) : sizeof(int16_t)) : c->esz;
   long const n = (long)k * f->ilen;
   void const *win = c->d_win[f->next_jobnum % ND];
   if (sring_copy(c, (char const *)win + (size_t)(f->impulse_length - 1) * esz, LONG_MAX, 0, c->sring_pos, n, esz,
@@ -697,6 +823,11 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
   /* the ring slots' previous occupants (job - ND) must have drained */
   for (int j = 0; j < k; j++)
     cudaEventSynchronize(c->done[slot + j]);
+  if (c->stats_on && !c->i16_mode && !c->raw_fmt)
+    c->stats_on = false; /* fed floats: the driver counts in its own loop */
+  while (c->stats_on && c->folded + ND < c->issued + (unsigned long long)k)
+    fold_one(f, c); /* the statistics of the slots about to be reused */
+  struct kgpu_block_stats *const bst = c->stats_on ? c->d_bstats + slot : NULL;
   if (c->timed[slot]) { /* forward+channels device time of that older job, for main.c:154-164 */
     float ms = 0;
     if (cudaEventElapsedTime(&ms, c->t0[slot], c->done[slot]) == cudaSuccess) {
@@ -726,6 +857,15 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     c->i16_rp += c->i16_esz * (size_t)f->ilen * (size_t)k;
     if (c->i16_rp >= (char *)c->i16_ring + c->i16_ring_size)
       c->i16_rp -= c->i16_ring_size;
+  } else if (c->raw_fmt) { /* packed-12 goes on as int16 with the drivers' float scale; 8-bit as floats */
+    bool const cplx = f->in_type == COMPLEX;
+    src = c->raw_rp;
+    bytes = raw_bytes(c->raw_fmt, cplx, span);
+    fmt = c->raw_fmt == FILTER_RAW_PACKED12 ? KGPU_FMT_I16 : KGPU_FMT_F32;
+    scale = (float)c->raw_scale;
+    c->raw_rp += raw_bytes(c->raw_fmt, cplx, (size_t)f->ilen * (size_t)k);
+    if (c->raw_rp >= (char *)c->raw_ring + c->raw_ring_size)
+      c->raw_rp -= c->raw_ring_size;
   } else if (f->in_type == COMPLEX) {
     src = f->input_read_pointer.c;
     bytes = sizeof(float complex) * span;
@@ -741,9 +881,17 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
   for (int j = 0; j < k; j++) /* nothing of the previous occupants may be served for these jobs */
     for (int i = 0; i < c->nslots; i++)
       c->snap[slot + j][i].ok = false;
-  if (window_h2d(c->d_win[slot], src, bytes, c->i16_mode ? c->i16_ring : f->input_buffer,
-                 c->i16_mode ? c->i16_ring_size : f->input_buffer_size, c->st) != 0)
+  void const *const ring = c->i16_mode ? c->i16_ring : c->raw_fmt ? c->raw_ring : f->input_buffer;
+  size_t const ring_size = c->i16_mode ? c->i16_ring_size : c->raw_fmt ? c->raw_ring_size : f->input_buffer_size;
+  if (window_h2d(c->raw_fmt ? c->d_raw : c->d_win[slot], src, bytes, ring, ring_size, c->st) != 0)
     rc = kgf_fail("execute_filter_input: H2D of the window");
+  long const M1 = f->impulse_length - 1;
+  if (rc == 0 && c->raw_fmt && raw_unpack(f, c, c->d_raw, M1, k, c->d_win[slot], bst, c->st) != 0)
+    rc = kgf_fail("execute_filter_input: raw unpack");
+  if (rc == 0 && c->i16_mode && bst &&
+      kgpu_block_stats_i16(c->d_win[slot], f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL, M1, f->ilen, k, c->i16_derand, 32767,
+                           bst, c->st) != 0)
+    rc = kgf_fail("execute_filter_input: kgpu_block_stats_i16");
   if (rc == 0 && kgpu_forward(c->km, c->d_win[slot], fmt, scale, c->i16_derand, k, spec, NULL, c->st) != 0)
     rc = kgf_fail("execute_filter_input: kgpu_forward");
   if (rc == 0 && c->d_sring)
@@ -803,6 +951,8 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
   }
   cudaEventRecord(c->kev, c->st);
   cudaStreamWaitEvent(c->st_d2h, c->kev, 0);
+  if (rc == 0 && bst && cudaMemcpyAsync(c->h_bstats + slot, bst, sizeof *bst * (size_t)k, cudaMemcpyDeviceToHost, c->st_d2h) != cudaSuccess)
+    rc = kgf_fail("execute_filter_input: D2H of the A/D statistics");
   if (rc == 0 && c->spectrum_d2h) {
     if (c->spectrum_d2h == 1 && c->ranges_dirty)
       rebuild_ranges(f, c);
@@ -1250,11 +1400,12 @@ int filter_spectrum_poll(struct filter_out *slave, int shift, int fft_avg, doubl
   while (sp && sp->slave != slave)
     sp = sp->next;
   int rc = sp ? 0 : -1;
-  if (rc == 0 && (c->d_sring == NULL || c->sring_i16 != c->i16_mode))
+  if (rc == 0 && (c->d_sring == NULL || c->sring_i16 != ingest_i16(c)))
     rc = sring_seed(f, c);
   uint64_t const end = (uint64_t)f->ilen * c->issued;
+  float const scale = c->raw_fmt ? (float)c->raw_scale : c->i16_scale; /* packed-12: the drivers' float scale */
   if (rc == 0 && kgpu_spectrum_run(sp->ks, c->d_sring, c->sring_cap, c->sring_pos, c->sring_i16 ? KGPU_FMT_I16 : KGPU_FMT_F32,
-                                   c->i16_scale, c->i16_derand, shift, fft_avg, overlap, sp->d_bins, c->st) != 0)
+                                   scale, c->i16_mode && c->i16_derand, shift, fft_avg, overlap, sp->d_bins, c->st) != 0)
     rc = kgf_fail("filter_spectrum_poll: kgpu_spectrum_run");
   if (rc == 0 && (cudaMemcpyAsync(sp->h_bins, sp->d_bins, sizeof(float) * (size_t)sp->bin_count, cudaMemcpyDeviceToHost,
                                   c->st) != cudaSuccess ||
@@ -1445,8 +1596,10 @@ int delete_filter_input(struct filter_in *master) { /* filter.c:930-942 */
 }
 
 /* ---------------------------------------------------------------- write_*filter ------------- */
+/* a master fed raw words takes no floats */
+static bool raw_fed(struct filter_in const *f) { return f->fwd_plan && ((struct master_ctx const *)f->fwd_plan)->raw_fmt; }
 int write_cfilter(struct filter_in *f, float complex const *buffer, int size) { /* filter.c:1093-1113 */
-  if (f == NULL)
+  if (f == NULL || raw_fed(f))
     return -1;
   if ((f->wcnt + size) * sizeof *buffer >= f->input_buffer_size)
     return -1;
@@ -1458,7 +1611,7 @@ int write_cfilter(struct filter_in *f, float complex const *buffer, int size) { 
   return fire_ready_blocks(f);
 }
 int write_rfilter(struct filter_in *f, float const *buffer, int size) { /* filter.c:1114-1134 */
-  if (f == NULL)
+  if (f == NULL || raw_fed(f))
     return -1;
   if ((f->wcnt + size) * sizeof *buffer >= f->input_buffer_size)
     return -1;
@@ -1492,7 +1645,7 @@ int write_i16filter(struct filter_in *f, int16_t const *samples, int n, float sc
 /* where a driver may deposit the next raw samples itself (mirrored, pinned ring: up to one block contiguous),
  * e.g. as the libusb transfer buffer of rx888.c:797-826; publish with write_i16filter(f, NULL, n, ...) */
 int16_t *filter_i16_write_pointer(struct filter_in *f) {
-  if (f == NULL || f->fwd_plan == NULL)
+  if (f == NULL || f->fwd_plan == NULL || raw_fed(f))
     return NULL;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
   if (!c->i16_mode) {
@@ -1506,6 +1659,76 @@ int16_t *filter_i16_write_pointer(struct filter_in *f) {
     c->i16_mode = true;
   }
   return (int16_t *)c->i16_wp;
+}
+
+/* EXTENSION: raw packed 12-bit or 8-bit ADC words, unpacked on the device (see include/ka9q_gpu_filter.h).  The drivers
+ * (airspy.c:388-434, hydrasdr.c:663-679, :759-830, rtlsdr.c:316-343) get their buffers from their vendor libraries, so
+ * there is no zero-copy write pointer: the bytes are copied into the raw ring. */
+int write_rawfilter(struct filter_in *f, void const *samples, int n, int format, double scale) {
+  if (f == NULL || f->fwd_plan == NULL || samples == NULL || n < 0)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (format != FILTER_RAW_PACKED12 && format != FILTER_RAW_U8 && format != FILTER_RAW_S8) {
+    fprintf(stderr, "write_rawfilter: unknown format %d\n", format);
+    return -1;
+  }
+  if (!c->raw_fmt && raw_start(f, c, format) != 0)
+    return -1;
+  if (format != c->raw_fmt) {
+    fprintf(stderr, "write_rawfilter: format %d on a master fed format %d\n", format, c->raw_fmt);
+    return -1;
+  }
+  if (format == FILTER_RAW_PACKED12 && n % 8 != 0) {
+    fprintf(stderr, "write_rawfilter: %d packed 12-bit samples: not a multiple of 8\n", n);
+    return -1;
+  }
+  bool const cplx = f->in_type == COMPLEX;
+  if (raw_bytes(format, cplx, (size_t)f->wcnt + (size_t)n) >= c->raw_ring_size)
+    return -1;
+  c->raw_scale = scale;
+  size_t const bytes = raw_bytes(format, cplx, (size_t)n);
+  memcpy(c->raw_wp, samples, bytes); /* the mirror view keeps a write across the end contiguous */
+  c->raw_wp += bytes;
+  if (c->raw_wp >= (char *)c->raw_ring + c->raw_ring_size)
+    c->raw_wp -= c->raw_ring_size;
+  f->wcnt += n;
+  return fire_ready_blocks(f);
+}
+
+/* EXTENSION: the A/D statistics of the blocks whose device work completed since the previous call (see
+ * include/ka9q_gpu_filter.h).  The slots about to be reused are folded in by execute_filter_input_n, which has already
+ * waited for them; this call folds, in job order, whatever else has completed, without waiting. */
+int filter_ingest_stats(struct filter_in *f, struct filter_ingest_stats *stats) {
+  if (f == NULL || f->fwd_plan == NULL || stats == NULL)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  int rc = 0;
+  pthread_mutex_lock(&c->mu);
+  if (!c->i16_mode && !c->raw_fmt && (c->issued > 0 || f->wcnt > 0))
+    rc = -1; /* fed floats */
+  else if (!c->stats_on) {
+    if (c->d_bstats == NULL &&
+        (cudaMalloc((void **)&c->d_bstats, sizeof *c->d_bstats * ND) != cudaSuccess ||
+         cudaHostAlloc((void **)&c->h_bstats, sizeof *c->h_bstats * ND, cudaHostAllocPortable) != cudaSuccess)) {
+      cudaFree(c->d_bstats);
+      c->d_bstats = NULL;
+      rc = kgf_fail("filter_ingest_stats: buffers");
+    } else {
+      c->stats_on = true;
+      c->folded = c->issued; /* blocks already issued carry no statistics */
+      memset(&c->acc, 0, sizeof c->acc);
+      memset(stats, 0, sizeof *stats);
+    }
+  } else {
+    while (c->folded < c->issued && cudaEventQuery(c->done[c->folded % ND]) == cudaSuccess)
+      fold_one(f, c);
+    *stats = c->acc;
+    uint64_t const since = c->acc.since_over;
+    memset(&c->acc, 0, sizeof c->acc);
+    c->acc.since_over = since;
+  }
+  pthread_mutex_unlock(&c->mu);
+  return rc;
 }
 
 /* ---------------------------------------------------------------- housekeeping -------------- */

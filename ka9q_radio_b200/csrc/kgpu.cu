@@ -29,6 +29,7 @@
 #include "spectrum_kernels.cuh"
 #include "bluestein_master.cuh"
 #include "bluestein_chan.cuh"
+#include "raw_ingest.cuh"
 
 using namespace kfft;
 
@@ -272,6 +273,42 @@ extern "C" int kgpu_unpack_airspy12(const void *d_packed, long sampcount, void *
   if (d_stats) CUDA_OK(cudaMemsetAsync(d_stats, 0, sizeof(IngestStats), st));
   long const ng = sampcount / 8;
   airspy_unpack_kernel<<<(unsigned)((ng + 255) / 256), 256, 0, st>>>((uint32_t const *)d_packed, ng, (uint4 *)d_i16, (IngestStats *)d_stats);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---- 8-bit ingest and per-block statistics of raw ingest (raw_ingest.cuh) -------------------------------------------
+extern "C" int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, int nblocks, double scale, void *d_out,
+                            void *d_stats, void *stream) {
+  if (!d_raw || !d_out || history < 0 || nblocks < 0 || (nblocks > 0 && L < 1) || nblocks >= 65535 ||
+      (fmt != KGPU_RAW_U8 && fmt != KGPU_RAW_S8) || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX))
+    return fail("kgpu_unpack8: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  BlockStats *stats = (BlockStats *)d_stats;
+  if (stats && nblocks) CUDA_OK(cudaMemsetAsync(stats, 0, sizeof(BlockStats) * (size_t)nblocks, st));
+  long const longest = std::max(nblocks ? L : 0L, history);
+  if (longest == 0) return 0;
+  dim3 const g((unsigned)((longest + kRawThreads - 1) / kRawThreads), (unsigned)nblocks + 1);
+  bool const s8 = fmt == KGPU_RAW_S8, cplx = in_type == KGPU_COMPLEX;
+  auto const k = s8 ? (cplx ? unpack8_kernel<true, true> : unpack8_kernel<true, false>)
+                    : (cplx ? unpack8_kernel<false, true> : unpack8_kernel<false, false>);
+  k<<<g, kRawThreads, 0, st>>>((uint8_t const *)d_raw, history, L, nblocks, scale, (float *)d_out, stats);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int kgpu_block_stats_i16(const void *d_in, int in_type, long history, long L, int nblocks, int derandomize, int limit,
+                                    void *d_stats, void *stream) {
+  if (!d_in || !d_stats || history < 0 || L < 1 || nblocks < 1 || nblocks >= 65535 || limit < 1 ||
+      (in_type != KGPU_REAL && in_type != KGPU_COMPLEX))
+    return fail("kgpu_block_stats_i16: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  CUDA_OK(cudaMemsetAsync(d_stats, 0, sizeof(BlockStats) * (size_t)nblocks, st));
+  dim3 const g((unsigned)((L + kRawThreads - 1) / kRawThreads), (unsigned)nblocks);
+  auto const k = in_type == KGPU_COMPLEX ? block_stats_i16_kernel<true> : block_stats_i16_kernel<false>;
+  k<<<g, kRawThreads, 0, st>>>((short const *)d_in, history, L, derandomize != 0, limit, (BlockStats *)d_stats);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
