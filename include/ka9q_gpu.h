@@ -132,6 +132,55 @@ int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, 
 int kgpu_block_stats_i16(const void *d_in, int in_type, long history, long L, int nblocks, int derandomize, int limit,
                          void *d_stats, void *stream);
 
+/* I/Q correction of the HackRF and FUNcube drivers (hackrf.c:297-375, funcube.c:194-310) by exact moments; see
+ * csrc/iq_correct.cuh.  Words of kgpu_iq_moments / kgpu_iq_apply, apart from kgpu_format and kgpu_raw8: */
+enum kgpu_iq_fmt {
+  KGPU_IQ_S8 = 1, /* HackRF: signed byte pairs, -128 clipped to -127 and counted (hackrf.c:325-332) */
+  KGPU_IQ_S16 = 2 /* FUNcube: int16 pairs as they are, |x| >= 32767 counted (funcube.c:256-266) */
+};
+/* One write (one transfer) in the device's ring table of writes, indexed by write number modulo the table's capacity.
+ * The caller fills first, n and scale and zeroes the rest (last_over = -1); kgpu_iq_moments accumulates the rest. */
+struct kgpu_iq_write {
+  long long first;     /* absolute index of its first I/Q pair (0 = the first pair ever written) */
+  long long n;         /* I/Q pairs */
+  double scale;        /* the scale of exactly these pairs */
+  long long m[5];      /* sum i, sum q, sum i*i, sum q*q, sum i*q over the (clipped) words */
+  long long overs;     /* components at the limits */
+  long long last_over; /* absolute component index (2 * pair, + 1 for Q) of the last one, -1 if none */
+};
+/* The correction state: what a write is corrected with (the state its predecessor left), and what it leaves. */
+struct kgpu_iq_state {
+  double dc_i, dc_q, sinphi, imbalance, gain_i, gain_q, secphi, tanphi;
+};
+/* The state update's constants: kind 1 (HackRF) weighs gain and phase by gp * n and holds DC when n == 0
+ * (hackrf.c:317, :359, :367-369); kind 2 (FUNcube) by gp = gainphase_alpha (funcube.c:209). */
+struct kgpu_iq_params {
+  int kind;
+  double dc_alpha; /* per sample: 1e-7 (hackrf.c:34), 1e-6 (funcube.c:28) */
+  double gp;
+};
+/* What a driver's state block computes for one write, and the state after it. */
+struct kgpu_iq_record {
+  long long seq;        /* write number */
+  long long n, sum_i, sum_q;
+  double i_energy, q_energy, dotprod; /* the drivers' sums over the write */
+  long long overs;      /* HackRF clips, FUNcube components at the limits */
+  long long since_over; /* components after the last one at the limits, -1 if none */
+  struct kgpu_iq_state state;
+};
+/* Moments of I/Q pairs [a0, a0 + count) whose words start at d_raw, into the table entries of writes
+ * [w_lo, w_lo + nw), which must hold every one of those pairs; a write may be summed over several calls. */
+int kgpu_iq_moments(const void *d_raw, int fmt, long long a0, long count, struct kgpu_iq_write *d_tab, int cap,
+                    long long w_lo, int nw, void *stream);
+/* Writes [w_from, w_from + nw), complete, in order: d_coef[w % cap] is the state write w was corrected with; its record
+ * goes to d_rec[w % cap] and the state after it to d_coef[(w + 1) % cap].  One thread. */
+int kgpu_iq_scan(const struct kgpu_iq_write *d_tab, struct kgpu_iq_state *d_coef, int cap, long long w_from, int nw,
+                 const struct kgpu_iq_params *params, struct kgpu_iq_record *d_rec, void *stream);
+/* Corrected float I/Q of pairs [a0, a0 + count) to d_out (float2 per pair); pairs a >= 0 lie in writes [w_lo, w_lo + nw)
+ * whose coefficients d_coef holds, pairs a < 0 precede the first write and are 0.0f. */
+int kgpu_iq_apply(const void *d_raw, int fmt, long long a0, long count, const struct kgpu_iq_write *d_tab,
+                  const struct kgpu_iq_state *d_coef, int cap, long long w_lo, int nw, void *d_out, void *stream);
+
 /* Notch EWMA on listed bins (apply_notch_filters, filter.c:464-474); list ends with bin 0. The state
  * lives in the master; blocks are processed in order. */
 int kgpu_master_set_notches(kgpu_master *m, int const *bins, double const *alpha, int n);

@@ -20,6 +20,8 @@
  *   write_rawfilter               (EXTENSION) raw 8-bit and packed 12-bit ingest: the conversion loops of rtlsdr.c,
  *                                 hydrasdr.c and airspy-unpack.c on the device
  *   filter_ingest_stats           (EXTENSION) the A/D energy and overranges those loops return, per drained block
+ *   filter_iq_correction_setup    (EXTENSION) HackRF's and FUNcube's DC and I/Q gain and phase correction on the device
+ *   filter_iq_records             (EXTENSION) the per-transfer sums and state those drivers' loops produce
  *
  * Semantics kept: return 0 / -1 (write_*: 1 if a block fired), ND-deep spectrum ring with
  * lap -> zeros + block_drops++ (filter.c:690-701), owner-thread shortcut (filter.c:681-683),
@@ -140,7 +142,13 @@ int16_t *filter_i16_write_pointer(struct filter_in *master);
  * L and M - 1 multiples of 8 so every window starts on a group boundary (Airspy R2: L = 400000 / 200000, M - 1 = L/4);
  * other geometries are rejected with -1 and a message at the first write.  A master fed one format (raw, int16 or
  * float) rejects writes in another with -1.  Returns -1 on error, 1 if a block fired, else 0. */
-enum filter_raw_format { FILTER_RAW_PACKED12 = 1, FILTER_RAW_U8 = 2, FILTER_RAW_S8 = 3 };
+enum filter_raw_format {
+  FILTER_RAW_PACKED12 = 1,
+  FILTER_RAW_U8 = 2,
+  FILTER_RAW_S8 = 3,
+  FILTER_RAW_S8_IQCORR = 4, /* HackRF: signed byte I/Q with the driver's DC and I/Q correction (filter_iq_correction_setup) */
+  FILTER_RAW_S16_IQCORR = 5 /* FUNcube: int16 I/Q with the same correction */
+};
 int write_rawfilter(struct filter_in *master, void const *samples, int n, int format, double scale);
 /* Pure host code: the byte size of the raw ring write_rawfilter allocates for a master of this geometry and format (a
  * whole number of pages, and for PACKED12 of 12-byte groups, holding at least the master's float ring of samples), or -1
@@ -159,6 +167,43 @@ struct filter_ingest_stats {
   uint64_t since_over;        /* samples after the last summed block that had an overrange (over all calls) */
 };
 int filter_ingest_stats(struct filter_in *master, struct filter_ingest_stats *stats);
+/* EXTENSION: the DC removal and I/Q gain and phase correction of hackrf.c:297-375 and funcube.c:194-310 on the device, for
+ * COMPLEX masters fed FILTER_RAW_S8_IQCORR (HackRF: -128 is clipped to -127 and counted) or FILTER_RAW_S16_IQCORR
+ * (FUNcube: words as they are; |x| >= 32767 is counted).  Each write_rawfilter call is one transfer: its samples are
+ * corrected with the state the previous write left, and its scale applies to exactly its own samples.  The state update
+ * after each write is the drivers', in their expression order, from exact integer moments of the write's words.
+ * Call filter_iq_correction_setup once, before the first write; a write in these formats without it returns -1.
+ *   dc_alpha  per sample: 1e-7 (hackrf.c:34), 1e-6 (funcube.c:28)
+ *   gp_rate   HackRF: gain/phase weight gp_rate * n per write (rate_factor, hackrf.c:317): 1 / samprate;  else 0
+ *   gp_alpha  FUNcube: the fixed weight per write (gainphase_alpha, funcube.c:209), with gp_rate 0
+ *   dc_i .. tanphi: the driver's initial state (HackRF: imbalance 0, gains and secphi 1; FUNcube: the same)
+ * Writes shorter than FILTER_IQ_MIN_WRITE pairs are rejected with -1 and a message (FUNcube at a 5 ms Blocktime writes
+ * 960).  filter_ingest_stats returns -1 on such a master: filter_iq_records replaces it.  Samples before the first write
+ * (the first window's M-1 history) are 0.0f. */
+#define FILTER_IQ_MIN_WRITE 512
+struct filter_iq_params {
+  double dc_alpha, gp_rate, gp_alpha;
+  double dc_i, dc_q, sinphi, imbalance, gain_i, gain_q, secphi, tanphi;
+};
+int filter_iq_correction_setup(struct filter_in *master, int format, struct filter_iq_params const *params);
+/* Pure host code: the writes the device table of a master of this geometry holds (every write the raw ring can hold, at
+ * FILTER_IQ_MIN_WRITE pairs each, and the launches in flight), or -1 where the format cannot feed it. */
+long filter_iq_table_writes(int L, int M, enum filtertype in_type, int format);
+/* One write's record: what the driver's state block computes, and the state after it.  The driver keeps its own
+ * if_power rule (hackrf.c:364, funcube.c:293-294) and counters (clips, overranges, samp_since_over) from these. */
+struct filter_iq_record {
+  int64_t seq;        /* write number, from 0 */
+  int64_t n;          /* I/Q pairs */
+  int64_t sum_i, sum_q; /* samp_sum */
+  double i_energy, q_energy, dotprod; /* as the drivers' loops sum them */
+  int64_t overs;      /* HackRF clips, FUNcube components at the limits */
+  int64_t since_over; /* components after the last one at the limits, -1 if none (funcube.c:256-267's samp_since_over) */
+  double dc_i, dc_q, sinphi, imbalance, gain_i, gain_q, secphi, tanphi; /* after the update */
+};
+/* Never blocks: up to max records of the writes whose last sample's launch has completed, in write order, each once.
+ * Records arrive up to one launch after their write.  A caller that falls more than the table's writes behind loses the
+ * oldest.  Returns the count, or -1 on a master without I/Q correction. */
+int filter_iq_records(struct filter_in *master, struct filter_iq_record *recs, int max);
 /* EXTENSION: serve many slaves with one call (what 1024 channel threads would each do): one wait per block. */
 int execute_filter_output_batch(struct filter_out *const *slaves, int const *shifts, int n);
 /* EXTENSION (downconvert()'s per-sample work, radio.c:1476-1501 and :1515-1520, on the device): execute_filter_output

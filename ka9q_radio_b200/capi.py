@@ -85,6 +85,10 @@ def load() -> C.CDLL:
     L.kgpu_unpack_airspy12.argtypes = [vp, l, vp, vp, vp]
     L.kgpu_unpack8.argtypes = [vp, i, i, l, l, i, d, vp, vp, vp]
     L.kgpu_block_stats_i16.argtypes = [vp, i, l, l, i, i, i, vp, vp]
+    ll = C.c_longlong
+    L.kgpu_iq_moments.argtypes = [vp, i, ll, l, vp, i, ll, i, vp]
+    L.kgpu_iq_scan.argtypes = [vp, vp, i, ll, i, vp, vp, vp]
+    L.kgpu_iq_apply.argtypes = [vp, i, ll, l, vp, vp, i, ll, i, vp, vp]
     L.kgpu_bank_define_ex.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_wide.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_huge.argtypes = [vp, i, i, i]
@@ -185,6 +189,33 @@ def block_stats_i16(d_in: int, in_type: int, history: int, L: int, nblocks: int,
     2047 for unpacked packed-12 values."""
     check(load().kgpu_block_stats_i16(d_in, in_type, history, L, nblocks, int(derandomize), limit, d_stats, stream or None),
           "kgpu_block_stats_i16")
+
+
+KGPU_IQ_S8, KGPU_IQ_S16 = 1, 2   # kgpu_iq_moments / kgpu_iq_apply words
+IQ_HACKRF, IQ_FUNCUBE = 1, 2     # struct kgpu_iq_params kind
+
+
+class IqParams(C.Structure):
+    """struct kgpu_iq_params"""
+    _fields_ = [("kind", C.c_int), ("dc_alpha", C.c_double), ("gp", C.c_double)]
+
+
+def iq_moments(d_raw: int, fmt: int, a0: int, count: int, d_tab: int, cap: int, w_lo: int, nw: int, stream: int = 0) -> None:
+    """Moments of I/Q pairs [a0, a0 + count) into the ring table entries of writes [w_lo, w_lo + nw) (kgpu_iq_moments)."""
+    check(load().kgpu_iq_moments(d_raw, fmt, a0, count, d_tab, cap, w_lo, nw, stream or None), "kgpu_iq_moments")
+
+
+def iq_scan(d_tab: int, d_coef: int, cap: int, w_from: int, nw: int, kind: int, dc_alpha: float, gp: float, d_rec: int,
+            stream: int = 0) -> None:
+    """Records and states of the complete writes [w_from, w_from + nw), in order (kgpu_iq_scan)."""
+    p = IqParams(kind, dc_alpha, gp)
+    check(load().kgpu_iq_scan(d_tab, d_coef, cap, w_from, nw, C.byref(p), d_rec, stream or None), "kgpu_iq_scan")
+
+
+def iq_apply(d_raw: int, fmt: int, a0: int, count: int, d_tab: int, d_coef: int, cap: int, w_lo: int, nw: int, d_out: int,
+             stream: int = 0) -> None:
+    """Corrected float I/Q of pairs [a0, a0 + count); pairs before 0 are 0.0 (kgpu_iq_apply)."""
+    check(load().kgpu_iq_apply(d_raw, fmt, a0, count, d_tab, d_coef, cap, w_lo, nw, d_out, stream or None), "kgpu_iq_apply")
 
 
 MASTER_DIRECT, MASTER_EXTENDED, MASTER_BLUESTEIN = 0, 1, 2

@@ -142,6 +142,22 @@ struct master_ctx {
   struct kgpu_block_stats *d_bstats, *h_bstats;
   unsigned long long folded; /* blocks folded (or, before stats_on, skipped) so far */
   struct filter_ingest_stats acc;
+  /* I/Q correction (FILTER_RAW_*_IQCORR): a ring table of the writes (host copy, device copy), the device's coefficient
+   * set and record of each write, and the pinned copy of the records */
+  bool iq_on;
+  struct kgpu_iq_params iq_par;
+  int iq_cap;
+  struct kgpu_iq_write *h_iqw, *d_iqw;
+  struct kgpu_iq_state *d_iqc;
+  struct kgpu_iq_record *d_iqr, *h_iqr;
+  unsigned long long iq_writes;          /* writes so far */
+  long long iq_total;                    /* their I/Q pairs */
+  unsigned long long iq_sent;            /* writes whose table entry is on the device */
+  unsigned long long iq_scanned;         /* writes whose record a launch computes */
+  unsigned long long iq_rec_from;        /* iq_scanned before the current launch */
+  unsigned long long iq_job_done[ND];    /* iq_scanned after the launch of each ring slot's job */
+  unsigned long long iq_checked;         /* jobs whose completion filter_iq_records has taken in */
+  unsigned long long iq_avail, iq_given; /* records complete on the host; records handed to the caller */
   unsigned long long issued; /* blocks issued to the device so far */
   /* wideband spectrum analyzer (extension): a device copy of the input ring, in the ingest format, with the host float
    * ring's capacity and positions; created by the first filter_spectrum_setup, then appended by every launch */
@@ -293,6 +309,11 @@ static void master_teardown(struct filter_in *master) {
     cudaFree(c->d_raw);
     cudaFree(c->d_bstats);
     cudaFreeHost(c->h_bstats);
+    cudaFreeHost(c->h_iqw);
+    cudaFree(c->d_iqw);
+    cudaFree(c->d_iqc);
+    cudaFree(c->d_iqr);
+    cudaFreeHost(c->h_iqr);
     while (c->specs) {
       struct spec_slave *sp = c->specs;
       c->specs = sp->next;
@@ -634,9 +655,14 @@ static void rebuild_ranges(struct filter_in *f, struct master_ctx *c) {
 
 /* ---------------------------------------------------------------- raw ingest ---------------- */
 /* bytes of n samples (REAL) or I/Q pairs (COMPLEX) in a raw format; a packed-12 n is a multiple of 8 (three words) */
-static size_t raw_bytes(int fmt, bool cplx, size_t n) { return fmt == FILTER_RAW_PACKED12 ? n / 8 * 12 : n * (cplx ? 2 : 1); }
+static bool iq_format(int fmt) { return fmt == FILTER_RAW_S8_IQCORR || fmt == FILTER_RAW_S16_IQCORR; }
+/* bytes per component */
+static size_t raw_word(int fmt) { return fmt == FILTER_RAW_S16_IQCORR ? 2 : 1; }
+static size_t raw_bytes(int fmt, bool cplx, size_t n) {
+  return fmt == FILTER_RAW_PACKED12 ? n / 8 * 12 : n * (cplx ? 2 : 1) * raw_word(fmt);
+}
 static long raw_samples(int fmt, bool cplx, size_t bytes) {
-  return (long)(fmt == FILTER_RAW_PACKED12 ? bytes / 12 * 8 : bytes / (cplx ? 2 : 1));
+  return (long)(fmt == FILTER_RAW_PACKED12 ? bytes / 12 * 8 : bytes / ((cplx ? 2 : 1) * raw_word(fmt)));
 }
 /* the device window holds int16 words (int16 ingest, or packed-12 after the unpack) rather than floats */
 static bool ingest_i16(struct master_ctx const *c) { return c->i16_mode || c->raw_fmt == FILTER_RAW_PACKED12; }
@@ -650,6 +676,9 @@ long filter_raw_ring_bytes(int L, int M, enum filtertype in_type, int format) {
     if (cplx || L % 8 != 0 || (M - 1) % 8 != 0)
       return -1;
     unit = unit / (size_t)gcd((long)unit, 12) * 12;
+  } else if (iq_format(format)) {
+    if (!cplx)
+      return -1;
   } else if (format != FILTER_RAW_U8 && format != FILTER_RAW_S8)
     return -1;
   size_t const fsz = cplx ? sizeof(float complex) : sizeof(float);
@@ -664,7 +693,9 @@ static int raw_start(struct filter_in *f, struct master_ctx *c, int format) {
   long const size = filter_raw_ring_bytes(f->ilen, f->impulse_length, f->in_type, format);
   if (size < 0) {
     fprintf(stderr, "write_rawfilter(L=%d M=%d): format %d cannot feed this master%s\n", f->ilen, f->impulse_length, format,
-            format == FILTER_RAW_PACKED12 ? " (packed 12-bit needs a REAL master with L and M-1 multiples of 8)" : "");
+            format == FILTER_RAW_PACKED12 ? " (packed 12-bit needs a REAL master with L and M-1 multiples of 8)"
+            : iq_format(format)          ? " (I/Q correction needs a COMPLEX master)"
+                                         : "");
     return -1;
   }
   if (c->i16_mode || f->wcnt != 0 || c->issued != 0) {
@@ -697,16 +728,92 @@ static int raw_start(struct filter_in *f, struct master_ctx *c, int format) {
 }
 
 /* raw bytes on the device (history samples, then nblocks blocks of L) -> the master's device samples at d_dst: floats for
- * the 8-bit formats, int16 for packed-12, which kgpu_forward then scales.  d_stats: NULL or nblocks block statistics. */
-static int raw_unpack(struct filter_in const *f, struct master_ctx const *c, void const *d_src, long history, int nblocks,
-                      void *d_dst, void *d_stats, cudaStream_t st) {
+ * the 8-bit and I/Q corrected formats, int16 for packed-12, which kgpu_forward then scales.  d_stats: NULL or nblocks
+ * block statistics (not for I/Q correction, whose records replace them). */
+static int iq_apply(struct master_ctx const *c, void const *d_src, long long a0, long count, void *d_dst, cudaStream_t st);
+static int raw_unpack(struct filter_in const *f, struct master_ctx const *c, void const *d_src, long long a0, long history,
+                      int nblocks, void *d_dst, void *d_stats, cudaStream_t st) {
   int const type = f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL;
+  if (c->iq_on) /* a0: the absolute index of the first sample (I/Q correction needs to know whose write it is) */
+    return iq_apply(c, d_src, a0, history + (long)nblocks * f->ilen, d_dst, st);
   if (c->raw_fmt != FILTER_RAW_PACKED12)
     return kgpu_unpack8(d_src, c->raw_fmt == FILTER_RAW_U8 ? KGPU_RAW_U8 : KGPU_RAW_S8, type, history, f->ilen, nblocks,
                         c->raw_scale, d_dst, d_stats, st);
   if (kgpu_unpack_airspy12(d_src, history + (long)nblocks * f->ilen, d_dst, NULL, st) != 0)
     return -1;
   return d_stats ? kgpu_block_stats_i16(d_dst, type, history, f->ilen, nblocks, 0, 2047, d_stats, st) : 0;
+}
+
+/* ---------------------------------------------------------------- I/Q correction ------------ */
+/* Writes live in a ring table of iq_cap entries (write w at w % iq_cap), on the host and on the device.  It holds twice
+ * the writes the raw ring can hold at FILTER_IQ_MIN_WRITE pairs each, plus the writes of the launches that may be in
+ * flight: the writes of the analyzer's seeding window and those written but not yet launched both fit, so no entry is
+ * overwritten while a launch or the seeding can still read it. */
+long filter_iq_table_writes(int L, int M, enum filtertype in_type, int format) {
+  if (!iq_format(format))
+    return -1;
+  long const bytes = filter_raw_ring_bytes(L, M, in_type, format);
+  if (bytes < 0)
+    return -1;
+  return 2 * (raw_samples(format, true, (size_t)bytes) / FILTER_IQ_MIN_WRITE) + 2 * ND + 2;
+}
+
+/* the newest write among [lo, hi) whose first pair is at or before absolute pair a (lo if none) */
+static unsigned long long iq_find(struct master_ctx const *c, unsigned long long lo, unsigned long long hi, long long a) {
+  while (hi - lo > 1) {
+    unsigned long long const mid = lo + (hi - lo) / 2;
+    if (c->h_iqw[mid % (unsigned long long)c->iq_cap].first <= a)
+      lo = mid;
+    else
+      hi = mid;
+  }
+  return lo;
+}
+/* the oldest write the table still holds, of the first `upto` */
+static unsigned long long iq_oldest(struct master_ctx const *c, unsigned long long upto) {
+  return upto > (unsigned long long)c->iq_cap ? upto - (unsigned long long)c->iq_cap : 0;
+}
+
+/* corrected floats of pairs [a0, a0 + count) from their raw words at d_src, into d_dst; every write they lie in has
+ * been sent to the device (c->iq_sent) and its predecessor scanned */
+static int iq_apply(struct master_ctx const *c, void const *d_src, long long a0, long count, void *d_dst, cudaStream_t st) {
+  unsigned long long w_lo = 0, w_hi = 0;
+  if (a0 + count > 0 && c->iq_sent > 0) {
+    unsigned long long const old = iq_oldest(c, c->iq_sent);
+    w_lo = iq_find(c, old, c->iq_sent, a0 > 0 ? a0 : 0);
+    w_hi = iq_find(c, old, c->iq_sent, a0 + count - 1);
+  }
+  return kgpu_iq_apply(d_src, c->raw_fmt == FILTER_RAW_S8_IQCORR ? KGPU_IQ_S8 : KGPU_IQ_S16, a0, count, c->d_iqw, c->d_iqc,
+                       c->iq_cap, (long long)w_lo, (int)(w_hi - w_lo + 1), d_dst, st);
+}
+
+/* the table entries, moments and records of the k blocks about to be issued (new pairs [issued L, (issued + k) L)),
+ * whose raw window is in d_raw, on the pipeline stream; the apply follows in raw_unpack */
+static int iq_launch(struct filter_in const *f, struct master_ctx *c, int k) {
+  long long const a = (long long)f->ilen * (long long)c->issued, end = a + (long long)k * f->ilen;
+  unsigned long long const cap = (unsigned long long)c->iq_cap, old = iq_oldest(c, c->iq_writes);
+  unsigned long long const last = iq_find(c, old, c->iq_writes, end - 1); /* the write of the launch's last pair */
+  for (unsigned long long w = c->iq_sent; w <= last;) { /* the writes that start in this launch */
+    unsigned long long const n = last + 1 - w < cap - w % cap ? last + 1 - w : cap - w % cap;
+    if (cudaMemcpyAsync(c->d_iqw + w % cap, c->h_iqw + w % cap, sizeof *c->h_iqw * (size_t)n, cudaMemcpyHostToDevice, c->st) !=
+        cudaSuccess)
+      return -1;
+    w += n;
+  }
+  c->iq_sent = last + 1;
+  int const fmt = c->raw_fmt == FILTER_RAW_S8_IQCORR ? KGPU_IQ_S8 : KGPU_IQ_S16;
+  unsigned long long const first = iq_find(c, old, c->iq_writes, a);
+  char const *d_new = (char const *)c->d_raw + raw_bytes(c->raw_fmt, true, (size_t)(f->impulse_length - 1));
+  if (kgpu_iq_moments(d_new, fmt, a, (long)(end - a), c->d_iqw, c->iq_cap, (long long)first, (int)(last - first + 1), c->st) != 0)
+    return -1;
+  struct kgpu_iq_write const *lw = &c->h_iqw[last % cap];
+  unsigned long long const done = lw->first + lw->n <= end ? last + 1 : last; /* writes complete at the launch's end */
+  c->iq_rec_from = c->iq_scanned;
+  if (kgpu_iq_scan(c->d_iqw, c->d_iqc, c->iq_cap, (long long)c->iq_scanned, (int)(done - c->iq_scanned), &c->iq_par, c->d_iqr,
+                   c->st) != 0)
+    return -1;
+  c->iq_scanned = done;
+  return 0;
 }
 
 /* the block statistics of job c->folded into c->acc (its slot's device work has completed) */
@@ -767,9 +874,11 @@ static int sring_seed(struct filter_in *f, struct master_ctx *c) {
     rc = rc ? rc
             : window_h2d(tmp, (char *)c->raw_ring + raw_bytes(c->raw_fmt, cplx, (size_t)src), raw_bytes(c->raw_fmt, cplx, (size_t)n),
                          c->raw_ring, c->raw_ring_size, c->st);
-    rc = rc ? rc : raw_unpack(f, c, tmp, first, 0, (char *)c->d_sring + (size_t)dst * esz, NULL, c->st);
+    long long const a0 = (long long)f->ilen * (long long)c->issued - n; /* the absolute index of the first seeded sample */
+    rc = rc ? rc : raw_unpack(f, c, tmp, a0, first, 0, (char *)c->d_sring + (size_t)dst * esz, NULL, c->st);
     if (rc == 0 && dst > 0)
-      rc = raw_unpack(f, c, (char *)tmp + raw_bytes(c->raw_fmt, cplx, (size_t)first), dst, 0, c->d_sring, NULL, c->st);
+      rc = raw_unpack(f, c, (char *)tmp + raw_bytes(c->raw_fmt, cplx, (size_t)first), a0 + first, dst, 0, c->d_sring, NULL,
+                      c->st);
     if (cudaStreamSynchronize(c->st) != cudaSuccess)
       rc = -1;
     cudaFree(tmp);
@@ -827,6 +936,8 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     c->stats_on = false; /* fed floats: the driver counts in its own loop */
   while (c->stats_on && c->folded + ND < c->issued + (unsigned long long)k)
     fold_one(f, c); /* the statistics of the slots about to be reused */
+  while (c->iq_on && c->iq_checked + ND < c->issued + (unsigned long long)k)
+    c->iq_avail = c->iq_job_done[c->iq_checked++ % ND]; /* the records of the slots about to be reused have arrived */
   struct kgpu_block_stats *const bst = c->stats_on ? c->d_bstats + slot : NULL;
   if (c->timed[slot]) { /* forward+channels device time of that older job, for main.c:154-164 */
     float ms = 0;
@@ -886,7 +997,10 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
   if (window_h2d(c->raw_fmt ? c->d_raw : c->d_win[slot], src, bytes, ring, ring_size, c->st) != 0)
     rc = kgf_fail("execute_filter_input: H2D of the window");
   long const M1 = f->impulse_length - 1;
-  if (rc == 0 && c->raw_fmt && raw_unpack(f, c, c->d_raw, M1, k, c->d_win[slot], bst, c->st) != 0)
+  if (rc == 0 && c->iq_on && iq_launch(f, c, k) != 0)
+    rc = kgf_fail("execute_filter_input: I/Q correction");
+  if (rc == 0 && c->raw_fmt && raw_unpack(f, c, c->d_raw, (long long)f->ilen * (long long)c->issued - M1, M1, k, c->d_win[slot],
+                                          bst, c->st) != 0)
     rc = kgf_fail("execute_filter_input: raw unpack");
   if (rc == 0 && c->i16_mode && bst &&
       kgpu_block_stats_i16(c->d_win[slot], f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL, M1, f->ilen, k, c->i16_derand, 32767,
@@ -953,6 +1067,21 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
   cudaStreamWaitEvent(c->st_d2h, c->kev, 0);
   if (rc == 0 && bst && cudaMemcpyAsync(c->h_bstats + slot, bst, sizeof *bst * (size_t)k, cudaMemcpyDeviceToHost, c->st_d2h) != cudaSuccess)
     rc = kgf_fail("execute_filter_input: D2H of the A/D statistics");
+  if (c->iq_on) {
+    unsigned long long const from = c->iq_rec_from, to = c->iq_scanned;
+    for (unsigned long long w = from; rc == 0 && w < to;) { /* the records of the writes this launch completed */
+      unsigned long long const n = to - w < (unsigned long long)c->iq_cap - w % (unsigned long long)c->iq_cap
+                                       ? to - w
+                                       : (unsigned long long)c->iq_cap - w % (unsigned long long)c->iq_cap;
+      size_t const at = (size_t)(w % (unsigned long long)c->iq_cap);
+      if (cudaMemcpyAsync(c->h_iqr + at, c->d_iqr + at, sizeof *c->h_iqr * (size_t)n, cudaMemcpyDeviceToHost, c->st_d2h) !=
+          cudaSuccess)
+        rc = kgf_fail("execute_filter_input: D2H of the I/Q records");
+      w += n;
+    }
+    for (int j = 0; j < k; j++)
+      c->iq_job_done[slot + j] = to;
+  }
   if (rc == 0 && c->spectrum_d2h) {
     if (c->spectrum_d2h == 1 && c->ranges_dirty)
       rebuild_ranges(f, c);
@@ -1668,8 +1797,12 @@ int write_rawfilter(struct filter_in *f, void const *samples, int n, int format,
   if (f == NULL || f->fwd_plan == NULL || samples == NULL || n < 0)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (format != FILTER_RAW_PACKED12 && format != FILTER_RAW_U8 && format != FILTER_RAW_S8) {
+  if (format != FILTER_RAW_PACKED12 && format != FILTER_RAW_U8 && format != FILTER_RAW_S8 && !iq_format(format)) {
     fprintf(stderr, "write_rawfilter: unknown format %d\n", format);
+    return -1;
+  }
+  if (iq_format(format) && !c->iq_on) {
+    fprintf(stderr, "write_rawfilter: format %d needs filter_iq_correction_setup first\n", format);
     return -1;
   }
   if (!c->raw_fmt && raw_start(f, c, format) != 0)
@@ -1685,6 +1818,20 @@ int write_rawfilter(struct filter_in *f, void const *samples, int n, int format,
   bool const cplx = f->in_type == COMPLEX;
   if (raw_bytes(format, cplx, (size_t)f->wcnt + (size_t)n) >= c->raw_ring_size)
     return -1;
+  if (c->iq_on) { /* one transfer: its table entry */
+    if (n < FILTER_IQ_MIN_WRITE) {
+      fprintf(stderr, "write_rawfilter: %d I/Q pairs: writes with I/Q correction take at least %d\n", n, FILTER_IQ_MIN_WRITE);
+      return -1;
+    }
+    struct kgpu_iq_write *w = &c->h_iqw[c->iq_writes % (unsigned long long)c->iq_cap];
+    memset(w, 0, sizeof *w);
+    w->first = c->iq_total;
+    w->n = n;
+    w->scale = scale;
+    w->last_over = -1;
+    c->iq_writes++;
+    c->iq_total += n;
+  }
   c->raw_scale = scale;
   size_t const bytes = raw_bytes(format, cplx, (size_t)n);
   memcpy(c->raw_wp, samples, bytes); /* the mirror view keeps a write across the end contiguous */
@@ -1702,6 +1849,8 @@ int filter_ingest_stats(struct filter_in *f, struct filter_ingest_stats *stats) 
   if (f == NULL || f->fwd_plan == NULL || stats == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (c->iq_on)
+    return -1; /* I/Q corrected: filter_iq_records replaces the block statistics */
   int rc = 0;
   pthread_mutex_lock(&c->mu);
   if (!c->i16_mode && !c->raw_fmt && (c->issued > 0 || f->wcnt > 0))
@@ -1729,6 +1878,82 @@ int filter_ingest_stats(struct filter_in *f, struct filter_ingest_stats *stats) 
   }
   pthread_mutex_unlock(&c->mu);
   return rc;
+}
+
+/* EXTENSION: HackRF's and FUNcube's DC and I/Q correction on the device (see include/ka9q_gpu_filter.h): the raw ring,
+ * the table of writes and the initial coefficient set, before the first write. */
+int filter_iq_correction_setup(struct filter_in *f, int format, struct filter_iq_params const *p) {
+  if (f == NULL || f->fwd_plan == NULL || p == NULL || !iq_format(format))
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (c->raw_fmt || c->iq_on) {
+    fprintf(stderr, "filter_iq_correction_setup: the master is already fed raw words\n");
+    return -1;
+  }
+  long const cap = filter_iq_table_writes(f->ilen, f->impulse_length, f->in_type, format);
+  if (cap < 0) {
+    fprintf(stderr, "filter_iq_correction_setup(L=%d M=%d): I/Q correction needs a COMPLEX master\n", f->ilen, f->impulse_length);
+    return -1;
+  }
+  if (raw_start(f, c, format) != 0)
+    return -1;
+  c->iq_cap = (int)cap;
+  size_t const nw = (size_t)cap;
+  bool ok = cudaHostAlloc((void **)&c->h_iqw, sizeof *c->h_iqw * nw, cudaHostAllocPortable) == cudaSuccess;
+  ok = ok && cudaMalloc((void **)&c->d_iqw, sizeof *c->d_iqw * nw) == cudaSuccess;
+  ok = ok && cudaMalloc((void **)&c->d_iqc, sizeof *c->d_iqc * nw) == cudaSuccess;
+  ok = ok && cudaMalloc((void **)&c->d_iqr, sizeof *c->d_iqr * nw) == cudaSuccess;
+  ok = ok && cudaHostAlloc((void **)&c->h_iqr, sizeof *c->h_iqr * nw, cudaHostAllocPortable) == cudaSuccess;
+  struct kgpu_iq_state const init = {p->dc_i, p->dc_q, p->sinphi, p->imbalance, p->gain_i, p->gain_q, p->secphi, p->tanphi};
+  ok = ok && cudaMemcpy(c->d_iqc, &init, sizeof init, cudaMemcpyHostToDevice) == cudaSuccess; /* write 0's coefficients */
+  if (!ok)
+    return kgf_fail("filter_iq_correction_setup: table buffers"); /* freed with the master */
+  c->iq_par.kind = p->gp_rate != 0 ? 1 : 2;
+  c->iq_par.dc_alpha = p->dc_alpha;
+  c->iq_par.gp = p->gp_rate != 0 ? p->gp_rate : p->gp_alpha;
+  c->iq_on = true;
+  return 0;
+}
+
+/* EXTENSION: the records of the writes whose launch has completed (see include/ka9q_gpu_filter.h).  The launches' slots
+ * about to be reused are taken in by execute_filter_input_n, which has already waited for them; this call takes in, in
+ * job order, whatever else has completed, without waiting. */
+int filter_iq_records(struct filter_in *f, struct filter_iq_record *recs, int max) {
+  if (f == NULL || f->fwd_plan == NULL || (recs == NULL && max > 0))
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (!c->iq_on)
+    return -1;
+  pthread_mutex_lock(&c->mu);
+  while (c->iq_checked < c->issued && cudaEventQuery(c->done[c->iq_checked % ND]) == cudaSuccess)
+    c->iq_avail = c->iq_job_done[c->iq_checked++ % ND];
+  unsigned long long const cap = (unsigned long long)c->iq_cap;
+  if (c->iq_scanned > cap && c->iq_given < c->iq_scanned - cap)
+    c->iq_given = c->iq_scanned - cap; /* overwritten by later launches' records */
+  int n = 0;
+  for (; n < max && c->iq_given < c->iq_avail; n++, c->iq_given++) {
+    struct kgpu_iq_record const *r = &c->h_iqr[c->iq_given % cap];
+    struct filter_iq_record *o = &recs[n];
+    o->seq = r->seq;
+    o->n = r->n;
+    o->sum_i = r->sum_i;
+    o->sum_q = r->sum_q;
+    o->i_energy = r->i_energy;
+    o->q_energy = r->q_energy;
+    o->dotprod = r->dotprod;
+    o->overs = r->overs;
+    o->since_over = r->since_over;
+    o->dc_i = r->state.dc_i;
+    o->dc_q = r->state.dc_q;
+    o->sinphi = r->state.sinphi;
+    o->imbalance = r->state.imbalance;
+    o->gain_i = r->state.gain_i;
+    o->gain_q = r->state.gain_q;
+    o->secphi = r->state.secphi;
+    o->tanphi = r->state.tanphi;
+  }
+  pthread_mutex_unlock(&c->mu);
+  return n;
 }
 
 /* ---------------------------------------------------------------- housekeeping -------------- */

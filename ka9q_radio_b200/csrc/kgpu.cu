@@ -30,6 +30,7 @@
 #include "bluestein_master.cuh"
 #include "bluestein_chan.cuh"
 #include "raw_ingest.cuh"
+#include "iq_correct.cuh"
 
 using namespace kfft;
 
@@ -309,6 +310,53 @@ extern "C" int kgpu_block_stats_i16(const void *d_in, int in_type, long history,
   dim3 const g((unsigned)((L + kRawThreads - 1) / kRawThreads), (unsigned)nblocks);
   auto const k = in_type == KGPU_COMPLEX ? block_stats_i16_kernel<true> : block_stats_i16_kernel<false>;
   k<<<g, kRawThreads, 0, st>>>((short const *)d_in, history, L, derandomize != 0, limit, (BlockStats *)d_stats);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---- I/Q correction of the HackRF and FUNcube drivers (iq_correct.cuh) ----------------------------------------------
+static_assert(sizeof(IqWrite) == sizeof(kgpu_iq_write) && sizeof(IqState) == sizeof(kgpu_iq_state) &&
+                  sizeof(IqRecord) == sizeof(kgpu_iq_record),
+              "iq_correct.cuh mirrors include/ka9q_gpu.h");
+static bool iq_args(const void *d_raw, int fmt, long count, const void *d_tab, int cap, int nw) {
+  return d_raw && d_tab && count >= 0 && cap > 0 && nw > 0 && nw <= cap && (fmt == KGPU_IQ_S8 || fmt == KGPU_IQ_S16) &&
+         (count + kIqChunk - 1) / kIqChunk < 0x7fffffffL;
+}
+
+extern "C" int kgpu_iq_moments(const void *d_raw, int fmt, long long a0, long count, kgpu_iq_write *d_tab, int cap,
+                               long long w_lo, int nw, void *stream) {
+  if (!iq_args(d_raw, fmt, count, d_tab, cap, nw) || a0 < 0 || w_lo < 0) return fail("kgpu_iq_moments: bad arguments");
+  if (count == 0) return 0;
+  auto const k = fmt == KGPU_IQ_S16 ? iq_moments_kernel<true> : iq_moments_kernel<false>;
+  k<<<(unsigned)((count + kIqChunk - 1) / kIqChunk), kIqThreads, 0, (cudaStream_t)stream>>>(d_raw, a0, count, (IqWrite *)d_tab,
+                                                                                           cap, w_lo, nw);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int kgpu_iq_scan(const kgpu_iq_write *d_tab, kgpu_iq_state *d_coef, int cap, long long w_from, int nw,
+                            const kgpu_iq_params *params, kgpu_iq_record *d_rec, void *stream) {
+  if (!d_tab || !d_coef || !d_rec || !params || cap < 2 || nw < 0 || nw >= cap || w_from < 0 ||
+      (params->kind != 1 && params->kind != 2))
+    return fail("kgpu_iq_scan: bad arguments");
+  if (nw == 0) return 0;
+  IqParams const p = {params->kind, params->dc_alpha, params->gp};
+  iq_scan_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((IqWrite const *)d_tab, (IqState *)d_coef, cap, w_from, nw, p,
+                                                    (IqRecord *)d_rec);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int kgpu_iq_apply(const void *d_raw, int fmt, long long a0, long count, const kgpu_iq_write *d_tab,
+                             const kgpu_iq_state *d_coef, int cap, long long w_lo, int nw, void *d_out, void *stream) {
+  if (!iq_args(d_raw, fmt, count, d_tab, cap, nw) || !d_coef || !d_out || w_lo < 0) return fail("kgpu_iq_apply: bad arguments");
+  if (count == 0) return 0;
+  auto const k = fmt == KGPU_IQ_S16 ? iq_apply_kernel<true> : iq_apply_kernel<false>;
+  k<<<(unsigned)((count + kIqChunk - 1) / kIqChunk), kIqThreads, 0, (cudaStream_t)stream>>>(
+      d_raw, a0, count, (IqWrite const *)d_tab, (IqState const *)d_coef, cap, w_lo, nw, (float2 *)d_out);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
