@@ -118,13 +118,28 @@ struct kgpu_block_stats {
   unsigned int overs;        /* components at the format's limits */
   unsigned int over_samples; /* samples with at least one component at the limits */
 };
+/* A front end's change of scale between two writes: from absolute sample `at` on (0 = the first sample a master was
+ * written), samples take `scale`.  The conversions that take a device array of n of them, sorted by `at`, give each
+ * sample the scale of the last change at or before it, or their `scale` argument before the first. */
+struct kgpu_scale_change {
+  long long at;
+  double scale;
+};
 /* 8-bit ingest (replaces the conversion loops cited at kgpu_raw8): the bytes of an overlap-save launch -- `history`
  * samples, then nblocks blocks of L new samples, laid out as kgpu_forward's d_in -- to floats at d_out (4-byte aligned),
  * each (float)(scale * (double)x) with x = byte - 128 (U8) or the signed byte (S8), bitwise what the drivers' loops
- * store; then kgpu_forward(..., KGPU_FMT_F32, ...) reads d_out.  d_stats: NULL or nblocks kgpu_block_stats, zeroed by the
- * call; at the limits: x >= 127 or x <= -128.  nblocks may be 0 (conversion only: history samples). */
-int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, int nblocks, double scale, void *d_out,
-                 void *d_stats, void *stream);
+ * store; then kgpu_forward(..., KGPU_FMT_F32, ...) reads d_out.  d_chg: NULL, or nchg scale changes, the first history
+ * sample being absolute sample a0.  d_stats: NULL or nblocks kgpu_block_stats, zeroed by the call; at the limits:
+ * x >= 127 or x <= -128.  nblocks may be 0 (conversion only: history samples). */
+int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, int nblocks, double scale,
+                 const struct kgpu_scale_change *d_chg, int nchg, long long a0, void *d_out, void *d_stats, void *stream);
+/* int16 words laid out as kgpu_forward's KGPU_FMT_I16 d_in (count samples, the first being absolute sample a0) to floats
+ * at d_out, each (float)x * (float)s after the optional derandomization (rx888.c:707-712, 764-765; airspy-unpack.c:124
+ * for kgpu_unpack_airspy12's words), s its own scale: `scale` before the first of the nchg changes at d_chg, else the
+ * last change at or before it.  For windows that hold more than one scale; kgpu_forward(..., KGPU_FMT_F32, ...) then
+ * reads d_out. */
+int kgpu_scale_i16(const void *d_in, int in_type, long count, long long a0, double scale, const struct kgpu_scale_change *d_chg,
+                   int nchg, int derandomize, float *d_out, void *stream);
 /* Per-block statistics of int16 words on the device, laid out as kgpu_forward's KGPU_FMT_I16 d_in (history samples, then
  * nblocks blocks of L): the RX888's words after the optional derandomization (rx888.c:707-712, 759-762; limit 32767, i.e.
  * x > 32766 or x < -32766), or kgpu_unpack_airspy12's output (airspy-unpack.c:121-124; limit 2047).  A component is at the
@@ -327,11 +342,13 @@ int kgpu_spectrum_set_window(kgpu_spectrum *s, float const *window);
  *   end           ring position just past the newest sample (taken modulo ring_samples); segments start at
  *                 end - adjust + i*hop (REAL) or end - adjust - i*hop (COMPLEX), adjust and hop as spectrum.c:364,407
  *   scale, derandomize  int16 samples are scale * (float)x after the randomizer flip (rx888.c:707-712,765)
+ *   d_chg, nchg, end_index  NULL, or nchg scale changes of an int16 ring: the sample just before ring position end is
+ *                 absolute sample end_index - 1, samples before the first change take `scale`
  *   shift         spectrum.c:347; fft_avg >= 1; 0 <= overlap < 1
  * Enqueued on `stream`; the analyzer's scratch is reused by the next run, so runs of one analyzer go on one stream.
  * A REAL walk index the reference would take below 0 (out of its array) contributes 0. */
 int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring_samples, long end, int fmt, float scale,
-                      int derandomize, int shift, int fft_avg, double overlap, float *d_bins, void *stream);
+                      const struct kgpu_scale_change *d_chg, int nchg, long long end_index, int derandomize, int shift, int fft_avg, double overlap, float *d_bins, void *stream);
 /* One narrowband poll (narrowband_poll, spectrum.c:206-306) on an analyzer created with in_type KGPU_COMPLEX:
  *   d_ring        device ring of ring_size float2 samples (>= fft_n), the channel's delivered blocks as spectrum.c:147-151
  *                 appends them (kgpu_spectrum_ring_append); ring_idx the position the next sample would take

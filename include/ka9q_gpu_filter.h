@@ -127,7 +127,10 @@ int set_filter_weights(struct filter_out *slave, double complex i_weight, double
 int write_cfilter(struct filter_in *master, float complex const *samples, int n);
 int write_rfilter(struct filter_in *master, float const *samples, int n);
 /* EXTENSION: raw ADC words.  n int16 samples (REAL master) or n I/Q pairs (COMPLEX master); a
- * master fed this way must not also be fed through write_rfilter/write_cfilter. */
+ * master fed this way must not also be fed through write_rfilter/write_cfilter.  Each sample becomes
+ * (float)x * scale with the scale of its own write, as rx888.c:764 converts each transfer (see FILTER_SCALE_CHANGES
+ * for gain changes between writes).  derandomize is a per-device constant (rx888.c): the last write's applies to every
+ * launch from then on. */
 int write_i16filter(struct filter_in *master, int16_t const *samples, int n, float scale, bool derandomize);
 /* Where a driver may deposit the next raw samples itself (pinned, mirrored ring: a block's worth stays contiguous),
  * e.g. as the libusb transfer buffer of rx888.c:797-826; publish with write_i16filter(master, NULL, n, scale, derand). */
@@ -137,8 +140,8 @@ int16_t *filter_i16_write_pointer(struct filter_in *master);
  * (COMPLEX master) are copied into a pinned, mirrored ring of their own and fire blocks as write_i16filter does; each
  * launch sends the raw bytes of its windows to the device, unpacks them there, then runs the usual forward, notch,
  * channel and noise work.  U8 and S8 give floats bitwise equal to the drivers' (float)(scale * x) with a double scale;
- * PACKED12 (REAL masters only) gives (float)scale * (float)x, the drivers' float scale.  scale applies from the next
- * launch on, to that launch's whole window.  PACKED12 needs n a multiple of 8 (whole groups of three 32-bit words), and
+ * PACKED12 (REAL masters only) gives (float)scale * (float)x, the drivers' float scale.  Each write's scale applies to
+ * exactly its own samples.  PACKED12 needs n a multiple of 8 (whole groups of three 32-bit words), and
  * L and M - 1 multiples of 8 so every window starts on a group boundary (Airspy R2: L = 400000 / 200000, M - 1 = L/4);
  * other geometries are rejected with -1 and a message at the first write.  A master fed one format (raw, int16 or
  * float) rejects writes in another with -1.  Returns -1 on error, 1 if a block fired, else 0. */
@@ -154,6 +157,13 @@ int write_rawfilter(struct filter_in *master, void const *samples, int n, int fo
  * whole number of pages, and for PACKED12 of 12-byte groups, holding at least the master's float ring of samples), or -1
  * where write_rawfilter would reject the geometry. */
 long filter_raw_ring_bytes(int L, int M, enum filtertype in_type, int format);
+/* Scale changes of write_i16filter and write_rawfilter (U8, S8, PACKED12): a write whose scale differs from the previous
+ * write's records a change at its first sample, in a table of FILTER_SCALE_CHANGES(L, S) entries, S the samples of the
+ * master's float ring (input_buffer_size over the sample size).  A change leaves the table once S samples have been
+ * launched after it (the wideband analyzer's device ring holds S samples).  A write whose change would overflow the
+ * table returns -1 with a message and stores nothing.  A launch whose window holds one scale converts inside the first
+ * FFT pass as before; one that holds more converts each sample with its own scale in a kernel of its own. */
+#define FILTER_SCALE_CHANGES(L, S) (64 + 16 * (((S) + (L)-1) / (L)))
 /* EXTENSION: the A/D statistics the drivers' conversion loops return (in_energy, overranges, samp_since_over), for masters
  * fed through write_rawfilter or write_i16filter.  Never blocks: sums over the blocks whose device work completed since
  * the previous call, each block counted once however rarely the caller asks.  Collection starts with the first call on

@@ -83,7 +83,7 @@ def load() -> C.CDLL:
     L.kgpu_bank_run_one.argtypes = [vp, i, vp, vp, vp]
     L.kgpu_bank_commit.argtypes = [vp, vp]
     L.kgpu_unpack_airspy12.argtypes = [vp, l, vp, vp, vp]
-    L.kgpu_unpack8.argtypes = [vp, i, i, l, l, i, d, vp, vp, vp]
+    L.kgpu_unpack8.argtypes = [vp, i, i, l, l, i, d, vp, i, C.c_longlong, vp, vp, vp]
     L.kgpu_block_stats_i16.argtypes = [vp, i, l, l, i, i, i, vp, vp]
     ll = C.c_longlong
     L.kgpu_iq_moments.argtypes = [vp, i, ll, l, vp, i, ll, i, vp]
@@ -120,7 +120,7 @@ def load() -> C.CDLL:
     L.kgpu_spectrum_create.restype = vp
     L.kgpu_spectrum_create.argtypes = [i, i, i]
     L.kgpu_spectrum_set_window.argtypes = [vp, vp]
-    L.kgpu_spectrum_run.argtypes = [vp, vp, l, l, i, f, i, i, i, d, vp, vp]
+    L.kgpu_spectrum_run.argtypes = [vp, vp, l, l, i, f, vp, i, C.c_longlong, i, i, i, d, vp, vp]
     L.kgpu_spectrum_run_narrow.argtypes = [vp, vp, l, l, i, d, vp, vp, vp]
     L.kgpu_spectrum_ring_append.argtypes = [vp, l, l, vp, l, vp]
     L.kgpu_spectrum_describe.argtypes = [vp, C.c_char_p, i]
@@ -179,8 +179,8 @@ def unpack8(d_raw: int, fmt: int, in_type: int, history: int, L: int, nblocks: i
     """8-bit ingest (kgpu_unpack8): the u8 / s8 bytes of `history` samples then nblocks blocks of L to float32 at d_out,
     each (float)(scale * (double)x); d_stats: 0 or nblocks kgpu_block_stats (uint64 energy, uint32 overs, uint32
     over_samples)."""
-    check(load().kgpu_unpack8(d_raw, fmt, in_type, history, L, nblocks, scale, d_out, d_stats or None, stream or None),
-          "kgpu_unpack8")
+    check(load().kgpu_unpack8(d_raw, fmt, in_type, history, L, nblocks, scale, None, 0, 0, d_out, d_stats or None,
+                              stream or None), "kgpu_unpack8")
 
 
 def block_stats_i16(d_in: int, in_type: int, history: int, L: int, nblocks: int, d_stats: int, derandomize: bool = False,
@@ -462,8 +462,8 @@ class Spectrum:
         samples = ring.numel() // (2 if self.in_type == KGPU_COMPLEX else 1)
         if bins.numel() < self.bin_count:
             raise ValueError(f"bins holds fewer than {self.bin_count} floats")
-        check(self.lib.kgpu_spectrum_run(self.h, ring.data_ptr(), samples, int(end), fmt, float(scale), int(derandomize),
-                                         int(shift), int(fft_avg), float(overlap), bins.data_ptr(), stream or None),
+        check(self.lib.kgpu_spectrum_run(self.h, ring.data_ptr(), samples, int(end), fmt, float(scale), None, 0, 0,
+                                         int(derandomize), int(shift), int(fft_avg), float(overlap), bins.data_ptr(), stream or None),
               "kgpu_spectrum_run")
 
     def run_narrow(self, ring, ring_idx: int, fft_avg: int, overlap: float, bins, stream: int = 0) -> int:

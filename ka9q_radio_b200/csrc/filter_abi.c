@@ -127,7 +127,6 @@ struct master_ctx {
   void *i16_ring;
   size_t i16_ring_size, i16_esz;
   char *i16_wp, *i16_rp;
-  float i16_scale;
   bool i16_derand;
   /* raw 8-bit / packed 12-bit ingest (extension): the bytes in a mirrored ring of their own, unpacked on the device from
    * d_raw into d_win[slot] */
@@ -135,8 +134,19 @@ struct master_ctx {
   void *raw_ring;
   size_t raw_ring_size;
   char *raw_wp, *raw_rp;
-  double raw_scale;
   void *d_raw;
+  /* the scale of every int16, 8-bit and packed-12 sample (the I/Q corrected formats keep theirs per write): samples
+   * before chg[0].at take chg_base, those from chg[i].at on chg[i].scale.  A change enters where a write's scale differs
+   * from the previous write's; changes leave once no launch, analyzer seeding or poll can read their samples.  d_chg takes
+   * the changes of one launch's or poll's samples, copied from pinned staging h_stg (ND + 1 regions of chg_cap: one per
+   * ring slot for the launches, one for the seedings and polls, whose reuse waits on stg_ev); d_conv the floats of a
+   * window that holds more than one scale. */
+  bool chg_started;
+  double chg_base;
+  struct kgpu_scale_change *chg, *d_chg, *h_stg;
+  cudaEvent_t stg_ev;
+  int nchg, chg_cap;
+  float *d_conv;
   /* A/D statistics (filter_ingest_stats): one kgpu_block_stats per ring slot, folded in job order into `acc` */
   bool stats_on;
   struct kgpu_block_stats *d_bstats, *h_bstats;
@@ -307,6 +317,12 @@ static void master_teardown(struct filter_in *master) {
     ring_free(c->i16_ring, c->i16_ring_size);
     ring_free(c->raw_ring, c->raw_ring_size);
     cudaFree(c->d_raw);
+    free(c->chg);
+    cudaFree(c->d_chg);
+    cudaFreeHost(c->h_stg);
+    if (c->stg_ev)
+      cudaEventDestroy(c->stg_ev);
+    cudaFree(c->d_conv);
     cudaFree(c->d_bstats);
     cudaFreeHost(c->h_bstats);
     cudaFreeHost(c->h_iqw);
@@ -727,18 +743,108 @@ static int raw_start(struct filter_in *f, struct master_ctx *c, int format) {
   return 0;
 }
 
+/* ---------------------------------------------------------------- scale changes ------------- */
+/* FILTER_SCALE_CHANGES entries, S the samples of the master's float ring: every consumer reads samples from (blocks
+ * issued) L - S on (the analyzer's device ring holds S samples, a window M - 1 + k L of them), so a change leaves the
+ * table once S samples have been issued after it. */
+static int chg_capacity(struct filter_in const *f, struct master_ctx const *c) {
+  return (int)FILTER_SCALE_CHANGES((long)f->ilen, (long)(f->input_buffer_size / c->esz));
+}
+/* drop the changes whose samples no launch, seeding or poll can still read, folding them into chg_base */
+static void chg_prune(struct filter_in const *f, struct master_ctx *c) {
+  long long const oldest = (long long)f->ilen * (long long)c->issued - (long long)(f->input_buffer_size / c->esz);
+  int i = 0;
+  while (i < c->nchg && c->chg[i].at <= oldest)
+    c->chg_base = c->chg[i++].scale;
+  if (i > 0) {
+    memmove(c->chg, c->chg + i, sizeof *c->chg * (size_t)(c->nchg - i));
+    c->nchg -= i;
+  }
+}
+/* the scale of the write about to be stored, whose first sample is the next one; -1 (and a message) when its change
+ * would overflow the table.  Caller holds c->mu. */
+static int chg_note(struct filter_in const *f, struct master_ctx *c, double scale, char const *who) {
+  long long const at = (long long)f->ilen * (long long)c->issued + f->wcnt;
+  if (!c->chg_started) { /* the first write: the samples before it are zeros */
+    c->chg_started = true;
+    c->chg_base = scale;
+    return 0;
+  }
+  if (c->nchg > 0 && c->chg[c->nchg - 1].at == at)
+    c->nchg--; /* the previous write was empty: its change covers no sample */
+  if (scale == (c->nchg > 0 ? c->chg[c->nchg - 1].scale : c->chg_base))
+    return 0;
+  if (c->chg == NULL) {
+    c->chg_cap = chg_capacity(f, c);
+    c->chg = malloc(sizeof *c->chg * (size_t)c->chg_cap);
+    if (!c->chg || cudaMalloc((void **)&c->d_chg, sizeof *c->chg * (size_t)c->chg_cap) != cudaSuccess ||
+        cudaHostAlloc((void **)&c->h_stg, sizeof *c->chg * (size_t)c->chg_cap * (ND + 1), cudaHostAllocPortable) != cudaSuccess ||
+        cudaEventCreateWithFlags(&c->stg_ev, cudaEventDisableTiming) != cudaSuccess ||
+        (ingest_i16(c) && cudaMalloc((void **)&c->d_conv, c->win_bytes) != cudaSuccess)) {
+      free(c->chg);
+      c->chg = NULL;
+      cudaFree(c->d_chg);
+      c->d_chg = NULL;
+      cudaFreeHost(c->h_stg);
+      c->h_stg = NULL;
+      if (c->stg_ev)
+        cudaEventDestroy(c->stg_ev);
+      c->stg_ev = NULL;
+      return kgf_fail(who);
+    }
+  }
+  if (c->nchg == c->chg_cap)
+    chg_prune(f, c);
+  if (c->nchg == c->chg_cap) {
+    fprintf(stderr, "%s: a scale change at sample %lld would overflow the table of %d changes of the last %ld samples\n", who, at,
+            c->chg_cap, (long)(f->input_buffer_size / c->esz));
+    return -1;
+  }
+  c->chg[c->nchg].at = at;
+  c->chg[c->nchg].scale = scale;
+  c->nchg++;
+  return 0;
+}
+/* samples [lo, hi): *scale that of sample lo, and the *n changes after it that fall inside, copied to d_chg on the
+ * pipeline stream through staging region `stage`: a launch's first ring slot (whose previous user the launch has already
+ * waited for), or ND for seedings and polls.  Caller holds c->mu. */
+static int chg_span(struct master_ctx const *c, int stage, long long lo, long long hi, double *scale, int *n) {
+  int i = 0;
+  while (i < c->nchg && c->chg[i].at <= lo)
+    i++;
+  *scale = i > 0 ? c->chg[i - 1].scale : c->chg_base;
+  int j = i;
+  while (j < c->nchg && c->chg[j].at < hi)
+    j++;
+  *n = j - i;
+  if (*n == 0)
+    return 0;
+  struct kgpu_scale_change *const stg = c->h_stg + (size_t)stage * (size_t)c->chg_cap;
+  if (stage == ND && cudaEventSynchronize(c->stg_ev) != cudaSuccess) /* the previous seeding's or poll's copy has read it */
+    return -1;
+  memcpy(stg, c->chg + i, sizeof *c->chg * (size_t)*n);
+  if (cudaMemcpyAsync(c->d_chg, stg, sizeof *c->chg * (size_t)*n, cudaMemcpyHostToDevice, c->st) != cudaSuccess)
+    return -1;
+  return stage == ND && cudaEventRecord(c->stg_ev, c->st) != cudaSuccess ? -1 : 0;
+}
+
 /* raw bytes on the device (history samples, then nblocks blocks of L) -> the master's device samples at d_dst: floats for
  * the 8-bit and I/Q corrected formats, int16 for packed-12, which kgpu_forward then scales.  d_stats: NULL or nblocks
  * block statistics (not for I/Q correction, whose records replace them). */
 static int iq_apply(struct master_ctx const *c, void const *d_src, long long a0, long count, void *d_dst, cudaStream_t st);
-static int raw_unpack(struct filter_in const *f, struct master_ctx const *c, void const *d_src, long long a0, long history,
-                      int nblocks, void *d_dst, void *d_stats, cudaStream_t st) {
+static int raw_unpack(struct filter_in const *f, struct master_ctx const *c, int stage, void const *d_src, long long a0,
+                      long history, int nblocks, void *d_dst, void *d_stats, cudaStream_t st) {
   int const type = f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL;
   if (c->iq_on) /* a0: the absolute index of the first sample (I/Q correction needs to know whose write it is) */
     return iq_apply(c, d_src, a0, history + (long)nblocks * f->ilen, d_dst, st);
-  if (c->raw_fmt != FILTER_RAW_PACKED12)
-    return kgpu_unpack8(d_src, c->raw_fmt == FILTER_RAW_U8 ? KGPU_RAW_U8 : KGPU_RAW_S8, type, history, f->ilen, nblocks,
-                        c->raw_scale, d_dst, d_stats, st);
+  if (c->raw_fmt != FILTER_RAW_PACKED12) {
+    double scale;
+    int n;
+    if (chg_span(c, stage, a0, a0 + history + (long long)nblocks * f->ilen, &scale, &n) != 0)
+      return -1;
+    return kgpu_unpack8(d_src, c->raw_fmt == FILTER_RAW_U8 ? KGPU_RAW_U8 : KGPU_RAW_S8, type, history, f->ilen, nblocks, scale,
+                        n ? c->d_chg : NULL, n, a0, d_dst, d_stats, st);
+  }
   if (kgpu_unpack_airspy12(d_src, history + (long)nblocks * f->ilen, d_dst, NULL, st) != 0)
     return -1;
   return d_stats ? kgpu_block_stats_i16(d_dst, type, history, f->ilen, nblocks, 0, 2047, d_stats, st) : 0;
@@ -875,9 +981,9 @@ static int sring_seed(struct filter_in *f, struct master_ctx *c) {
             : window_h2d(tmp, (char *)c->raw_ring + raw_bytes(c->raw_fmt, cplx, (size_t)src), raw_bytes(c->raw_fmt, cplx, (size_t)n),
                          c->raw_ring, c->raw_ring_size, c->st);
     long long const a0 = (long long)f->ilen * (long long)c->issued - n; /* the absolute index of the first seeded sample */
-    rc = rc ? rc : raw_unpack(f, c, tmp, a0, first, 0, (char *)c->d_sring + (size_t)dst * esz, NULL, c->st);
+    rc = rc ? rc : raw_unpack(f, c, ND, tmp, a0, first, 0, (char *)c->d_sring + (size_t)dst * esz, NULL, c->st);
     if (rc == 0 && dst > 0)
-      rc = raw_unpack(f, c, (char *)tmp + raw_bytes(c->raw_fmt, cplx, (size_t)first), a0 + first, dst, 0, c->d_sring, NULL,
+      rc = raw_unpack(f, c, ND, (char *)tmp + raw_bytes(c->raw_fmt, cplx, (size_t)first), a0 + first, dst, 0, c->d_sring, NULL,
                       c->st);
     if (cudaStreamSynchronize(c->st) != cudaSuccess)
       rc = -1;
@@ -964,7 +1070,6 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     src = c->i16_rp;
     bytes = c->i16_esz * span;
     fmt = KGPU_FMT_I16;
-    scale = c->i16_scale;
     c->i16_rp += c->i16_esz * (size_t)f->ilen * (size_t)k;
     if (c->i16_rp >= (char *)c->i16_ring + c->i16_ring_size)
       c->i16_rp -= c->i16_ring_size;
@@ -973,7 +1078,6 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     src = c->raw_rp;
     bytes = raw_bytes(c->raw_fmt, cplx, span);
     fmt = c->raw_fmt == FILTER_RAW_PACKED12 ? KGPU_FMT_I16 : KGPU_FMT_F32;
-    scale = (float)c->raw_scale;
     c->raw_rp += raw_bytes(c->raw_fmt, cplx, (size_t)f->ilen * (size_t)k);
     if (c->raw_rp >= (char *)c->raw_ring + c->raw_ring_size)
       c->raw_rp -= c->raw_ring_size;
@@ -997,16 +1101,34 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
   if (window_h2d(c->raw_fmt ? c->d_raw : c->d_win[slot], src, bytes, ring, ring_size, c->st) != 0)
     rc = kgf_fail("execute_filter_input: H2D of the window");
   long const M1 = f->impulse_length - 1;
+  long long const a0 = (long long)f->ilen * (long long)c->issued - M1; /* the window's first sample */
+  if (c->chg)
+    chg_prune(f, c);
   if (rc == 0 && c->iq_on && iq_launch(f, c, k) != 0)
     rc = kgf_fail("execute_filter_input: I/Q correction");
-  if (rc == 0 && c->raw_fmt && raw_unpack(f, c, c->d_raw, (long long)f->ilen * (long long)c->issued - M1, M1, k, c->d_win[slot],
-                                          bst, c->st) != 0)
+  if (rc == 0 && c->raw_fmt && raw_unpack(f, c, slot, c->d_raw, a0, M1, k, c->d_win[slot], bst, c->st) != 0)
     rc = kgf_fail("execute_filter_input: raw unpack");
   if (rc == 0 && c->i16_mode && bst &&
       kgpu_block_stats_i16(c->d_win[slot], f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL, M1, f->ilen, k, c->i16_derand, 32767,
                            bst, c->st) != 0)
     rc = kgf_fail("execute_filter_input: kgpu_block_stats_i16");
-  if (rc == 0 && kgpu_forward(c->km, c->d_win[slot], fmt, scale, c->i16_derand, k, spec, NULL, c->st) != 0)
+  void const *fwd_in = c->d_win[slot];
+  if (rc == 0 && fmt == KGPU_FMT_I16) { /* one scale: fwd_cols converts; more: floats with each sample's own scale */
+    double s;
+    int n;
+    if (chg_span(c, slot, a0, a0 + (long long)span, &s, &n) != 0)
+      rc = kgf_fail("execute_filter_input: scale changes");
+    else if (n == 0)
+      scale = (float)s;
+    else if (kgpu_scale_i16(c->d_win[slot], f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL, (long)span, a0, s, c->d_chg, n,
+                            c->i16_mode && c->i16_derand, c->d_conv, c->st) != 0)
+      rc = kgf_fail("execute_filter_input: kgpu_scale_i16");
+    else {
+      fwd_in = c->d_conv;
+      fmt = KGPU_FMT_F32;
+    }
+  }
+  if (rc == 0 && kgpu_forward(c->km, fwd_in, fmt, scale, fmt == KGPU_FMT_I16 && c->i16_derand, k, spec, NULL, c->st) != 0)
     rc = kgf_fail("execute_filter_input: kgpu_forward");
   if (rc == 0 && c->d_sring)
     rc = sring_append(f, c, k);
@@ -1532,9 +1654,13 @@ int filter_spectrum_poll(struct filter_out *slave, int shift, int fft_avg, doubl
   if (rc == 0 && (c->d_sring == NULL || c->sring_i16 != ingest_i16(c)))
     rc = sring_seed(f, c);
   uint64_t const end = (uint64_t)f->ilen * c->issued;
-  float const scale = c->raw_fmt ? (float)c->raw_scale : c->i16_scale; /* packed-12: the drivers' float scale */
+  double scale = 1.0; /* int16 rings: that of the ring's oldest sample, then each change (packed-12: the drivers' float scale) */
+  int n = 0;
+  if (rc == 0 && c->sring_i16 && chg_span(c, ND, (long long)end - c->sring_cap, (long long)end, &scale, &n) != 0)
+    rc = kgf_fail("filter_spectrum_poll: scale changes");
   if (rc == 0 && kgpu_spectrum_run(sp->ks, c->d_sring, c->sring_cap, c->sring_pos, c->sring_i16 ? KGPU_FMT_I16 : KGPU_FMT_F32,
-                                   scale, c->i16_mode && c->i16_derand, shift, fft_avg, overlap, sp->d_bins, c->st) != 0)
+                                   (float)scale, n ? c->d_chg : NULL, n, (long long)end, c->i16_mode && c->i16_derand, shift,
+                                   fft_avg, overlap, sp->d_bins, c->st) != 0)
     rc = kgf_fail("filter_spectrum_poll: kgpu_spectrum_run");
   if (rc == 0 && (cudaMemcpyAsync(sp->h_bins, sp->d_bins, sizeof(float) * (size_t)sp->bin_count, cudaMemcpyDeviceToHost,
                                   c->st) != cudaSuccess ||
@@ -1761,7 +1887,11 @@ int write_i16filter(struct filter_in *f, int16_t const *samples, int n, float sc
     return -1;
   if (((size_t)f->wcnt + (size_t)n) * c->i16_esz >= c->i16_ring_size)
     return -1;
-  c->i16_scale = scale;
+  pthread_mutex_lock(&c->mu);
+  int const rc = chg_note(f, c, scale, "write_i16filter");
+  pthread_mutex_unlock(&c->mu);
+  if (rc != 0)
+    return -1;
   c->i16_derand = derandomize;
   if (samples != NULL)
     memcpy(c->i16_wp, samples, (size_t)n * c->i16_esz);
@@ -1832,7 +1962,13 @@ int write_rawfilter(struct filter_in *f, void const *samples, int n, int format,
     c->iq_writes++;
     c->iq_total += n;
   }
-  c->raw_scale = scale;
+  if (!c->iq_on) {
+    pthread_mutex_lock(&c->mu);
+    int const rc = chg_note(f, c, scale, "write_rawfilter");
+    pthread_mutex_unlock(&c->mu);
+    if (rc != 0)
+      return -1;
+  }
   size_t const bytes = raw_bytes(format, cplx, (size_t)n);
   memcpy(c->raw_wp, samples, bytes); /* the mirror view keeps a write across the end contiguous */
   c->raw_wp += bytes;

@@ -280,9 +280,10 @@ extern "C" int kgpu_unpack_airspy12(const void *d_packed, long sampcount, void *
 }
 
 // ---- 8-bit ingest and per-block statistics of raw ingest (raw_ingest.cuh) -------------------------------------------
-extern "C" int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, int nblocks, double scale, void *d_out,
-                            void *d_stats, void *stream) {
-  if (!d_raw || !d_out || history < 0 || nblocks < 0 || (nblocks > 0 && L < 1) || nblocks >= 65535 ||
+static_assert(sizeof(ScaleChange) == sizeof(kgpu_scale_change), "raw_ingest.cuh mirrors include/ka9q_gpu.h");
+extern "C" int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, int nblocks, double scale,
+                            const kgpu_scale_change *d_chg, int nchg, long long a0, void *d_out, void *d_stats, void *stream) {
+  if (!d_raw || !d_out || history < 0 || nblocks < 0 || (nblocks > 0 && L < 1) || nblocks >= 65535 || nchg < 0 || (nchg && !d_chg) ||
       (fmt != KGPU_RAW_U8 && fmt != KGPU_RAW_S8) || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX))
     return fail("kgpu_unpack8: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
@@ -294,7 +295,21 @@ extern "C" int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long histor
   bool const s8 = fmt == KGPU_RAW_S8, cplx = in_type == KGPU_COMPLEX;
   auto const k = s8 ? (cplx ? unpack8_kernel<true, true> : unpack8_kernel<true, false>)
                     : (cplx ? unpack8_kernel<false, true> : unpack8_kernel<false, false>);
-  k<<<g, kRawThreads, 0, st>>>((uint8_t const *)d_raw, history, L, nblocks, scale, (float *)d_out, stats);
+  k<<<g, kRawThreads, 0, st>>>((uint8_t const *)d_raw, history, L, nblocks, scale, (ScaleChange const *)d_chg, nchg, a0,
+                               (float *)d_out, stats);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int kgpu_scale_i16(const void *d_in, int in_type, long count, long long a0, double scale, const kgpu_scale_change *d_chg,
+                              int nchg, int derandomize, float *d_out, void *stream) {
+  if (!d_in || !d_out || count < 0 || nchg < 0 || (nchg && !d_chg) || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX))
+    return fail("kgpu_scale_i16: bad arguments");
+  if (count == 0) return 0;
+  auto const k = in_type == KGPU_COMPLEX ? scale_i16_kernel<true> : scale_i16_kernel<false>;
+  k<<<(unsigned)((count + kRawThreads - 1) / kRawThreads), kRawThreads, 0, (cudaStream_t)stream>>>(
+      (short const *)d_in, count, a0, scale, (ScaleChange const *)d_chg, nchg, derandomize != 0, d_out);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
@@ -2548,8 +2563,9 @@ static int spectrum_chunks(kgpu_spectrum *s, SpecWindowArgs w, SpecPowerArgs p, 
 }
 
 extern "C" int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring_samples, long end, int fmt, float scale,
-                                 int derandomize, int shift, int fft_avg, double overlap, float *d_bins, void *stream) {
-  if (!s || !d_ring || !d_bins || fft_avg < 1 || !(overlap >= 0.0 && overlap < 1.0) ||
+                                 const kgpu_scale_change *d_chg, int nchg, long long end_index, int derandomize, int shift,
+                                 int fft_avg, double overlap, float *d_bins, void *stream) {
+  if (!s || !d_ring || !d_bins || fft_avg < 1 || !(overlap >= 0.0 && overlap < 1.0) || nchg < 0 || (nchg && !d_chg) ||
       (fmt != KGPU_FMT_F32 && fmt != KGPU_FMT_I16))
     return fail("kgpu_spectrum_run: bad arguments");
   int const fft_n = s->fft_n;
@@ -2575,6 +2591,10 @@ extern "C" int kgpu_spectrum_run(kgpu_spectrum *s, const void *d_ring, long ring
   w.complex_out = s->pl.path != SP_R2C;
   w.chirp = s->pl.path == SP_BLUESTEIN;
   w.scale = scale;
+  w.chg = (ScaleChange const *)d_chg;
+  w.nchg = w.i16 ? nchg : 0;
+  w.end = (end % ring_samples + ring_samples) % ring_samples;
+  w.end_index = end_index;
   w.window = s->d_window;
   w.out = s->d_in;
   SpecPowerArgs p;
@@ -2619,6 +2639,7 @@ extern "C" int kgpu_spectrum_run_narrow(kgpu_spectrum *s, const void *d_ring, lo
   w.complex_out = 1;
   w.chirp = s->pl.path == SP_BLUESTEIN;
   w.scale = 1.0f;
+  w.nchg = 0;
   w.window = s->d_window;
   w.out = s->d_in;
   SpecPowerArgs p;

@@ -13,6 +13,7 @@
 #include <cuda_runtime.h>
 
 #include "bluestein_master.cuh"
+#include "raw_ingest.cuh"
 
 namespace kfft {
 
@@ -30,7 +31,11 @@ struct SpecWindowArgs {
   int flip;          // REAL with shift < 0: odd samples negated, odd fft_n's last sample zeroed (spectrum.c:385-390)
   int complex_out;   // float2 output (c2c and Bluestein); float for the r2c
   int chirp;         // multiply by w_n = exp(-i pi n^2 / fft_n)
-  float scale;       // int16 samples: scale * (float)x (rx888.c:765)
+  float scale;       // int16 samples: scale * (float)x (rx888.c:765) ...
+  ScaleChange const *chg;  // ... or, with nchg > 0, each sample's own scale: `scale` before chg[0].at
+  int nchg;
+  long end;          // ring position just past the newest sample, which is absolute sample end_index - 1
+  long long end_index;
   float const *window;
   void *out;         // [segment][out_len]
 };
@@ -52,12 +57,17 @@ __global__ void __launch_bounds__(kSpecThreads) spectrum_window_kernel(SpecWindo
     long pos = base + k;
     if (pos >= a.cap) pos -= a.cap;
     float const w = a.window[k];
+    float scale = a.scale;
+    if (a.nchg) {
+      long const back = a.end > pos ? a.end - pos : a.end - pos + a.cap;  // 1 for the newest sample
+      scale = (float)scale_at(a.chg, a.nchg, (double)a.scale, a.end_index - back);
+    }
     if (a.complex_in) {
       float xr, xi;
       if (a.i16) {
         short2 const v = reinterpret_cast<short2 const *>(a.ring)[pos];
-        xr = spec_i16(v.x, a.derandomize, a.scale);
-        xi = spec_i16(v.y, a.derandomize, a.scale);
+        xr = spec_i16(v.x, a.derandomize, scale);
+        xi = spec_i16(v.y, a.derandomize, scale);
       } else {
         float2 const v = reinterpret_cast<float2 const *>(a.ring)[pos];
         xr = v.x;
@@ -66,7 +76,7 @@ __global__ void __launch_bounds__(kSpecThreads) spectrum_window_kernel(SpecWindo
       re = __fmul_rn(w, xr);
       im = __fmul_rn(w, xi);
     } else {
-      float const x = a.i16 ? spec_i16(reinterpret_cast<short const *>(a.ring)[pos], a.derandomize, a.scale)
+      float const x = a.i16 ? spec_i16(reinterpret_cast<short const *>(a.ring)[pos], a.derandomize, scale)
                             : reinterpret_cast<float const *>(a.ring)[pos];
       re = __fmul_rn(w, x);
       if (a.flip) {

@@ -72,34 +72,44 @@ int rd_write_float(struct rd_session *s, void const *x, int n) {
 }
 
 /* the same writes from a thread of their own (joined before returning), so that the caller is not the master's owner
- * and its slaves can be lapped (filter.c:681-701); kind 0 floats, 1 raw, 2 int16 */
+ * and its slaves can be lapped (filter.c:681-701), or are served their blocks in order; kind 0 floats, 1 raw, 2 int16,
+ * 3 int16 derandomized */
 struct rd_prod {
   struct rd_session *s;
   void const *x;
   int n, chunks, kind, format;
   double scale;
   size_t esz; /* bytes per chunk */
+  int rc;     /* the last write's return */
 };
 static void *rd_producer(void *p) {
   struct rd_prod *a = p;
   for (int i = 0; i < a->chunks; i++) {
     void const *x = (char const *)a->x + (size_t)i * a->esz;
     if (a->kind == 1)
-      rd_write_raw(a->s, x, a->n, a->format, a->scale);
-    else if (a->kind == 2)
-      rd_write_i16(a->s, x, a->n, (float)a->scale, 0);
+      a->rc = rd_write_raw(a->s, x, a->n, a->format, a->scale);
+    else if (a->kind == 2 || a->kind == 3)
+      a->rc = rd_write_i16(a->s, x, a->n, (float)a->scale, a->kind == 3);
     else
-      rd_write_float(a->s, x, a->n);
+      a->rc = rd_write_float(a->s, x, a->n);
   }
   return NULL;
 }
 int rd_write_from_thread(struct rd_session *s, void const *x, int n, int chunks, size_t chunk_bytes, int kind, int format,
                          double scale) {
-  struct rd_prod a = {s, x, n, chunks, kind, format, scale, chunk_bytes};
+  struct rd_prod a = {s, x, n, chunks, kind, format, scale, chunk_bytes, 0};
   pthread_t t;
   if (pthread_create(&t, NULL, rd_producer, &a) != 0)
     return -1;
   return pthread_join(t, NULL);
+}
+/* one write from a thread of its own: its return (-2 if the thread could not run) */
+int rd_write_once_from_thread(struct rd_session *s, void const *x, int n, int kind, int format, double scale) {
+  struct rd_prod a = {s, x, n, 1, kind, format, scale, 0, 0};
+  pthread_t t;
+  if (pthread_create(&t, NULL, rd_producer, &a) != 0 || pthread_join(t, NULL) != 0)
+    return -2;
+  return a.rc;
 }
 
 int rd_execute(struct rd_session *s, int ch, int shift, float complex *dst) {
@@ -116,6 +126,11 @@ int rd_execute_tuned(struct rd_session *s, int ch, int shift, double remainder, 
   return r;
 }
 unsigned rd_drops(struct rd_session *s, int ch) { return s->out[ch].block_drops; }
+/* the master's host copy of job `job`'s spectrum (master->fdomain[], filter.c:640); returns its bins */
+int rd_fdomain(struct rd_session *s, unsigned job, float complex *dst) {
+  memcpy(dst, s->in.fdomain[job % ND], sizeof(float complex) * (size_t)s->in.bins);
+  return s->in.bins;
+}
 int rd_enable_noise(struct rd_session *s, double samprate) { return filter_input_enable_noise(&s->in, samprate); }
 double rd_noise(struct rd_session *s, int ch) { return filter_noise_estimate(&s->out[ch]); }
 /* out[6]: blocks, samples, energy, overranges, overrange_samples, since_over */

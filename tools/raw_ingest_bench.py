@@ -9,6 +9,12 @@
           blocks' device work) of a stream fed as raw words (write_rawfilter, statistics drained every write) against the
           same stream fed as the restated floats (write_cfilter / write_rfilter), two channels, writes alternated round
           by round; the float figure leaves out the drivers' CPU conversion loop, which raw ingest removes
+  scale   wall time per block through filter.h of an RX888 int16 stream (L = 48 000, M = 12 001) whose scale changes
+          every --every blocks, against the same stream at one scale, alternated round by round; the difference over
+          the mixed-scale launches, counted as the extra kernel launches of the changing stream (one kgpu_scale_i16
+          each), is the wall time each adds; and the device time a mixed-scale launch adds to one block's forward
+          transform: kgpu_scale_i16 (two changes in the window) + kgpu_forward on floats, against kgpu_forward's fused
+          int16 conversion, CUDA events around --reps launches, median of --rounds rounds
 
 Prints one JSON line per measurement, each with the card's name and power limit read in the same run.
 """
@@ -153,15 +159,88 @@ def bench_filter(blocks, rounds, info):
                           "float_us_per_block": round(float(np.median(times["float"])), 1), "blocks": n // L, **info}))
 
 
+def bench_scale(blocks, rounds, every, info):
+    from ka9q_radio_b200 import capi
+
+    lib = capi.load()
+    drv = C.CDLL(str(ROOT / "tests" / "abi" / "_build" / "raw_driver.so"))
+    vp, i, d = C.c_void_p, C.c_int, C.c_double
+    drv.rd_open.restype = vp
+    drv.rd_open.argtypes = [i, i, i, i]
+    drv.rd_add_channel.argtypes = [vp, i, d, d, d]
+    drv.rd_write_i16.argtypes = [vp, vp, i, C.c_float, i]
+    drv.rd_execute.argtypes = [vp, i, i, vp]
+    drv.rd_close.argtypes = [vp]
+    L, M, chunk = 48000, 12001, 16000
+    x = np.random.default_rng(2).integers(-3000, 3000, blocks * L).astype(np.int16)
+    scales = (float(np.float32(1 / 32768)), float(np.float32(10 ** (-1 / 20) / 32768)))
+    y = np.empty(960, np.complex64)
+    sessions = {}
+    for kind in ("one", "changing"):
+        h = drv.rd_open(L, M, 0, 0)
+        for olen in (480, 960):
+            drv.rd_add_channel(h, olen, -0.3, 0.3, 11.0)
+        sessions[kind] = h
+    times = {"one": [], "changing": []}
+    launches = {"one": [], "changing": []}
+    for r in range(rounds + 1):
+        for kind in ("one", "changing") if r % 2 == 0 else ("changing", "one"):
+            h = sessions[kind]
+            k0 = lib.kgpu_launch_count()
+            t0 = time.perf_counter()
+            for w in range(blocks * L // chunk):
+                sc = scales[(w * chunk // (every * L)) % 2] if kind == "changing" else scales[0]
+                if drv.rd_write_i16(h, x[w * chunk:].ctypes.data, chunk, sc, 0) == 1:
+                    drv.rd_execute(h, 0, 1000, y.ctypes.data)
+                    drv.rd_execute(h, 1, -2000, y.ctypes.data)
+            if r > 0:
+                times[kind].append((time.perf_counter() - t0) * 1e6 / blocks)
+                launches[kind].append(lib.kgpu_launch_count() - k0)
+    for h in sessions.values():
+        drv.rd_close(h)
+    one, changing = float(np.median(times["one"])), float(np.median(times["changing"]))
+    mixed = float(np.median(np.subtract(launches["changing"], launches["one"])))   # mixed-scale launches per round
+    import torch
+
+    m = capi.Master(L, M, capi.KGPU_REAL)
+    n = L + M - 1
+    d_i16 = torch.from_numpy(x[:n].copy()).cuda()
+    d_f32 = torch.empty(n, device="cuda")
+    d_spec = torch.empty(2 * m.spec_stride, device="cuda")
+    chg = np.array([(n // 3, scales[1]), (2 * n // 3, scales[0])], dtype=[("at", "<i8"), ("scale", "<f8")])
+    d_chg = torch.from_numpy(chg.view(np.uint8).copy()).cuda()
+    lib.kgpu_scale_i16.argtypes = [C.c_void_p, C.c_int, C.c_long, C.c_longlong, C.c_double, C.c_void_p, C.c_int, C.c_int,
+                                   C.c_void_p, C.c_void_p]
+    fused = lambda: m.forward(d_i16.data_ptr(), capi.KGPU_FMT_I16, scales[0], 1, d_spec.data_ptr())  # noqa: E731
+
+    def mixed_fwd():
+        lib.kgpu_scale_i16(d_i16.data_ptr(), capi.KGPU_REAL, n, 0, scales[0], d_chg.data_ptr(), 2, 0, d_f32.data_ptr(), None)
+        m.forward(d_f32.data_ptr(), capi.KGPU_FMT_F32, 1.0, 1, d_spec.data_ptr())
+
+    for f in (fused, mixed_fwd):
+        f()
+    torch.cuda.synchronize()
+    t_fused, t_mixed = timed(fused, 200, rounds), timed(mixed_fwd, 200, rounds)
+    print(json.dumps({"bench": "scale_changes", "case": "rx888_48k_i16", "every_blocks": every,
+                      "fused_forward_us": round(t_fused, 2), "mixed_scale_forward_us": round(t_mixed, 2),
+                      "added_device_us_per_mixed_launch": round(t_mixed - t_fused, 2),
+                      "one_scale_us_per_block": round(one, 1), "changing_us_per_block": round(changing, 1),
+                      "mixed_launches_per_round": mixed,
+                      "added_us_per_mixed_launch": round((changing - one) * blocks / mixed, 1) if mixed else None,
+                      "blocks": blocks, **info}))
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=60)
+    ap.add_argument("--every", type=int, default=5, help="blocks between scale changes (the scale case)")
     a = ap.parse_args()
     info = card()
     bench_kernels(a.reps, a.rounds, info)
     bench_filter(a.blocks, a.rounds, info)
+    bench_scale(a.blocks, a.rounds, a.every, info)
 
 
 if __name__ == "__main__":
