@@ -306,6 +306,15 @@ int kgpu_bank_commit(kgpu_bank *b, void *stream);
  * A master's forward kernel pair (specialised where its split has one, generic otherwise) is chosen when it is created;
  * kgpu_master_describe prints it.  Kernel variants that lost on H100 are not in the library. */
 int kgpu_use_static_kernels(int on);
+/* fwd_cols_r36, the column pass of masters split 1296 x n2, copies each CTA's input tile into shared memory with tensor
+ * copies (TMA) where the input allows a tensor map: d_in 16-byte aligned, the hop between windows and the row pitch of
+ * n2 points multiples of 16 bytes.  Any other input, or on = 0, runs the same kernel reading its inputs with global loads;
+ * the spectra and statistics are bitwise the same.  The default is on, or what the environment variable KA9Q_COLS_TMA
+ * (0 / 1) says when the first launch reads it; a call takes effect at the next launch, also for existing masters. */
+int kgpu_use_cols_tma(int on);
+/* Pure host code: 1 if kgpu_forward of the master kgpu_master_create_any(L, M, in_type) builds, fed `fmt` input at d_in,
+ * runs fwd_cols_r36 on tensor copies (with kgpu_use_cols_tma on), 0 if it does not, -1 for a length with no master. */
+int kgpu_cols_tma_fits(int L, int M, int in_type, int fmt, const void *d_in);
 
 /* Planner introspection, pure host code (works without a GPU): the in-register radices chosen for
  * a column transform of length len (returns their count, -1 if unplannable) and the two-pass split

@@ -106,6 +106,8 @@ def load() -> C.CDLL:
     L.kgpu_bank_noise.argtypes = [vp, vp, i, d, vp, vp]
     L.kgpu_bank_fm_front.argtypes = [vp, vp, l, i, vp, vp, vp]
     L.kgpu_use_static_kernels.argtypes = [i]
+    L.kgpu_use_cols_tma.argtypes = [i]
+    L.kgpu_cols_tma_fits.argtypes = [i, i, i, i, vp]
     L.kgpu_profile_enable.argtypes = [i]
     L.kgpu_profile_name.argtypes = [i]
     L.kgpu_profile_name.restype = C.c_char_p

@@ -154,6 +154,12 @@ __device__ __forceinline__ void bulk_g2s(void *dst, void const *src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// a box of a 3-D tensor map into shared memory (128-byte aligned); coordinates in elements, outside the tensor zero-filled
+__device__ __forceinline__ void tensor_g2s_3d(void *dst, void const *map, int x, int y, int z, uint64_t *bar) {
+  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+               ::"r"(smem_u32(dst)), "l"(map), "r"(x), "r"(y), "r"(z), "r"(smem_u32(bar))
+               : "memory");
+}
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"

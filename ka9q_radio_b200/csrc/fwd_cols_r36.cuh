@@ -4,7 +4,8 @@
 // traffic: one store, one load + store and one load per point, plus stage twiddles (on H100 it took 14.4 us per cfg-2 block
 // against 9.8 for this kernel).  With 1296 = 36 x 36 a point crosses shared memory ONCE (stage 0 store, stage 1 load), there
 // is one block barrier instead of two, and the 36-point butterfly is a Good-Thomas 4 x 9 split with no inner twiddles
-// (fft_radix.cuh).  Stage 0 reads its 36 inputs straight from global memory (int16 pairs -> float in registers) and
+// (fft_radix.cuh).  Stage 0 reads its 36 inputs from global memory, or from the tile tensor copies fetched
+// (fwd_cols_r36_tma, below), converting int16 pairs to floats in registers, and
 // stage 1 stores X[k1] * W^{n2 k1} straight to the inter-pass buffer, 8 adjacent columns per warp row.
 //
 // Twiddles: a thread needs W^{j t}, t = 1..35.  Ten are loaded (t = 1..5 and 6, 12, .., 30), the other 25 are one product
@@ -15,6 +16,8 @@
 // 18 LDS.128 (a quarter-warp = the 8 columns of one butterfly: 8 x 16 B at a column pitch of 4 banks = all 32 banks once)
 // instead of 36 LDS.64.  Inter-pass rows are padded to 128 B when the row pass is fwd_rows_v2 (N2C = 1250).
 #pragma once
+#include <cuda.h>  // CUtensorMap (a type only: the library does not link the driver)
+
 #include "static_kernels_v2.cuh"
 
 namespace kfft {
@@ -38,8 +41,69 @@ struct ColsR36Shape {
   static constexpr size_t smem = sizeof(float2) * (size_t)(8 * CP + 360 + 80);  // tile, tw0, twB of the 8 columns
 };
 
-template <int FMT, int N2C>
-__global__ void __launch_bounds__(ColsR36Shape::T, 2) fwd_cols_r36(Pass1Args const a, ColsR36Tables const tb) {
+// ---- the raw tile by tensor copies: fwd_cols_r36_tma ------------------------------------------------------------------
+// With global loads a warp's stage-0 load reads 4 rows x 32 bytes (int16) or x 64 bytes (float); at the row pitch of n2
+// points most of those pieces straddle a 32-byte sector, and all 36 loads of a thread occupy the LSU pipe that the
+// shared-memory traffic of both stages also needs.  fwd_cols_r36_tma has the tensor-memory accelerator copy the CTA's
+// 8 columns x 1296 rows into shared memory instead (tensor maps built by the host per launch, kgpu.cu cols_tma_map);
+// stage 0 then reads its inputs from there and does exactly what the global-load form does with them.  Every box starts
+// 16-byte aligned in global memory, inside the rows it covers.
+//  * float (FMT 0): map [2 n2 floats][n1 rows][nblocks], 6 boxes of 16 floats x 216 rows, one 64-byte row after the
+//    other.  A warp's rows ul = 4w .. 4w+3 are 256 contiguous bytes: LDS.64 without bank conflicts.
+//  * int16 (FMT 1, 2): the row pitch 4 n2 bytes is not a multiple of 16, so the map's rows are row pairs of 32-bit words
+//    (one int16 pair each): [2 n2 words][n1/2 pairs][nblocks].  Even rows are the first half of a pair (x = c0), odd rows
+//    the second (x = n2 + c0), which starts 8 bytes off 16-byte alignment when n2 = 2 mod 4: their boxes start
+//    s = n2 & 2 words earlier.  Both parities take boxes 12 words wide (48 bytes: the 8 columns and the s words before
+//    them), 3 boxes of 216 pairs each.  A thread's rows ul + 36m all have the parity of ul.  At a pitch of 12 words the
+//    even and odd pieces a warp reads share banks: its LDS.32 take 2 wavefronts, as the LDS.64 of the float form do.
+// The raw tile lies in the float tile's memory: a CTA barrier separates the last raw read from stage 0's first store.
+// Columns past n2 (the last group of 1250 = 156 * 8 + 2) hold zeros or the next row's first words and are never used.
+struct ColsR36Tma {
+  static constexpr int BOX_ROWS = 216;  // rows (float) or row pairs (int16) of a box: 1296 = 6 x 216 = 2 x 3 x 216
+  static constexpr int F32_BOX_BYTES = BOX_ROWS * 64;
+  static constexpr int I16_BOX_WORDS = 12, I16_BOX_BYTES = BOX_ROWS * I16_BOX_WORDS * 4;
+  static constexpr int I16_ODD_OFF = 3 * I16_BOX_BYTES;  // the odd rows' boxes, after the even rows' ones
+  static constexpr uint32_t bytes(int fmt) { return fmt == 0 ? 6 * F32_BOX_BYTES : 6 * I16_BOX_BYTES; }
+};
+static_assert(ColsR36Tma::bytes(0) + 112 <= sizeof(float2) * 8 * ColsR36Shape::CP &&
+              ColsR36Tma::bytes(1) + 112 <= sizeof(float2) * 8 * ColsR36Shape::CP, "the raw tile lies in the float tile");
+static_assert(ColsR36Tma::F32_BOX_BYTES % 128 == 0 && ColsR36Tma::I16_BOX_BYTES % 128 == 0, "box destinations 128-B aligned");
+
+// one int16 pair of stage 0 -> float2, with de-randomisation and the statistics of FMT 2; row, col: its place in the window
+template <int FMT>
+__device__ __forceinline__ float2 r36_ingest(int raw, int row, int col, int n2, Pass1Args const &a, unsigned long long &energy,
+                                             unsigned int &clips) {
+  int lo, hi;
+  unpack_i16(raw, lo, hi);
+  if (FMT == 2) {
+    if (a.derandomize) {  // rx888.c:707-712 on the sign-extended words
+      lo ^= (lo & 1) ? 0xfffffffe : 0;
+      hi ^= (hi & 1) ? 0xfffffffe : 0;
+    }
+    if (a.stats && (long)row * n2 + col >= a.first_new) {
+      energy += (unsigned long long)(lo * lo) + (unsigned long long)(hi * hi);
+      clips += (lo > 32766 || lo < -32766) + (hi > 32766 || hi < -32766);
+    }
+  }
+  return make_float2(i32_to_f32(lo), i32_to_f32(hi));  // the int16 scale rides on the inter-pass twiddle
+}
+
+// stage 0's twiddles and its stores into the float tile
+__device__ __forceinline__ void r36_stage0_store(float2 (&x)[36], float2 const *s_tw0, float2 *d, int ul) {
+  constexpr int R = 36, BLK = ColsR36Shape::BLK;
+  float2 wb[6], wa[6];
+#pragma unroll
+  for (int b = 1; b < 6; b++) {
+    wb[b] = s_tw0[(b - 1) * 36 + ul];
+    wa[b] = s_tw0[(4 + b) * 36 + ul];
+  }
+  d[0] = x[0];
+#pragma unroll
+  for (int t = 1; t < R; t++) d[t * BLK] = cmul(x[t], r36_power(wb, wa, t));
+}
+
+template <int FMT, int N2C, bool TMA>
+__device__ __forceinline__ void fwd_cols_r36_body(Pass1Args const &a, ColsR36Tables const &tb, CUtensorMap const *tmap) {
   constexpr int R = 36, BLK = ColsR36Shape::BLK, CP = ColsR36Shape::CP;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // [8][CP]
@@ -57,10 +121,27 @@ __global__ void __launch_bounds__(ColsR36Shape::T, 2) fwd_cols_r36(Pass1Args con
   bool const col_ok = c < ncols;
   int const n2g = c0 + c;
   float2 *mycol = tile + c * CP;
+  // tensor copies land 128-byte aligned (an extern alignment of 128 would move every kernel's shared memory)
+  unsigned char *const rtile = smem_raw + ((0u - smem_u32(smem_raw)) & 127u);
   if (tid == 0) {
     mbar_init(&tbar, 1);
     mbar_fence_init();
-    mbar_expect_tx(&tbar, 360 * 8 + 80 * 8);
+    if constexpr (TMA) {
+      using T = ColsR36Tma;
+      mbar_expect_tx(&tbar, 360 * 8 + 80 * 8 + T::bytes(FMT));
+      if (FMT == 0) {
+#pragma unroll
+        for (int k = 0; k < 6; k++) tensor_g2s_3d(rtile + k * T::F32_BOX_BYTES, tmap, 2 * c0, k * T::BOX_ROWS, blk, &tbar);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+          tensor_g2s_3d(rtile + k * T::I16_BOX_BYTES, tmap, c0, k * T::BOX_ROWS, blk, &tbar);
+          tensor_g2s_3d(rtile + T::I16_ODD_OFF + k * T::I16_BOX_BYTES, tmap, n2 + c0 - (n2 & 2), k * T::BOX_ROWS, blk, &tbar);
+        }
+      }
+    } else {
+      mbar_expect_tx(&tbar, 360 * 8 + 80 * 8);
+    }
     bulk_g2s(s_tw0, tb.tw0, 360 * 8, &tbar);
     bulk_g2s(s_twB, tb.twB + (long)c0 * 10, 80 * 8, &tbar);  // table padded by 8 columns
   }
@@ -70,7 +151,28 @@ __global__ void __launch_bounds__(ColsR36Shape::T, 2) fwd_cols_r36(Pass1Args con
   // ---- stage 0 fused with the load: x[j + 36 m], m = 0..35, j = ul --------------------------------------------
   unsigned long long energy = 0;
   unsigned int clips = 0;
-  if (col_ok) {
+  if constexpr (TMA) {
+    float2 x[R];
+    mbar_wait(&tbar, 0);
+    if (col_ok) {
+      if (FMT == 0) {
+        float2 const *src = reinterpret_cast<float2 const *>(rtile) + ul * 8 + c;
+#pragma unroll
+        for (int m = 0; m < R; m++) x[m] = src[R * 8 * m];
+      } else {
+        using T = ColsR36Tma;
+        int const odd = ul & 1;
+        int const *src = reinterpret_cast<int const *>(rtile + odd * T::I16_ODD_OFF) + (ul >> 1) * T::I16_BOX_WORDS + c +
+                         odd * (n2 & 2);
+#pragma unroll
+        for (int m = 0; m < R; m++)
+          x[m] = r36_ingest<FMT>(src[(R / 2) * T::I16_BOX_WORDS * m], ul + R * m, n2g, n2, a, energy, clips);
+      }
+      Dft<R, false>::run(x);
+    }
+    __syncthreads();  // the raw tile is read: stage 0 may overwrite it
+    if (col_ok) r36_stage0_store(x, s_tw0, mycol + ul, ul);
+  } else if (col_ok) {
     float2 x[R];
     if (FMT == 0) {
       float2 const *src = reinterpret_cast<float2 const *>(a.in) + (long)blk * a.hop + n2g + (long)ul * n2;
@@ -82,34 +184,11 @@ __global__ void __launch_bounds__(ColsR36Shape::T, 2) fwd_cols_r36(Pass1Args con
 #pragma unroll
       for (int m = 0; m < R; m++) raw[m] = ldg_stream_b32(src + (long)(R * m) * n2);
 #pragma unroll
-      for (int m = 0; m < R; m++) {
-        int lo, hi;
-        unpack_i16(raw[m], lo, hi);
-        if (FMT == 2) {
-          if (a.derandomize) {  // rx888.c:707-712 on the sign-extended words
-            lo ^= (lo & 1) ? 0xfffffffe : 0;
-            hi ^= (hi & 1) ? 0xfffffffe : 0;
-          }
-          if (a.stats && (long)(ul + R * m) * n2 + n2g >= a.first_new) {
-            energy += (unsigned long long)(lo * lo) + (unsigned long long)(hi * hi);
-            clips += (lo > 32766 || lo < -32766) + (hi > 32766 || hi < -32766);
-          }
-        }
-        x[m] = make_float2(i32_to_f32(lo), i32_to_f32(hi));  // the int16 scale rides on the inter-pass twiddle
-      }
+      for (int m = 0; m < R; m++) x[m] = r36_ingest<FMT>(raw[m], ul + R * m, n2g, n2, a, energy, clips);
     }
     mbar_wait(&tbar, 0);
     Dft<R, false>::run(x);
-    float2 wb[6], wa[6];
-#pragma unroll
-    for (int b = 1; b < 6; b++) {
-      wb[b] = s_tw0[(b - 1) * 36 + ul];
-      wa[b] = s_tw0[(4 + b) * 36 + ul];
-    }
-    float2 *d = mycol + ul;
-    d[0] = x[0];
-#pragma unroll
-    for (int t = 1; t < R; t++) d[t * BLK] = cmul(x[t], r36_power(wb, wa, t));
+    r36_stage0_store(x, s_tw0, mycol + ul, ul);
   } else {
     mbar_wait(&tbar, 0);
   }
@@ -149,6 +228,18 @@ __global__ void __launch_bounds__(ColsR36Shape::T, 2) fwd_cols_r36(Pass1Args con
 #pragma unroll
     for (int k = 1; k < R; k++) dst[(long)(R * k) * ld] = cmul(x[k], cmul(w0, r36_power(wb, wa, k)));
   }
+}
+
+// stage 0 from global loads: any input layout
+template <int FMT, int N2C>
+__global__ void __launch_bounds__(ColsR36Shape::T, 2) fwd_cols_r36(Pass1Args const a, ColsR36Tables const tb) {
+  fwd_cols_r36_body<FMT, N2C, false>(a, tb, nullptr);
+}
+// stage 0 from the raw tile the tensor copies fetch: inputs whose tensor map the host could build (kgpu.cu cols_tma_fits)
+template <int FMT, int N2C>
+__global__ void __launch_bounds__(ColsR36Shape::T, 2)
+    fwd_cols_r36_tma(Pass1Args const a, ColsR36Tables const tb, const __grid_constant__ CUtensorMap tmap) {
+  fwd_cols_r36_body<FMT, N2C, true>(a, tb, &tmap);
 }
 
 }  // namespace kfft

@@ -2,6 +2,7 @@
 // launchers behind the C-ABI declared in include/ka9q_gpu.h.  No CPU fallback anywhere: every
 // entry point either launches the sm_90a kernels or fails with -1.
 #include <cuda_runtime.h>
+#include <cudaTypedefs.h>  // PFN_cuTensorMapEncodeTiled: taken from the runtime, the library does not link the driver
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -42,6 +43,22 @@ static std::atomic<int> g_static_on{1};  // tests can force the generic kernels
 extern "C" int kgpu_use_static_kernels(int on) {
   g_static_on.store(on != 0);
   return 0;
+}
+// fwd_cols_r36 fetches its raw tile by tensor copies wherever the input allows (kgpu_use_cols_tma); -1: not yet read
+// from KA9Q_COLS_TMA
+static std::atomic<int> g_cols_tma{-1};
+extern "C" int kgpu_use_cols_tma(int on) {
+  g_cols_tma.store(on != 0);
+  return 0;
+}
+static bool cols_tma_on() {
+  int v = g_cols_tma.load();
+  if (v < 0) {
+    char const *e = getenv("KA9Q_COLS_TMA");
+    g_cols_tma.compare_exchange_strong(v, (e && *e) ? (atoi(e) != 0) : 1);
+    v = g_cols_tma.load();
+  }
+  return v != 0;
 }
 
 static int fail(char const *fmt, ...) {
@@ -784,6 +801,9 @@ static std::vector<float2> bluestein_bspec(long n, long P) {
 // When both passes of a REAL master are specialised (1296 x 1250) the 1/2 of the real split rides on the column pass's
 // inter-pass twiddle, and the inter-pass rows of a specialised pair are padded to 128 bytes.  kgpu_use_static_kernels(0)
 // runs the generic pair instead, at launch time.
+// fwd_cols_r36 comes in two forms with the same arithmetic, chosen per launch (forward_span): fwd_cols_r36_tma has its
+// input tile copied into shared memory by tensor copies, wherever cols_tma_fits finds the input's base and strides 16-byte
+// aligned; fwd_cols_r36 reads it with global loads for any other input, or with kgpu_use_cols_tma(0) / KA9Q_COLS_TMA=0.
 enum ColsKernel { COLS_GENERIC, COLS_R36, COLS_2S };
 enum RowsKernel { ROWS_GENERIC, ROWS_V2, ROWS_2S };
 
@@ -824,6 +844,7 @@ struct kgpu_master {
 
 // the specialised kernels of a master's pair; f: 0 float input, 1 int16, 2 int16 with de-randomisation or statistics
 using ColsR36Fn = void (*)(Pass1Args, ColsR36Tables);
+using ColsR36TmaFn = void (*)(Pass1Args, ColsR36Tables, CUtensorMap);
 using Cols2sFn = void (*)(Pass1Args, Cols2sTables);
 using RowsV2Fn = void (*)(Pass2Args, FwdTables);
 using Cols2s = Cols2sShape<25, 32>;
@@ -831,6 +852,11 @@ using Rows2s = Rows2sShape<25, 25>;
 static ColsR36Fn cols_r36_kernel(kgpu_master const *m, int f) {
   static ColsR36Fn const k[2][3] = {{fwd_cols_r36<0, 0>, fwd_cols_r36<1, 0>, fwd_cols_r36<2, 0>},
                                     {fwd_cols_r36<0, 1250>, fwd_cols_r36<1, 1250>, fwd_cols_r36<2, 1250>}};
+  return k[m->n2c == 1250][f];
+}
+static ColsR36TmaFn cols_r36_tma_kernel(kgpu_master const *m, int f) {
+  static ColsR36TmaFn const k[2][3] = {{fwd_cols_r36_tma<0, 0>, fwd_cols_r36_tma<1, 0>, fwd_cols_r36_tma<2, 0>},
+                                       {fwd_cols_r36_tma<0, 1250>, fwd_cols_r36_tma<1, 1250>, fwd_cols_r36_tma<2, 1250>}};
   return k[m->n2c == 1250][f];
 }
 static Cols2sFn cols_2s_kernel(int f) {
@@ -937,7 +963,9 @@ static int master_setup(kgpu_master *m) {
     }
     if (upload(&m->d_tw0, t0) || upload(&m->d_twA, tA) || upload(&m->d_twB, tB)) return -1;
     for (int f = 0; f < 3; f++)
-      if (allow_smem((const void *)cols_r36_kernel(m, f), ColsR36Shape::smem)) return -1;
+      if (allow_smem((const void *)cols_r36_kernel(m, f), ColsR36Shape::smem) ||
+          allow_smem((const void *)cols_r36_tma_kernel(m, f), ColsR36Shape::smem))
+        return -1;
   }
   if (m->cols == COLS_2S) {  // (25 x 32) x (25 x 25)
     constexpr int RA = 25, RB = 32, RC = 25, RD = 25;
@@ -1164,6 +1192,52 @@ extern "C" int kgpu_master_plan(int L, int M, int in_type, char *buf, int buflen
   return (int)pl.path;
 }
 
+// Whether fwd_cols_r36 can take its raw tile by tensor copies (fwd_cols_r36.cuh): a tensor map needs a 16-byte aligned
+// base and strides that are multiples of 16 bytes.  Its rows are n2 points apart (8 n2 bytes: a row of floats, or a pair of
+// int16 rows, which also needs n1 even) and its windows hop points apart.  Any other input runs the global-load form.
+static bool cols_tma_fits(kgpu_master const *m, void const *d_in, int fmt) {
+  long const point = fmt == KGPU_FMT_I16 ? 4 : 8;  // bytes of a complex input point
+  long const hop = m->in_type == KGPU_REAL ? m->L / 2 : m->L;
+  return m->cols == COLS_R36 && (uintptr_t)d_in % 16 == 0 && hop * point % 16 == 0 && 8L * m->sp.n2 % 16 == 0 &&
+         m->sp.n1 % 2 == 0;
+}
+
+extern "C" int kgpu_cols_tma_fits(int L, int M, int in_type, int fmt, const void *d_in) {
+  MasterPlan pl;
+  if (master_plan(L, M, in_type, MP_BLUESTEIN, "kgpu_cols_tma_fits", &pl)) return -1;
+  if (pl.path != MP_DIRECT) return 0;
+  kgpu_master m;
+  master_shape(&m, L, M, in_type, pl.sp, false);
+  return cols_tma_fits(&m, d_in, fmt) ? 1 : 0;
+}
+
+// The tensor map of the windows of `nblocks` blocks from d_in that fwd_cols_r36_tma reads, for a master and input that
+// cols_tma_fits accepts.  L2 fills in 128-byte pieces: on H100 the column pass took 7.9 us per cfg-2 block so, 8.1 with
+// 256-byte pieces and 8.2 without promotion (int16, tools/cols_tma_ab.py).
+static int cols_tma_map(kgpu_master const *m, void const *d_in, int fmt, int nblocks, CUtensorMap *map) {
+  static PFN_cuTensorMapEncodeTiled const encode = [] {
+    void *fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      fn = nullptr;
+    return (PFN_cuTensorMapEncodeTiled)fn;
+  }();
+  if (!encode) return fail("kgpu_forward: the driver has no cuTensorMapEncodeTiled");
+  bool const i16 = fmt == KGPU_FMT_I16;
+  cuuint64_t const n1 = (cuuint64_t)m->sp.n1, n2 = (cuuint64_t)m->sp.n2;
+  cuuint64_t const hop = (cuuint64_t)(m->in_type == KGPU_REAL ? m->L / 2 : m->L);
+  cuuint64_t const dim[3] = {2 * n2, i16 ? n1 / 2 : n1, (cuuint64_t)nblocks};
+  cuuint64_t const stride[2] = {8 * n2, hop * (i16 ? 4 : 8)};
+  cuuint32_t const box[3] = {(cuuint32_t)(i16 ? ColsR36Tma::I16_BOX_WORDS : 16), ColsR36Tma::BOX_ROWS, 1};
+  cuuint32_t const unit[3] = {1, 1, 1};
+  CUresult const r = encode(map, i16 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void *>(d_in),
+                            dim, stride, box, unit, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("kgpu_forward: cuTensorMapEncodeTiled failed (%d)", (int)r);
+  return 0;
+}
+
 // One launch pair (column pass, row pass) over `nblocks` consecutive blocks on stream `st`, inter-pass data in `mid`.
 static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, int derandomize, int nblocks, void *d_spec,
                         void *d_stats, cudaStream_t st, float2 *mid) {
@@ -1195,7 +1269,13 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
         cols_2s_kernel(f)<<<g1, Cols2s::T, Cols2s::smem, st>>>(a1, Cols2sTables{m->d_tw0, m->d_twA, m->d_twB});
         break;
       case COLS_R36:
-        cols_r36_kernel(m, f)<<<g1, ColsR36Shape::T, ColsR36Shape::smem, st>>>(a1, ColsR36Tables{m->d_tw0, m->d_twA, m->d_twB});
+        if (cols_tma_on() && cols_tma_fits(m, d_in, fmt)) {
+          CUtensorMap map;
+          if (cols_tma_map(m, d_in, fmt, nblocks, &map)) return -1;
+          cols_r36_tma_kernel(m, f)<<<g1, ColsR36Shape::T, ColsR36Shape::smem, st>>>(a1, ColsR36Tables{m->d_tw0, m->d_twA, m->d_twB}, map);
+        } else {
+          cols_r36_kernel(m, f)<<<g1, ColsR36Shape::T, ColsR36Shape::smem, st>>>(a1, ColsR36Tables{m->d_tw0, m->d_twA, m->d_twB});
+        }
         break;
       case COLS_GENERIC:
         if (m->ext && f) fwd_cols_ext<1><<<g1, kFwdThreads, m->smem1, st>>>(a1, m->xplan1);
