@@ -315,6 +315,26 @@ int kgpu_use_cols_tma(int on);
 /* Pure host code: 1 if kgpu_forward of the master kgpu_master_create_any(L, M, in_type) builds, fed `fmt` input at d_in,
  * runs fwd_cols_r36 on tensor copies (with kgpu_use_cols_tma on), 0 if it does not, -1 for a length with no master. */
 int kgpu_cols_tma_fits(int L, int M, int in_type, int fmt, const void *d_in);
+/* REAL masters split 1296 x 1250 run their column and row passes as one launch, fwd_fused_r36_v2, wherever the column
+ * pass could take its tile by tensor copies (kgpu_cols_tma_fits, with kgpu_use_cols_tma on), in launches of 2 or more
+ * blocks: each block's row pass then overlaps the next block's column pass and reads its inter-pass rows from L2.  Every other master and input runs the two-kernel pair.  The
+ * spectra and statistics are bitwise the same either way.  The default is on, or what the environment variable
+ * KA9Q_FUSED_FWD (0 / 1) says when the first launch reads it; a call takes effect at the next launch. */
+int kgpu_use_fused_forward(int on);
+/* Pure host code: 1 if kgpu_forward of the master kgpu_master_create_any(L, M, in_type), fed `fmt` input at d_in, runs
+ * the fused launch for 2 or more blocks (with kgpu_use_fused_forward and kgpu_use_cols_tma on), 0 if not, -1 for a length with no master. */
+int kgpu_fused_forward_fits(int L, int M, int in_type, int fmt, const void *d_in);
+/* Testing and measuring aids of the fused launch.  kgpu_fused_forward_options: `lead` (0 .. the C items per block) column
+ * items of the next block go before a block's first row item; discard = 1 drops each inter-pass row from L2 once it is
+ * read (default 0).  Takes effect at the next launch.  kgpu_fused_shape fills out[5] = {C items per block,
+ * R items per block, n1, inter-pass row pitch in points, default lead}.  kgpu_fused_schedule fills out[5] = {kind
+ * (0 C, 1 R), block, item, the block whose C items it waits for (-1: none), how many} for a ticket of a launch of
+ * nblocks blocks.  kgpu_fused_discards writes the 128-byte lines (from the inter-pass buffer's start) that item R(blk, idx)
+ * discards to lines[0 .. max-1] and returns their count.  All pure host code. */
+int kgpu_fused_forward_options(int lead, int discard);
+int kgpu_fused_shape(int *out);
+int kgpu_fused_schedule(int nblocks, int lead, int ticket, int *out);
+long kgpu_fused_discards(int blk, int idx, long *lines, long max);
 
 /* Planner introspection, pure host code (works without a GPU): the in-register radices chosen for
  * a column transform of length len (returns their count, -1 if unplannable) and the two-pass split

@@ -108,6 +108,13 @@ def load() -> C.CDLL:
     L.kgpu_use_static_kernels.argtypes = [i]
     L.kgpu_use_cols_tma.argtypes = [i]
     L.kgpu_cols_tma_fits.argtypes = [i, i, i, i, vp]
+    L.kgpu_use_fused_forward.argtypes = [i]
+    L.kgpu_fused_forward_fits.argtypes = [i, i, i, i, vp]
+    L.kgpu_fused_forward_options.argtypes = [i, i]
+    L.kgpu_fused_shape.argtypes = [vp]
+    L.kgpu_fused_schedule.argtypes = [i, i, i, vp]
+    L.kgpu_fused_discards.argtypes = [i, i, vp, l]
+    L.kgpu_fused_discards.restype = l
     L.kgpu_profile_enable.argtypes = [i]
     L.kgpu_profile_name.argtypes = [i]
     L.kgpu_profile_name.restype = C.c_char_p

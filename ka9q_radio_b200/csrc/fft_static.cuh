@@ -160,6 +160,11 @@ __device__ __forceinline__ void tensor_g2s_3d(void *dst, void const *map, int x,
                ::"r"(smem_u32(dst)), "l"(map), "r"(x), "r"(y), "r"(z), "r"(smem_u32(bar))
                : "memory");
 }
+// orders this thread's earlier generic-proxy view of global memory (what an acquire made visible) before its later
+// async-proxy accesses (bulk and tensor copies)
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+// drops one 128-byte L2 line (128-byte aligned) without writing it back: its contents become undefined
+__device__ __forceinline__ void discard_l2_line(void *p) { asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory"); }
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"

@@ -102,17 +102,18 @@ __device__ __forceinline__ void r36_stage0_store(float2 (&x)[36], float2 const *
   for (int t = 1; t < R; t++) d[t * BLK] = cmul(x[t], r36_power(wb, wa, t));
 }
 
-template <int FMT, int N2C, bool TMA>
-__device__ __forceinline__ void fwd_cols_r36_body(Pass1Args const &a, ColsR36Tables const &tb, CUtensorMap const *tmap) {
+// One column tile: columns c0 .. c0+7 of block blk, by the 288 threads tid = 0..287 that `sync` (a barrier of exactly
+// those threads) joins, in ColsR36Shape::smem bytes of shared memory at smem_raw (16-byte aligned), with tbar its
+// copies' mbarrier.  The kernels below run one tile per CTA; fwd_fused_r36_v2 (fwd_fused.cuh) two side by side.
+template <int FMT, int N2C, bool TMA, class Sync>
+__device__ __forceinline__ void fwd_cols_r36_body(Pass1Args const &a, ColsR36Tables const &tb, CUtensorMap const *tmap,
+                                                  unsigned char *smem_raw, uint64_t &tbar, int tid, int c0, int blk,
+                                                  Sync const &sync) {
   constexpr int R = 36, BLK = ColsR36Shape::BLK, CP = ColsR36Shape::CP;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
   float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // [8][CP]
   float2 *s_tw0 = tile + 8 * CP;                        // [10][36]
   float2 *s_twB = s_tw0 + 360;                          // [8][10]
-  __shared__ __align__(8) uint64_t tbar;
-  int const tid = threadIdx.x;
   int const c = tid & 7, ul = tid >> 3;  // column of the tile, butterfly 0..35
-  int const c0 = blockIdx.x * 8, blk = blockIdx.y;
   int const n2 = N2C ? N2C : a.n2;  // N2C: number of columns as a compile-time constant (0 = from the arguments)
   // rows of the inter-pass buffer padded to whole 128-byte lines: every 64-byte store piece of this kernel then lies in ONE
   // line (with the natural pitch of 10 000 bytes 3 of 8 pieces straddle two: +27 % L1TEX wavefronts for the stores)
@@ -145,7 +146,7 @@ __device__ __forceinline__ void fwd_cols_r36_body(Pass1Args const &a, ColsR36Tab
     bulk_g2s(s_tw0, tb.tw0, 360 * 8, &tbar);
     bulk_g2s(s_twB, tb.twB + (long)c0 * 10, 80 * 8, &tbar);  // table padded by 8 columns
   }
-  __syncthreads();  // barrier initialised before anybody waits on it
+  sync();  // barrier initialised before anybody waits on it
   float2 const twA = col_ok ? ldg_stream_f2(tb.twA + (long)n2g * 36 + ul) : make_float2(1.f, 0.f);
 
   // ---- stage 0 fused with the load: x[j + 36 m], m = 0..35, j = ul --------------------------------------------
@@ -170,7 +171,7 @@ __device__ __forceinline__ void fwd_cols_r36_body(Pass1Args const &a, ColsR36Tab
       }
       Dft<R, false>::run(x);
     }
-    __syncthreads();  // the raw tile is read: stage 0 may overwrite it
+    sync();  // the raw tile is read: stage 0 may overwrite it
     if (col_ok) r36_stage0_store(x, s_tw0, mycol + ul, ul);
   } else if (col_ok) {
     float2 x[R];
@@ -203,7 +204,7 @@ __device__ __forceinline__ void fwd_cols_r36_body(Pass1Args const &a, ColsR36Tab
       atomicAdd(&a.stats[blk].clips, clips);
     }
   }
-  __syncthreads();
+  sync();
 
   // ---- stage 1 fused with the store: sub-transform t = ul, X[t + 36 k'] * W_nc^{n2 (t + 36 k')} -> mid ------------
   if (col_ok) {
@@ -233,13 +234,19 @@ __device__ __forceinline__ void fwd_cols_r36_body(Pass1Args const &a, ColsR36Tab
 // stage 0 from global loads: any input layout
 template <int FMT, int N2C>
 __global__ void __launch_bounds__(ColsR36Shape::T, 2) fwd_cols_r36(Pass1Args const a, ColsR36Tables const tb) {
-  fwd_cols_r36_body<FMT, N2C, false>(a, tb, nullptr);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  __shared__ __align__(8) uint64_t tbar;
+  fwd_cols_r36_body<FMT, N2C, false>(a, tb, nullptr, smem_raw, tbar, threadIdx.x, blockIdx.x * 8, blockIdx.y,
+                                     [] { __syncthreads(); });
 }
 // stage 0 from the raw tile the tensor copies fetch: inputs whose tensor map the host could build (kgpu.cu cols_tma_fits)
 template <int FMT, int N2C>
 __global__ void __launch_bounds__(ColsR36Shape::T, 2)
     fwd_cols_r36_tma(Pass1Args const a, ColsR36Tables const tb, const __grid_constant__ CUtensorMap tmap) {
-  fwd_cols_r36_body<FMT, N2C, true>(a, tb, &tmap);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  __shared__ __align__(8) uint64_t tbar;
+  fwd_cols_r36_body<FMT, N2C, true>(a, tb, &tmap, smem_raw, tbar, threadIdx.x, blockIdx.x * 8, blockIdx.y,
+                                    [] { __syncthreads(); });
 }
 
 }  // namespace kfft

@@ -182,7 +182,7 @@ struct RowItem {   // one unit of pass-2 work: a row, or a mirrored pair of rows
 
 // Pass-2 work item p.  REAL: row 0 | pairs (k1, n1-k1) | row n1/2 (n1 even) | empty padding, n1/2 + 1 items in all.
 // COMPLEX: row p | empty padding.
-__device__ __forceinline__ RowItem row_item(int p, int n1, bool real_split) {
+__host__ __device__ __forceinline__ RowItem row_item(int p, int n1, bool real_split) {
   RowItem it;
   if (!real_split) {
     it.kind = p < n1 ? kRowPlain : kRowEmpty;

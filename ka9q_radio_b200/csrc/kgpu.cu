@@ -26,6 +26,7 @@
 #include "static_kernels.cuh"
 #include "static_kernels_v2.cuh"
 #include "fwd_cols_r36.cuh"
+#include "fwd_fused.cuh"
 #include "fwd_2s.cuh"
 #include "spectrum_kernels.cuh"
 #include "bluestein_master.cuh"
@@ -57,6 +58,24 @@ static bool cols_tma_on() {
     char const *e = getenv("KA9Q_COLS_TMA");
     g_cols_tma.compare_exchange_strong(v, (e && *e) ? (atoi(e) != 0) : 1);
     v = g_cols_tma.load();
+  }
+  return v != 0;
+}
+// REAL 1296 x 1250 masters run both passes as one launch (fwd_fused_r36_v2) wherever the column pass could take its
+// tile by tensor copies (kgpu_use_fused_forward); -1: not yet read from KA9Q_FUSED_FWD
+static std::atomic<int> g_fused{-1};
+// The L2 discard of the inter-pass rows is off by default: on H100 it cost 0.6 us per cfg-2 block (DESIGN.md section 4).
+static std::atomic<int> g_fused_lead{FusedShape::DEFAULT_LEAD}, g_fused_discard{0};
+extern "C" int kgpu_use_fused_forward(int on) {
+  g_fused.store(on != 0);
+  return 0;
+}
+static bool fused_on() {
+  int v = g_fused.load();
+  if (v < 0) {
+    char const *e = getenv("KA9Q_FUSED_FWD");
+    g_fused.compare_exchange_strong(v, (e && *e) ? (atoi(e) != 0) : 1);
+    v = g_fused.load();
   }
   return v != 0;
 }
@@ -127,8 +146,8 @@ static int grow(StreamBuf &s, size_t bytes, cudaStream_t st, char const *who) {
 // ------------------------------------------------------------------ per-launch profiling -----
 // When enabled, every kernel launch is bracketed by CUDA events on the launching stream; bench.py
 // reads the per-kernel totals for its roofline line (events are markers, they do not serialise).
-enum KernelId { K_FWD_COLS = 0, K_FWD_ROWS, K_CHAN, K_NOTCH, K_RESPONSE, K_NOISE, K_COUNT };
-static char const *const kKernelNames[K_COUNT] = {"fwd_cols", "fwd_rows", "chan", "notch", "response_fft", "noise"};
+enum KernelId { K_FWD_COLS = 0, K_FWD_ROWS, K_CHAN, K_NOTCH, K_RESPONSE, K_NOISE, K_FWD_FUSED, K_COUNT };
+static char const *const kKernelNames[K_COUNT] = {"fwd_cols", "fwd_rows", "chan", "notch", "response_fft", "noise", "fwd_fused"};
 struct ProfRec {
   cudaEvent_t a, b;
   int kid;
@@ -825,6 +844,7 @@ struct kgpu_master {
   float2 *d_tw0 = nullptr, *d_twA = nullptr, *d_twB = nullptr;  // tables of fwd_cols_r36 / fwd_cols_2s
   float2 *d_rtw0 = nullptr;        // stage-0 powers of fwd_rows_2s
   StreamBuf mid;                   // the inter-pass buffer
+  StreamBuf fused_ctr;             // fwd_fused_r36_v2's ticket and done counters (FusedArgs::ctr)
   size_t smem1 = 0, smem2 = 0;     // generic kernels
   // kgpu_master_create_ex with a prime factor 11 .. 23: the master owns its two plans (plan1 / plan2 stay -1) and runs
   // the extended pair fwd_cols_ext / fwd_rows_ext, which take them by value
@@ -866,6 +886,17 @@ static Cols2sFn cols_2s_kernel(int f) {
 static RowsV2Fn rows_v2_kernel(kgpu_master const *m) {
   if (m->in_type == KGPU_REAL) return m->halved ? fwd_rows_v2<true, 1296, true> : fwd_rows_v2<true, 0, false>;
   return m->n1c ? fwd_rows_v2<false, 1296, false> : fwd_rows_v2<false, 0, false>;
+}
+// Whether a master's pair can run as one launch (fwd_fused.cuh): REAL with the 1296 x 1250 pair and the real split's 1/2
+// folded into the column pass.  The input decides the rest (fused_fits).
+static bool fused_pair(kgpu_master const *m) {
+  return m->in_type == KGPU_REAL && m->cols == COLS_R36 && m->rows == ROWS_V2 && m->halved && m->n2c == FusedShape::N2 &&
+         m->n1c == FusedShape::N1 && m->mid_ld % 16 == 0;
+}
+using FusedFn = void (*)(Pass1Args, ColsR36Tables, Pass2Args, FwdTables, FusedArgs, CUtensorMap);
+static FusedFn fused_kernel(int f) {
+  static FusedFn const k[3] = {fwd_fused_r36_v2<0>, fwd_fused_r36_v2<1>, fwd_fused_r36_v2<2>};
+  return k[f];
 }
 static int rows_v2_threads(kgpu_master const *m) { return m->in_type == KGPU_REAL ? RowsV2Shape<true>::T : RowsV2Shape<false>::T; }
 static size_t rows_v2_smem(kgpu_master const *m) {
@@ -985,6 +1016,9 @@ static int master_setup(kgpu_master *m) {
     if (allow_smem((const void *)fwd_rows_2s<25, 25>, Rows2s::smem)) return -1;
   }
   if (m->rows == ROWS_V2 && allow_smem((const void *)rows_v2_kernel(m), rows_v2_smem(m))) return -1;
+  if (fused_pair(m))
+    for (int f = 0; f < 3; f++)
+      if (allow_smem((const void *)fused_kernel(f), FusedShape::smem)) return -1;
   // an extended master runs the extended pair; the generic pair can run for every other one (kgpu_use_static_kernels(0))
   if (m->ext) {
     if (allow_smem((const void *)fwd_cols_ext<0>, m->smem1) || allow_smem((const void *)fwd_cols_ext<1>, m->smem1) ||
@@ -1010,6 +1044,7 @@ extern "C" void kgpu_master_destroy(kgpu_master *m) {
   cudaFree(m->d_twB);
   cudaFree(m->d_rtw0);
   cudaFree(m->mid.p);
+  cudaFree(m->fused_ctr.p);
   cudaFree(m->d_notch);
   kgpu_master_destroy(m->bs);
   cudaFree(m->blue.d_b);
@@ -1211,6 +1246,64 @@ extern "C" int kgpu_cols_tma_fits(int L, int M, int in_type, int fmt, const void
   return cols_tma_fits(&m, d_in, fmt) ? 1 : 0;
 }
 
+// Whether both passes run as one launch (fwd_fused.cuh): a master whose pair allows it and an input the column pass can
+// take by tensor copies.
+static bool fused_fits(kgpu_master const *m, void const *d_in, int fmt) { return fused_pair(m) && cols_tma_fits(m, d_in, fmt); }
+
+extern "C" int kgpu_fused_forward_fits(int L, int M, int in_type, int fmt, const void *d_in) {
+  MasterPlan pl;
+  if (master_plan(L, M, in_type, MP_BLUESTEIN, "kgpu_fused_forward_fits", &pl)) return -1;
+  if (pl.path != MP_DIRECT) return 0;
+  kgpu_master m;
+  master_shape(&m, L, M, in_type, pl.sp, false);
+  return fused_fits(&m, d_in, fmt) ? 1 : 0;
+}
+
+extern "C" int kgpu_fused_forward_options(int lead, int discard) {
+  if (lead < 0 || lead > FusedShape::NC) return fail("kgpu_fused_forward_options: lead %d outside 0..%d", lead, FusedShape::NC);
+  g_fused_lead.store(lead);
+  g_fused_discard.store(discard != 0);
+  return 0;
+}
+
+extern "C" int kgpu_fused_shape(int *out) {
+  if (!out) return fail("kgpu_fused_shape: bad arguments");
+  out[0] = FusedShape::NC;
+  out[1] = FusedShape::NR;
+  out[2] = FusedShape::N1;
+  out[3] = (FusedShape::N2 + 15) / 16 * 16;
+  out[4] = FusedShape::DEFAULT_LEAD;
+  return 0;
+}
+
+extern "C" int kgpu_fused_schedule(int nblocks, int lead, int ticket, int *out) {
+  if (nblocks < 1 || lead < 0 || lead > FusedShape::NC || ticket < 0 || ticket >= nblocks * (FusedShape::NC + FusedShape::NR) ||
+      !out)
+    return fail("kgpu_fused_schedule: bad arguments");
+  FusedItem const it = fused_item(ticket, nblocks, lead);
+  out[0] = it.kind;
+  out[1] = it.blk;
+  out[2] = it.idx;
+  out[3] = it.kind == kFusedRow ? it.blk : -1;  // the done counter it waits on, and for what count
+  out[4] = it.kind == kFusedRow ? FusedShape::NC : 0;
+  return 0;
+}
+
+extern "C" long kgpu_fused_discards(int blk, int idx, long *lines, long max) {
+  using S = RowsV2Shape<true>;
+  if (blk < 0 || idx < 0 || idx >= FusedShape::NR || max < 0) return fail("kgpu_fused_discards: bad arguments");
+  int const ld = (FusedShape::N2 + 15) / 16 * 16;
+  long n = 0;
+  for (int col = 0; col < S::COLS; col++) {  // the rows fwd_rows_v2_body's tile columns hold
+    RowItem const it = row_item(idx * S::IPC + (col >> 1), FusedShape::N1, true);
+    int const row = (col & 1) == 0 ? (it.kind != kRowEmpty ? it.row_a : -1) : (it.kind == kRowPair ? it.row_b : -1);
+    if (row < 0) continue;
+    for (int l = 0; l < mid_row_lines(ld); l++, n++)
+      if (lines && n < max) lines[n] = mid_line(blk, FusedShape::N1, row, ld, l);
+  }
+  return n;
+}
+
 // The tensor map of the windows of `nblocks` blocks from d_in that fwd_cols_r36_tma reads, for a master and input that
 // cols_tma_fits accepts.  L2 fills in 128-byte pieces: on H100 the column pass took 7.9 us per cfg-2 block so, 8.1 with
 // 256-byte pieces and 8.2 without promotion (int16, tools/cols_tma_ab.py).
@@ -1238,6 +1331,47 @@ static int cols_tma_map(kgpu_master const *m, void const *d_in, int fmt, int nbl
   return 0;
 }
 
+// The Pass2Args of the row pass, for the Pass1Args a1 of the same launch
+static Pass2Args rows_args(kgpu_master const *m, Pass1Args const &a1, void *d_spec) {
+  Pass2Args a2;
+  a2.mid = a1.mid;
+  a2.n1 = m->sp.n1;
+  a2.n2 = m->sp.n2;
+  a2.nc = m->nc;
+  a2.plan = m->plan2;
+  a2.pitch = m->pitch2;
+  a2.real_split = (m->in_type == KGPU_REAL);
+  a2.rootD = m->d_rootD;
+  a2.spec = (float2 *)d_spec;
+  a2.spec_stride = m->spec_stride;
+  a2.mid_ld = a1.mid_ld;
+  return a2;
+}
+
+// Both passes over `nblocks` blocks as one launch of fwd_fused_r36_v2, for a master and input fused_fits accepts.
+static int fused_span(kgpu_master *m, const void *d_in, int fmt, int f, int nblocks, void *d_spec, cudaStream_t st,
+                      Pass1Args const &a1) {
+  using F = FusedShape;
+  size_t const ctr_bytes = sizeof(unsigned) * (size_t)(1 + nblocks);
+  if (grow(m->fused_ctr, ctr_bytes, st, "kgpu_forward")) return -1;
+  CUtensorMap map;
+  if (cols_tma_map(m, d_in, fmt, nblocks, &map)) return -1;
+  FusedArgs fa;
+  fa.ctr = (unsigned *)m->fused_ctr.p;
+  fa.nblocks = nblocks;
+  fa.lead = g_fused_lead.load();
+  fa.discard = g_fused_discard.load();
+  CUDA_OK(cudaMemsetAsync(fa.ctr, 0, ctr_bytes, st));
+  {
+    ProfScope ps(K_FWD_FUSED, st);
+    fused_kernel(f)<<<(unsigned)(nblocks * (F::NC + F::NR)), F::T, F::smem, st>>>(a1, ColsR36Tables{m->d_tw0, m->d_twA, m->d_twB},
+                                                                       rows_args(m, a1, d_spec), FwdTables{m->d_rootC}, fa, map);
+  }
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 // One launch pair (column pass, row pass) over `nblocks` consecutive blocks on stream `st`, inter-pass data in `mid`.
 static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, int derandomize, int nblocks, void *d_spec,
                         void *d_stats, cudaStream_t st, float2 *mid) {
@@ -1261,6 +1395,8 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
   a1.out_scale = (fmt == KGPU_FMT_I16 ? scale : 1.0f) * (m->halved ? 0.5f : 1.0f);
   a1.mid_ld = use_static ? m->mid_ld : m->sp.n2;
   int const f = (fmt != KGPU_FMT_I16) ? 0 : ((derandomize || a1.stats) ? 2 : 1);
+  // one block has nothing to overlap: its row items could only wait for its column items, so it runs the pair
+  if (nblocks >= 2 && use_static && cols_tma_on() && fused_on() && fused_fits(m, d_in, fmt)) return fused_span(m, d_in, fmt, f, nblocks, d_spec, st, a1);
   dim3 const g1((unsigned)((m->sp.n2 + kTile - 1) / kTile), (unsigned)nblocks);
   {
     ProfScope ps(K_FWD_COLS, st);
@@ -1286,18 +1422,7 @@ static int forward_span(kgpu_master *m, const void *d_in, int fmt, float scale, 
     }
   }
   g_launches++;
-  Pass2Args a2;
-  a2.mid = mid;
-  a2.n1 = m->sp.n1;
-  a2.n2 = m->sp.n2;
-  a2.nc = m->nc;
-  a2.plan = m->plan2;
-  a2.pitch = m->pitch2;
-  a2.real_split = (m->in_type == KGPU_REAL);
-  a2.rootD = m->d_rootD;
-  a2.spec = (float2 *)d_spec;
-  a2.spec_stride = m->spec_stride;
-  a2.mid_ld = a1.mid_ld;
+  Pass2Args const a2 = rows_args(m, a1, d_spec);
   dim3 const g2((unsigned)(rows == ROWS_GENERIC ? m->n_item_ctas : m->n_rows_ctas), (unsigned)nblocks);
   {
     ProfScope ps(K_FWD_ROWS, st);

@@ -73,22 +73,31 @@ __device__ constexpr float kRowsTw0[3][4][2] = {
 // butterfly.  Variants tried and removed again: warp-per-column stages 0/1, stage-0 butterflies in groups of 2 / 4,
 // stage-1 twiddles by products, a persistent double-buffered form, an L2 prefetch of a later CTA's rows, blocks first-to-last,
 // REAL with 4 row pairs per 256-thread CTA (32-byte store runs; 18.2 against 13.5 us per cfg-2 block, DESIGN.md section 4).
-template <bool REAL_SPLIT, int N1C = 0, bool HALVED = false>
-__global__ void __launch_bounds__(RowsV2Shape<REAL_SPLIT>::T, REAL_SPLIT ? 1 : 2) fwd_rows_v2(Pass2Args const a, FwdTables const tb) {
+// The 128-byte lines of the inter-pass buffer (rows of mid_ld points, a multiple of 16): line l of row `row` of block
+// blk, counted from the buffer's start
+__host__ __device__ constexpr int mid_row_lines(int mid_ld) { return mid_ld * 8 / 128; }
+__host__ __device__ constexpr long mid_line(int blk, int n1, int row, int mid_ld, int l) {
+  return ((long)blk * n1 + row) * mid_row_lines(mid_ld) + l;
+}
+
+// The row tile of items item0 .. item0+IPC-1 of block blk, by the S::T threads tid = 0..T-1, in S::smem bytes of shared
+// memory at smem_raw with the mbarriers bars[COLS] and tbar.  sync / sync_or: a barrier (and its OR reduction) of exactly
+// those threads; the groups' barriers are 1 and 2.  FUSED (fwd_fused.cuh): the caller has acquired the block's inter-pass
+// rows, written by other SMs; each row's copy is ordered after that through the async proxy, and the row's L2 lines are
+// discarded once it is in shared memory (nothing reads them again, so they never have to be written back to DRAM).
+template <bool REAL_SPLIT, int N1C, bool HALVED, bool FUSED, class Sync, class SyncOr>
+__device__ __forceinline__ void fwd_rows_v2_body(Pass2Args const &a, FwdTables const &tb, unsigned char *smem_raw,
+                                                 uint64_t *bars, uint64_t &tbar, int tid, int blk, int item0,
+                                                 Sync const &sync, SyncOr const &sync_or, bool discard = false) {
   using S = RowsV2Shape<REAL_SPLIT>;
   using P = typename S::P;
   constexpr int N2 = S::N2, T = S::T, GT = S::GT, COLS = S::COLS, IPC = S::IPC;
   constexpr int R0 = 10, S0 = 125, R1 = 25, NSUB1 = 125, S1 = 5, R2 = 5;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
   float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // COLS columns at S::col_off(c)
   float2 *s_tw = tile + S::TILE;
-  __shared__ __align__(8) uint64_t bars[COLS];
-  __shared__ __align__(8) uint64_t tbar;
   TilePlan const &pl = c_plans[a.plan];
-  int const tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  int const blk = gridDim.y - 1 - blockIdx.y;
+  int const lane = tid & 31, warp = tid >> 5;
   int const n1 = N1C ? N1C : a.n1;
-  int const item0 = blockIdx.x * IPC;
   // which global row sits in which tile column
   auto row_of = [&](int col) -> int {
     RowItem const it = row_item(item0 + (REAL_SPLIT ? col >> 1 : col), n1, REAL_SPLIT);
@@ -104,6 +113,7 @@ __global__ void __launch_bounds__(RowsV2Shape<REAL_SPLIT>::T, REAL_SPLIT ? 1 : 2
     if (warp == 0) mbar_init(&tbar, 1);
     mbar_fence_init();
     if (row >= 0) {
+      if (FUSED) fence_proxy_async_global();
       mbar_expect_tx(&bars[warp], N2 * 8);
       bulk_g2s(tile + S::col_off(warp), a.mid + ((long)blk * n1 + row) * a.mid_ld, N2 * 8, &bars[warp]);
     }
@@ -113,17 +123,21 @@ __global__ void __launch_bounds__(RowsV2Shape<REAL_SPLIT>::T, REAL_SPLIT ? 1 : 2
       bulk_g2s(s_tw, pl.tw, TWB, &tbar);
     }
   }
-  __syncthreads();
+  sync();
   int const g = tid / GT;                                  // group
   int const c = (tid & 7) + 8 * g, ul = (tid % GT) >> 3;  // column, butterfly lane 0..31
   // stages 0 and 1 of a group touch only its own columns: the groups meet only before stage 2
   auto group_sync = [&] {
-    if (S::NG == 1) __syncthreads();
+    if (S::NG == 1) sync();
     else asm volatile("bar.sync %0, %1;" ::"r"(1 + g), "n"(GT) : "memory");
   };
   bool const col_ok = row_of(c) >= 0;
   mbar_wait(&tbar, 0);
   if (col_ok) mbar_wait(&bars[c], 0);
+  if (FUSED && discard && col_ok) {  // the 32 threads of column c discard its row's lines (scratch: no result changes)
+    char *const mid = const_cast<char *>(reinterpret_cast<char const *>(a.mid));
+    for (int l = ul; l < mid_row_lines(a.mid_ld); l += GT / 8) discard_l2_line(mid + 128 * mid_line(blk, n1, row_of(c), a.mid_ld, l));
+  }
   float2 *mycol = tile + S::col_off(c);
 
   // ---- stage 0: radix 10, stride 125 (125 butterflies per column) ------------------------------
@@ -188,7 +202,7 @@ __global__ void __launch_bounds__(RowsV2Shape<REAL_SPLIT>::T, REAL_SPLIT ? 1 : 2
       rd[q] = (it.kind == kRowPair && u < N2 / R2) ? __ldg(a.rootD + t0 + 10 * t1) : make_float2(1.f, 0.f);
     }
   }
-  int const has_self = __syncthreads_or(self_item);
+  int const has_self = sync_or(self_item);
 
   float2 *spec = a.spec + (long)blk * a.spec_stride;
   float const hf = HALVED ? 1.0f : 0.5f;
@@ -261,7 +275,7 @@ __global__ void __launch_bounds__(RowsV2Shape<REAL_SPLIT>::T, REAL_SPLIT ? 1 : 2
       for (int m = 0; m < R2; m++) col[u * R2 + m] = x[m];
     }
   }
-  __syncthreads();
+  sync();
   for (int s = 0; s < IPC; s++) {
     RowItem const its = row_item(item0 + s, n1, true);
     if (its.kind != kRowSelf0 && its.kind != kRowSelfMid) continue;
@@ -281,6 +295,16 @@ __global__ void __launch_bounds__(RowsV2Shape<REAL_SPLIT>::T, REAL_SPLIT ? 1 : 2
       if (nc - k != k) spec[nc - k] = make_float2(E.x - Pp.y, -(E.y + Pp.x));
     }
   }
+}
+
+template <bool REAL_SPLIT, int N1C = 0, bool HALVED = false>
+__global__ void __launch_bounds__(RowsV2Shape<REAL_SPLIT>::T, REAL_SPLIT ? 1 : 2) fwd_rows_v2(Pass2Args const a, FwdTables const tb) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  __shared__ __align__(8) uint64_t bars[RowsV2Shape<REAL_SPLIT>::COLS];
+  __shared__ __align__(8) uint64_t tbar;
+  fwd_rows_v2_body<REAL_SPLIT, N1C, HALVED, false>(a, tb, smem_raw, bars, tbar, threadIdx.x, gridDim.y - 1 - blockIdx.y,
+                                                   blockIdx.x * RowsV2Shape<REAL_SPLIT>::IPC, [] { __syncthreads(); },
+                                                   [](int p) { return __syncthreads_or(p); });
 }
 
 // ------------------------------------------------------------------ channels ------------------
