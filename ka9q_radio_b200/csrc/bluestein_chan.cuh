@@ -22,7 +22,7 @@ __global__ void __launch_bounds__(kBluesteinThreads) bluestein_chan_in(ChanArgs 
   long const k = (long)blockIdx.x * kBluesteinThreads + threadIdx.x;
   if (k >= P) return;
   int const oi = blockIdx.y;
-  int const ci = a.order ? a.order[oi] : a.chan_base + oi;
+  int const ci = chan_index(a, oi);
   ChanDesc const d = a.desc[ci];
   if (d.plan < 0) return;
   int const blk = blockIdx.z;
@@ -41,9 +41,8 @@ __global__ void __launch_bounds__(kBluesteinThreads) bluestein_chan_in(ChanArgs 
 // partial: [row][gridDim.x] per-CTA power sums of kChanOsc channels.
 __global__ void __launch_bounds__(kBluesteinThreads) bluestein_chan_out(ChanArgs const a, double inv_p, float2 const *y, long y_stride,
                                                                        float *partial) {
-  __shared__ float red[kBluesteinThreads / 32];
   int const oi = blockIdx.y;
-  int const ci = a.order ? a.order[oi] : a.chan_base + oi;
+  int const ci = chan_index(a, oi);
   ChanDesc const d = a.desc[ci];
   if (d.plan < 0) return;
   int const blk = blockIdx.z, tid = threadIdx.x;
@@ -64,19 +63,9 @@ __global__ void __launch_bounds__(kBluesteinThreads) bluestein_chan_out(ChanArgs
   if (d.flags & kChanOsc) {
     ChanAux const ax = a.aux[ci];
     float pw = 0.f;
-    if (live) {
-      v = osc_rotate(v, osc_phase_cycles(ax, a.block0 + blk - ax.osc_epoch, d.olen, i));
-      dst[i] = v;
-      pw = v.x * v.x + v.y * v.y;
-    }
-    pw = warp_sum(pw);
-    if ((tid & 31) == 0) red[tid >> 5] = pw;
-    __syncthreads();
-    if (partial && tid == 0) {
-      float s = 0.f;
-      for (int w = 0; w < kBluesteinThreads / 32; w++) s += red[w];
-      partial[row * gridDim.x + blockIdx.x] = s;
-    }
+    if (live) dst[i] = osc_sample(ax, a.block0 + blk - ax.osc_epoch, d.olen, i, v, pw);
+    float const s = cta_power_sum<kBluesteinThreads>(pw);
+    if (partial && tid == 0) partial[row * gridDim.x + blockIdx.x] = s;
     return;
   }
   if (live) dst[i] = v;

@@ -35,73 +35,34 @@ struct HugeGeom {
   int plan1, plan2;    // registry plans of length n1 (pass A) and n2 (pass B)
 };
 
-// The slice element w of chan_wide's load (plain walk, conjugate walk, COMPLEX wrap, beam), Nyquist slot zero.
-__device__ __forceinline__ float2 huge_base(ChanArgs const &a, ChanDesc const &d, ChanAux const &ax, float2 const *X,
-                                            float2 const *R, int w, int top) {
-  int const ns = d.points;
-  int t = w - top;
-  if (t < 0) t += ns;
-  int const u = t - d.zlead;
-  if (!(u >= 0 && u < d.ncopy && w != top)) return make_float2(0.f, 0.f);  // filter.c:911 zeroes the Nyquist slot
-  int q = d.q0 + d.dir * u;
-  if (a.wrap && q >= a.m_bins) q -= a.m_bins;
-  float2 const r = __ldg(R + w);
-  float2 x = __ldg(X + q);
-  if (d.flags & kChanBeam) {  // filter.c:756-775 in double complex, rounded to float once
-    int const m = a.m_bins;
-    double sr, si_;
-    if (q == 0 || q == m / 2) {
-      sr = (double)x.x * ax.are + (double)x.y * ax.bre;
-      si_ = (double)x.x * ax.aim + (double)x.y * ax.bim;
-    } else {
-      float2 const y = __ldg(X + (m - q));
-      sr = ax.are * x.x - ax.aim * x.y + ax.bre * y.x + ax.bim * y.y;
-      si_ = ax.are * x.y + ax.aim * x.x - ax.bre * y.y + ax.bim * y.x;
-    }
-    return make_float2((float)(sr * r.x - si_ * r.y), (float)(sr * r.y + si_ * r.x));
-  }
-  if (d.dir < 0) x.y = -x.y;  // inverted REAL spectrum => conjugate (filter.c:876)
-  return cmul(x, r);
-}
-
-// Element si of a REAL-output slave's half spectrum (filter.c:794-809, as chan_wide): zero at (sb+1)/2.
-__device__ __forceinline__ float2 huge_half(ChanArgs const &a, ChanDesc const &d, float2 const *X, float2 const *R, int si) {
-  int const shift = d.q0, sb = d.points / 2 + 1, m = a.m_bins;
-  if (si == (sb + 1) / 2) return make_float2(0.f, 0.f);
-  int const mi = si + shift;
-  if (!a.wrap) return (mi >= 0 && mi < m) ? cmul(__ldg(X + mi), __ldg(R + si)) : make_float2(0.f, 0.f);
-  if (!(mi >= -(m / 2) && mi < m / 2)) return make_float2(0.f, 0.f);
-  int q1 = mi % m, q2 = (m - mi) % m;
-  if (q1 < 0) q1 += m;
-  if (q2 < 0) q2 += m;
-  float2 const xa = __ldg(X + q1), xb = __ldg(X + q2);
-  return cmul(__ldg(R + si), make_float2(xa.x + xb.x, xa.y - xb.y));
-}
-
-// Element w of the slice chan_wide hands its inverse transform, computed from the spectrum alone.
+// Element w of the slice chan_wide hands its inverse transform, computed from the spectrum alone (chan_slice.cuh's
+// steps, element by element).
 __device__ __forceinline__ float2 huge_slice(ChanArgs const &a, ChanDesc const &d, ChanAux const &ax, float2 const *X,
                                              float2 const *R, int w) {
   int const ns = d.points, top = (ns + 1) / 2, half = ns / 2;
   if (d.flags & kChanRealOut) {  // the Hermitian extension the c2r inverse implies
     if (w <= half) {
-      float2 const v = huge_half(a, d, X, R, w);
+      float2 const v = real_half(a, d, X, R, w);
       return (w == 0 || 2 * w == ns) ? make_float2(v.x, 0.f) : v;
     }
-    float2 const v = huge_half(a, d, X, R, ns - w);
+    float2 const v = real_half(a, d, X, R, ns - w);
     return make_float2(v.x, -v.y);
   }
-  if (!(d.flags & kChanIsb)) return huge_base(a, d, ax, X, R, w, top);
-  // ISB (filter.c:895-909): (S[p], S[ns-p]) <- (S[p] + conj S[ns-p], S[ns-p] - conj S[p]) for 0 < p < ns/2; S[0] = 0
+  auto base = [&](int v) {  // slot v before the ISB fold
+    bool live;
+    int const u = walk_pos(d, ns, top, v, live);
+    if (!live) return make_float2(0.f, 0.f);
+    int const q = walk_bin(a, d, u);
+    float2 const r = __ldg(R + v);
+    return (d.flags & kChanBeam) ? beam_product(ax, X, a.m_bins, q, r) : slice_product(d, __ldg(X + q), r);
+  };
+  if (!(d.flags & kChanIsb)) return base(w);
   if (w == 0 || w == top) return make_float2(0.f, 0.f);
-  if (w < half) {
-    float2 const pos = huge_base(a, d, ax, X, R, w, top), neg = huge_base(a, d, ax, X, R, ns - w, top);
-    return make_float2(pos.x + neg.x, pos.y - neg.y);
-  }
-  if (ns - w < half) {
-    float2 const neg = huge_base(a, d, ax, X, R, w, top), pos = huge_base(a, d, ax, X, R, ns - w, top);
-    return make_float2(neg.x - pos.x, neg.y + pos.y);
-  }
-  return huge_base(a, d, ax, X, R, w, top);
+  bool const lower = w < half;
+  if (!lower && ns - w >= half) return base(w);  // the middle slot, which the fold leaves alone
+  float2 pos = base(lower ? w : ns - w), neg = base(lower ? ns - w : w);
+  isb_fold(pos, neg);
+  return lower ? pos : neg;
 }
 
 // Pass A after the tile's columns k2 = c0 .. c0+ncols-1 are loaded (tile[c * pitch1 + k1]): transform each column,
@@ -143,7 +104,7 @@ __global__ void __launch_bounds__(kHugeThreads, 2) chan_huge_cols(ChanArgs const
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // [kTile][pitch1]
   int const oi = blockIdx.y;
-  int const ci = a.order ? a.order[oi] : a.chan_base + oi;
+  int const ci = chan_index(a, oi);
   ChanDesc const d = a.desc[ci];
   if (d.plan < 0) return;
   int const blk = blockIdx.z, tid = threadIdx.x, c = tid % kTile, r = tid / kTile;
@@ -162,10 +123,9 @@ __global__ void __launch_bounds__(kHugeThreads, 2) chan_huge_cols(ChanArgs const
 __global__ void __launch_bounds__(kHugeThreads, 2) chan_huge_rows(ChanArgs const a, HugeGeom const g, float2 const *scratch,
                                                                float *partial) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  __shared__ float red[kHugeThreads / 32];
   float2 *tile = reinterpret_cast<float2 *>(smem_raw);  // [kTile][pitch2]
   int const oi = blockIdx.y;
-  int const ci = a.order ? a.order[oi] : a.chan_base + oi;
+  int const ci = chan_index(a, oi);
   ChanDesc const d = a.desc[ci];
   if (d.plan < 0) return;
   int const blk = blockIdx.z, tid = threadIdx.x;
@@ -194,18 +154,10 @@ __global__ void __launch_bounds__(kHugeThreads, 2) chan_huge_rows(ChanArgs const
     if (row_ok)
       for (int j2 = j2lo + q; j2 < g.n2; j2 += kHugeRowsPerIt) {
         int const n = j1 + g.n1 * j2 - first;
-        float2 const v = osc_rotate(colp[__ldg(perm2 + j2)], osc_phase_cycles(ax, k, d.olen, n));
-        dst[n] = v;
-        pw += v.x * v.x + v.y * v.y;
+        dst[n] = osc_sample(ax, k, d.olen, n, colp[__ldg(perm2 + j2)], pw);
       }
-    pw = warp_sum(pw);
-    if ((tid & 31) == 0) red[tid >> 5] = pw;
-    __syncthreads();
-    if (partial && tid == 0) {
-      float s = 0.f;
-      for (int w = 0; w < kHugeThreads / 32; w++) s += red[w];
-      partial[slot * gridDim.x + blockIdx.x] = s;
-    }
+    float const s = cta_power_sum<kHugeThreads>(pw);
+    if (partial && tid == 0) partial[slot * gridDim.x + blockIdx.x] = s;
     return;
   }
   if (row_ok)
@@ -215,7 +167,7 @@ __global__ void __launch_bounds__(kHugeThreads, 2) chan_huge_rows(ChanArgs const
 // grid (channels, blocks), one warp: the block power of each kChanOsc channel from pass B's ntiles partial sums
 __global__ void __launch_bounds__(32) huge_power_kernel(ChanArgs const a, float const *partial, int ntiles) {
   int const oi = blockIdx.x, blk = blockIdx.y, lane = threadIdx.x;
-  int const ci = a.order ? a.order[oi] : a.chan_base + oi;
+  int const ci = chan_index(a, oi);
   ChanDesc const d = a.desc[ci];
   if (d.plan < 0 || !(d.flags & kChanOsc) || (d.flags & kChanRealOut)) return;
   float const *p = partial + ((long)blk * gridDim.x + oi) * ntiles;

@@ -101,6 +101,10 @@ struct ChanArgs {
   long power_stride;
 };
 
+}  // namespace kfft
+#include "chan_slice.cuh"
+namespace kfft {
+
 __global__ void __launch_bounds__(kChanWarps * 32) chan_kernel(ChanArgs const a) {
 #define KFFT_CHAN_EXT false
 #include "chan_body.cuh"

@@ -2252,28 +2252,14 @@ extern "C" long kgpu_bank_out_offset(kgpu_bank const *b, int idx) {
   return idx < b->nchan ? b->out_off[(size_t)idx] : -1;
 }
 
-template <class P> static int launch_chan_v2(ChanArgs const &a, int n, int nblocks, cudaStream_t st, bool osc) {
-  size_t const sm = sizeof(float2) * ((size_t)(2 * P::len + 4) * kChanWarps + static_tw_count<P>() + 2);
-  static bool attr_done = false;
-  if (!attr_done) {
-    if (allow_smem((const void *)chan_v2<P, false>, sm) || allow_smem((const void *)chan_v2<P, true>, sm)) return -1;
-    attr_done = true;
-  }
-  dim3 const g((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks);
-  if (osc) chan_v2<P, true><<<g, kChanWarps * 32, sm, st>>>(a);
-  else chan_v2<P, false><<<g, kChanWarps * 32, sm, st>>>(a);
-  return 0;
-}
-
-template <class P> static int launch_chan_static(ChanArgs const &a, int n, int nblocks, cudaStream_t st) {
-  size_t const sm = sizeof(float2) * ((size_t)(2 * P::len + 4) * kChanWarps + static_tw_count<P>() + 2);
-  static bool attr_done = false;
-  if (!attr_done) {
-    if (allow_smem((const void *)chan_static<P>, sm)) return -1;
-    attr_done = true;
-  }
-  dim3 const g((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks);
-  chan_static<P><<<g, kChanWarps * 32, sm, st>>>(a);
+// The specialised channel kernel of static plan P: chan_v2 (with the oscillator compiled in when `osc`) for a two-stage
+// plan, chan_static for the others.
+template <class P> static int launch_chan_static(ChanArgs const &a, int n, int nblocks, cudaStream_t st, bool osc) {
+  void (*k)(ChanArgs);
+  if constexpr (P::nst == 2) k = osc ? chan_v2<P, true> : chan_v2<P, false>;
+  else k = chan_static<P>;
+  if (allow_smem((const void *)k, StaticChan<P>::smem)) return -1;
+  k<<<dim3((unsigned)((n + kChanWarps - 1) / kChanWarps), (unsigned)nblocks), kChanWarps * 32, StaticChan<P>::smem, st>>>(a);
   return 0;
 }
 
@@ -2414,9 +2400,9 @@ static int launch_chan(kgpu_bank *b, const void *d_spec, int nblocks, void *d_ou
   g_launches++;
   TilePlan const *tp = host_tile_plan(g.plan);
   if (g_static_on.load() && !generic) {
-    if (plan_is<S600>(tp)) return launch_chan_v2<S600>(a, n, nblocks, st, b->any_osc);
-    if (plan_is<S300>(tp)) return launch_chan_v2<S300>(a, n, nblocks, st, b->any_osc);
-    if (plan_is<S1200>(tp)) return launch_chan_static<S1200>(a, n, nblocks, st);
+    if (plan_is<S600>(tp)) return launch_chan_static<S600>(a, n, nblocks, st, b->any_osc);
+    if (plan_is<S300>(tp)) return launch_chan_static<S300>(a, n, nblocks, st, b->any_osc);
+    if (plan_is<S1200>(tp)) return launch_chan_static<S1200>(a, n, nblocks, st, b->any_osc);
   }
   if (allow_smem((const void *)chan_kernel, warp_smem)) return -1;
   chan_kernel<<<warps, kChanWarps * 32, warp_smem, st>>>(a);

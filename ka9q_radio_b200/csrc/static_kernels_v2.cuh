@@ -318,113 +318,38 @@ __global__ void __launch_bounds__(RowsV2Shape<REAL_SPLIT>::T, REAL_SPLIT ? 1 : 2
 template <class P, bool OSC = false>
 __global__ void __launch_bounds__(kChanWarps * 32) chan_v2(ChanArgs const a) {
   static_assert(P::nst == 2, "two-stage plans only");
-  extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ __align__(8) uint64_t bars[kChanWarps];
   __shared__ __align__(8) uint64_t tbar;
-  constexpr int NS = P::len, TOP = (NS + 1) / 2, R0 = P::rad(0), R1 = P::rad(1), S0 = NS / R0;
-  static_assert(S0 == R1 && NS % 2 == 0, "plan shape");
-  constexpr int XS = NS + 4;
-  int const lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int const oi = blockIdx.x * kChanWarps + warp;
-  float2 *s_tw = reinterpret_cast<float2 *>(smem_raw) + kChanWarps * (NS + XS);
-  bool const active = oi < a.norder;
-  ChanDesc d;
-  d.plan = -1;
-  if (active) d = a.desc[a.order ? a.order[oi] : a.chan_base + oi];
-  if (threadIdx.x == 0) {
-    int p0 = -1;
-    for (int w = 0; w < kChanWarps && p0 < 0; w++) {
-      int const o = blockIdx.x * kChanWarps + w;
-      if (o < a.norder) p0 = a.desc[a.order ? a.order[o] : a.chan_base + o].plan;
-    }
-    mbar_init(&tbar, 1);
-    mbar_fence_init();
-    if (p0 >= 0) {
-      constexpr uint32_t TWB = (uint32_t)((static_tw_count<P>() + 1) & ~1) * 8u;
-      mbar_expect_tx(&tbar, TWB);
-      bulk_g2s(s_tw, c_plans[p0].tw, TWB, &tbar);
-    }
-  }
-  __syncthreads();
-  if (!active || d.plan < 0) return;
-  int const blk = blockIdx.y;
-  float2 *col = reinterpret_cast<float2 *>(smem_raw) + warp * (NS + XS);
-  float2 *xs = col + NS;
-  float2 const *X = a.spec + (long)blk * a.spec_stride;
-  float2 const *R = a.resp + d.resp_off;
-  float2 *dst = a.out + (long)blk * a.out_stride + d.out_off;
-  if (d.ncopy <= 0) {
-    for (int i = lane; i < d.olen; i += 32) dst[i] = make_float2(0.f, 0.f);
-    if ((d.flags & kChanOsc) && a.power && lane == 0) a.power[(long)blk * a.power_stride + (a.order ? a.order[oi] : a.chan_base + oi)] = 0.f;
-    mbar_wait(&tbar, 0);  // the CTA's twiddle copy targets this CTA's shared memory: never retire with it in flight
-    return;
-  }
-  int const qlo = d.dir > 0 ? d.q0 : d.q0 - (d.ncopy - 1);
-  bool const wraps = a.wrap && (d.q0 + d.ncopy > a.m_bins);
-  int const qa = qlo & ~1;
-  if (!wraps) {
-    int const qhi = qlo + d.ncopy - 1;
-    uint32_t const nx = (uint32_t)(((qhi - qa + 1) + 1) & ~1);
-    if (lane == 0) {
-      mbar_init(&bars[warp], 1);
-      mbar_fence_init();
-      mbar_expect_tx(&bars[warp], nx * 8 + NS * 8);
-      bulk_g2s(xs, X + qa, nx * 8, &bars[warp]);
-      bulk_g2s(col, R, NS * 8, &bars[warp]);
-    }
-    __syncwarp();
-    mbar_wait(&bars[warp], 0);
-  } else {
-    for (int i = lane; i < NS; i += 32) col[i] = __ldg(R + i);
-    for (int u = lane; u < d.ncopy; u += 32) {
-      int q = d.q0 + u;
-      if (q >= a.m_bins) q -= a.m_bins;
-      xs[u] = __ldg(X + q);
-    }
-    __syncwarp();
-  }
+  using S = StaticChan<P>;
+  constexpr int NS = S::NS, R0 = P::rad(0), R1 = P::rad(1), S0 = NS / R0;
+  static_assert(S0 == R1, "plan shape");
+  S s;
+  if (!static_prologue<P>(a, bars, tbar, s)) return;
+  ChanDesc const &d = s.d;
+  float2 *col = s.col;
+  int const lane = s.lane;
   mbar_wait(&tbar, 0);
-  auto product = [&](int wp) -> float2 {  // S[wp] = X[q(wp)] * R[wp], zero outside the master (filter.c:728-911)
-    int t = wp - TOP;
-    if (t < 0) t += NS;
-    int const u = t - d.zlead;
-    bool const live = (u >= 0 && u < d.ncopy && wp != TOP);
-    int const xi = wraps ? u : (d.q0 + d.dir * u - qa);
-    float2 x = xs[live ? xi : 0];
-    if (d.dir < 0) x.y = -x.y;
-    float2 const v = cmul(x, col[wp]);
-    return live ? v : make_float2(0.f, 0.f);
-  };
   if (d.flags & kChanIsb) {  // ISB: whole product in shared memory first, then the plain two stages
-    for (int wp = lane; wp < NS; wp += 32) col[wp] = product(wp);  // same lane reads R[wp] and writes S[wp]
+    for (int wp = lane; wp < NS; wp += 32) col[wp] = s.product(wp);  // same lane reads R[wp] and writes S[wp]
     __syncwarp();
-    for (int p = 1 + lane; p < NS / 2; p += 32) {
-      float2 const pos = col[p], neg = col[NS - p];
-      col[p] = make_float2(pos.x + neg.x, pos.y - neg.y);
-      col[NS - p] = make_float2(neg.x - pos.x, neg.y + pos.y);
-    }
-    if (lane == 0) {
-      col[0] = make_float2(0.f, 0.f);
-      col[TOP] = make_float2(0.f, 0.f);
-    }
-    __syncwarp();
-    static_stage<P, true, 0, true, 1>(col, s_tw, lane);
+    isb_fold_warp(col, NS, S::TOP, lane);
+    static_stage<P, true, 0, true, 1>(col, s.s_tw, lane);
     __syncwarp();
   } else if (lane < S0) {
     // ---- stage 0 with the product formed on the fly ------------------------------------------
     float2 x[R0];
 #pragma unroll
-    for (int m = 0; m < R0; m++) x[m] = product(lane + S0 * m);
+    for (int m = 0; m < R0; m++) x[m] = s.product(lane + S0 * m);
     Dft<R0, true>::run(x);
     col[lane] = x[0];
 #pragma unroll
-    for (int t = 1; t < R0; t++) col[lane + S0 * t] = cmulc(x[t], s_tw[(t - 1) * S0 + lane]);
+    for (int t = 1; t < R0; t++) col[lane + S0 * t] = cmulc(x[t], s.s_tw[(t - 1) * S0 + lane]);
   }
   __syncwarp();
   // ---- stage 1 fused with the store: y[n], n = u + R0*t, keep n >= NS - olen ---------------------
   bool const osc = OSC && (d.flags & kChanOsc) != 0;  // warp-uniform
   float pw = 0.f;
-  int const ci = a.order ? a.order[oi] : a.chan_base + oi;
+  int const ci = chan_index(a, s.oi);
   if (lane < R0) {
     float2 x[R1];
 #pragma unroll
@@ -435,25 +360,21 @@ __global__ void __launch_bounds__(kChanWarps * 32) chan_v2(ChanArgs const a) {
 #pragma unroll
       for (int t = 0; t < R1; t++) {
         int const n = lane + R0 * t;
-        if (n >= first) dst[n - first] = x[t];
+        if (n >= first) s.dst[n - first] = x[t];
       }
     } else if (OSC) {  // fine-tuning rotation + block power fused into the store (radio.c:1476-1501, :1515-1520)
       ChanAux const ax = a.aux[ci];
-      long const k = a.block0 + blk - ax.osc_epoch;
+      long const k = a.block0 + s.blk - ax.osc_epoch;
 #pragma unroll
       for (int t = 0; t < R1; t++) {
         int const n = lane + R0 * t;
-        if (n >= first) {
-          float2 const v = osc_rotate(x[t], osc_phase_cycles(ax, k, d.olen, n - first));
-          dst[n - first] = v;
-          pw += v.x * v.x + v.y * v.y;
-        }
+        if (n >= first) s.dst[n - first] = osc_sample(ax, k, d.olen, n - first, x[t], pw);
       }
     }
   }
   if (OSC && osc && a.power) {
     pw = warp_sum(pw);
-    if (lane == 0) a.power[(long)blk * a.power_stride + ci] = pw / (float)d.olen;
+    if (lane == 0) a.power[(long)s.blk * a.power_stride + ci] = pw / (float)d.olen;
   }
 }
 

@@ -51,3 +51,36 @@ def test_launches_per_path(cuda_dev, case):
     finally:
         b.close()
         m.close()
+
+
+def test_static_kernel_on_two_devices(cuda_dev):
+    """A 1200-point bank (chan_static, about 77 kB of dynamic shared memory) run on device 0 and then on device 1 in one
+    process: each device needs the kernel's shared-memory attribute of its own, and both compute the same output."""
+    import numpy as np
+    from ka9q_radio_b200 import capi
+    from ka9q_radio_b200.channelizer import Channelizer
+
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs two CUDA devices")
+    lib = capi.load()
+    lib.kgpu_use_static_kernels(1)
+    x = np.random.default_rng(1200).standard_normal(3 * L, dtype=np.float32)
+    outs = []
+    try:
+        for dev in (torch.device("cuda:0"), torch.device("cuda:1")):
+            cz = Channelizer(L, M, capi.KGPU_REAL, dev, capacity=2)
+            try:
+                assert cz.add_channel(960, 3000, -0.4, 0.4, 7.0) == 0 and cz._olen[0][1] == 1200
+                spec, out = cz.alloc_spectra(3), cz.alloc_outputs(3)
+                cz.forward(cz.stage_stream(x), 3, spec)
+                out.zero_()
+                cz.channels(spec, 3, out)
+                torch.cuda.synchronize(dev)
+                outs.append(cz.channel_slice(out, 0).cpu().numpy())
+            finally:
+                cz.close()
+    finally:
+        capi.check(lib.kgpu_set_device(0), "kgpu_set_device")
+        torch.cuda.set_device(cuda_dev)
+    assert np.abs(outs[0]).max() > 0
+    assert np.array_equal(outs[0].view(np.int32), outs[1].view(np.int32))

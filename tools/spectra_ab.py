@@ -8,7 +8,12 @@ Cases: cfg-2 (REAL int16, 32 blocks from block 3, the workload's 1024 channels),
 on fwd_rows_v2 with other row counts (odd n1 included), plus the COMPLEX 1296 x 1250 master.  Then every Bluestein
 transform: REAL 62 MS/s and COMPLEX 2.9 MS/s masters (kgpu_master_create_any; int16 with statistics, float), a bank of
 725-, 1550- and 44 000-point channels on each (responses, outputs, oscillator channels with block power), and spectrum
-polls at the REAL and COMPLEX fft_n 104 400, short and long enough to run in chunks of segments."""
+polls at the REAL and COMPLEX fft_n 104 400, short and long enough to run in chunks of segments.  Then every channel
+path on a REAL and a COMPLEX master (L = 48000, M = 12001): one bank with every length of PATH_POINTS in every variant
+that length's path serves, run batched with and without block power, again with the specialised kernels off, and one
+channel of each length alone (kgpu_bank_run_one_ex).
+
+--lib PATH dumps with another build of libka9qgpu.so, such as the parent commit's, in place of this tree's."""
 import argparse, sys
 from pathlib import Path
 import numpy as np
@@ -36,6 +41,78 @@ BLUESTEIN_SPECTRA = [  # (name, fft_n, real, int16 ring, fft_avg); 100 segments 
     ("s104400_c_f32", 104400, False, False, 3),
     ("s104400_c_f32_long", 104400, False, False, 100),
 ]
+# Every channel path: chan_v2 (600, 300), chan_static (1200), chan_kernel (480: 7-smooth, no specialised kernel), wide
+# (9600), huge (38 400), extended narrow and wide (5500, 8800) and Bluestein (725, 1550, 44 000); points = 5 olen / 4.
+PATH_POINTS = (600, 300, 1200, 480, 9600, 38400, 5500, 8800, 725, 1550, 44000)
+PATH_NB = 3
+
+
+def _path_variants(real: bool, bins: int, pts: int):
+    """(name, shift, flags, REAL output, oscillator) of each variant a channel path serves on this master"""
+    from ka9q_radio_b200 import capi
+
+    v = [("up", bins // 5, 0, False, False), ("isb", bins // 3, capi.KGPU_CHAN_ISB, False, False),
+         ("osc", bins // 4, 0, False, True)]
+    if pts % 2 == 0:  # REAL output needs an even length
+        v.append(("realout", bins // 6, 0, True, False))
+    if real:  # an inverted spectrum, and a channel with no overlap at all (with its zero block power)
+        return v + [("inv", -(bins // 5), 0, False, True), ("none", bins + pts, 0, False, True)]
+    return v + [("wrap", 17, 0, False, True), ("beam", bins // 7, capi.KGPU_CHAN_BEAM, False, False)]
+
+
+def dump_paths(out: Path, dev):
+    import torch
+    from ka9q_radio_b200 import capi
+
+    lib = capi.load()
+    st = torch.cuda.current_stream(dev).cuda_stream
+    L, M, nb = 48000, 12001, PATH_NB
+    for name, real in (("paths_r", True), ("paths_c", False)):
+        rng = np.random.default_rng(L + M + real)
+        host = rng.standard_normal((nb * L + M - 1) * (1 if real else 2), dtype=np.float32)
+        m = capi.Master(L, M, capi.KGPU_REAL if real else capi.KGPU_COMPLEX)
+        chans = [(pts,) + v for pts in PATH_POINTS for v in _path_variants(real, m.bins, pts)]
+        b = capi.Bank(m, len(chans))
+        try:
+            print(f"{name}: {m.describe()}, {len(chans)} channels")
+            for i, (pts, _, shift, flags, realout, osc) in enumerate(chans):
+                assert b.define_any(i, pts * 4 // 5, capi.KGPU_REAL if realout else capi.KGPU_COMPLEX) == pts
+                b.set_filter(i, 0.05 if realout else -0.3, 0.4 if realout else 0.35, 11.0)
+                b.set_shift(i, shift)
+                if flags & capi.KGPU_CHAN_BEAM:
+                    b.set_weights(i, 0.6, 0.3)
+                if flags:
+                    b.set_flags(i, flags)
+                if osc:
+                    b.set_osc(i, True, 0.1 + 0.01 * i, 1e-3, 1e-9, 0.01)
+            spec = torch.empty((nb, m.spec_stride), dtype=torch.complex64, device=dev)
+            m.forward(torch.from_numpy(host).to(dev).data_ptr(), capi.KGPU_FMT_F32, 1.0, nb, spec.data_ptr(), st)
+            res = {"spec": spec[:, :m.bins]}
+            for static in (1, 0):
+                lib.kgpu_use_static_kernels(static)
+                o = torch.zeros((nb, b.out_stride), dtype=torch.complex64, device=dev)
+                b.run(spec.data_ptr(), nb, o.data_ptr(), st)
+                res[f"chan_s{static}"] = o
+                o = torch.zeros((nb, b.out_stride), dtype=torch.complex64, device=dev)
+                power = torch.zeros((nb, len(chans)), dtype=torch.float32, device=dev)
+                b.run(spec.data_ptr(), nb, o.data_ptr(), st, power.data_ptr())
+                res[f"chan_pw_s{static}"], res[f"power_s{static}"] = o, power
+            lib.kgpu_use_static_kernels(1)
+            for i, (pts, vname, *_rest) in enumerate(chans):  # one channel of each length alone: its oscillator variant
+                if vname != "osc":
+                    continue
+                o = torch.zeros(pts, dtype=torch.complex64, device=dev)
+                power = torch.zeros(1, dtype=torch.float32, device=dev)
+                capi.check(lib.kgpu_bank_run_one_ex(b.h, i, spec[1].data_ptr(), o.data_ptr(), power.data_ptr(), st),
+                           "kgpu_bank_run_one_ex")
+                res[f"one{pts}"], res[f"one{pts}_power"] = o, power
+            torch.cuda.synchronize()
+            for k, v in res.items():
+                _save(out, f"{name}.{k}", v)
+        finally:
+            lib.kgpu_use_static_kernels(1)
+            b.close()
+            m.close()
 
 
 def _save(out: Path, name: str, v):
@@ -104,10 +181,13 @@ def dump_bluestein(out: Path, dev):
             s.close()
 
 
-def dump(out: Path):
+def dump(out: Path, lib: Path | None):
     import torch
     sys.path.insert(0, str(ROOT))
     from ka9q_radio_b200 import capi, workloads
+
+    if lib:
+        capi.LIB_PATH = lib.resolve()
     from ka9q_radio_b200.channelizer import Channelizer
 
     out.mkdir(parents=True, exist_ok=True)
@@ -137,6 +217,7 @@ def dump(out: Path):
         finally:
             cz.close()
     dump_bluestein(out, dev)
+    dump_paths(out, dev)
 
 
 def compare(a: Path, b: Path) -> int:
@@ -158,8 +239,9 @@ ap = argparse.ArgumentParser()
 g = ap.add_mutually_exclusive_group(required=True)
 g.add_argument("--dump", type=Path)
 g.add_argument("--compare", type=Path, nargs=2)
+ap.add_argument("--lib", type=Path, help="with --dump: the libka9qgpu.so to dump with (default: this tree's)")
 a = ap.parse_args()
 if a.dump:
-    dump(a.dump)
+    dump(a.dump, a.lib)
 else:
     sys.exit(compare(*a.compare))
