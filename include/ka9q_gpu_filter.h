@@ -17,8 +17,9 @@
  *   delete_filter_input/output    filter.c:930-957
  *   write_i16filter               (EXTENSION, not in the reference) raw int16 ingest: fuses
  *                                 rx888.c:753-767 convert() into the first FFT pass
- *   write_rawfilter               (EXTENSION) raw 8-bit and packed 12-bit ingest: the conversion loops of rtlsdr.c,
- *                                 hydrasdr.c and airspy-unpack.c on the device
+ *   write_rawfilter               (EXTENSION) raw 8-bit, packed 12-bit and 16-bit ingest: the conversion loops of
+ *                                 rtlsdr.c, hydrasdr.c, airspy-unpack.c, bladerf.c and sdrplay.c on the device
+ *   write_rawfilter_planar        (EXTENSION) SDRplay's separate int16 I and Q arrays as FILTER_RAW_S16 pairs
  *   filter_ingest_stats           (EXTENSION) the A/D energy and overranges those loops return, per drained block
  *   filter_iq_correction_setup    (EXTENSION) HackRF's and FUNcube's DC and I/Q gain and phase correction on the device
  *   filter_iq_records             (EXTENSION) the per-transfer sums and state those drivers' loops produce
@@ -149,15 +150,26 @@ enum filter_raw_format {
   FILTER_RAW_PACKED12 = 1,
   FILTER_RAW_U8 = 2,
   FILTER_RAW_S8 = 3,
-  FILTER_RAW_S8_IQCORR = 4, /* HackRF: signed byte I/Q with the driver's DC and I/Q correction (filter_iq_correction_setup) */
-  FILTER_RAW_S16_IQCORR = 5 /* FUNcube: int16 I/Q with the same correction */
+  FILTER_RAW_S8_IQCORR = 4,  /* HackRF: signed byte I/Q with the driver's DC and I/Q correction (filter_iq_correction_setup) */
+  FILTER_RAW_S16_IQCORR = 5, /* FUNcube: int16 I/Q with the same correction */
+  FILTER_RAW_S16 = 6,        /* int16, REAL or I/Q: HydraSDR INT16_REAL / INT16_IQ; SDRplay through write_rawfilter_planar */
+  FILTER_RAW_U16 = 7,        /* offset-binary uint16 (x = w - 32768), REAL only: HydraSDR UINT16_REAL */
+  FILTER_RAW_SC16Q11 = 8     /* bladeRF SC16_Q11 I/Q, COMPLEX only: bits 0-11 of each word, sign-extended from bit 11 */
 };
+/* The 16-bit formats (hydrasdr.c:681-716, :729-747, bladerf.c:215-246, sdrplay.c:1234-1246) give floats bitwise equal to
+ * the drivers' (float)(scale * x) with a double scale; bladerf.c stores (float)x, i.e. scale 1.0.  Their limits, as the
+ * drivers test them: x >= 32767 or x <= -32768 (S16, U16), x == 2047 or x == -2048 (SC16Q11).  Samples before the first
+ * write are 0.0f (the U16 ring is prefilled with 0x8000 words). */
 int write_rawfilter(struct filter_in *master, void const *samples, int n, int format, double scale);
+/* EXTENSION: SDRplay's separate I and Q arrays (sdrplay.c:1210-1246): n pairs i[k], q[k] interleaved into the raw ring of
+ * a COMPLEX master fed FILTER_RAW_S16, then exactly a write_rawfilter(..., FILTER_RAW_S16, scale) of those pairs.  -1 on a
+ * REAL master or one fed any other format. */
+int write_rawfilter_planar(struct filter_in *master, int16_t const *i, int16_t const *q, int n, double scale);
 /* Pure host code: the byte size of the raw ring write_rawfilter allocates for a master of this geometry and format (a
  * whole number of pages, and for PACKED12 of 12-byte groups, holding at least the master's float ring of samples), or -1
  * where write_rawfilter would reject the geometry. */
 long filter_raw_ring_bytes(int L, int M, enum filtertype in_type, int format);
-/* Scale changes of write_i16filter and write_rawfilter (U8, S8, PACKED12): a write whose scale differs from the previous
+/* Scale changes of write_i16filter and write_rawfilter (every format without I/Q correction): a write whose scale differs from the previous
  * write's records a change at its first sample, in a table of FILTER_SCALE_CHANGES(L, S) entries, S the samples of the
  * master's float ring (input_buffer_size over the sample size).  A change leaves the table once S samples have been
  * launched after it (the wideband analyzer's device ring holds S samples).  A write whose change would overflow the

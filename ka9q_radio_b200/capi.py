@@ -17,6 +17,7 @@ LIB_PATH = PKG / "libka9qgpu.so"
 KGPU_COMPLEX, KGPU_REAL = 1, 2
 KGPU_FMT_F32, KGPU_FMT_I16 = 0, 1
 KGPU_RAW_U8, KGPU_RAW_S8 = 1, 2   # kgpu_unpack8's formats, apart from kgpu_format
+KGPU_RAW_S16, KGPU_RAW_U16, KGPU_RAW_SC16Q11 = 3, 4, 5   # its 16-bit formats (U16 REAL, SC16Q11 COMPLEX only)
 KGPU_CHAN_ISB = 1
 KGPU_CHAN_BEAM = 4
 
@@ -184,12 +185,13 @@ def check(rc: int, what: str = "") -> int:
 
 
 def unpack8(d_raw: int, fmt: int, in_type: int, history: int, L: int, nblocks: int, scale: float, d_out: int,
-            d_stats: int = 0, stream: int = 0) -> None:
-    """8-bit ingest (kgpu_unpack8): the u8 / s8 bytes of `history` samples then nblocks blocks of L to float32 at d_out,
-    each (float)(scale * (double)x); d_stats: 0 or nblocks kgpu_block_stats (uint64 energy, uint32 overs, uint32
-    over_samples)."""
-    check(load().kgpu_unpack8(d_raw, fmt, in_type, history, L, nblocks, scale, None, 0, 0, d_out, d_stats or None,
-                              stream or None), "kgpu_unpack8")
+            d_stats: int = 0, stream: int = 0, d_chg: int = 0, nchg: int = 0, a0: int = 0) -> None:
+    """8- and 16-bit ingest (kgpu_unpack8): the u8 / s8 bytes or s16 / u16 / sc16q11 words of `history` samples then
+    nblocks blocks of L to float32 at d_out, each (float)(scale * (double)x); d_stats: 0 or nblocks kgpu_block_stats
+    (uint64 energy, uint32 overs, uint32 over_samples); d_chg: 0 or nchg kgpu_scale_change (int64 at, float64 scale),
+    the first history sample being absolute sample a0."""
+    check(load().kgpu_unpack8(d_raw, fmt, in_type, history, L, nblocks, scale, d_chg or None, nchg, a0, d_out,
+                              d_stats or None, stream or None), "kgpu_unpack8")
 
 
 def block_stats_i16(d_in: int, in_type: int, history: int, L: int, nblocks: int, d_stats: int, derandomize: bool = False,

@@ -673,7 +673,9 @@ static void rebuild_ranges(struct filter_in *f, struct master_ctx *c) {
 /* bytes of n samples (REAL) or I/Q pairs (COMPLEX) in a raw format; a packed-12 n is a multiple of 8 (three words) */
 static bool iq_format(int fmt) { return fmt == FILTER_RAW_S8_IQCORR || fmt == FILTER_RAW_S16_IQCORR; }
 /* bytes per component */
-static size_t raw_word(int fmt) { return fmt == FILTER_RAW_S16_IQCORR ? 2 : 1; }
+static size_t raw_word(int fmt) {
+  return fmt == FILTER_RAW_S16_IQCORR || fmt == FILTER_RAW_S16 || fmt == FILTER_RAW_U16 || fmt == FILTER_RAW_SC16Q11 ? 2 : 1;
+}
 static size_t raw_bytes(int fmt, bool cplx, size_t n) {
   return fmt == FILTER_RAW_PACKED12 ? n / 8 * 12 : n * (cplx ? 2 : 1) * raw_word(fmt);
 }
@@ -692,10 +694,13 @@ long filter_raw_ring_bytes(int L, int M, enum filtertype in_type, int format) {
     if (cplx || L % 8 != 0 || (M - 1) % 8 != 0)
       return -1;
     unit = unit / (size_t)gcd((long)unit, 12) * 12;
-  } else if (iq_format(format)) {
+  } else if (iq_format(format) || format == FILTER_RAW_SC16Q11) {
     if (!cplx)
       return -1;
-  } else if (format != FILTER_RAW_U8 && format != FILTER_RAW_S8)
+  } else if (format == FILTER_RAW_U16) {
+    if (cplx)
+      return -1;
+  } else if (format != FILTER_RAW_U8 && format != FILTER_RAW_S8 && format != FILTER_RAW_S16)
     return -1;
   size_t const fsz = cplx ? sizeof(float complex) : sizeof(float);
   size_t const samples = page_round((size_t)ND * (size_t)(L + M - 1) * fsz) / fsz; /* the float ring's capacity */
@@ -711,6 +716,8 @@ static int raw_start(struct filter_in *f, struct master_ctx *c, int format) {
     fprintf(stderr, "write_rawfilter(L=%d M=%d): format %d cannot feed this master%s\n", f->ilen, f->impulse_length, format,
             format == FILTER_RAW_PACKED12 ? " (packed 12-bit needs a REAL master with L and M-1 multiples of 8)"
             : iq_format(format)          ? " (I/Q correction needs a COMPLEX master)"
+            : format == FILTER_RAW_SC16Q11 ? " (SC16 Q11 samples are I/Q)"
+            : format == FILTER_RAW_U16   ? " (offset-binary 16-bit samples are real)"
                                          : "");
     return -1;
   }
@@ -725,7 +732,11 @@ static int raw_start(struct filter_in *f, struct master_ctx *c, int format) {
   c->raw_ring_size = (size_t)size;
   if (format == FILTER_RAW_U8)
     memset(c->raw_ring, 128, c->raw_ring_size);
-  else if (format == FILTER_RAW_PACKED12) { /* eight offset-binary 2048s per three words (airspy-unpack.c:110-117) */
+  else if (format == FILTER_RAW_U16) { /* offset binary: 0x8000 is 0 */
+    uint16_t *const w = c->raw_ring;
+    for (size_t o = 0; o < c->raw_ring_size / sizeof *w; o++)
+      w[o] = 0x8000;
+  } else if (format == FILTER_RAW_PACKED12) { /* eight offset-binary 2048s per three words (airspy-unpack.c:110-117) */
     uint32_t const g[3] = {0x80080080u, 0x08008008u, 0x00800800u};
     for (size_t o = 0; o < c->raw_ring_size; o += sizeof g)
       memcpy((char *)c->raw_ring + o, g, sizeof g);
@@ -828,8 +839,18 @@ static int chg_span(struct master_ctx const *c, int stage, long long lo, long lo
   return stage == ND && cudaEventRecord(c->stg_ev, c->st) != cudaSuccess ? -1 : 0;
 }
 
+/* kgpu_unpack8's word format of a filter_raw_format it serves */
+static int kgpu_raw_format(int fmt) {
+  switch (fmt) {
+  case FILTER_RAW_U8: return KGPU_RAW_U8;
+  case FILTER_RAW_S8: return KGPU_RAW_S8;
+  case FILTER_RAW_S16: return KGPU_RAW_S16;
+  case FILTER_RAW_U16: return KGPU_RAW_U16;
+  default: return KGPU_RAW_SC16Q11;
+  }
+}
 /* raw bytes on the device (history samples, then nblocks blocks of L) -> the master's device samples at d_dst: floats for
- * the 8-bit and I/Q corrected formats, int16 for packed-12, which kgpu_forward then scales.  d_stats: NULL or nblocks
+ * the 8-bit, 16-bit and I/Q corrected formats, int16 for packed-12, which kgpu_forward then scales.  d_stats: NULL or nblocks
  * block statistics (not for I/Q correction, whose records replace them). */
 static int iq_apply(struct master_ctx const *c, void const *d_src, long long a0, long count, void *d_dst, cudaStream_t st);
 static int raw_unpack(struct filter_in const *f, struct master_ctx const *c, int stage, void const *d_src, long long a0,
@@ -842,8 +863,8 @@ static int raw_unpack(struct filter_in const *f, struct master_ctx const *c, int
     int n;
     if (chg_span(c, stage, a0, a0 + history + (long long)nblocks * f->ilen, &scale, &n) != 0)
       return -1;
-    return kgpu_unpack8(d_src, c->raw_fmt == FILTER_RAW_U8 ? KGPU_RAW_U8 : KGPU_RAW_S8, type, history, f->ilen, nblocks, scale,
-                        n ? c->d_chg : NULL, n, a0, d_dst, d_stats, st);
+    return kgpu_unpack8(d_src, kgpu_raw_format(c->raw_fmt), type, history, f->ilen, nblocks, scale, n ? c->d_chg : NULL, n, a0,
+                        d_dst, d_stats, st);
   }
   if (kgpu_unpack_airspy12(d_src, history + (long)nblocks * f->ilen, d_dst, NULL, st) != 0)
     return -1;
@@ -1073,7 +1094,7 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     c->i16_rp += c->i16_esz * (size_t)f->ilen * (size_t)k;
     if (c->i16_rp >= (char *)c->i16_ring + c->i16_ring_size)
       c->i16_rp -= c->i16_ring_size;
-  } else if (c->raw_fmt) { /* packed-12 goes on as int16 with the drivers' float scale; 8-bit as floats */
+  } else if (c->raw_fmt) { /* packed-12 goes on as int16 with the drivers' float scale; 8- and 16-bit as floats */
     bool const cplx = f->in_type == COMPLEX;
     src = c->raw_rp;
     bytes = raw_bytes(c->raw_fmt, cplx, span);
@@ -1920,37 +1941,33 @@ int16_t *filter_i16_write_pointer(struct filter_in *f) {
   return (int16_t *)c->i16_wp;
 }
 
-/* EXTENSION: raw packed 12-bit or 8-bit ADC words, unpacked on the device (see include/ka9q_gpu_filter.h).  The drivers
- * (airspy.c:388-434, hydrasdr.c:663-679, :759-830, rtlsdr.c:316-343) get their buffers from their vendor libraries, so
- * there is no zero-copy write pointer: the bytes are copied into the raw ring. */
-int write_rawfilter(struct filter_in *f, void const *samples, int n, int format, double scale) {
-  if (f == NULL || f->fwd_plan == NULL || samples == NULL || n < 0)
-    return -1;
-  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (format != FILTER_RAW_PACKED12 && format != FILTER_RAW_U8 && format != FILTER_RAW_S8 && !iq_format(format)) {
-    fprintf(stderr, "write_rawfilter: unknown format %d\n", format);
+/* the checks, table entry and scale of a write of n samples in `format` about to be stored at c->raw_wp (starting the
+ * raw ring at a master's first write); 0, or -1 with nothing stored */
+static int raw_admit(struct filter_in *f, struct master_ctx *c, int n, int format, double scale, char const *who) {
+  if (format != FILTER_RAW_PACKED12 && format != FILTER_RAW_U8 && format != FILTER_RAW_S8 && format != FILTER_RAW_S16 &&
+      format != FILTER_RAW_U16 && format != FILTER_RAW_SC16Q11 && !iq_format(format)) {
+    fprintf(stderr, "%s: unknown format %d\n", who, format);
     return -1;
   }
   if (iq_format(format) && !c->iq_on) {
-    fprintf(stderr, "write_rawfilter: format %d needs filter_iq_correction_setup first\n", format);
+    fprintf(stderr, "%s: format %d needs filter_iq_correction_setup first\n", who, format);
     return -1;
   }
   if (!c->raw_fmt && raw_start(f, c, format) != 0)
     return -1;
   if (format != c->raw_fmt) {
-    fprintf(stderr, "write_rawfilter: format %d on a master fed format %d\n", format, c->raw_fmt);
+    fprintf(stderr, "%s: format %d on a master fed format %d\n", who, format, c->raw_fmt);
     return -1;
   }
   if (format == FILTER_RAW_PACKED12 && n % 8 != 0) {
-    fprintf(stderr, "write_rawfilter: %d packed 12-bit samples: not a multiple of 8\n", n);
+    fprintf(stderr, "%s: %d packed 12-bit samples: not a multiple of 8\n", who, n);
     return -1;
   }
-  bool const cplx = f->in_type == COMPLEX;
-  if (raw_bytes(format, cplx, (size_t)f->wcnt + (size_t)n) >= c->raw_ring_size)
+  if (raw_bytes(format, f->in_type == COMPLEX, (size_t)f->wcnt + (size_t)n) >= c->raw_ring_size)
     return -1;
   if (c->iq_on) { /* one transfer: its table entry */
     if (n < FILTER_IQ_MIN_WRITE) {
-      fprintf(stderr, "write_rawfilter: %d I/Q pairs: writes with I/Q correction take at least %d\n", n, FILTER_IQ_MIN_WRITE);
+      fprintf(stderr, "%s: %d I/Q pairs: writes with I/Q correction take at least %d\n", who, n, FILTER_IQ_MIN_WRITE);
       return -1;
     }
     struct kgpu_iq_write *w = &c->h_iqw[c->iq_writes % (unsigned long long)c->iq_cap];
@@ -1961,21 +1978,54 @@ int write_rawfilter(struct filter_in *f, void const *samples, int n, int format,
     w->last_over = -1;
     c->iq_writes++;
     c->iq_total += n;
+    return 0;
   }
-  if (!c->iq_on) {
-    pthread_mutex_lock(&c->mu);
-    int const rc = chg_note(f, c, scale, "write_rawfilter");
-    pthread_mutex_unlock(&c->mu);
-    if (rc != 0)
-      return -1;
-  }
-  size_t const bytes = raw_bytes(format, cplx, (size_t)n);
-  memcpy(c->raw_wp, samples, bytes); /* the mirror view keeps a write across the end contiguous */
-  c->raw_wp += bytes;
+  pthread_mutex_lock(&c->mu);
+  int const rc = chg_note(f, c, scale, who);
+  pthread_mutex_unlock(&c->mu);
+  return rc;
+}
+/* publish the n samples just stored at c->raw_wp, and fire the blocks they complete */
+static int raw_commit(struct filter_in *f, struct master_ctx *c, int n) {
+  c->raw_wp += raw_bytes(c->raw_fmt, f->in_type == COMPLEX, (size_t)n);
   if (c->raw_wp >= (char *)c->raw_ring + c->raw_ring_size)
     c->raw_wp -= c->raw_ring_size;
   f->wcnt += n;
   return fire_ready_blocks(f);
+}
+
+/* EXTENSION: raw packed 12-bit, 8-bit or 16-bit ADC words, unpacked on the device (see include/ka9q_gpu_filter.h).  The
+ * drivers (airspy.c:388-434, hydrasdr.c:663-830, rtlsdr.c:316-343, bladerf.c:215-246) get their buffers from their vendor
+ * libraries, so there is no zero-copy write pointer: the bytes are copied into the raw ring. */
+int write_rawfilter(struct filter_in *f, void const *samples, int n, int format, double scale) {
+  if (f == NULL || f->fwd_plan == NULL || samples == NULL || n < 0)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (raw_admit(f, c, n, format, scale, "write_rawfilter") != 0)
+    return -1;
+  memcpy(c->raw_wp, samples, raw_bytes(format, f->in_type == COMPLEX, (size_t)n)); /* the mirror view keeps a write across
+                                                                                      the end contiguous */
+  return raw_commit(f, c, n);
+}
+
+/* EXTENSION: SDRplay's separate I and Q arrays (sdrplay.c:1234-1246), interleaved into the FILTER_RAW_S16 ring: a copy
+ * like write_rawfilter's memcpy, after which the pairs are an S16 write like any other. */
+int write_rawfilter_planar(struct filter_in *f, int16_t const *i, int16_t const *q, int n, double scale) {
+  if (f == NULL || f->fwd_plan == NULL || i == NULL || q == NULL || n < 0)
+    return -1;
+  if (f->in_type != COMPLEX) {
+    fprintf(stderr, "write_rawfilter_planar: the master is not COMPLEX\n");
+    return -1;
+  }
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (raw_admit(f, c, n, FILTER_RAW_S16, scale, "write_rawfilter_planar") != 0)
+    return -1;
+  int16_t *restrict const w = (int16_t *)c->raw_wp; /* the mirror view keeps a write across the end contiguous */
+  for (int k = 0; k < n; k++) {
+    w[2 * k] = i[k];
+    w[2 * k + 1] = q[k];
+  }
+  return raw_commit(f, c, n);
 }
 
 /* EXTENSION: the A/D statistics of the blocks whose device work completed since the previous call (see

@@ -315,12 +315,24 @@ extern "C" int kgpu_unpack_airspy12(const void *d_packed, long sampcount, void *
   return 0;
 }
 
-// ---- 8-bit ingest and per-block statistics of raw ingest (raw_ingest.cuh) -------------------------------------------
+// ---- 8- and 16-bit ingest and per-block statistics of raw ingest (raw_ingest.cuh) ------------------------------------
 static_assert(sizeof(ScaleChange) == sizeof(kgpu_scale_change), "raw_ingest.cuh mirrors include/ka9q_gpu.h");
+// REAL_OK / CPLX_OK: the master types the format exists for (only those kernels are instantiated)
+template <class D, bool REAL_OK = true, bool CPLX_OK = true>
+static void launch_unpack(dim3 g, cudaStream_t st, bool cplx, const void *d_raw, long history, long L, int nblocks, double scale,
+                          ScaleChange const *chg, int nchg, long long a0, float *out, BlockStats *stats) {
+  auto const *w = (typename D::Word const *)d_raw;
+  if constexpr (CPLX_OK)
+    if (cplx) unpack_kernel<D, true><<<g, kRawThreads, 0, st>>>(w, history, L, nblocks, scale, chg, nchg, a0, out, stats);
+  if constexpr (REAL_OK)
+    if (!cplx) unpack_kernel<D, false><<<g, kRawThreads, 0, st>>>(w, history, L, nblocks, scale, chg, nchg, a0, out, stats);
+}
 extern "C" int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, int nblocks, double scale,
                             const kgpu_scale_change *d_chg, int nchg, long long a0, void *d_out, void *d_stats, void *stream) {
   if (!d_raw || !d_out || history < 0 || nblocks < 0 || (nblocks > 0 && L < 1) || nblocks >= 65535 || nchg < 0 || (nchg && !d_chg) ||
-      (fmt != KGPU_RAW_U8 && fmt != KGPU_RAW_S8) || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX))
+      fmt < KGPU_RAW_U8 || fmt > KGPU_RAW_SC16Q11 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX) ||
+      (fmt == KGPU_RAW_U16 && in_type != KGPU_REAL) || (fmt == KGPU_RAW_SC16Q11 && in_type != KGPU_COMPLEX) ||
+      (fmt >= KGPU_RAW_S16 && ((uintptr_t)d_raw & 1)))
     return fail("kgpu_unpack8: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   BlockStats *stats = (BlockStats *)d_stats;
@@ -328,11 +340,18 @@ extern "C" int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long histor
   long const longest = std::max(nblocks ? L : 0L, history);
   if (longest == 0) return 0;
   dim3 const g((unsigned)((longest + kRawThreads - 1) / kRawThreads), (unsigned)nblocks + 1);
-  bool const s8 = fmt == KGPU_RAW_S8, cplx = in_type == KGPU_COMPLEX;
-  auto const k = s8 ? (cplx ? unpack8_kernel<true, true> : unpack8_kernel<true, false>)
-                    : (cplx ? unpack8_kernel<false, true> : unpack8_kernel<false, false>);
-  k<<<g, kRawThreads, 0, st>>>((uint8_t const *)d_raw, history, L, nblocks, scale, (ScaleChange const *)d_chg, nchg, a0,
-                               (float *)d_out, stats);
+  bool const cplx = in_type == KGPU_COMPLEX;
+  auto const *chg = (ScaleChange const *)d_chg;
+  auto *out = (float *)d_out;
+#define KGPU_UNPACK(...) launch_unpack<__VA_ARGS__>(g, st, cplx, d_raw, history, L, nblocks, scale, chg, nchg, a0, out, stats)
+  switch (fmt) {
+    case KGPU_RAW_U8: KGPU_UNPACK(DecodeU8); break;
+    case KGPU_RAW_S8: KGPU_UNPACK(DecodeS8); break;
+    case KGPU_RAW_S16: KGPU_UNPACK(DecodeS16); break;
+    case KGPU_RAW_U16: KGPU_UNPACK(DecodeU16, true, false); break;    // REAL only
+    default: KGPU_UNPACK(DecodeSC16Q11, false, true); break;           // COMPLEX only
+  }
+#undef KGPU_UNPACK
   g_launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -1,8 +1,9 @@
-// raw_ingest.cuh -- the 8-bit front ends' sample conversion (rtlsdr.c:316-343, hydrasdr.c:759-830) and the per-block A/D
-// statistics of every raw ingest format (energy, components at the limits, samples with a component at the limits).
+// raw_ingest.cuh -- the 8- and 16-bit front ends' sample conversion (rtlsdr.c:316-343, hydrasdr.c:681-716, :729-747,
+// :759-830, bladerf.c:215-246, sdrplay.c:1234-1246) and the per-block A/D statistics of every raw ingest format (energy,
+// components at the limits, samples with a component at the limits).
 //
 // Both kernels walk one overlap-save launch: a window of `history` samples followed by nblocks blocks of L new samples.
-// grid.y picks the segment: y < nblocks is block y's new samples, whose statistics go to stats[y]; for the 8-bit unpack
+// grid.y picks the segment: y < nblocks is block y's new samples, whose statistics go to stats[y]; for the unpack
 // y == nblocks is the history, converted but never counted (the drivers count each sample once).  A sample is one value
 // (REAL) or one I/Q pair (COMPLEX); every component counts in the energy and in the component count.
 #pragma once
@@ -51,14 +52,40 @@ __device__ __forceinline__ double scale_at(ScaleChange const *chg, int n, double
   return lo ? chg[lo - 1].scale : base;
 }
 
-// u8 (excess-128) or s8 words -> float, one thread per sample.  The value is (float)(scale * (double)x) as the drivers'
-// loops store it: a double product rounded once more to float (no float multiply, no FMA), with the sample's own scale
-// where nchg changes are given (in[0] being absolute sample a0).  At the limits: x >= 127 or x <= -128, i.e. bytes 0 and
-// 255 of u8 (rtlsdr.c:324-333) and 127, -128 of s8 (hydrasdr.c:781).
-template <bool SIGNED, bool CPLX>
-__global__ void __launch_bounds__(kRawThreads) unpack8_kernel(uint8_t const *__restrict__ in, long history, long L, int nblocks,
-                                                              double scale, ScaleChange const *__restrict__ chg, int nchg,
-                                                              long long a0, float *__restrict__ out, BlockStats *stats) {
+// The word decodes of unpack_kernel: each gives a word's integer x and whether x is at the format's limits.
+struct DecodeU8 {  // excess-128 bytes: RTL-SDR (rtlsdr.c:316-343), HydraSDR UINT8_* (hydrasdr.c:759-775, :793-811)
+  using Word = uint8_t;
+  static __device__ __forceinline__ int x(Word w) { return (int)w - 128; }
+  static __device__ __forceinline__ bool over(int x) { return x >= 127 || x <= -128; }
+};
+struct DecodeS8 {  // signed bytes: HydraSDR INT8_* (hydrasdr.c:776-791, :812-830)
+  using Word = uint8_t;
+  static __device__ __forceinline__ int x(Word w) { return (int)(int8_t)w; }
+  static __device__ __forceinline__ bool over(int x) { return x >= 127 || x <= -128; }
+};
+struct DecodeS16 {  // int16: HydraSDR INT16_REAL / INT16_IQ (hydrasdr.c:700-716, :729-747), SDRplay (sdrplay.c:1238-1242)
+  using Word = uint16_t;
+  static __device__ __forceinline__ int x(Word w) { return (int)(int16_t)w; }
+  static __device__ __forceinline__ bool over(int x) { return x >= 32767 || x <= -32768; }
+};
+struct DecodeU16 {  // offset-binary uint16: HydraSDR UINT16_REAL at 16 bits per sample (hydrasdr.c:681-699, :265-267)
+  using Word = uint16_t;
+  static __device__ __forceinline__ int x(Word w) { return (int)w - 32768; }
+  static __device__ __forceinline__ bool over(int x) { return x >= 32767 || x <= -32768; }
+};
+struct DecodeSC16Q11 {  // bladeRF SC16_Q11 (bladerf.c:226-235): bits 0-11 sign-extended from bit 11, bits 12-15 ignored
+  using Word = uint16_t;
+  static __device__ __forceinline__ int x(Word w) { return (int)((w & 0xfffu) ^ 0x800u) - 0x800; }
+  static __device__ __forceinline__ bool over(int x) { return x == 2047 || x == -2048; }  // s == 0x7ff || s == 0x800
+};
+
+// Raw words -> float, one thread per sample.  The value is (float)(scale * (double)x) as the drivers' loops store it: a
+// double product rounded once more to float (no float multiply, no FMA), with the sample's own scale where nchg changes
+// are given (in[0] being absolute sample a0).  D decodes each word (above).
+template <class D, bool CPLX>
+__global__ void __launch_bounds__(kRawThreads) unpack_kernel(typename D::Word const *__restrict__ in, long history, long L,
+                                                             int nblocks, double scale, ScaleChange const *__restrict__ chg,
+                                                             int nchg, long long a0, float *__restrict__ out, BlockStats *stats) {
   int const seg = blockIdx.y;
   long const len = seg < nblocks ? L : history;
   if ((long)blockIdx.x * kRawThreads >= len) return;  // the whole CTA lies past its segment
@@ -72,11 +99,10 @@ __global__ void __launch_bounds__(kRawThreads) unpack8_kernel(uint8_t const *__r
     double const sc = nchg ? scale_at(chg, nchg, scale, a0 + base + i) : scale;
 #pragma unroll
     for (int c = 0; c < C; c++) {
-      uint8_t const b = in[s + c];
-      int const x = SIGNED ? (int)(int8_t)b : (int)b - 128;
+      int const x = D::x(in[s + c]);
       out[s + c] = __double2float_rn(__dmul_rn(sc, (double)x));
       e += (unsigned)(x * x);
-      o += (x >= 127 || x <= -128);
+      o += D::over(x);
     }
   }
   if (stats && seg < nblocks) block_stats_add(stats + seg, e, o, o != 0);
