@@ -200,6 +200,31 @@ int kgpu_iq_scan(const struct kgpu_iq_write *d_tab, struct kgpu_iq_state *d_coef
 int kgpu_iq_apply(const void *d_raw, int fmt, long long a0, long count, const struct kgpu_iq_write *d_tab,
                   const struct kgpu_iq_state *d_coef, int cap, long long w_lo, int nw, void *d_out, void *stream);
 
+/* sig_gen.c's CW source (proc_sig_gen, sig_gen.c:286-346) on the device; see csrc/siggen.cuh.  freq and rate are cycles
+ * per sample and per sample^2, what set_osc receives (sig_gen.c:221-224); amplitude and noise sdr->amplitude and
+ * sdr->noise; seed rand_init's xoshiro256** seed (1). */
+struct kgpu_siggen_params {
+  double freq, rate, amplitude, noise;
+  uint64_t seed;
+};
+typedef struct kgpu_siggen kgpu_siggen;
+/* A generator of REAL samples or COMPLEX pairs (pure host code; the device's jump matrices are copied at the first
+ * generate); NULL and kgpu_last_error() on failure. */
+kgpu_siggen *kgpu_siggen_create(int in_type, const struct kgpu_siggen_params *params);
+void kgpu_siggen_destroy(kgpu_siggen *g);
+/* The floats of samples [a0, a0 + count) at d_out (float per REAL sample, float2 per pair), each (float)(samp * scale) as
+ * the driver's loop stores it, scale that of the sample (`scale` before the first of the nchg changes at d_chg, else the
+ * last change at or before it); samples a < 0 precede the stream and are 0.0f (they must lie in the history).  The window is laid out as kgpu_forward's
+ * d_in: `history` samples, then nblocks blocks of L (L >= 64 when nblocks > 0).  d_block_energy: NULL or nblocks
+ * doubles, block j's sum of |samp|^2 (unscaled) over its L new samples.  Enqueued on `stream`; calls of one generator go
+ * on one stream (its scratch is reused). */
+int kgpu_siggen_generate(kgpu_siggen *g, long long a0, long count, double scale, const struct kgpu_scale_change *d_chg, int nchg,
+                         void *d_out, double *d_block_energy, int nblocks, long L, long history, void *stream);
+/* Pure host code: the xoshiro256** state before draw `draw` (out[4]), by GF(2) jumps from the seeded state; and the
+ * step and sweep angles the carrier uses, in cycles as 128-bit fractions: out[4] = {F low, F high, R low, R high}. */
+int kgpu_siggen_state(const kgpu_siggen *g, unsigned long long draw, uint64_t *out);
+int kgpu_siggen_angles(const kgpu_siggen *g, uint64_t *out);
+
 /* Notch EWMA on listed bins (apply_notch_filters, filter.c:464-474); list ends with bin 0. The state
  * lives in the master; blocks are processed in order. */
 int kgpu_master_set_notches(kgpu_master *m, int const *bins, double const *alpha, int n);

@@ -23,6 +23,9 @@
  *   filter_ingest_stats           (EXTENSION) the A/D energy and overranges those loops return, per drained block
  *   filter_iq_correction_setup    (EXTENSION) HackRF's and FUNcube's DC and I/Q gain and phase correction on the device
  *   filter_iq_records             (EXTENSION) the per-transfer sums and state those drivers' loops produce
+ *   filter_siggen_setup           (EXTENSION) sig_gen.c's carrier and noise generated on the device
+ *   write_genfilter               (EXTENSION) advance a generated master, replacing sig_gen.c's sample loop
+ *   filter_siggen_stats           (EXTENSION) the energy that loop sums, per drained block
  *
  * Semantics kept: return 0 / -1 (write_*: 1 if a block fired), ND-deep spectrum ring with
  * lap -> zeros + block_drops++ (filter.c:690-701), owner-thread shortcut (filter.c:681-683),
@@ -226,6 +229,35 @@ struct filter_iq_record {
  * Records arrive up to one launch after their write.  A caller that falls more than the table's writes behind loses the
  * oldest.  Returns the count, or -1 on a master without I/Q correction. */
 int filter_iq_records(struct filter_in *master, struct filter_iq_record *recs, int max);
+/* EXTENSION: sig_gen.c's CW source (proc_sig_gen, sig_gen.c:286-346) generated on the device: no samples cross PCIe and
+ * the host float ring is never written.  Call filter_siggen_setup once, before the first write (-1 on a master already
+ * fed floats, int16 or raw words).  The master then rejects write_rfilter, write_cfilter, write_i16filter and
+ * write_rawfilter with -1.  write_genfilter(master, n, scale) replaces the driver's per-sample loop and its
+ * write_rfilter / write_cfilter: it advances the stream by n samples (REAL) or pairs (COMPLEX), each the loop's
+ * (float)(samp * scale) with this write's scale, and fires blocks as write_rfilter does (1 if a block fired).  Samples
+ * before the first write are 0.0f.  The noise is bitwise the reference's (xoshiro256** seeded by rand_init through
+ * splitmix64, real_gauss); the carrier is within 1 ulp of its phasor chain.  Only CW is served (FM is CW in the reference);
+ * AM and DSB read an audio source and stay with the driver's loop.
+ *   freq, rate  cycles per sample and per sample^2, what set_osc receives: carrier / samprate (REAL),
+ *               (carrier - frequency) / samprate (COMPLEX), sig_gen.c:221-224
+ *   amplitude, noise  sdr->amplitude, sdr->noise;  seed  rand_init's (1) */
+struct filter_siggen_params {
+  double freq, rate;
+  double amplitude, noise;
+  uint64_t seed;
+};
+int filter_siggen_setup(struct filter_in *master, struct filter_siggen_params const *params);
+int write_genfilter(struct filter_in *master, int n, double scale);
+/* The generated energy, as filter_ingest_stats counts its statistics: never blocks, sums over the blocks whose device
+ * work completed since the previous call, each block once; the first call starts collection and returns zeros.  energy
+ * is the sum of samp^2 (REAL, as sig_gen.c:294) or |samp|^2 (COMPLEX) of the unscaled samples; the reference's COMPLEX
+ * loop adds re^2 - im^2 (sig_gen.c:324).  -1 on a master that is not generated. */
+struct filter_siggen_stats {
+  uint64_t blocks;  /* blocks summed by this call */
+  uint64_t samples; /* their new samples (blocks * L) */
+  double energy;
+};
+int filter_siggen_stats(struct filter_in *master, struct filter_siggen_stats *stats);
 /* EXTENSION: serve many slaves with one call (what 1024 channel threads would each do): one wait per block. */
 int execute_filter_output_batch(struct filter_out *const *slaves, int const *shifts, int n);
 /* EXTENSION (downconvert()'s per-sample work, radio.c:1476-1501 and :1515-1520, on the device): execute_filter_output

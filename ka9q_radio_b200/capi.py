@@ -90,6 +90,15 @@ def load() -> C.CDLL:
     L.kgpu_iq_moments.argtypes = [vp, i, ll, l, vp, i, ll, i, vp]
     L.kgpu_iq_scan.argtypes = [vp, vp, i, ll, i, vp, vp, vp]
     L.kgpu_iq_apply.argtypes = [vp, i, ll, l, vp, vp, i, ll, i, vp, vp]
+    L.kgpu_siggen_create.restype = vp
+    L.kgpu_siggen_create.argtypes = [i, vp]
+    L.kgpu_siggen_destroy.argtypes = [vp]
+    L.kgpu_siggen_generate.argtypes = [vp, ll, l, d, vp, i, vp, vp, i, l, l, vp]
+    L.kgpu_siggen_state.argtypes = [vp, C.c_ulonglong, vp]
+    L.kgpu_siggen_angles.argtypes = [vp, vp]
+    L.filter_siggen_setup.argtypes = [vp, vp]
+    L.write_genfilter.argtypes = [vp, i, d]
+    L.filter_siggen_stats.argtypes = [vp, vp]
     L.kgpu_bank_define_ex.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_wide.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_huge.argtypes = [vp, i, i, i]
@@ -227,6 +236,58 @@ def iq_apply(d_raw: int, fmt: int, a0: int, count: int, d_tab: int, d_coef: int,
              stream: int = 0) -> None:
     """Corrected float I/Q of pairs [a0, a0 + count); pairs before 0 are 0.0 (kgpu_iq_apply)."""
     check(load().kgpu_iq_apply(d_raw, fmt, a0, count, d_tab, d_coef, cap, w_lo, nw, d_out, stream or None), "kgpu_iq_apply")
+
+
+class SiggenParams(C.Structure):
+    """struct kgpu_siggen_params (and filter.h's struct filter_siggen_params, the same layout)"""
+    _fields_ = [("freq", C.c_double), ("rate", C.c_double), ("amplitude", C.c_double), ("noise", C.c_double),
+                ("seed", C.c_uint64)]
+
+
+class SiggenStats(C.Structure):
+    """filter.h's struct filter_siggen_stats"""
+    _fields_ = [("blocks", C.c_uint64), ("samples", C.c_uint64), ("energy", C.c_double)]
+
+
+class Siggen:
+    """sig_gen.c's CW source on the device (kgpu_siggen_*): carrier freq / rate in cycles per sample (per sample^2),
+    amplitude, noise and the xoshiro256** seed as rand_init gives it (1)."""
+
+    def __init__(self, in_type: int, freq: float, amplitude: float, noise: float, rate: float = 0.0, seed: int = 1):
+        self.cplx = in_type == KGPU_COMPLEX
+        p = SiggenParams(freq, rate, amplitude, noise, seed)
+        self.h = load().kgpu_siggen_create(in_type, C.byref(p))
+        if not self.h:
+            raise KgpuError(f"kgpu_siggen_create: {load().kgpu_last_error().decode()}")
+
+    def generate(self, a0: int, count: int, scale: float, d_out: int, d_energy: int = 0, nblocks: int = 0, L: int = 0,
+                 history: int | None = None, d_chg: int = 0, nchg: int = 0, stream: int = 0) -> None:
+        """floats of samples [a0, a0 + count) at d_out; d_energy: 0 or nblocks float64 block energies of a window of
+        `history` samples then nblocks blocks of L (history defaults to count - nblocks * L)"""
+        if history is None:
+            history = count - nblocks * L
+        check(load().kgpu_siggen_generate(self.h, a0, count, scale, d_chg or None, nchg, d_out, d_energy or None, nblocks, L,
+                                          history, stream or None), "kgpu_siggen_generate")
+
+    def state(self, draw: int) -> tuple[int, int, int, int]:
+        """the xoshiro256** state before draw `draw` (host jump)"""
+        out = (C.c_uint64 * 4)()
+        check(load().kgpu_siggen_state(self.h, draw, C.cast(out, C.c_void_p)), "kgpu_siggen_state")
+        return tuple(int(v) for v in out)
+
+    def angles(self) -> tuple[int, int]:
+        """the carrier's step and sweep angles, cycles times 2^128"""
+        out = (C.c_uint64 * 4)()
+        check(load().kgpu_siggen_angles(self.h, C.cast(out, C.c_void_p)), "kgpu_siggen_angles")
+        return int(out[0]) | int(out[1]) << 64, int(out[2]) | int(out[3]) << 64
+
+    def close(self) -> None:
+        if self.h:
+            load().kgpu_siggen_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        self.close()
 
 
 MASTER_DIRECT, MASTER_EXTENDED, MASTER_BLUESTEIN = 0, 1, 2

@@ -176,6 +176,13 @@ struct master_ctx {
   long sring_cap; /* samples */
   long sring_pos; /* just past the newest issued sample */
   bool sring_i16;
+  /* sig_gen's CW source (filter_siggen_setup): the device generates every window, the host ring is never written.
+   * d_gen_energy / h_gen_energy: each ring slot's block energies, folded in job order into gen_acc once asked for */
+  kgpu_siggen *gen;
+  double *d_gen_energy, *h_gen_energy;
+  bool gen_stats_on;
+  unsigned long long gen_folded;
+  struct filter_siggen_stats gen_acc;
 };
 
 /* ---------------------------------------------------------------- mirrored ring ------------- */
@@ -336,6 +343,9 @@ static void master_teardown(struct filter_in *master) {
       spec_slave_free(sp);
     }
     cudaFree(c->d_sring);
+    kgpu_siggen_destroy(c->gen);
+    cudaFree(c->d_gen_energy);
+    cudaFreeHost(c->h_gen_energy);
     pthread_mutex_destroy(&c->mu);
     free(c);
     master->fwd_plan = NULL;
@@ -721,8 +731,8 @@ static int raw_start(struct filter_in *f, struct master_ctx *c, int format) {
                                          : "");
     return -1;
   }
-  if (c->i16_mode || f->wcnt != 0 || c->issued != 0) {
-    fprintf(stderr, "write_rawfilter: the master is already fed int16 or float samples\n");
+  if (c->i16_mode || c->gen || f->wcnt != 0 || c->issued != 0) {
+    fprintf(stderr, "write_rawfilter: the master is already fed int16, generated or float samples\n");
     return -1;
   }
   bool const cplx = f->in_type == COMPLEX;
@@ -955,6 +965,14 @@ static void fold_one(struct filter_in const *f, struct master_ctx *c) {
   c->folded++;
 }
 
+/* the generated energy of job c->gen_folded into c->gen_acc (its slot's device work has completed) */
+static void gen_fold_one(struct filter_in const *f, struct master_ctx *c) {
+  c->gen_acc.blocks++;
+  c->gen_acc.samples += (uint64_t)f->ilen;
+  c->gen_acc.energy += c->h_gen_energy[c->gen_folded % ND];
+  c->gen_folded++;
+}
+
 /* ---------------------------------------------------------------- spectrum device ring ------ */
 /* n samples of esz bytes from a ring (src_cap samples, position src) to the device ring at position dst, both modular */
 static int sring_copy(struct master_ctx *c, char const *src_base, long src_cap, long src, long dst, long n, size_t esz,
@@ -989,6 +1007,22 @@ static int sring_seed(struct filter_in *f, struct master_ctx *c) {
   }
   long const M1 = f->impulse_length - 1;
   c->sring_pos = (long)((M1 + (unsigned long long)f->ilen * c->issued) % (unsigned long long)c->sring_cap);
+  if (c->gen) { /* the host ring holds nothing: generate the last sring_cap samples again */
+    long const n = c->sring_cap, dst = c->sring_pos, first = n - dst;
+    long long const a0 = (long long)f->ilen * (long long)c->issued - n;
+    double scale;
+    int nc;
+    int rc = chg_span(c, ND, a0, a0 + n, &scale, &nc);
+    struct kgpu_scale_change const *chg = nc ? c->d_chg : NULL;
+    rc = rc ? rc
+            : kgpu_siggen_generate(c->gen, a0, first, scale, chg, nc, (char *)c->d_sring + (size_t)dst * esz, NULL, 0, 0, first,
+                                   c->st);
+    if (rc == 0 && dst > 0)
+      rc = kgpu_siggen_generate(c->gen, a0 + first, dst, scale, chg, nc, c->d_sring, NULL, 0, 0, dst, c->st);
+    if (cudaStreamSynchronize(c->st) != cudaSuccess)
+      rc = -1;
+    return rc ? kgf_fail("filter_spectrum_setup: generating the device ring") : 0;
+  }
   if (c->raw_fmt) { /* the host ring holds raw bytes: send the last sring_cap samples' bytes over and unpack them there */
     bool const cplx = f->in_type == COMPLEX;
     long const n = c->sring_cap, cap = raw_samples(c->raw_fmt, cplx, c->raw_ring_size);
@@ -1063,6 +1097,8 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     c->stats_on = false; /* fed floats: the driver counts in its own loop */
   while (c->stats_on && c->folded + ND < c->issued + (unsigned long long)k)
     fold_one(f, c); /* the statistics of the slots about to be reused */
+  while (c->gen_stats_on && c->gen_folded + ND < c->issued + (unsigned long long)k)
+    gen_fold_one(f, c);
   while (c->iq_on && c->iq_checked + ND < c->issued + (unsigned long long)k)
     c->iq_avail = c->iq_job_done[c->iq_checked++ % ND]; /* the records of the slots about to be reused have arrived */
   struct kgpu_block_stats *const bst = c->stats_on ? c->d_bstats + slot : NULL;
@@ -1102,6 +1138,9 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     c->raw_rp += raw_bytes(c->raw_fmt, cplx, (size_t)f->ilen * (size_t)k);
     if (c->raw_rp >= (char *)c->raw_ring + c->raw_ring_size)
       c->raw_rp -= c->raw_ring_size;
+  } else if (c->gen) { /* generated on the device below: nothing crosses PCIe */
+    src = NULL;
+    bytes = 0;
   } else if (f->in_type == COMPLEX) {
     src = f->input_read_pointer.c;
     bytes = sizeof(float complex) * span;
@@ -1119,7 +1158,7 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
       c->snap[slot + j][i].ok = false;
   void const *const ring = c->i16_mode ? c->i16_ring : c->raw_fmt ? c->raw_ring : f->input_buffer;
   size_t const ring_size = c->i16_mode ? c->i16_ring_size : c->raw_fmt ? c->raw_ring_size : f->input_buffer_size;
-  if (window_h2d(c->raw_fmt ? c->d_raw : c->d_win[slot], src, bytes, ring, ring_size, c->st) != 0)
+  if (!c->gen && window_h2d(c->raw_fmt ? c->d_raw : c->d_win[slot], src, bytes, ring, ring_size, c->st) != 0)
     rc = kgf_fail("execute_filter_input: H2D of the window");
   long const M1 = f->impulse_length - 1;
   long long const a0 = (long long)f->ilen * (long long)c->issued - M1; /* the window's first sample */
@@ -1127,6 +1166,14 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     chg_prune(f, c);
   if (rc == 0 && c->iq_on && iq_launch(f, c, k) != 0)
     rc = kgf_fail("execute_filter_input: I/Q correction");
+  if (rc == 0 && c->gen) {
+    double s;
+    int n;
+    if (chg_span(c, slot, a0, a0 + (long long)span, &s, &n) != 0 ||
+        kgpu_siggen_generate(c->gen, a0, (long)span, s, n ? c->d_chg : NULL, n, c->d_win[slot],
+                             c->gen_stats_on ? c->d_gen_energy + slot : NULL, k, f->ilen, M1, c->st) != 0)
+      rc = kgf_fail("execute_filter_input: kgpu_siggen_generate");
+  }
   if (rc == 0 && c->raw_fmt && raw_unpack(f, c, slot, c->d_raw, a0, M1, k, c->d_win[slot], bst, c->st) != 0)
     rc = kgf_fail("execute_filter_input: raw unpack");
   if (rc == 0 && c->i16_mode && bst &&
@@ -1210,6 +1257,10 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
   cudaStreamWaitEvent(c->st_d2h, c->kev, 0);
   if (rc == 0 && bst && cudaMemcpyAsync(c->h_bstats + slot, bst, sizeof *bst * (size_t)k, cudaMemcpyDeviceToHost, c->st_d2h) != cudaSuccess)
     rc = kgf_fail("execute_filter_input: D2H of the A/D statistics");
+  if (rc == 0 && c->gen_stats_on &&
+      cudaMemcpyAsync(c->h_gen_energy + slot, c->d_gen_energy + slot, sizeof(double) * (size_t)k, cudaMemcpyDeviceToHost,
+                      c->st_d2h) != cudaSuccess)
+    rc = kgf_fail("execute_filter_input: D2H of the generated energies");
   if (c->iq_on) {
     unsigned long long const from = c->iq_rec_from, to = c->iq_scanned;
     for (unsigned long long w = from; rc == 0 && w < to;) { /* the records of the writes this launch completed */
@@ -1872,8 +1923,10 @@ int delete_filter_input(struct filter_in *master) { /* filter.c:930-942 */
 }
 
 /* ---------------------------------------------------------------- write_*filter ------------- */
-/* a master fed raw words takes no floats */
-static bool raw_fed(struct filter_in const *f) { return f->fwd_plan && ((struct master_ctx const *)f->fwd_plan)->raw_fmt; }
+/* a master fed raw words, or generating its own, takes no floats */
+static bool raw_fed(struct filter_in const *f) {
+  return f->fwd_plan && (((struct master_ctx const *)f->fwd_plan)->raw_fmt || ((struct master_ctx const *)f->fwd_plan)->gen);
+}
 int write_cfilter(struct filter_in *f, float complex const *buffer, int size) { /* filter.c:1093-1113 */
   if (f == NULL || raw_fed(f))
     return -1;
@@ -2035,8 +2088,8 @@ int filter_ingest_stats(struct filter_in *f, struct filter_ingest_stats *stats) 
   if (f == NULL || f->fwd_plan == NULL || stats == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (c->iq_on)
-    return -1; /* I/Q corrected: filter_iq_records replaces the block statistics */
+  if (c->iq_on || c->gen)
+    return -1; /* I/Q corrected: filter_iq_records replaces the block statistics; generated: filter_siggen_stats */
   int rc = 0;
   pthread_mutex_lock(&c->mu);
   if (!c->i16_mode && !c->raw_fmt && (c->issued > 0 || f->wcnt > 0))
@@ -2072,8 +2125,8 @@ int filter_iq_correction_setup(struct filter_in *f, int format, struct filter_iq
   if (f == NULL || f->fwd_plan == NULL || p == NULL || !iq_format(format))
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (c->raw_fmt || c->iq_on) {
-    fprintf(stderr, "filter_iq_correction_setup: the master is already fed raw words\n");
+  if (c->raw_fmt || c->iq_on || c->gen) {
+    fprintf(stderr, "filter_iq_correction_setup: the master is already fed raw words or generated\n");
     return -1;
   }
   long const cap = filter_iq_table_writes(f->ilen, f->impulse_length, f->in_type, format);
@@ -2140,6 +2193,76 @@ int filter_iq_records(struct filter_in *f, struct filter_iq_record *recs, int ma
   }
   pthread_mutex_unlock(&c->mu);
   return n;
+}
+
+/* ---------------------------------------------------------------- sig_gen ------------------- */
+/* EXTENSION: sig_gen's CW source on the device (see include/ka9q_gpu_filter.h), before the first write. */
+int filter_siggen_setup(struct filter_in *f, struct filter_siggen_params const *p) {
+  if (f == NULL || f->fwd_plan == NULL || p == NULL)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (c->gen || c->raw_fmt || c->i16_mode || f->wcnt != 0 || c->issued != 0) {
+    fprintf(stderr, "filter_siggen_setup: the master is already fed or generated\n");
+    return -1;
+  }
+  struct kgpu_siggen_params const kp = {p->freq, p->rate, p->amplitude, p->noise, p->seed};
+  kgpu_siggen *g = kgpu_siggen_create(f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL, &kp);
+  if (!g) {
+    fprintf(stderr, "filter_siggen_setup: %s\n", kgpu_last_error());
+    return -1;
+  }
+  if (cudaMalloc((void **)&c->d_gen_energy, sizeof(double) * ND) != cudaSuccess ||
+      cudaHostAlloc((void **)&c->h_gen_energy, sizeof(double) * ND, cudaHostAllocPortable) != cudaSuccess) {
+    kgpu_siggen_destroy(g);
+    return kgf_fail("filter_siggen_setup: energy buffers"); /* freed with the master */
+  }
+  pthread_mutex_lock(&c->mu);
+  c->gen = g;
+  pthread_mutex_unlock(&c->mu);
+  return 0;
+}
+
+/* EXTENSION: advance a generated master by n samples (REAL) or pairs (COMPLEX), stored with this write's scale; fires
+ * the blocks they complete as write_rfilter does. */
+int write_genfilter(struct filter_in *f, int n, double scale) {
+  if (f == NULL || f->fwd_plan == NULL || n < 0)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (!c->gen)
+    return -1;
+  if (((size_t)f->wcnt + (size_t)n) * c->esz >= f->input_buffer_size)
+    return -1;
+  pthread_mutex_lock(&c->mu);
+  int const rc = chg_note(f, c, scale, "write_genfilter");
+  pthread_mutex_unlock(&c->mu);
+  if (rc != 0)
+    return -1;
+  f->wcnt += n;
+  return fire_ready_blocks(f);
+}
+
+/* EXTENSION: the generated energy of the blocks whose device work completed since the previous call, as
+ * filter_ingest_stats counts them. */
+int filter_siggen_stats(struct filter_in *f, struct filter_siggen_stats *stats) {
+  if (f == NULL || f->fwd_plan == NULL || stats == NULL)
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (!c->gen)
+    return -1;
+  pthread_mutex_lock(&c->mu);
+  if (!c->gen_stats_on) {
+    c->gen_stats_on = true;
+    c->gen_folded = c->issued; /* blocks already issued carry no energy */
+    memset(&c->gen_acc, 0, sizeof c->gen_acc);
+    memset(stats, 0, sizeof *stats);
+  } else {
+    while (c->gen_folded < c->issued && cudaEventQuery(c->done[c->gen_folded % ND]) == cudaSuccess)
+      gen_fold_one(f, c);
+    *stats = c->gen_acc;
+    memset(&c->gen_acc, 0, sizeof c->gen_acc);
+  }
+  pthread_mutex_unlock(&c->mu);
+  return 0;
 }
 
 /* ---------------------------------------------------------------- housekeeping -------------- */

@@ -33,6 +33,7 @@
 #include "bluestein_chan.cuh"
 #include "raw_ingest.cuh"
 #include "iq_correct.cuh"
+#include "siggen.cuh"
 
 using namespace kfft;
 
@@ -429,6 +430,185 @@ extern "C" int kgpu_iq_apply(const void *d_raw, int fmt, long long a0, long coun
       d_raw, a0, count, (IqWrite const *)d_tab, (IqState const *)d_coef, cap, w_lo, nw, (float2 *)d_out);
   g_launches++;
   CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---- sig_gen.c's CW source (siggen.cuh) ------------------------------------------------------------------------------
+extern "C" void kgpu_siggen_angle128(double f, uint64_t *out);  // siggen_host.c
+namespace {
+// T^(2^b), b = 0 .. 63, of xoshiro256**'s state transition, in siggen.cuh's nibble-table form; built once per process
+std::vector<unsigned long long> g_jump;
+std::once_flag g_jump_once;
+void xo_step_host(unsigned long long s[4]) {
+  unsigned long long const t = s[1] << 17;
+  s[2] ^= s[0];
+  s[3] ^= s[1];
+  s[1] ^= s[2];
+  s[0] ^= s[3];
+  s[2] ^= t;
+  s[3] = (s[3] << 45) | (s[3] >> 19);
+}
+void gf2_apply_host(unsigned long long const *tab, unsigned long long s[4]) {
+  unsigned long long y[4] = {0, 0, 0, 0};
+  for (int w = 0; w < 4; w++)
+    for (int q = 0; q < 16; q++) {
+      unsigned long long const *e = tab + ((w * 16 + q) * 16 + (int)((s[w] >> (4 * q)) & 15)) * 4;
+      for (int k = 0; k < 4; k++) y[k] ^= e[k];
+    }
+  for (int k = 0; k < 4; k++) s[k] = y[k];
+}
+// nibble tables of the matrix whose column j (the image of state bit j = bit j % 64 of word j / 64) is cols[j]
+void gf2_tables(unsigned long long const (*cols)[4], unsigned long long *tab) {
+  for (int w = 0; w < 4; w++)
+    for (int q = 0; q < 16; q++)
+      for (int v = 0; v < 16; v++) {
+        unsigned long long *e = tab + ((w * 16 + q) * 16 + v) * 4;
+        e[0] = e[1] = e[2] = e[3] = 0;
+        for (int i = 0; i < 4; i++)
+          if ((v >> i) & 1)
+            for (int k = 0; k < 4; k++) e[k] ^= cols[w * 64 + 4 * q + i][k];
+      }
+}
+void build_jumps() {
+  g_jump.assign((size_t)64 * kGf2Table, 0);
+  static unsigned long long cols[256][4];
+  for (int j = 0; j < 256; j++) {
+    for (int k = 0; k < 4; k++) cols[j][k] = 0;
+    cols[j][j / 64] = 1ULL << (j % 64);
+    xo_step_host(cols[j]);
+  }
+  gf2_tables(cols, g_jump.data());
+  for (int b = 1; b < 64; b++) {  // T^(2^b) = T^(2^(b-1)) applied to each column of itself
+    for (int j = 0; j < 256; j++) gf2_apply_host(g_jump.data() + (size_t)(b - 1) * kGf2Table, cols[j]);
+    gf2_tables(cols, g_jump.data() + (size_t)b * kGf2Table);
+  }
+}
+unsigned long long splitmix64(unsigned long long *x) {  // gauss.c:24-29
+  unsigned long long z = (*x += 0x9E3779B97F4A7C15ULL);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
+  return z ^ (z >> 31);
+}
+}  // namespace
+
+struct kgpu_siggen {
+  bool cplx;
+  kgpu_siggen_params p;
+  unsigned long long seeded[4];  // xoshiro256ss_seed (gauss.c:32-44)
+  U128 F, R;
+  unsigned long long *d_tabs;  // T^(kGenRun 2^b), b < kGenJumpBits
+  double *d_part;
+  long part_cap;
+};
+constexpr int kGenLog2Run = 6;
+static_assert(kGenRun == 64, "kGenLog2Run");
+
+extern "C" kgpu_siggen *kgpu_siggen_create(int in_type, const kgpu_siggen_params *p) {
+  if (!p || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX) || !std::isfinite(p->freq) || !std::isfinite(p->rate) ||
+      !std::isfinite(p->amplitude) || !std::isfinite(p->noise)) {
+    fail("kgpu_siggen_create: bad arguments");
+    return nullptr;
+  }
+  std::call_once(g_jump_once, build_jumps);
+  auto *g = new kgpu_siggen();
+  g->cplx = in_type == KGPU_COMPLEX;
+  g->p = *p;
+  unsigned long long x = p->seed;
+  for (int k = 0; k < 4; k++) g->seeded[k] = splitmix64(&x);
+  if ((g->seeded[0] | g->seeded[1] | g->seeded[2] | g->seeded[3]) == 0) g->seeded[0] = 1;
+  uint64_t a[2];
+  kgpu_siggen_angle128(p->freq, a);
+  g->F = {a[0], a[1]};
+  kgpu_siggen_angle128(p->rate, a);
+  g->R = {a[0], a[1]};
+  return g;
+}
+
+extern "C" void kgpu_siggen_destroy(kgpu_siggen *g) {
+  if (!g) return;
+  cudaFree(g->d_tabs);
+  cudaFree(g->d_part);
+  delete g;
+}
+
+extern "C" int kgpu_siggen_state(const kgpu_siggen *g, unsigned long long draw, uint64_t *out) {
+  if (!g || !out) return fail("kgpu_siggen_state: bad arguments");
+  unsigned long long s[4] = {g->seeded[0], g->seeded[1], g->seeded[2], g->seeded[3]};
+  for (int b = 0; b < 64; b++)
+    if ((draw >> b) & 1) gf2_apply_host(g_jump.data() + (size_t)b * kGf2Table, s);
+  for (int k = 0; k < 4; k++) out[k] = s[k];
+  return 0;
+}
+
+extern "C" int kgpu_siggen_angles(const kgpu_siggen *g, uint64_t *out) {
+  if (!g || !out) return fail("kgpu_siggen_angles: bad arguments");
+  out[0] = g->F.lo;
+  out[1] = g->F.hi;
+  out[2] = g->R.lo;
+  out[3] = g->R.hi;
+  return 0;
+}
+
+extern "C" int kgpu_siggen_generate(kgpu_siggen *g, long long a0, long count, double scale, const kgpu_scale_change *d_chg, int nchg,
+                                    void *d_out, double *d_block_energy, int nblocks, long L, long history, void *stream) {
+  int const C = g && g->cplx ? 2 : 1, S = kGenRun / C;
+  if (!g || !d_out || count < 0 || history < 0 || nblocks < 0 || nchg < 0 || (nchg && !d_chg) ||
+      (nblocks > 0 && (L < S || count != history + (long)nblocks * L)) || (a0 < 0 && std::min(-a0, (long long)count) > history))
+    return fail("kgpu_siggen_generate: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  float *out = (float *)d_out;
+  if (a0 < 0) {  // the samples before the stream's first: zeros, all inside the history
+    long const z = (long)std::min(-a0, (long long)count);
+    CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)C * (size_t)z, st));
+    out += (size_t)C * (size_t)z;
+    count -= z;
+    history -= z;
+    a0 = 0;
+  }
+  long const nthreads = (count + S - 1) / S;
+  if (nthreads >= (1L << kGenJumpBits)) return fail("kgpu_siggen_generate: %ld samples exceed one launch", count);
+  if (count == 0) return 0;
+  long const grid = (nthreads + kGenThreads - 1) / kGenThreads;
+  if (!g->d_tabs) {  // the device's jump matrices, at the first launch (create is pure host code)
+    size_t const bytes = sizeof(unsigned long long) * (size_t)kGenJumpBits * kGf2Table;
+    CUDA_OK(cudaMalloc((void **)&g->d_tabs, bytes));
+    CUDA_OK(cudaMemcpy(g->d_tabs, g_jump.data() + (size_t)kGenLog2Run * kGf2Table, bytes, cudaMemcpyHostToDevice));
+  }
+  if (d_block_energy && nblocks > 0 && 2 * grid * kGenThreads > g->part_cap) {
+    CUDA_OK(cudaStreamSynchronize(st));  // the previous launch may still write the old scratch
+    cudaFree(g->d_part);
+    g->d_part = nullptr;
+    g->part_cap = 0;
+    CUDA_OK(cudaMalloc((void **)&g->d_part, sizeof(double) * 2 * (size_t)grid * kGenThreads));
+    g->part_cap = 2 * grid * kGenThreads;
+  }
+  GenArgs a;
+  uint64_t base[4];
+  kgpu_siggen_state(g, (unsigned long long)a0 * (unsigned long long)C, base);
+  for (int k = 0; k < 4; k++) a.base[k] = base[k];
+  a.F = g->F;
+  a.R = g->R;
+  a.amplitude = g->p.amplitude;
+  a.noise = g->p.noise;
+  a.scale = scale;
+  a.chg = (ScaleChange const *)d_chg;
+  a.nchg = nchg;
+  a.a0 = a0;
+  a.count = count;
+  a.history = history;
+  a.L = nblocks > 0 ? L : 1;
+  a.tabs = g->d_tabs;
+  a.out = out;
+  a.part = d_block_energy && nblocks > 0 ? g->d_part : nullptr;
+  if (g->cplx) siggen_kernel<true><<<(unsigned)grid, kGenThreads, 0, st>>>(a);
+  else siggen_kernel<false><<<(unsigned)grid, kGenThreads, 0, st>>>(a);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  if (a.part) {
+    siggen_energy_kernel<<<nblocks, 256, 0, st>>>(a.part, history, L, S, nthreads, d_block_energy);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+  }
   return 0;
 }
 
