@@ -106,20 +106,28 @@ int kgpu_forward(kgpu_master *m, const void *d_in, int fmt, float scale, int der
  * d_stats: NULL or ONE kgpu_ingest_stats receiving the energy and the clip count (x == 2047 || x <= -2047). */
 int kgpu_unpack_airspy12(const void *d_packed, long sampcount, void *d_i16, void *d_stats, void *stream);
 
-/* 8- and 16-bit sample words of kgpu_unpack8.  Kept apart from kgpu_format: kgpu_forward does not read them. */
+/* 8-bit, 16-bit and float sample words of kgpu_unpack8.  Kept apart from kgpu_format: kgpu_forward does not read them. */
 enum kgpu_raw8 {
   KGPU_RAW_U8 = 1,  /* excess-128 bytes: RTL-SDR (rtlsdr.c:316-343), HydraSDR UINT8_REAL / UINT8_IQ (hydrasdr.c:759-775, :793-811) */
   KGPU_RAW_S8 = 2,  /* signed bytes: HydraSDR INT8_REAL / INT8_IQ (hydrasdr.c:776-791, :812-830) */
   KGPU_RAW_S16 = 3, /* int16: HydraSDR INT16_REAL / INT16_IQ (hydrasdr.c:700-716, :729-747), SDRplay (sdrplay.c:1238-1242) */
   KGPU_RAW_U16 = 4, /* offset-binary uint16, x = w - 32768, REAL only: HydraSDR UINT16_REAL (hydrasdr.c:681-699) */
-  KGPU_RAW_SC16Q11 = 5 /* bladeRF SC16_Q11, COMPLEX only: x = bits 0-11 sign-extended from bit 11 (bladerf.c:226-235) */
+  KGPU_RAW_SC16Q11 = 5, /* bladeRF SC16_Q11, COMPLEX only: x = bits 0-11 sign-extended from bit 11 (bladerf.c:226-235) */
+  /* floats (4-byte aligned).  Energy per block: the sum of the loop's terms as its source writes them, in double in a fixed order. */
+  KGPU_RAW_F32 = 6,         /* REAL only: (float)(scale * (double)x), terms x * x in float (hydrasdr.c:717-728) */
+  KGPU_RAW_CF32 = 7,        /* COMPLEX only: (float)(scale * (double)x), terms cnrm in double (hydrasdr.c:748-758) */
+  KGPU_RAW_CF32_CNRMF = 8,  /* COMPLEX only: (float)(scale * (double)x), terms cnrmf in float (airspyhf.c:313-318) */
+  KGPU_RAW_CF32_FSCALE = 9  /* COMPLEX only: x * (float)scale in float, terms x * x in float (fobos.c:410-420) */
 };
 /* A/D statistics of one block's L new samples (never its M-1 history samples).  A sample is one value (REAL) or one I/Q
  * pair (COMPLEX). */
 struct kgpu_block_stats {
-  unsigned long long energy; /* sum of x*x over every component */
-  unsigned int overs;        /* components at the format's limits */
-  unsigned int over_samples; /* samples with at least one component at the limits */
+  union {
+    unsigned long long energy; /* integer formats: sum of x*x over every component */
+    double fenergy;            /* float formats: the sum of the driver loop's energy terms, non-finite if one is */
+  };
+  unsigned int overs;        /* components at the format's limits (float formats: 0) */
+  unsigned int over_samples; /* samples with at least one component at the limits (float formats: 0) */
 };
 /* A front end's change of scale between two writes: from absolute sample `at` on (0 = the first sample a master was
  * written), samples take `scale`.  The conversions that take a device array of n of them, sorted by `at`, give each
@@ -128,13 +136,14 @@ struct kgpu_scale_change {
   long long at;
   double scale;
 };
-/* 8- and 16-bit ingest (replaces the conversion loops cited at kgpu_raw8): the words of an overlap-save launch --
- * `history` samples, then nblocks blocks of L new samples, laid out as kgpu_forward's d_in (16-bit words 2-byte aligned)
- * -- to floats at d_out (4-byte aligned), each (float)(scale * (double)x) with x the word's integer as kgpu_raw8 gives
- * it, bitwise what the drivers' loops store; then kgpu_forward(..., KGPU_FMT_F32, ...) reads d_out.  d_chg: NULL, or nchg
- * scale changes, the first history sample being absolute sample a0.  d_stats: NULL or nblocks kgpu_block_stats, zeroed
- * by the call; at the limits: x >= 127 or x <= -128 (U8, S8), x >= 32767 or x <= -32768 (S16, U16), x == 2047 or
- * x == -2048 (SC16Q11).  nblocks may be 0 (conversion only: history samples). */
+/* 8-bit, 16-bit and float ingest (replaces the conversion loops cited at kgpu_raw8): the words of an overlap-save launch
+ * -- `history` samples, then nblocks blocks of L new samples, laid out as kgpu_forward's d_in (16-bit words 2-byte
+ * aligned, floats 4-byte aligned) -- to floats at d_out (4-byte aligned), each (float)(scale * (double)x) with x the
+ * word's integer as kgpu_raw8 gives it, or the float formats' own rule, bitwise what the drivers' loops store; then
+ * kgpu_forward(..., KGPU_FMT_F32, ...) reads d_out.  d_chg: NULL, or nchg scale changes, the first history sample being
+ * absolute sample a0.  d_stats: NULL or nblocks kgpu_block_stats, zeroed by the call; at the limits: x >= 127 or x <= -128
+ * (U8, S8), x >= 32767 or x <= -32768 (S16, U16), x == 2047 or x == -2048 (SC16Q11); the float formats fill fenergy.
+ * nblocks may be 0 (conversion only: history samples). */
 int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, int nblocks, double scale,
                  const struct kgpu_scale_change *d_chg, int nchg, long long a0, void *d_out, void *d_stats, void *stream);
 /* int16 words laid out as kgpu_forward's KGPU_FMT_I16 d_in (count samples, the first being absolute sample a0) to floats

@@ -17,8 +17,9 @@
  *   delete_filter_input/output    filter.c:930-957
  *   write_i16filter               (EXTENSION, not in the reference) raw int16 ingest: fuses
  *                                 rx888.c:753-767 convert() into the first FFT pass
- *   write_rawfilter               (EXTENSION) raw 8-bit, packed 12-bit and 16-bit ingest: the conversion loops of
- *                                 rtlsdr.c, hydrasdr.c, airspy-unpack.c, bladerf.c and sdrplay.c on the device
+ *   write_rawfilter               (EXTENSION) raw 8-bit, packed 12-bit, 16-bit and float ingest: the conversion loops
+ *                                 of rtlsdr.c, hydrasdr.c, airspy-unpack.c, bladerf.c, sdrplay.c, airspyhf.c and
+ *                                 fobos.c on the device
  *   write_rawfilter_planar        (EXTENSION) SDRplay's separate int16 I and Q arrays as FILTER_RAW_S16 pairs
  *   filter_ingest_stats           (EXTENSION) the A/D energy and overranges those loops return, per drained block
  *   filter_iq_correction_setup    (EXTENSION) HackRF's and FUNcube's DC and I/Q gain and phase correction on the device
@@ -157,12 +158,26 @@ enum filter_raw_format {
   FILTER_RAW_S16_IQCORR = 5, /* FUNcube: int16 I/Q with the same correction */
   FILTER_RAW_S16 = 6,        /* int16, REAL or I/Q: HydraSDR INT16_REAL / INT16_IQ; SDRplay through write_rawfilter_planar */
   FILTER_RAW_U16 = 7,        /* offset-binary uint16 (x = w - 32768), REAL only: HydraSDR UINT16_REAL */
-  FILTER_RAW_SC16Q11 = 8     /* bladeRF SC16_Q11 I/Q, COMPLEX only: bits 0-11 of each word, sign-extended from bit 11 */
+  FILTER_RAW_SC16Q11 = 8,    /* bladeRF SC16_Q11 I/Q, COMPLEX only: bits 0-11 of each word, sign-extended from bit 11 */
+  FILTER_RAW_F32 = 9,        /* float, REAL only: HydraSDR FLOAT32_REAL */
+  FILTER_RAW_CF32 = 10,      /* float I/Q, COMPLEX only: HydraSDR FLOAT32_IQ */
+  FILTER_RAW_CF32_CNRMF = 11, /* float I/Q, COMPLEX only: AirspyHF+ */
+  FILTER_RAW_CF32_FSCALE = 12 /* float I/Q, COMPLEX only: Fobos */
 };
 /* The 16-bit formats (hydrasdr.c:681-716, :729-747, bladerf.c:215-246, sdrplay.c:1234-1246) give floats bitwise equal to
  * the drivers' (float)(scale * x) with a double scale; bladerf.c stores (float)x, i.e. scale 1.0.  Their limits, as the
  * drivers test them: x >= 32767 or x <= -32768 (S16, U16), x == 2047 or x == -2048 (SC16Q11).  Samples before the first
  * write are 0.0f (the U16 ring is prefilled with 0x8000 words). */
+/* The float formats take the floats the vendor libraries deliver and store each driver's own value, bitwise:
+ * (float)(scale * (double)x) with a double scale for F32, CF32 and CF32_CNRMF (hydrasdr.c:717-728, :748-758,
+ * airspyhf.c:313-318), x * (float)scale in float for CF32_FSCALE (fobos.c:410-420).  They test no limits.  Their energy
+ * (filter_ingest_stats' fenergy) sums the terms as each loop's source writes them: x * x in float (F32, CF32_FSCALE),
+ * cnrm in double (CF32), cnrmf in float with both products rounded (CF32_CNRMF; the reference's build contracts it into a
+ * fused multiply-add), added in double in a fixed order; the drivers' sums differ from it by their compiler's
+ * reassociation (fobos.c's is a float sum).  A block with a NaN or Inf sample, or a float term past FLT_MAX, has a
+ * non-finite energy, and so has every filter_ingest_stats result whose drained blocks include it: a driver's isfinite
+ * guard on that result skips all of that call's blocks (draining after each write that fires a block keeps that to the
+ * blocks the write fired).  Samples before the first write are 0.0f. */
 int write_rawfilter(struct filter_in *master, void const *samples, int n, int format, double scale);
 /* EXTENSION: SDRplay's separate I and Q arrays (sdrplay.c:1210-1246): n pairs i[k], q[k] interleaved into the raw ring of
  * a COMPLEX master fed FILTER_RAW_S16, then exactly a write_rawfilter(..., FILTER_RAW_S16, scale) of those pairs.  -1 on a
@@ -186,8 +201,11 @@ long filter_raw_ring_bytes(int L, int M, enum filtertype in_type, int format);
 struct filter_ingest_stats {
   uint64_t blocks;            /* blocks summed by this call */
   uint64_t samples;           /* their new samples (blocks * L): samples (REAL) or I/Q pairs (COMPLEX) */
-  uint64_t energy;            /* sum of x * x over every component of those samples */
-  uint64_t overranges;        /* components at the format's limits */
+  union {
+    uint64_t energy;          /* integer formats: sum of x * x over every component of those samples */
+    double fenergy;           /* float formats (FILTER_RAW_F32 ..): the sum of the driver loop's energy terms */
+  };
+  uint64_t overranges;        /* components at the format's limits (float formats: 0) */
   uint64_t overrange_samples; /* samples with at least one component at the limits */
   uint64_t since_over;        /* samples after the last summed block that had an overrange (over all calls) */
 };

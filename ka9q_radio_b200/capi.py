@@ -18,6 +18,7 @@ KGPU_COMPLEX, KGPU_REAL = 1, 2
 KGPU_FMT_F32, KGPU_FMT_I16 = 0, 1
 KGPU_RAW_U8, KGPU_RAW_S8 = 1, 2   # kgpu_unpack8's formats, apart from kgpu_format
 KGPU_RAW_S16, KGPU_RAW_U16, KGPU_RAW_SC16Q11 = 3, 4, 5   # its 16-bit formats (U16 REAL, SC16Q11 COMPLEX only)
+KGPU_RAW_F32, KGPU_RAW_CF32, KGPU_RAW_CF32_CNRMF, KGPU_RAW_CF32_FSCALE = 6, 7, 8, 9   # its float formats (F32 REAL, the rest COMPLEX only)
 KGPU_CHAN_ISB = 1
 KGPU_CHAN_BEAM = 4
 
@@ -195,10 +196,11 @@ def check(rc: int, what: str = "") -> int:
 
 def unpack8(d_raw: int, fmt: int, in_type: int, history: int, L: int, nblocks: int, scale: float, d_out: int,
             d_stats: int = 0, stream: int = 0, d_chg: int = 0, nchg: int = 0, a0: int = 0) -> None:
-    """8- and 16-bit ingest (kgpu_unpack8): the u8 / s8 bytes or s16 / u16 / sc16q11 words of `history` samples then
-    nblocks blocks of L to float32 at d_out, each (float)(scale * (double)x); d_stats: 0 or nblocks kgpu_block_stats
-    (uint64 energy, uint32 overs, uint32 over_samples); d_chg: 0 or nchg kgpu_scale_change (int64 at, float64 scale),
-    the first history sample being absolute sample a0."""
+    """8-bit, 16-bit and float ingest (kgpu_unpack8): the u8 / s8 bytes, s16 / u16 / sc16q11 words or floats of
+    `history` samples then nblocks blocks of L to float32 at d_out, each (float)(scale * (double)x) (x * (float)scale for
+    KGPU_RAW_CF32_FSCALE); d_stats: 0 or nblocks kgpu_block_stats (uint64 energy, or float64 fenergy for the float
+    formats, uint32 overs, uint32 over_samples); d_chg: 0 or nchg kgpu_scale_change (int64 at, float64 scale), the first
+    history sample being absolute sample a0."""
     check(load().kgpu_unpack8(d_raw, fmt, in_type, history, L, nblocks, scale, d_chg or None, nchg, a0, d_out,
                               d_stats or None, stream or None), "kgpu_unpack8")
 

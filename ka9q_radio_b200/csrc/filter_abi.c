@@ -682,8 +682,12 @@ static void rebuild_ranges(struct filter_in *f, struct master_ctx *c) {
 /* ---------------------------------------------------------------- raw ingest ---------------- */
 /* bytes of n samples (REAL) or I/Q pairs (COMPLEX) in a raw format; a packed-12 n is a multiple of 8 (three words) */
 static bool iq_format(int fmt) { return fmt == FILTER_RAW_S8_IQCORR || fmt == FILTER_RAW_S16_IQCORR; }
+/* the formats of floats the vendor libraries deliver (AirspyHF+, Fobos, HydraSDR FLOAT32_*) */
+static bool float_format(int fmt) { return fmt >= FILTER_RAW_F32 && fmt <= FILTER_RAW_CF32_FSCALE; }
 /* bytes per component */
 static size_t raw_word(int fmt) {
+  if (float_format(fmt))
+    return sizeof(float);
   return fmt == FILTER_RAW_S16_IQCORR || fmt == FILTER_RAW_S16 || fmt == FILTER_RAW_U16 || fmt == FILTER_RAW_SC16Q11 ? 2 : 1;
 }
 static size_t raw_bytes(int fmt, bool cplx, size_t n) {
@@ -704,10 +708,10 @@ long filter_raw_ring_bytes(int L, int M, enum filtertype in_type, int format) {
     if (cplx || L % 8 != 0 || (M - 1) % 8 != 0)
       return -1;
     unit = unit / (size_t)gcd((long)unit, 12) * 12;
-  } else if (iq_format(format) || format == FILTER_RAW_SC16Q11) {
+  } else if (iq_format(format) || format == FILTER_RAW_SC16Q11 || (float_format(format) && format != FILTER_RAW_F32)) {
     if (!cplx)
       return -1;
-  } else if (format == FILTER_RAW_U16) {
+  } else if (format == FILTER_RAW_U16 || format == FILTER_RAW_F32) {
     if (cplx)
       return -1;
   } else if (format != FILTER_RAW_U8 && format != FILTER_RAW_S8 && format != FILTER_RAW_S16)
@@ -728,6 +732,8 @@ static int raw_start(struct filter_in *f, struct master_ctx *c, int format) {
             : iq_format(format)          ? " (I/Q correction needs a COMPLEX master)"
             : format == FILTER_RAW_SC16Q11 ? " (SC16 Q11 samples are I/Q)"
             : format == FILTER_RAW_U16   ? " (offset-binary 16-bit samples are real)"
+            : format == FILTER_RAW_F32   ? " (FILTER_RAW_F32 samples are real)"
+            : float_format(format)       ? " (float I/Q formats need a COMPLEX master)"
                                          : "");
     return -1;
   }
@@ -856,6 +862,10 @@ static int kgpu_raw_format(int fmt) {
   case FILTER_RAW_S8: return KGPU_RAW_S8;
   case FILTER_RAW_S16: return KGPU_RAW_S16;
   case FILTER_RAW_U16: return KGPU_RAW_U16;
+  case FILTER_RAW_F32: return KGPU_RAW_F32;
+  case FILTER_RAW_CF32: return KGPU_RAW_CF32;
+  case FILTER_RAW_CF32_CNRMF: return KGPU_RAW_CF32_CNRMF;
+  case FILTER_RAW_CF32_FSCALE: return KGPU_RAW_CF32_FSCALE;
   default: return KGPU_RAW_SC16Q11;
   }
 }
@@ -958,7 +968,10 @@ static void fold_one(struct filter_in const *f, struct master_ctx *c) {
   struct kgpu_block_stats const *s = &c->h_bstats[c->folded % ND];
   c->acc.blocks++;
   c->acc.samples += (uint64_t)f->ilen;
-  c->acc.energy += s->energy;
+  if (float_format(c->raw_fmt))
+    c->acc.fenergy += s->fenergy;
+  else
+    c->acc.energy += s->energy;
   c->acc.overranges += s->overs;
   c->acc.overrange_samples += s->over_samples;
   c->acc.since_over = s->over_samples ? 0 : c->acc.since_over + (uint64_t)f->ilen;
@@ -1998,7 +2011,7 @@ int16_t *filter_i16_write_pointer(struct filter_in *f) {
  * raw ring at a master's first write); 0, or -1 with nothing stored */
 static int raw_admit(struct filter_in *f, struct master_ctx *c, int n, int format, double scale, char const *who) {
   if (format != FILTER_RAW_PACKED12 && format != FILTER_RAW_U8 && format != FILTER_RAW_S8 && format != FILTER_RAW_S16 &&
-      format != FILTER_RAW_U16 && format != FILTER_RAW_SC16Q11 && !iq_format(format)) {
+      format != FILTER_RAW_U16 && format != FILTER_RAW_SC16Q11 && !iq_format(format) && !float_format(format)) {
     fprintf(stderr, "%s: unknown format %d\n", who, format);
     return -1;
   }
@@ -2047,9 +2060,10 @@ static int raw_commit(struct filter_in *f, struct master_ctx *c, int n) {
   return fire_ready_blocks(f);
 }
 
-/* EXTENSION: raw packed 12-bit, 8-bit or 16-bit ADC words, unpacked on the device (see include/ka9q_gpu_filter.h).  The
- * drivers (airspy.c:388-434, hydrasdr.c:663-830, rtlsdr.c:316-343, bladerf.c:215-246) get their buffers from their vendor
- * libraries, so there is no zero-copy write pointer: the bytes are copied into the raw ring. */
+/* EXTENSION: raw packed 12-bit, 8-bit or 16-bit ADC words, or floats, converted on the device (see
+ * include/ka9q_gpu_filter.h).  The drivers (airspy.c:388-434, hydrasdr.c:663-830, rtlsdr.c:316-343, bladerf.c:215-246,
+ * airspyhf.c:292-325, fobos.c:395-426) get their buffers from their vendor libraries, so there is no zero-copy write
+ * pointer: the bytes are copied into the raw ring. */
 int write_rawfilter(struct filter_in *f, void const *samples, int n, int format, double scale) {
   if (f == NULL || f->fwd_plan == NULL || samples == NULL || n < 0)
     return -1;

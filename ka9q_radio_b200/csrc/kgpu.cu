@@ -316,7 +316,7 @@ extern "C" int kgpu_unpack_airspy12(const void *d_packed, long sampcount, void *
   return 0;
 }
 
-// ---- 8- and 16-bit ingest and per-block statistics of raw ingest (raw_ingest.cuh) ------------------------------------
+// ---- 8-bit, 16-bit and float ingest and per-block statistics of raw ingest (raw_ingest.cuh) ---------------------------
 static_assert(sizeof(ScaleChange) == sizeof(kgpu_scale_change), "raw_ingest.cuh mirrors include/ka9q_gpu.h");
 // REAL_OK / CPLX_OK: the master types the format exists for (only those kernels are instantiated)
 template <class D, bool REAL_OK = true, bool CPLX_OK = true>
@@ -331,9 +331,10 @@ static void launch_unpack(dim3 g, cudaStream_t st, bool cplx, const void *d_raw,
 extern "C" int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long history, long L, int nblocks, double scale,
                             const kgpu_scale_change *d_chg, int nchg, long long a0, void *d_out, void *d_stats, void *stream) {
   if (!d_raw || !d_out || history < 0 || nblocks < 0 || (nblocks > 0 && L < 1) || nblocks >= 65535 || nchg < 0 || (nchg && !d_chg) ||
-      fmt < KGPU_RAW_U8 || fmt > KGPU_RAW_SC16Q11 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX) ||
-      (fmt == KGPU_RAW_U16 && in_type != KGPU_REAL) || (fmt == KGPU_RAW_SC16Q11 && in_type != KGPU_COMPLEX) ||
-      (fmt >= KGPU_RAW_S16 && ((uintptr_t)d_raw & 1)))
+      fmt < KGPU_RAW_U8 || fmt > KGPU_RAW_CF32_FSCALE || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX) ||
+      ((fmt == KGPU_RAW_U16 || fmt == KGPU_RAW_F32) && in_type != KGPU_REAL) ||
+      ((fmt == KGPU_RAW_SC16Q11 || fmt >= KGPU_RAW_CF32) && in_type != KGPU_COMPLEX) ||
+      (fmt >= KGPU_RAW_S16 && ((uintptr_t)d_raw & 1)) || (fmt >= KGPU_RAW_F32 && ((uintptr_t)d_raw & 3)))
     return fail("kgpu_unpack8: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   BlockStats *stats = (BlockStats *)d_stats;
@@ -350,11 +351,24 @@ extern "C" int kgpu_unpack8(const void *d_raw, int fmt, int in_type, long histor
     case KGPU_RAW_S8: KGPU_UNPACK(DecodeS8); break;
     case KGPU_RAW_S16: KGPU_UNPACK(DecodeS16); break;
     case KGPU_RAW_U16: KGPU_UNPACK(DecodeU16, true, false); break;    // REAL only
-    default: KGPU_UNPACK(DecodeSC16Q11, false, true); break;           // COMPLEX only
+    case KGPU_RAW_SC16Q11: KGPU_UNPACK(DecodeSC16Q11, false, true); break;  // COMPLEX only
+    case KGPU_RAW_F32: KGPU_UNPACK(DecodeF32, true, false); break;     // REAL only
+    case KGPU_RAW_CF32_FSCALE: KGPU_UNPACK(DecodeF32FScale, false, true); break;  // COMPLEX only
+    default: KGPU_UNPACK(DecodeF32, false, true); break;               // CF32, CF32_CNRMF: COMPLEX only
   }
 #undef KGPU_UNPACK
   g_launches++;
   CUDA_OK(cudaGetLastError());
+  if (fmt >= KGPU_RAW_F32 && stats && nblocks) {  // the float formats' energies: a double sum in a fixed order
+    dim3 const ge(kEnergyCluster, (unsigned)nblocks);
+    auto const *f = (float const *)d_raw;
+    int const C = cplx ? 2 : 1;
+    if (fmt == KGPU_RAW_CF32) float_energy_kernel<EnergyCnrm><<<ge, kEnergyThreads, 0, st>>>(f, history, L, C, stats);
+    else if (fmt == KGPU_RAW_CF32_CNRMF) float_energy_kernel<EnergyCnrmf><<<ge, kEnergyThreads, 0, st>>>(f, history, L, C, stats);
+    else float_energy_kernel<EnergySq><<<ge, kEnergyThreads, 0, st>>>(f, history, L, C, stats);
+    g_launches++;
+    CUDA_OK(cudaGetLastError());
+  }
   return 0;
 }
 
