@@ -148,8 +148,10 @@ int16_t *filter_i16_write_pointer(struct filter_in *master);
  * PACKED12 (REAL masters only) gives (float)scale * (float)x, the drivers' float scale.  Each write's scale applies to
  * exactly its own samples.  PACKED12 needs n a multiple of 8 (whole groups of three 32-bit words), and
  * L and M - 1 multiples of 8 so every window starts on a group boundary (Airspy R2: L = 400000 / 200000, M - 1 = L/4);
- * other geometries are rejected with -1 and a message at the first write.  A master fed one format (raw, int16 or
- * float) rejects writes in another with -1.  Returns -1 on error, 1 if a block fired, else 0. */
+ * other geometries are rejected with -1 and a message at the first write.  A master fed one format (raw, int16,
+ * float or generated) rejects writes in another with -1: a raw, int16 or generated master refuses write_rfilter and
+ * write_cfilter, and a float master refuses write_i16filter and filter_i16_write_pointer.  Returns -1 on error, 1 if
+ * a block fired, else 0. */
 enum filter_raw_format {
   FILTER_RAW_PACKED12 = 1,
   FILTER_RAW_U8 = 2,

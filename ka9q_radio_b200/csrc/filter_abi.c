@@ -86,6 +86,18 @@ struct spec_slave {
   struct spec_slave *next;
 };
 
+/* What feeds a master: nothing yet, floats, int16 words, raw words, or its own generator.  Floats are never recorded:
+ * the header-inline put_rfilter / put_cfilter store them without calling the library, so a master holds floats once
+ * its float ring has taken or launched a sample (ingest_of). */
+enum ingest { INGEST_NONE, INGEST_FLOAT, INGEST_INT16, INGEST_RAW, INGEST_GEN };
+
+/* The int16 or raw words of a master's stream: a mirrored, pinned host ring of `size` bytes, `group` bytes to every 8
+ * samples (REAL) or I/Q pairs, written at wp; rp is the first sample (history included) of the next launch's window. */
+struct word_ring {
+  char *base, *wp, *rp;
+  size_t size, group;
+};
+
 struct master_ctx {
   kgpu_master *km;
   kgpu_bank *bank;
@@ -122,19 +134,13 @@ struct master_ctx {
   bool ranges_dirty;
   struct notch_state *notches_seen;
   unsigned notch_hash;
-  /* raw int16 ingest (extension) */
-  bool i16_mode;
-  void *i16_ring;
-  size_t i16_ring_size, i16_esz;
-  char *i16_wp, *i16_rp;
-  bool i16_derand;
-  /* raw 8-bit / packed 12-bit ingest (extension): the bytes in a mirrored ring of their own, unpacked on the device from
-   * d_raw into d_win[slot] */
-  int raw_fmt; /* 0, or the enum filter_raw_format the master is fed */
-  void *raw_ring;
-  size_t raw_ring_size;
-  char *raw_wp, *raw_rp;
+  /* what feeds the master (see check_mode); int16 and raw words go through `ring`, raw ones are then unpacked on the
+   * device from d_raw into d_win[slot] */
+  enum ingest mode;
+  int raw_fmt; /* INGEST_RAW: the enum filter_raw_format, its row of raw_formats; else 0 */
+  struct word_ring ring;
   void *d_raw;
+  bool i16_derand;
   /* the scale of every int16, 8-bit and packed-12 sample (the I/Q corrected formats keep theirs per write): samples
    * before chg[0].at take chg_base, those from chg[i].at on chg[i].scale.  A change enters where a write's scale differs
    * from the previous write's; changes leave once no launch, analyzer seeding or poll can read their samples.  d_chg takes
@@ -152,11 +158,10 @@ struct master_ctx {
   struct kgpu_block_stats *d_bstats, *h_bstats;
   unsigned long long folded; /* blocks folded (or, before stats_on, skipped) so far */
   struct filter_ingest_stats acc;
-  /* I/Q correction (FILTER_RAW_*_IQCORR): a ring table of the writes (host copy, device copy), the device's coefficient
+  /* I/Q correction (the RAW_IQ formats): a ring table of the writes (host copy, device copy), the device's coefficient
    * set and record of each write, and the pinned copy of the records */
-  bool iq_on;
   struct kgpu_iq_params iq_par;
-  int iq_cap;
+  int iq_cap; /* 0 until filter_iq_correction_setup has succeeded */
   struct kgpu_iq_write *h_iqw, *d_iqw;
   struct kgpu_iq_state *d_iqc;
   struct kgpu_iq_record *d_iqr, *h_iqr;
@@ -225,6 +230,36 @@ static void ring_free(void *base, size_t size) {
   if (cudaHostUnregister(base) != cudaSuccess)
     (void)cudaGetLastError();
   munmap(base, 2 * size);
+}
+
+static size_t wring_bytes(struct word_ring const *r, size_t n) { return n * r->group / 8; } /* packed-12: n % 8 == 0 */
+static long wring_samples(struct word_ring const *r, size_t bytes) { return (long)(bytes * 8 / r->group); }
+/* a ring of `size` bytes prefilled with the three-word `zero`, so the history samples and whatever the wideband
+ * analyzer's seeding reads before the stream reaches it are 0.0 as in the float ring; wp past the M-1 history samples */
+static int wring_open(struct word_ring *r, size_t size, size_t group, long history, uint32_t const zero[3]) {
+  r->base = ring_alloc(size);
+  if (!r->base)
+    return -1;
+  r->size = size;
+  r->group = group;
+  if (zero[0] | zero[1] | zero[2]) /* size is a multiple of the zero's period: 4 bytes, or 12 for packed-12 */
+    for (size_t o = 0; o < size; o += sizeof *zero)
+      memcpy(r->base + o, &zero[o / sizeof *zero % 3], sizeof *zero);
+  r->rp = r->base;
+  r->wp = r->base + wring_bytes(r, (size_t)history);
+  return 0;
+}
+/* publish the n samples just stored at wp (the mirror view keeps a write across the end contiguous) */
+static void wring_push(struct word_ring *r, size_t n) {
+  r->wp += wring_bytes(r, n);
+  kgf_ring_wrap((void **)&r->wp, r->base, r->size);
+}
+/* the window of the launch about to be issued, whose n new samples then leave the ring */
+static char const *wring_advance(struct word_ring *r, size_t n) {
+  char const *const win = r->rp;
+  r->rp += wring_bytes(r, n);
+  kgf_ring_wrap((void **)&r->rp, r->base, r->size);
+  return win;
 }
 
 static int kgf_fail(char const *where) {
@@ -321,8 +356,7 @@ static void master_teardown(struct filter_in *master) {
     cudaStreamDestroy(c->st_one);
     cudaStreamDestroy(c->st_d2h);
     cudaEventDestroy(c->kev);
-    ring_free(c->i16_ring, c->i16_ring_size);
-    ring_free(c->raw_ring, c->raw_ring_size);
+    ring_free(c->ring.base, c->ring.size);
     cudaFree(c->d_raw);
     free(c->chg);
     cudaFree(c->d_chg);
@@ -679,94 +713,105 @@ static void rebuild_ranges(struct filter_in *f, struct master_ctx *c) {
   }
 }
 
-/* ---------------------------------------------------------------- raw ingest ---------------- */
-/* bytes of n samples (REAL) or I/Q pairs (COMPLEX) in a raw format; a packed-12 n is a multiple of 8 (three words) */
-static bool iq_format(int fmt) { return fmt == FILTER_RAW_S8_IQCORR || fmt == FILTER_RAW_S16_IQCORR; }
-/* the formats of floats the vendor libraries deliver (AirspyHF+, Fobos, HydraSDR FLOAT32_*) */
-static bool float_format(int fmt) { return fmt >= FILTER_RAW_F32 && fmt <= FILTER_RAW_CF32_FSCALE; }
-/* bytes per component */
-static size_t raw_word(int fmt) {
-  if (float_format(fmt))
-    return sizeof(float);
-  return fmt == FILTER_RAW_S16_IQCORR || fmt == FILTER_RAW_S16 || fmt == FILTER_RAW_U16 || fmt == FILTER_RAW_SC16Q11 ? 2 : 1;
+/* ---------------------------------------------------------------- ingest modes and formats -- */
+/* Every raw format (enum filter_raw_format) in one row: its words, the masters it serves, its ring's zero, how the device
+ * decodes it, what the device window then holds, and its block statistics. */
+enum raw_path { RAW_UNPACK, RAW_AIRSPY12, RAW_IQ }; /* kgpu_unpack8 (code KGPU_RAW_*), _unpack_airspy12, _iq_apply (KGPU_IQ_*) */
+enum raw_stats { STATS_NONE, STATS_INT, STATS_FLOAT }; /* none: I/Q correction, whose records replace them */
+struct raw_format {
+  unsigned char group; /* bytes of 8 components: 1, 2 or 4 per component, or packed-12's 8 samples in three words */
+  bool real, cplx;     /* the masters it serves */
+  enum raw_path path;
+  int code;
+  bool i16; /* the device window holds int16 words, which kgpu_forward scales, rather than floats */
+  enum raw_stats stats;
+  char const *why;  /* why a master it does not serve is refused */
+  uint32_t zero[3]; /* the ring's zero word(s), repeated */
+};
+static struct raw_format const raw_formats[] = {
+    [FILTER_RAW_PACKED12] = {12, true, false, RAW_AIRSPY12, 0, true, STATS_INT,
+                             " (packed 12-bit needs a REAL master with L and M-1 multiples of 8)",
+                             {0x80080080u, 0x08008008u, 0x00800800u}}, /* eight offset-binary 2048s (airspy-unpack.c:110-117) */
+    [FILTER_RAW_U8] = {8, true, true, RAW_UNPACK, KGPU_RAW_U8, false, STATS_INT, "", {0x80808080u, 0x80808080u, 0x80808080u}},
+    [FILTER_RAW_S8] = {8, true, true, RAW_UNPACK, KGPU_RAW_S8, false, STATS_INT, ""},
+    [FILTER_RAW_S8_IQCORR] = {8, false, true, RAW_IQ, KGPU_IQ_S8, false, STATS_NONE, " (I/Q correction needs COMPLEX)"},
+    [FILTER_RAW_S16_IQCORR] = {16, false, true, RAW_IQ, KGPU_IQ_S16, false, STATS_NONE, " (I/Q correction needs COMPLEX)"},
+    [FILTER_RAW_S16] = {16, true, true, RAW_UNPACK, KGPU_RAW_S16, false, STATS_INT, ""},
+    [FILTER_RAW_U16] = {16, true, false, RAW_UNPACK, KGPU_RAW_U16, false, STATS_INT, " (real)",
+                        {0x80008000u, 0x80008000u, 0x80008000u}}, /* offset binary: 0x8000 is 0 */
+    [FILTER_RAW_SC16Q11] = {16, false, true, RAW_UNPACK, KGPU_RAW_SC16Q11, false, STATS_INT, " (I/Q)"},
+    [FILTER_RAW_F32] = {32, true, false, RAW_UNPACK, KGPU_RAW_F32, false, STATS_FLOAT, " (real)"},
+    [FILTER_RAW_CF32] = {32, false, true, RAW_UNPACK, KGPU_RAW_CF32, false, STATS_FLOAT, " (I/Q)"},
+    [FILTER_RAW_CF32_CNRMF] = {32, false, true, RAW_UNPACK, KGPU_RAW_CF32_CNRMF, false, STATS_FLOAT, " (I/Q)"},
+    [FILTER_RAW_CF32_FSCALE] = {32, false, true, RAW_UNPACK, KGPU_RAW_CF32_FSCALE, false, STATS_FLOAT, " (I/Q)"},
+};
+/* the row of a format number; NULL for a number that names no format */
+static struct raw_format const *format_row(int fmt) {
+  return fmt >= 1 && fmt < (int)(sizeof raw_formats / sizeof *raw_formats) ? &raw_formats[fmt] : NULL;
 }
-static size_t raw_bytes(int fmt, bool cplx, size_t n) {
-  return fmt == FILTER_RAW_PACKED12 ? n / 8 * 12 : n * (cplx ? 2 : 1) * raw_word(fmt);
-}
-static long raw_samples(int fmt, bool cplx, size_t bytes) {
-  return (long)(fmt == FILTER_RAW_PACKED12 ? bytes / 12 * 8 : bytes / ((cplx ? 2 : 1) * raw_word(fmt)));
-}
+/* the row of the raw format a master is fed (row 0, all zero, for the other modes) */
+static struct raw_format const *fed_row(struct master_ctx const *c) { return &raw_formats[c->raw_fmt]; }
 /* the device window holds int16 words (int16 ingest, or packed-12 after the unpack) rather than floats */
-static bool ingest_i16(struct master_ctx const *c) { return c->i16_mode || c->raw_fmt == FILTER_RAW_PACKED12; }
+static bool ingest_i16(struct master_ctx const *c) { return c->mode == INGEST_INT16 || fed_row(c)->i16; }
+/* the master's blocks carry A/D statistics (filter_ingest_stats) */
+static bool ingest_counted(struct master_ctx const *c) {
+  return c->mode == INGEST_INT16 || (c->mode == INGEST_RAW && fed_row(c)->stats != STATS_NONE);
+}
+
+static enum ingest ingest_of(struct filter_in const *f, struct master_ctx const *c) {
+  return c->mode == INGEST_NONE && (f->wcnt != 0 || c->issued != 0) ? INGEST_FLOAT : c->mode;
+}
+/* May the master be fed mode m?  0 if it holds nothing yet or m already (for a setup, which starts m, only nothing);
+ * else -1 and a message.  The caller records m in c->mode once the mode's state exists. */
+static int check_mode(struct filter_in const *f, struct master_ctx const *c, enum ingest m, bool setup, char const *who) {
+  static char const *const name[] = {"nothing", "floats", "int16 words", "raw words", "generated samples"};
+  enum ingest const held = ingest_of(f, c);
+  if (held == INGEST_NONE || (held == m && !setup))
+    return 0;
+  fprintf(stderr, "%s: %s on a master already fed %s\n", who, name[m], name[held]);
+  return -1;
+}
 
 long filter_raw_ring_bytes(int L, int M, enum filtertype in_type, int format) {
-  if (L <= 0 || M <= 0 || (in_type != REAL && in_type != COMPLEX))
+  struct raw_format const *rf = format_row(format);
+  if (rf == NULL || L <= 0 || M <= 0 || !(in_type == REAL ? rf->real : in_type == COMPLEX && rf->cplx))
     return -1;
   bool const cplx = in_type == COMPLEX;
   size_t unit = page_round(1);
-  if (format == FILTER_RAW_PACKED12) { /* whole groups, so a group never straddles the end of the ring */
-    if (cplx || L % 8 != 0 || (M - 1) % 8 != 0)
+  if (rf->group % 8 != 0) { /* packed-12: whole groups, so a group never straddles the end of the ring */
+    if (L % 8 != 0 || (M - 1) % 8 != 0)
       return -1;
-    unit = unit / (size_t)gcd((long)unit, 12) * 12;
-  } else if (iq_format(format) || format == FILTER_RAW_SC16Q11 || (float_format(format) && format != FILTER_RAW_F32)) {
-    if (!cplx)
-      return -1;
-  } else if (format == FILTER_RAW_U16 || format == FILTER_RAW_F32) {
-    if (cplx)
-      return -1;
-  } else if (format != FILTER_RAW_U8 && format != FILTER_RAW_S8 && format != FILTER_RAW_S16)
-    return -1;
+    unit = unit / (size_t)gcd((long)unit, rf->group) * rf->group;
+  }
   size_t const fsz = cplx ? sizeof(float complex) : sizeof(float);
   size_t const samples = page_round((size_t)ND * (size_t)(L + M - 1) * fsz) / fsz; /* the float ring's capacity */
-  size_t const need = raw_bytes(format, cplx, (samples + 7) / 8 * 8);
+  size_t const need = (samples + 7) / 8 * rf->group * (cplx ? 2 : 1);
   return (long)((need + unit - 1) / unit * unit);
 }
 
-/* the first write_rawfilter on a master: its ring, prefilled with the format's zero so the M-1 history samples (and
- * whatever the wideband analyzer's seeding reads before the stream reaches it) are 0.0 as in the float ring */
-static int raw_start(struct filter_in *f, struct master_ctx *c, int format) {
+/* the first write_rawfilter on a master, or its filter_iq_correction_setup: its ring and device window */
+static int raw_start(struct filter_in *f, struct master_ctx *c, int format, bool setup, char const *who) {
   long const size = filter_raw_ring_bytes(f->ilen, f->impulse_length, f->in_type, format);
   if (size < 0) {
-    fprintf(stderr, "write_rawfilter(L=%d M=%d): format %d cannot feed this master%s\n", f->ilen, f->impulse_length, format,
-            format == FILTER_RAW_PACKED12 ? " (packed 12-bit needs a REAL master with L and M-1 multiples of 8)"
-            : iq_format(format)          ? " (I/Q correction needs a COMPLEX master)"
-            : format == FILTER_RAW_SC16Q11 ? " (SC16 Q11 samples are I/Q)"
-            : format == FILTER_RAW_U16   ? " (offset-binary 16-bit samples are real)"
-            : format == FILTER_RAW_F32   ? " (FILTER_RAW_F32 samples are real)"
-            : float_format(format)       ? " (float I/Q formats need a COMPLEX master)"
-                                         : "");
+    fprintf(stderr, "%s(L=%d M=%d): format %d cannot feed this master%s\n", who, f->ilen, f->impulse_length, format,
+            raw_formats[format].why);
     return -1;
   }
-  if (c->i16_mode || c->gen || f->wcnt != 0 || c->issued != 0) {
-    fprintf(stderr, "write_rawfilter: the master is already fed int16, generated or float samples\n");
+  if (check_mode(f, c, INGEST_RAW, setup, who) != 0)
     return -1;
-  }
-  bool const cplx = f->in_type == COMPLEX;
-  c->raw_ring = ring_alloc((size_t)size);
-  if (!c->raw_ring)
+  struct raw_format const *rf = &raw_formats[format];
+  size_t const group = rf->group * (f->in_type == COMPLEX ? 2u : 1u);
+  if (wring_open(&c->ring, (size_t)size, group, f->impulse_length - 1, rf->zero) != 0)
     return -1;
-  c->raw_ring_size = (size_t)size;
-  if (format == FILTER_RAW_U8)
-    memset(c->raw_ring, 128, c->raw_ring_size);
-  else if (format == FILTER_RAW_U16) { /* offset binary: 0x8000 is 0 */
-    uint16_t *const w = c->raw_ring;
-    for (size_t o = 0; o < c->raw_ring_size / sizeof *w; o++)
-      w[o] = 0x8000;
-  } else if (format == FILTER_RAW_PACKED12) { /* eight offset-binary 2048s per three words (airspy-unpack.c:110-117) */
-    uint32_t const g[3] = {0x80080080u, 0x08008008u, 0x00800800u};
-    for (size_t o = 0; o < c->raw_ring_size; o += sizeof g)
-      memcpy((char *)c->raw_ring + o, g, sizeof g);
-  }
   size_t const span = (size_t)(ND - 2) * (size_t)f->ilen + (size_t)f->points;
-  if (cudaMalloc(&c->d_raw, raw_bytes(format, cplx, span)) != cudaSuccess) {
+  if (cudaMalloc(&c->d_raw, wring_bytes(&c->ring, span)) != cudaSuccess) {
     c->d_raw = NULL;
-    ring_free(c->raw_ring, c->raw_ring_size);
-    c->raw_ring = NULL;
+    ring_free(c->ring.base, c->ring.size);
+    c->ring.base = NULL;
     return kgf_fail("write_rawfilter: device buffer");
   }
-  c->raw_rp = c->raw_ring;
-  c->raw_wp = c->raw_rp + raw_bytes(format, cplx, (size_t)(f->impulse_length - 1));
   c->raw_fmt = format;
+  c->mode = INGEST_RAW;
   return 0;
 }
 
@@ -855,40 +900,27 @@ static int chg_span(struct master_ctx const *c, int stage, long long lo, long lo
   return stage == ND && cudaEventRecord(c->stg_ev, c->st) != cudaSuccess ? -1 : 0;
 }
 
-/* kgpu_unpack8's word format of a filter_raw_format it serves */
-static int kgpu_raw_format(int fmt) {
-  switch (fmt) {
-  case FILTER_RAW_U8: return KGPU_RAW_U8;
-  case FILTER_RAW_S8: return KGPU_RAW_S8;
-  case FILTER_RAW_S16: return KGPU_RAW_S16;
-  case FILTER_RAW_U16: return KGPU_RAW_U16;
-  case FILTER_RAW_F32: return KGPU_RAW_F32;
-  case FILTER_RAW_CF32: return KGPU_RAW_CF32;
-  case FILTER_RAW_CF32_CNRMF: return KGPU_RAW_CF32_CNRMF;
-  case FILTER_RAW_CF32_FSCALE: return KGPU_RAW_CF32_FSCALE;
-  default: return KGPU_RAW_SC16Q11;
-  }
-}
 /* raw bytes on the device (history samples, then nblocks blocks of L) -> the master's device samples at d_dst: floats for
- * the 8-bit, 16-bit and I/Q corrected formats, int16 for packed-12, which kgpu_forward then scales.  d_stats: NULL or nblocks
- * block statistics (not for I/Q correction, whose records replace them). */
+ * the 8-bit, 16-bit, float and I/Q corrected formats, int16 for packed-12, which kgpu_forward then scales.  d_stats: NULL
+ * or nblocks block statistics (not for I/Q correction, whose records replace them). */
 static int iq_apply(struct master_ctx const *c, void const *d_src, long long a0, long count, void *d_dst, cudaStream_t st);
 static int raw_unpack(struct filter_in const *f, struct master_ctx const *c, int stage, void const *d_src, long long a0,
                       long history, int nblocks, void *d_dst, void *d_stats, cudaStream_t st) {
   int const type = f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL;
-  if (c->iq_on) /* a0: the absolute index of the first sample (I/Q correction needs to know whose write it is) */
-    return iq_apply(c, d_src, a0, history + (long)nblocks * f->ilen, d_dst, st);
-  if (c->raw_fmt != FILTER_RAW_PACKED12) {
-    double scale;
-    int n;
-    if (chg_span(c, stage, a0, a0 + history + (long long)nblocks * f->ilen, &scale, &n) != 0)
+  long const count = history + (long)nblocks * f->ilen;
+  if (fed_row(c)->path == RAW_IQ) /* a0: the absolute index of the first sample (whose write it is) */
+    return iq_apply(c, d_src, a0, count, d_dst, st);
+  if (fed_row(c)->path == RAW_AIRSPY12) {
+    if (kgpu_unpack_airspy12(d_src, count, d_dst, NULL, st) != 0)
       return -1;
-    return kgpu_unpack8(d_src, kgpu_raw_format(c->raw_fmt), type, history, f->ilen, nblocks, scale, n ? c->d_chg : NULL, n, a0,
-                        d_dst, d_stats, st);
+    return d_stats ? kgpu_block_stats_i16(d_dst, type, history, f->ilen, nblocks, 0, 2047, d_stats, st) : 0;
   }
-  if (kgpu_unpack_airspy12(d_src, history + (long)nblocks * f->ilen, d_dst, NULL, st) != 0)
+  double scale;
+  int n;
+  if (chg_span(c, stage, a0, a0 + count, &scale, &n) != 0)
     return -1;
-  return d_stats ? kgpu_block_stats_i16(d_dst, type, history, f->ilen, nblocks, 0, 2047, d_stats, st) : 0;
+  return kgpu_unpack8(d_src, fed_row(c)->code, type, history, f->ilen, nblocks, scale, n ? c->d_chg : NULL, n, a0, d_dst,
+                      d_stats, st);
 }
 
 /* ---------------------------------------------------------------- I/Q correction ------------ */
@@ -897,12 +929,11 @@ static int raw_unpack(struct filter_in const *f, struct master_ctx const *c, int
  * flight: the writes of the analyzer's seeding window and those written but not yet launched both fit, so no entry is
  * overwritten while a launch or the seeding can still read it. */
 long filter_iq_table_writes(int L, int M, enum filtertype in_type, int format) {
-  if (!iq_format(format))
-    return -1;
-  long const bytes = filter_raw_ring_bytes(L, M, in_type, format);
+  struct raw_format const *rf = format_row(format);
+  long const bytes = rf && rf->path == RAW_IQ ? filter_raw_ring_bytes(L, M, in_type, format) : -1;
   if (bytes < 0)
     return -1;
-  return 2 * (raw_samples(format, true, (size_t)bytes) / FILTER_IQ_MIN_WRITE) + 2 * ND + 2;
+  return 2 * (bytes * 8 / (2 * rf->group) / FILTER_IQ_MIN_WRITE) + 2 * ND + 2;
 }
 
 /* the newest write among [lo, hi) whose first pair is at or before absolute pair a (lo if none) */
@@ -930,8 +961,8 @@ static int iq_apply(struct master_ctx const *c, void const *d_src, long long a0,
     w_lo = iq_find(c, old, c->iq_sent, a0 > 0 ? a0 : 0);
     w_hi = iq_find(c, old, c->iq_sent, a0 + count - 1);
   }
-  return kgpu_iq_apply(d_src, c->raw_fmt == FILTER_RAW_S8_IQCORR ? KGPU_IQ_S8 : KGPU_IQ_S16, a0, count, c->d_iqw, c->d_iqc,
-                       c->iq_cap, (long long)w_lo, (int)(w_hi - w_lo + 1), d_dst, st);
+  return kgpu_iq_apply(d_src, fed_row(c)->code, a0, count, c->d_iqw, c->d_iqc, c->iq_cap, (long long)w_lo,
+                       (int)(w_hi - w_lo + 1), d_dst, st);
 }
 
 /* the table entries, moments and records of the k blocks about to be issued (new pairs [issued L, (issued + k) L)),
@@ -948,10 +979,10 @@ static int iq_launch(struct filter_in const *f, struct master_ctx *c, int k) {
     w += n;
   }
   c->iq_sent = last + 1;
-  int const fmt = c->raw_fmt == FILTER_RAW_S8_IQCORR ? KGPU_IQ_S8 : KGPU_IQ_S16;
   unsigned long long const first = iq_find(c, old, c->iq_writes, a);
-  char const *d_new = (char const *)c->d_raw + raw_bytes(c->raw_fmt, true, (size_t)(f->impulse_length - 1));
-  if (kgpu_iq_moments(d_new, fmt, a, (long)(end - a), c->d_iqw, c->iq_cap, (long long)first, (int)(last - first + 1), c->st) != 0)
+  char const *d_new = (char const *)c->d_raw + wring_bytes(&c->ring, (size_t)(f->impulse_length - 1));
+  if (kgpu_iq_moments(d_new, fed_row(c)->code, a, (long)(end - a), c->d_iqw, c->iq_cap, (long long)first, (int)(last - first + 1),
+                      c->st) != 0)
     return -1;
   struct kgpu_iq_write const *lw = &c->h_iqw[last % cap];
   unsigned long long const done = lw->first + lw->n <= end ? last + 1 : last; /* writes complete at the launch's end */
@@ -968,7 +999,7 @@ static void fold_one(struct filter_in const *f, struct master_ctx *c) {
   struct kgpu_block_stats const *s = &c->h_bstats[c->folded % ND];
   c->acc.blocks++;
   c->acc.samples += (uint64_t)f->ilen;
-  if (float_format(c->raw_fmt))
+  if (fed_row(c)->stats == STATS_FLOAT)
     c->acc.fenergy += s->fenergy;
   else
     c->acc.energy += s->energy;
@@ -1018,14 +1049,17 @@ static int sring_seed(struct filter_in *f, struct master_ctx *c) {
     c->d_sring = NULL;
     return kgf_fail("filter_spectrum_setup: device ring");
   }
-  long const M1 = f->impulse_length - 1;
+  long const M1 = f->impulse_length - 1, n = c->sring_cap;
   c->sring_pos = (long)((M1 + (unsigned long long)f->ilen * c->issued) % (unsigned long long)c->sring_cap);
-  if (c->gen) { /* the host ring holds nothing: generate the last sring_cap samples again */
-    long const n = c->sring_cap, dst = c->sring_pos, first = n - dst;
-    long long const a0 = (long long)f->ilen * (long long)c->issued - n;
+  long const dst = c->sring_pos, first = n - dst;                 /* (sring_pos - n) modulo sring_cap, n being sring_cap */
+  long long const a0 = (long long)f->ilen * (long long)c->issued - n; /* the absolute index of the first seeded sample */
+  struct word_ring const *r = &c->ring;
+  int rc = 0;
+  switch (c->mode) {
+  case INGEST_GEN: { /* the host ring holds nothing: generate the last sring_cap samples again */
     double scale;
     int nc;
-    int rc = chg_span(c, ND, a0, a0 + n, &scale, &nc);
+    rc = chg_span(c, ND, a0, a0 + n, &scale, &nc);
     struct kgpu_scale_change const *chg = nc ? c->d_chg : NULL;
     rc = rc ? rc
             : kgpu_siggen_generate(c->gen, a0, first, scale, chg, nc, (char *)c->d_sring + (size_t)dst * esz, NULL, 0, 0, first,
@@ -1036,46 +1070,34 @@ static int sring_seed(struct filter_in *f, struct master_ctx *c) {
       rc = -1;
     return rc ? kgf_fail("filter_spectrum_setup: generating the device ring") : 0;
   }
-  if (c->raw_fmt) { /* the host ring holds raw bytes: send the last sring_cap samples' bytes over and unpack them there */
-    bool const cplx = f->in_type == COMPLEX;
-    long const n = c->sring_cap, cap = raw_samples(c->raw_fmt, cplx, c->raw_ring_size);
-    long const end = raw_samples(c->raw_fmt, cplx, (size_t)(c->raw_rp - (char *)c->raw_ring)) + M1;
+  case INGEST_RAW: { /* the host ring holds raw bytes: send the last sring_cap samples' bytes over and unpack them there */
+    long const cap = wring_samples(r, r->size), end = wring_samples(r, (size_t)(r->rp - r->base)) + M1;
     long const src = ((end - n) % cap + cap) % cap;
-    long const dst = c->sring_pos; /* (sring_pos - n) modulo sring_cap, n being sring_cap */
-    long const first = n - dst;
     void *tmp = NULL;
-    int rc = cudaMalloc(&tmp, raw_bytes(c->raw_fmt, cplx, (size_t)n)) == cudaSuccess ? 0 : -1;
-    rc = rc ? rc
-            : window_h2d(tmp, (char *)c->raw_ring + raw_bytes(c->raw_fmt, cplx, (size_t)src), raw_bytes(c->raw_fmt, cplx, (size_t)n),
-                         c->raw_ring, c->raw_ring_size, c->st);
-    long long const a0 = (long long)f->ilen * (long long)c->issued - n; /* the absolute index of the first seeded sample */
+    rc = cudaMalloc(&tmp, wring_bytes(r, (size_t)n)) == cudaSuccess ? 0 : -1;
+    rc = rc ? rc : window_h2d(tmp, r->base + wring_bytes(r, (size_t)src), wring_bytes(r, (size_t)n), r->base, r->size, c->st);
     rc = rc ? rc : raw_unpack(f, c, ND, tmp, a0, first, 0, (char *)c->d_sring + (size_t)dst * esz, NULL, c->st);
     if (rc == 0 && dst > 0)
-      rc = raw_unpack(f, c, ND, (char *)tmp + raw_bytes(c->raw_fmt, cplx, (size_t)first), a0 + first, dst, 0, c->d_sring, NULL,
-                      c->st);
+      rc = raw_unpack(f, c, ND, (char *)tmp + wring_bytes(r, (size_t)first), a0 + first, dst, 0, c->d_sring, NULL, c->st);
     if (cudaStreamSynchronize(c->st) != cudaSuccess)
       rc = -1;
     cudaFree(tmp);
     return rc ? kgf_fail("filter_spectrum_setup: seeding the device ring from the raw ring") : 0;
   }
-  char const *base;
-  long src_cap, src_end;
-  if (c->sring_i16) {
-    base = c->i16_ring;
-    src_cap = (long)(c->i16_ring_size / c->i16_esz);
-    src_end = (long)((c->i16_rp - (char *)c->i16_ring) / (long)c->i16_esz) + M1;
-  } else {
-    base = f->input_buffer;
-    src_cap = c->sring_cap;
-    src_end = (long)(((char *)(f->in_type == COMPLEX ? (void *)f->input_read_pointer.c : (void *)f->input_read_pointer.r) -
-                      (char *)f->input_buffer) / (long)c->esz) + M1;
+  default: { /* int16 words or floats: the samples as they are (the int16 ring holds at least as many as the float ring) */
+    bool const words = c->mode == INGEST_INT16;
+    char const *const base = words ? r->base : (char const *)f->input_buffer;
+    char const *const rp =
+        words ? r->rp : f->in_type == COMPLEX ? (char const *)f->input_read_pointer.c : (char const *)f->input_read_pointer.r;
+    long const src_cap = words ? wring_samples(r, r->size) : c->sring_cap;
+    long const src_end = (long)((size_t)(rp - base) / esz) + M1;
+    long const src = ((src_end - n) % src_cap + src_cap) % src_cap;
+    if (sring_copy(c, base, src_cap, src, dst, n, esz, cudaMemcpyHostToDevice) != 0 ||
+        cudaStreamSynchronize(c->st) != cudaSuccess)
+      return kgf_fail("filter_spectrum_setup: seeding the device ring");
+    return 0;
   }
-  long const n = c->sring_cap; /* the i16 ring holds at least as many samples as the float ring */
-  long const src = ((src_end - n) % src_cap + src_cap) % src_cap;
-  long const dst = ((c->sring_pos - n) % c->sring_cap + c->sring_cap) % c->sring_cap;
-  if (sring_copy(c, base, src_cap, src, dst, n, esz, cudaMemcpyHostToDevice) != 0 || cudaStreamSynchronize(c->st) != cudaSuccess)
-    return kgf_fail("filter_spectrum_setup: seeding the device ring");
-  return 0;
+  }
 }
 /* the k*L new samples of the launch just issued from d_win[slot] (after its M-1 history samples), on the pipeline stream */
 static int sring_append(struct filter_in *f, struct master_ctx *c, int k) {
@@ -1095,24 +1117,82 @@ static int sring_append(struct filter_in *f, struct master_ctx *c, int k) {
   return 0;
 }
 
+/* The forward pass's input for the k blocks about to be issued from ring slot `slot`, in stages on the pipeline stream:
+ * H2D of the window (floats or int16 words into d_win[slot], raw words into d_raw), I/Q correction's launch, generation,
+ * unpack, int16 statistics into bst (NULL: none), and the conversion of an int16 window that holds more than one scale. */
+static int launch_input(struct filter_in *f, struct master_ctx *c, int slot, int k, struct kgpu_block_stats *bst,
+                        void const **fwd_in, int *fmt, float *scale) {
+  int const type = f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL;
+  long const M1 = f->impulse_length - 1;
+  size_t const span = (size_t)(k - 1) * (size_t)f->ilen + (size_t)f->points; /* samples covered by k overlapping windows */
+  long long const a0 = (long long)f->ilen * (long long)c->issued - M1;     /* the window's first sample */
+  void *const win = c->d_win[slot];
+  *fwd_in = win;
+  *fmt = ingest_i16(c) ? KGPU_FMT_I16 : KGPU_FMT_F32; /* packed-12 goes on as int16 with the drivers' float scale */
+  *scale = 1.0f;
+  if (c->chg)
+    chg_prune(f, c);
+  if (c->mode == INGEST_NONE) { /* floats */
+    void **const rp = f->in_type == COMPLEX ? (void **)&f->input_read_pointer.c : (void **)&f->input_read_pointer.r;
+    char const *const src = *rp;
+    *rp = (char *)*rp + c->esz * (size_t)f->ilen * (size_t)k;
+    kgf_ring_wrap(rp, f->input_buffer, f->input_buffer_size);
+    if (window_h2d(win, src, c->esz * span, f->input_buffer, f->input_buffer_size, c->st) != 0)
+      return kgf_fail("execute_filter_input: H2D of the window");
+    return 0;
+  }
+  double s;
+  int n;
+  if (c->mode == INGEST_GEN) { /* generated on the device: nothing crosses PCIe */
+    if (chg_span(c, slot, a0, a0 + (long long)span, &s, &n) != 0 ||
+        kgpu_siggen_generate(c->gen, a0, (long)span, s, n ? c->d_chg : NULL, n, win,
+                             c->gen_stats_on ? c->d_gen_energy + slot : NULL, k, f->ilen, M1, c->st) != 0)
+      return kgf_fail("execute_filter_input: kgpu_siggen_generate");
+    return 0;
+  }
+  bool const raw = c->mode == INGEST_RAW;
+  char const *const src = wring_advance(&c->ring, (size_t)f->ilen * (size_t)k);
+  if (window_h2d(raw ? c->d_raw : win, src, wring_bytes(&c->ring, span), c->ring.base, c->ring.size, c->st) != 0)
+    return kgf_fail("execute_filter_input: H2D of the window");
+  if (raw && fed_row(c)->path == RAW_IQ && iq_launch(f, c, k) != 0)
+    return kgf_fail("execute_filter_input: I/Q correction");
+  if (raw && raw_unpack(f, c, slot, c->d_raw, a0, M1, k, win, bst, c->st) != 0)
+    return kgf_fail("execute_filter_input: raw unpack");
+  if (!raw && bst && kgpu_block_stats_i16(win, type, M1, f->ilen, k, c->i16_derand, 32767, bst, c->st) != 0)
+    return kgf_fail("execute_filter_input: kgpu_block_stats_i16");
+  if (*fmt != KGPU_FMT_I16)
+    return 0;
+  if (chg_span(c, slot, a0, a0 + (long long)span, &s, &n) != 0)
+    return kgf_fail("execute_filter_input: scale changes");
+  if (n == 0) { /* one scale: fwd_cols converts; more: floats with each sample's own scale */
+    *scale = (float)s;
+    return 0;
+  }
+  if (kgpu_scale_i16(win, type, (long)span, a0, s, c->d_chg, n, c->i16_derand, c->d_conv, c->st) != 0)
+    return kgf_fail("execute_filter_input: kgpu_scale_i16");
+  *fwd_in = c->d_conv;
+  *fmt = KGPU_FMT_F32;
+  return 0;
+}
+
 /* k consecutive blocks (jobs next_jobnum .. +k-1, ring slots without wrap) as one device launch sequence.
  * filter.c:558-651 (+ run_fft :485-555) */
 static int execute_filter_input_n(struct filter_in *const f, int const k) {
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  int const N = f->points;
   pthread_mutex_lock(&c->mu);
   unsigned const jobnum = f->next_jobnum;
   int const slot = (int)(jobnum % ND);
   /* the ring slots' previous occupants (job - ND) must have drained */
   for (int j = 0; j < k; j++)
     cudaEventSynchronize(c->done[slot + j]);
-  if (c->stats_on && !c->i16_mode && !c->raw_fmt)
-    c->stats_on = false; /* fed floats: the driver counts in its own loop */
+  if (c->stats_on && !ingest_counted(c))
+    c->stats_on = false; /* fed floats (the driver counts in its own loop), generated or I/Q corrected */
   while (c->stats_on && c->folded + ND < c->issued + (unsigned long long)k)
     fold_one(f, c); /* the statistics of the slots about to be reused */
   while (c->gen_stats_on && c->gen_folded + ND < c->issued + (unsigned long long)k)
     gen_fold_one(f, c);
-  while (c->iq_on && c->iq_checked + ND < c->issued + (unsigned long long)k)
+  bool const iq = fed_row(c)->path == RAW_IQ;
+  while (iq && c->iq_checked + ND < c->issued + (unsigned long long)k)
     c->iq_avail = c->iq_job_done[c->iq_checked++ % ND]; /* the records of the slots about to be reused have arrived */
   struct kgpu_block_stats *const bst = c->stats_on ? c->d_bstats + slot : NULL;
   if (c->timed[slot]) { /* forward+channels device time of that older job, for main.c:154-164 */
@@ -1129,86 +1209,15 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
     }
   }
   sync_notches(f, c);
-  int rc = 0;
   cudaEventRecord(c->t0[slot], c->st);
-  void const *src;
-  int fmt = KGPU_FMT_F32;
-  float scale = 1.0f;
-  size_t bytes;
-  size_t const span = (size_t)(k - 1) * (size_t)f->ilen + (size_t)N; /* samples covered by k overlapping windows */
-  if (c->i16_mode) {
-    src = c->i16_rp;
-    bytes = c->i16_esz * span;
-    fmt = KGPU_FMT_I16;
-    c->i16_rp += c->i16_esz * (size_t)f->ilen * (size_t)k;
-    if (c->i16_rp >= (char *)c->i16_ring + c->i16_ring_size)
-      c->i16_rp -= c->i16_ring_size;
-  } else if (c->raw_fmt) { /* packed-12 goes on as int16 with the drivers' float scale; 8- and 16-bit as floats */
-    bool const cplx = f->in_type == COMPLEX;
-    src = c->raw_rp;
-    bytes = raw_bytes(c->raw_fmt, cplx, span);
-    fmt = c->raw_fmt == FILTER_RAW_PACKED12 ? KGPU_FMT_I16 : KGPU_FMT_F32;
-    c->raw_rp += raw_bytes(c->raw_fmt, cplx, (size_t)f->ilen * (size_t)k);
-    if (c->raw_rp >= (char *)c->raw_ring + c->raw_ring_size)
-      c->raw_rp -= c->raw_ring_size;
-  } else if (c->gen) { /* generated on the device below: nothing crosses PCIe */
-    src = NULL;
-    bytes = 0;
-  } else if (f->in_type == COMPLEX) {
-    src = f->input_read_pointer.c;
-    bytes = sizeof(float complex) * span;
-    f->input_read_pointer.c += (size_t)f->ilen * (size_t)k;
-    kgf_ring_wrap((void **)&f->input_read_pointer.c, f->input_buffer, f->input_buffer_size);
-  } else {
-    src = f->input_read_pointer.r;
-    bytes = sizeof(float) * span;
-    f->input_read_pointer.r += (size_t)f->ilen * (size_t)k;
-    kgf_ring_wrap((void **)&f->input_read_pointer.r, f->input_buffer, f->input_buffer_size);
-  }
   float complex *spec = c->d_spec + (size_t)slot * (size_t)c->spec_stride;
   for (int j = 0; j < k; j++) /* nothing of the previous occupants may be served for these jobs */
     for (int i = 0; i < c->nslots; i++)
       c->snap[slot + j][i].ok = false;
-  void const *const ring = c->i16_mode ? c->i16_ring : c->raw_fmt ? c->raw_ring : f->input_buffer;
-  size_t const ring_size = c->i16_mode ? c->i16_ring_size : c->raw_fmt ? c->raw_ring_size : f->input_buffer_size;
-  if (!c->gen && window_h2d(c->raw_fmt ? c->d_raw : c->d_win[slot], src, bytes, ring, ring_size, c->st) != 0)
-    rc = kgf_fail("execute_filter_input: H2D of the window");
-  long const M1 = f->impulse_length - 1;
-  long long const a0 = (long long)f->ilen * (long long)c->issued - M1; /* the window's first sample */
-  if (c->chg)
-    chg_prune(f, c);
-  if (rc == 0 && c->iq_on && iq_launch(f, c, k) != 0)
-    rc = kgf_fail("execute_filter_input: I/Q correction");
-  if (rc == 0 && c->gen) {
-    double s;
-    int n;
-    if (chg_span(c, slot, a0, a0 + (long long)span, &s, &n) != 0 ||
-        kgpu_siggen_generate(c->gen, a0, (long)span, s, n ? c->d_chg : NULL, n, c->d_win[slot],
-                             c->gen_stats_on ? c->d_gen_energy + slot : NULL, k, f->ilen, M1, c->st) != 0)
-      rc = kgf_fail("execute_filter_input: kgpu_siggen_generate");
-  }
-  if (rc == 0 && c->raw_fmt && raw_unpack(f, c, slot, c->d_raw, a0, M1, k, c->d_win[slot], bst, c->st) != 0)
-    rc = kgf_fail("execute_filter_input: raw unpack");
-  if (rc == 0 && c->i16_mode && bst &&
-      kgpu_block_stats_i16(c->d_win[slot], f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL, M1, f->ilen, k, c->i16_derand, 32767,
-                           bst, c->st) != 0)
-    rc = kgf_fail("execute_filter_input: kgpu_block_stats_i16");
-  void const *fwd_in = c->d_win[slot];
-  if (rc == 0 && fmt == KGPU_FMT_I16) { /* one scale: fwd_cols converts; more: floats with each sample's own scale */
-    double s;
-    int n;
-    if (chg_span(c, slot, a0, a0 + (long long)span, &s, &n) != 0)
-      rc = kgf_fail("execute_filter_input: scale changes");
-    else if (n == 0)
-      scale = (float)s;
-    else if (kgpu_scale_i16(c->d_win[slot], f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL, (long)span, a0, s, c->d_chg, n,
-                            c->i16_mode && c->i16_derand, c->d_conv, c->st) != 0)
-      rc = kgf_fail("execute_filter_input: kgpu_scale_i16");
-    else {
-      fwd_in = c->d_conv;
-      fmt = KGPU_FMT_F32;
-    }
-  }
+  void const *fwd_in;
+  int fmt;
+  float scale;
+  int rc = launch_input(f, c, slot, k, bst, &fwd_in, &fmt, &scale);
   if (rc == 0 && kgpu_forward(c->km, fwd_in, fmt, scale, fmt == KGPU_FMT_I16 && c->i16_derand, k, spec, NULL, c->st) != 0)
     rc = kgf_fail("execute_filter_input: kgpu_forward");
   if (rc == 0 && c->d_sring)
@@ -1274,7 +1283,7 @@ static int execute_filter_input_n(struct filter_in *const f, int const k) {
       cudaMemcpyAsync(c->h_gen_energy + slot, c->d_gen_energy + slot, sizeof(double) * (size_t)k, cudaMemcpyDeviceToHost,
                       c->st_d2h) != cudaSuccess)
     rc = kgf_fail("execute_filter_input: D2H of the generated energies");
-  if (c->iq_on) {
+  if (iq) {
     unsigned long long const from = c->iq_rec_from, to = c->iq_scanned;
     for (unsigned long long w = from; rc == 0 && w < to;) { /* the records of the writes this launch completed */
       unsigned long long const n = to - w < (unsigned long long)c->iq_cap - w % (unsigned long long)c->iq_cap
@@ -1744,7 +1753,7 @@ int filter_spectrum_poll(struct filter_out *slave, int shift, int fft_avg, doubl
   if (rc == 0 && c->sring_i16 && chg_span(c, ND, (long long)end - c->sring_cap, (long long)end, &scale, &n) != 0)
     rc = kgf_fail("filter_spectrum_poll: scale changes");
   if (rc == 0 && kgpu_spectrum_run(sp->ks, c->d_sring, c->sring_cap, c->sring_pos, c->sring_i16 ? KGPU_FMT_I16 : KGPU_FMT_F32,
-                                   (float)scale, n ? c->d_chg : NULL, n, (long long)end, c->i16_mode && c->i16_derand, shift,
+                                   (float)scale, n ? c->d_chg : NULL, n, (long long)end, c->mode == INGEST_INT16 && c->i16_derand, shift,
                                    fft_avg, overlap, sp->d_bins, c->st) != 0)
     rc = kgf_fail("filter_spectrum_poll: kgpu_spectrum_run");
   if (rc == 0 && (cudaMemcpyAsync(sp->h_bins, sp->d_bins, sizeof(float) * (size_t)sp->bin_count, cudaMemcpyDeviceToHost,
@@ -1936,33 +1945,24 @@ int delete_filter_input(struct filter_in *master) { /* filter.c:930-942 */
 }
 
 /* ---------------------------------------------------------------- write_*filter ------------- */
-/* a master fed raw words, or generating its own, takes no floats */
-static bool raw_fed(struct filter_in const *f) {
-  return f->fwd_plan && (((struct master_ctx const *)f->fwd_plan)->raw_fmt || ((struct master_ctx const *)f->fwd_plan)->gen);
-}
-int write_cfilter(struct filter_in *f, float complex const *buffer, int size) { /* filter.c:1093-1113 */
-  if (f == NULL || raw_fed(f))
+/* filter.c:1093-1134: n floats or float pairs of esz bytes to the float ring at its write pointer *wp */
+static int write_floats(struct filter_in *f, void **wp, void const *buffer, int size, size_t esz, char const *who) {
+  if (f->fwd_plan == NULL || check_mode(f, (struct master_ctx *)f->fwd_plan, INGEST_FLOAT, false, who) != 0)
     return -1;
-  if ((f->wcnt + size) * sizeof *buffer >= f->input_buffer_size)
+  if ((f->wcnt + size) * esz >= f->input_buffer_size)
     return -1;
   if (buffer != NULL)
-    memcpy(f->input_write_pointer.c, buffer, (size_t)size * sizeof *buffer);
-  f->input_write_pointer.c += size;
-  kgf_ring_wrap((void **)&f->input_write_pointer.c, f->input_buffer, f->input_buffer_size);
+    memcpy(*wp, buffer, (size_t)size * esz);
+  *wp = (char *)*wp + (ptrdiff_t)size * (ptrdiff_t)esz;
+  kgf_ring_wrap(wp, f->input_buffer, f->input_buffer_size);
   f->wcnt += size;
   return fire_ready_blocks(f);
 }
-int write_rfilter(struct filter_in *f, float const *buffer, int size) { /* filter.c:1114-1134 */
-  if (f == NULL || raw_fed(f))
-    return -1;
-  if ((f->wcnt + size) * sizeof *buffer >= f->input_buffer_size)
-    return -1;
-  if (buffer != NULL)
-    memcpy(f->input_write_pointer.r, buffer, (size_t)size * sizeof *buffer);
-  f->input_write_pointer.r += size;
-  kgf_ring_wrap((void **)&f->input_write_pointer.r, f->input_buffer, f->input_buffer_size);
-  f->wcnt += size;
-  return fire_ready_blocks(f);
+int write_cfilter(struct filter_in *f, float complex const *buffer, int size) {
+  return f ? write_floats(f, (void **)&f->input_write_pointer.c, buffer, size, sizeof *buffer, "write_cfilter") : -1;
+}
+int write_rfilter(struct filter_in *f, float const *buffer, int size) {
+  return f ? write_floats(f, (void **)&f->input_write_pointer.r, buffer, size, sizeof *buffer, "write_rfilter") : -1;
 }
 /* EXTENSION: raw ADC words straight to the device; conversion (rx888.c:753-767) happens in fwd_cols.
  * samples == NULL: the caller already wrote them through filter_i16_write_pointer() (the zero-copy driver path). */
@@ -1970,9 +1970,9 @@ int write_i16filter(struct filter_in *f, int16_t const *samples, int n, float sc
   if (f == NULL || f->fwd_plan == NULL || n < 0)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (!c->i16_mode && filter_i16_write_pointer(f) == NULL)
+  if (c->mode != INGEST_INT16 && filter_i16_write_pointer(f) == NULL)
     return -1;
-  if (((size_t)f->wcnt + (size_t)n) * c->i16_esz >= c->i16_ring_size)
+  if (wring_bytes(&c->ring, (size_t)f->wcnt + (size_t)n) >= c->ring.size)
     return -1;
   pthread_mutex_lock(&c->mu);
   int const rc = chg_note(f, c, scale, "write_i16filter");
@@ -1981,57 +1981,54 @@ int write_i16filter(struct filter_in *f, int16_t const *samples, int n, float sc
     return -1;
   c->i16_derand = derandomize;
   if (samples != NULL)
-    memcpy(c->i16_wp, samples, (size_t)n * c->i16_esz);
-  c->i16_wp += (size_t)n * c->i16_esz;
-  if (c->i16_wp >= (char *)c->i16_ring + c->i16_ring_size)
-    c->i16_wp -= c->i16_ring_size;
+    memcpy(c->ring.wp, samples, wring_bytes(&c->ring, (size_t)n));
+  wring_push(&c->ring, (size_t)n);
   f->wcnt += n;
   return fire_ready_blocks(f);
 }
 /* where a driver may deposit the next raw samples itself (mirrored, pinned ring: up to one block contiguous),
  * e.g. as the libusb transfer buffer of rx888.c:797-826; publish with write_i16filter(f, NULL, n, ...) */
 int16_t *filter_i16_write_pointer(struct filter_in *f) {
-  if (f == NULL || f->fwd_plan == NULL || raw_fed(f))
+  if (f == NULL || f->fwd_plan == NULL)
     return NULL;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (!c->i16_mode) {
-    c->i16_esz = (f->in_type == COMPLEX) ? 2 * sizeof(int16_t) : sizeof(int16_t);
-    c->i16_ring_size = page_round((size_t)ND * (size_t)f->points * c->i16_esz);
-    c->i16_ring = ring_alloc(c->i16_ring_size);
-    if (!c->i16_ring)
+  if (c->mode != INGEST_INT16) {
+    static uint32_t const zero[3];
+    size_t const group = 8 * ((f->in_type == COMPLEX) ? 2 * sizeof(int16_t) : sizeof(int16_t));
+    if (check_mode(f, c, INGEST_INT16, false, "filter_i16_write_pointer") != 0 ||
+        wring_open(&c->ring, page_round((size_t)ND * (size_t)f->points * group / 8), group, f->impulse_length - 1, zero) != 0)
       return NULL;
-    c->i16_rp = c->i16_ring;
-    c->i16_wp = c->i16_rp + c->i16_esz * (size_t)(f->impulse_length - 1);
-    c->i16_mode = true;
+    c->mode = INGEST_INT16;
   }
-  return (int16_t *)c->i16_wp;
+  return (int16_t *)c->ring.wp;
 }
 
-/* the checks, table entry and scale of a write of n samples in `format` about to be stored at c->raw_wp (starting the
- * raw ring at a master's first write); 0, or -1 with nothing stored */
+/* the checks, table entry and scale of a write of n samples in `format` about to be stored at the ring's write pointer
+ * (starting the raw ring at a master's first write); 0, or -1 with nothing stored */
 static int raw_admit(struct filter_in *f, struct master_ctx *c, int n, int format, double scale, char const *who) {
-  if (format != FILTER_RAW_PACKED12 && format != FILTER_RAW_U8 && format != FILTER_RAW_S8 && format != FILTER_RAW_S16 &&
-      format != FILTER_RAW_U16 && format != FILTER_RAW_SC16Q11 && !iq_format(format) && !float_format(format)) {
+  struct raw_format const *rf = format_row(format);
+  if (rf == NULL) {
     fprintf(stderr, "%s: unknown format %d\n", who, format);
     return -1;
   }
-  if (iq_format(format) && !c->iq_on) {
+  bool const iq = rf->path == RAW_IQ;
+  if (iq && c->iq_cap == 0) {
     fprintf(stderr, "%s: format %d needs filter_iq_correction_setup first\n", who, format);
     return -1;
   }
-  if (!c->raw_fmt && raw_start(f, c, format) != 0)
+  if (c->mode != INGEST_RAW && raw_start(f, c, format, false, who) != 0)
     return -1;
   if (format != c->raw_fmt) {
     fprintf(stderr, "%s: format %d on a master fed format %d\n", who, format, c->raw_fmt);
     return -1;
   }
-  if (format == FILTER_RAW_PACKED12 && n % 8 != 0) {
+  if (rf->group % 8 != 0 && n % 8 != 0) {
     fprintf(stderr, "%s: %d packed 12-bit samples: not a multiple of 8\n", who, n);
     return -1;
   }
-  if (raw_bytes(format, f->in_type == COMPLEX, (size_t)f->wcnt + (size_t)n) >= c->raw_ring_size)
+  if (wring_bytes(&c->ring, (size_t)f->wcnt + (size_t)n) >= c->ring.size)
     return -1;
-  if (c->iq_on) { /* one transfer: its table entry */
+  if (iq) { /* one transfer: its table entry */
     if (n < FILTER_IQ_MIN_WRITE) {
       fprintf(stderr, "%s: %d I/Q pairs: writes with I/Q correction take at least %d\n", who, n, FILTER_IQ_MIN_WRITE);
       return -1;
@@ -2051,11 +2048,9 @@ static int raw_admit(struct filter_in *f, struct master_ctx *c, int n, int forma
   pthread_mutex_unlock(&c->mu);
   return rc;
 }
-/* publish the n samples just stored at c->raw_wp, and fire the blocks they complete */
+/* publish the n samples just stored at the ring's write pointer, and fire the blocks they complete */
 static int raw_commit(struct filter_in *f, struct master_ctx *c, int n) {
-  c->raw_wp += raw_bytes(c->raw_fmt, f->in_type == COMPLEX, (size_t)n);
-  if (c->raw_wp >= (char *)c->raw_ring + c->raw_ring_size)
-    c->raw_wp -= c->raw_ring_size;
+  wring_push(&c->ring, (size_t)n);
   f->wcnt += n;
   return fire_ready_blocks(f);
 }
@@ -2070,8 +2065,7 @@ int write_rawfilter(struct filter_in *f, void const *samples, int n, int format,
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
   if (raw_admit(f, c, n, format, scale, "write_rawfilter") != 0)
     return -1;
-  memcpy(c->raw_wp, samples, raw_bytes(format, f->in_type == COMPLEX, (size_t)n)); /* the mirror view keeps a write across
-                                                                                      the end contiguous */
+  memcpy(c->ring.wp, samples, wring_bytes(&c->ring, (size_t)n)); /* the mirror view keeps a write across the end contiguous */
   return raw_commit(f, c, n);
 }
 
@@ -2087,7 +2081,7 @@ int write_rawfilter_planar(struct filter_in *f, int16_t const *i, int16_t const 
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
   if (raw_admit(f, c, n, FILTER_RAW_S16, scale, "write_rawfilter_planar") != 0)
     return -1;
-  int16_t *restrict const w = (int16_t *)c->raw_wp; /* the mirror view keeps a write across the end contiguous */
+  int16_t *restrict const w = (int16_t *)c->ring.wp; /* the mirror view keeps a write across the end contiguous */
   for (int k = 0; k < n; k++) {
     w[2 * k] = i[k];
     w[2 * k + 1] = q[k];
@@ -2102,12 +2096,10 @@ int filter_ingest_stats(struct filter_in *f, struct filter_ingest_stats *stats) 
   if (f == NULL || f->fwd_plan == NULL || stats == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (c->iq_on || c->gen)
-    return -1; /* I/Q corrected: filter_iq_records replaces the block statistics; generated: filter_siggen_stats */
   int rc = 0;
   pthread_mutex_lock(&c->mu);
-  if (!c->i16_mode && !c->raw_fmt && (c->issued > 0 || f->wcnt > 0))
-    rc = -1; /* fed floats */
+  if (ingest_of(f, c) != INGEST_NONE && !ingest_counted(c))
+    rc = -1; /* floats: the driver counts them; generated: filter_siggen_stats; I/Q corrected: filter_iq_records */
   else if (!c->stats_on) {
     if (c->d_bstats == NULL &&
         (cudaMalloc((void **)&c->d_bstats, sizeof *c->d_bstats * ND) != cudaSuccess ||
@@ -2136,22 +2128,13 @@ int filter_ingest_stats(struct filter_in *f, struct filter_ingest_stats *stats) 
 /* EXTENSION: HackRF's and FUNcube's DC and I/Q correction on the device (see include/ka9q_gpu_filter.h): the raw ring,
  * the table of writes and the initial coefficient set, before the first write. */
 int filter_iq_correction_setup(struct filter_in *f, int format, struct filter_iq_params const *p) {
-  if (f == NULL || f->fwd_plan == NULL || p == NULL || !iq_format(format))
+  struct raw_format const *rf = format_row(format);
+  if (f == NULL || f->fwd_plan == NULL || p == NULL || rf == NULL || rf->path != RAW_IQ)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (c->raw_fmt || c->iq_on || c->gen) {
-    fprintf(stderr, "filter_iq_correction_setup: the master is already fed raw words or generated\n");
+  if (raw_start(f, c, format, true, "filter_iq_correction_setup") != 0)
     return -1;
-  }
-  long const cap = filter_iq_table_writes(f->ilen, f->impulse_length, f->in_type, format);
-  if (cap < 0) {
-    fprintf(stderr, "filter_iq_correction_setup(L=%d M=%d): I/Q correction needs a COMPLEX master\n", f->ilen, f->impulse_length);
-    return -1;
-  }
-  if (raw_start(f, c, format) != 0)
-    return -1;
-  c->iq_cap = (int)cap;
-  size_t const nw = (size_t)cap;
+  size_t const nw = (size_t)filter_iq_table_writes(f->ilen, f->impulse_length, f->in_type, format);
   bool ok = cudaHostAlloc((void **)&c->h_iqw, sizeof *c->h_iqw * nw, cudaHostAllocPortable) == cudaSuccess;
   ok = ok && cudaMalloc((void **)&c->d_iqw, sizeof *c->d_iqw * nw) == cudaSuccess;
   ok = ok && cudaMalloc((void **)&c->d_iqc, sizeof *c->d_iqc * nw) == cudaSuccess;
@@ -2160,11 +2143,11 @@ int filter_iq_correction_setup(struct filter_in *f, int format, struct filter_iq
   struct kgpu_iq_state const init = {p->dc_i, p->dc_q, p->sinphi, p->imbalance, p->gain_i, p->gain_q, p->secphi, p->tanphi};
   ok = ok && cudaMemcpy(c->d_iqc, &init, sizeof init, cudaMemcpyHostToDevice) == cudaSuccess; /* write 0's coefficients */
   if (!ok)
-    return kgf_fail("filter_iq_correction_setup: table buffers"); /* freed with the master */
+    return kgf_fail("filter_iq_correction_setup: table buffers"); /* freed with the master, whose writes are refused */
+  c->iq_cap = (int)nw;
   c->iq_par.kind = p->gp_rate != 0 ? 1 : 2;
   c->iq_par.dc_alpha = p->dc_alpha;
   c->iq_par.gp = p->gp_rate != 0 ? p->gp_rate : p->gp_alpha;
-  c->iq_on = true;
   return 0;
 }
 
@@ -2175,7 +2158,7 @@ int filter_iq_records(struct filter_in *f, struct filter_iq_record *recs, int ma
   if (f == NULL || f->fwd_plan == NULL || (recs == NULL && max > 0))
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (!c->iq_on)
+  if (c->iq_cap == 0)
     return -1;
   pthread_mutex_lock(&c->mu);
   while (c->iq_checked < c->issued && cudaEventQuery(c->done[c->iq_checked % ND]) == cudaSuccess)
@@ -2215,10 +2198,8 @@ int filter_siggen_setup(struct filter_in *f, struct filter_siggen_params const *
   if (f == NULL || f->fwd_plan == NULL || p == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (c->gen || c->raw_fmt || c->i16_mode || f->wcnt != 0 || c->issued != 0) {
-    fprintf(stderr, "filter_siggen_setup: the master is already fed or generated\n");
+  if (check_mode(f, c, INGEST_GEN, true, "filter_siggen_setup") != 0)
     return -1;
-  }
   struct kgpu_siggen_params const kp = {p->freq, p->rate, p->amplitude, p->noise, p->seed};
   kgpu_siggen *g = kgpu_siggen_create(f->in_type == COMPLEX ? KGPU_COMPLEX : KGPU_REAL, &kp);
   if (!g) {
@@ -2232,6 +2213,7 @@ int filter_siggen_setup(struct filter_in *f, struct filter_siggen_params const *
   }
   pthread_mutex_lock(&c->mu);
   c->gen = g;
+  c->mode = INGEST_GEN;
   pthread_mutex_unlock(&c->mu);
   return 0;
 }
@@ -2242,8 +2224,8 @@ int write_genfilter(struct filter_in *f, int n, double scale) {
   if (f == NULL || f->fwd_plan == NULL || n < 0)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (!c->gen)
-    return -1;
+  if (check_mode(f, c, INGEST_GEN, false, "write_genfilter") != 0 || c->mode != INGEST_GEN)
+    return -1; /* only filter_siggen_setup starts a generated master */
   if (((size_t)f->wcnt + (size_t)n) * c->esz >= f->input_buffer_size)
     return -1;
   pthread_mutex_lock(&c->mu);
@@ -2261,7 +2243,7 @@ int filter_siggen_stats(struct filter_in *f, struct filter_siggen_stats *stats) 
   if (f == NULL || f->fwd_plan == NULL || stats == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
-  if (!c->gen)
+  if (c->mode != INGEST_GEN)
     return -1;
   pthread_mutex_lock(&c->mu);
   if (!c->gen_stats_on) {

@@ -402,7 +402,7 @@ def test_rejections(cuda_dev):
         assert s.raw(x, 16, R.U8) == -1                       # another format on the same master
         assert s.i16(xi[:16], 1.0) == -1
         assert s.flt(np.zeros(16, np.float32)) == -1
-        assert s.raw(x, 16, 9) == -1                          # unknown format
+        assert s.raw(x, 16, -1) == -1                         # unknown format
     with Session(lib, 48000, 12001, False) as s:
         assert s.i16(xi[:16], 1.0) == 0
         assert s.raw(x, 16, R.S8) == -1
@@ -415,3 +415,31 @@ def test_rejections(cuda_dev):
     with Session(lib, 48000, 12001, True) as s:
         assert s.raw(x, 16, R.PACKED12) == -1                 # packed 12-bit samples are real
         assert s.raw(x, 16, R.S8) == 0
+
+
+@pytest.mark.gpu
+def test_int16_and_float_writes_exclude_each_other(cuda_dev):
+    """Launches read the int16 ring of a master fed int16 words, so floats written to it would be lost: it refuses them,
+    and a master fed floats refuses int16 words, through write_i16filter and through filter_i16_write_pointer."""
+    from ka9q_radio_b200 import capi
+
+    lib, kg = _driver(), capi.load()
+    kg.filter_i16_write_pointer.restype = C.c_void_p
+    kg.filter_i16_write_pointer.argtypes = [C.c_void_p]
+    kg.write_i16filter.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_bool]
+    xi, xf = np.zeros(16, np.int16), np.zeros(16, np.float32)
+    # the session handle is the address of its struct filter_in
+    with Session(lib, 48000, 12001, False) as s:
+        assert s.i16(xi, 1.0) == 0
+        assert s.flt(xf) == -1
+    with Session(lib, 48000, 12001, False) as s:
+        assert kg.filter_i16_write_pointer(s.h)
+        assert kg.write_i16filter(s.h, None, 16, 1.0, False) == 0
+        assert s.flt(xf) == -1
+    with Session(lib, 48000, 12001, False) as s:
+        assert s.flt(xf) == 0
+        assert s.i16(xi, 1.0) == -1
+        assert not kg.filter_i16_write_pointer(s.h)
+    with Session(lib, 48000, 12001, False) as s:
+        assert s.flt(xf[:0]) == 0                             # a write of no floats claims nothing
+        assert s.i16(xi, 1.0) == 0

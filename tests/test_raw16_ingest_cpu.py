@@ -216,5 +216,5 @@ def test_raw16_ring_rejections():
     assert _ring_bytes(40000, 10001, COMPLEX, R.U16) == -1       # offset-binary 16-bit samples are real
     assert _ring_bytes(40000, 10001, REAL, R.SC16Q11) == -1      # SC16 Q11 samples are I/Q
     assert _ring_bytes(36000, 9001, COMPLEX, 7) == -1
-    assert _ring_bytes(40000, 10001, COMPLEX, 9) == -1           # unknown format
+    assert _ring_bytes(40000, 10001, COMPLEX, 13) == -1          # unknown format
     assert _ring_bytes(0, 10001, COMPLEX, R.S16) == -1

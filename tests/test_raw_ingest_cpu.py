@@ -71,6 +71,6 @@ def test_raw_ring_rejections_and_8bit_sizes():
     assert _ring_bytes(400004, 100001, 2, R.PACKED12) == -1    # windows would not start on a group boundary
     assert _ring_bytes(400000, 100003, 2, R.PACKED12) == -1
     assert _ring_bytes(400000, 100001, 1, R.PACKED12) == -1    # packed 12-bit samples are real
-    assert _ring_bytes(36000, 9001, 1, 7) == -1                # unknown format
+    assert _ring_bytes(36000, 9001, 1, 0) == -1                # unknown format
     n = _ring_bytes(36000, 9001, 1, R.U8)                      # RTL-SDR 1.8 MS/s I/Q: two bytes per pair
     assert n >= 2 * 4 * 45000 and n % 4096 == 0
