@@ -209,7 +209,7 @@ int kgpu_iq_scan(const struct kgpu_iq_write *d_tab, struct kgpu_iq_state *d_coef
 int kgpu_iq_apply(const void *d_raw, int fmt, long long a0, long count, const struct kgpu_iq_write *d_tab,
                   const struct kgpu_iq_state *d_coef, int cap, long long w_lo, int nw, void *d_out, void *stream);
 
-/* sig_gen.c's CW source (proc_sig_gen, sig_gen.c:286-346) on the device; see csrc/siggen.cuh.  freq and rate are cycles
+/* sig_gen.c's CW, AM and DSB sources (proc_sig_gen, sig_gen.c:286-346) on the device; see csrc/siggen.cuh.  freq and rate are cycles
  * per sample and per sample^2, what set_osc receives (sig_gen.c:221-224); amplitude and noise sdr->amplitude and
  * sdr->noise; seed rand_init's xoshiro256** seed (1). */
 struct kgpu_siggen_params {
@@ -229,6 +229,16 @@ void kgpu_siggen_destroy(kgpu_siggen *g);
  * on one stream (its scratch is reused). */
 int kgpu_siggen_generate(kgpu_siggen *g, long long a0, long count, double scale, const struct kgpu_scale_change *d_chg, int nchg,
                          void *d_out, double *d_block_energy, int nblocks, long L, long history, void *stream);
+/* sig_gen.c's AM and DSB sources (sig_gen.c:297-314, :327-344): turns g into a generator of
+ * (dc + m) * amplitude * carrier + noise * real_gauss, m the envelope libsamplerate produces at the front end's rate
+ * (dc: AM 1.0, DSB 0.0; -1 for a non-finite dc).  One draw per sample, for COMPLEX pairs too (the noise is on I only),
+ * so kgpu_siggen_state's draw d is then sample d.  A modulated generator is driven by kgpu_siggen_generate_mod only. */
+int kgpu_siggen_set_modulation(kgpu_siggen *g, double dc);
+/* kgpu_siggen_generate's window of a modulated generator: d_mod holds one envelope float per sample (REAL) or pair
+ * (COMPLEX) of the window, laid out as d_out; the entries of samples before the stream are not read. */
+int kgpu_siggen_generate_mod(kgpu_siggen *g, long long a0, long count, double scale, const struct kgpu_scale_change *d_chg,
+                             int nchg, void *d_out, const float *d_mod, double *d_block_energy, int nblocks, long L,
+                             long history, void *stream);
 /* Pure host code: the xoshiro256** state before draw `draw` (out[4]), by GF(2) jumps from the seeded state; and the
  * step and sweep angles the carrier uses, in cycles as 128-bit fractions: out[4] = {F low, F high, R low, R high}. */
 int kgpu_siggen_state(const kgpu_siggen *g, unsigned long long draw, uint64_t *out);

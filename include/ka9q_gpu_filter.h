@@ -27,6 +27,8 @@
  *   filter_siggen_setup           (EXTENSION) sig_gen.c's carrier and noise generated on the device
  *   write_genfilter               (EXTENSION) advance a generated master, replacing sig_gen.c's sample loop
  *   filter_siggen_stats           (EXTENSION) the energy that loop sums, per drained block
+ *   filter_siggen_modulate        (EXTENSION) sig_gen.c's AM and DSB: the carrier times the driver's resampled envelope
+ *   filter_siggen_mod_pointer     (EXTENSION) where src_callback_read puts that envelope
  *
  * Semantics kept: return 0 / -1 (write_*: 1 if a block fired), ND-deep spectrum ring with
  * lap -> zeros + block_drops++ (filter.c:690-701), owner-thread shortcut (filter.c:681-683),
@@ -256,8 +258,8 @@ int filter_iq_records(struct filter_in *master, struct filter_iq_record *recs, i
  * write_rfilter / write_cfilter: it advances the stream by n samples (REAL) or pairs (COMPLEX), each the loop's
  * (float)(samp * scale) with this write's scale, and fires blocks as write_rfilter does (1 if a block fired).  Samples
  * before the first write are 0.0f.  The noise is bitwise the reference's (xoshiro256** seeded by rand_init through
- * splitmix64, real_gauss); the carrier is within 1 ulp of its phasor chain.  Only CW is served (FM is CW in the reference);
- * AM and DSB read an audio source and stay with the driver's loop.
+ * splitmix64, real_gauss); the carrier is within 1 ulp of its phasor chain.  CW is served (FM is CW in the reference),
+ * and AM and DSB through filter_siggen_modulate.
  *   freq, rate  cycles per sample and per sample^2, what set_osc receives: carrier / samprate (REAL),
  *               (carrier - frequency) / samprate (COMPLEX), sig_gen.c:221-224
  *   amplitude, noise  sdr->amplitude, sdr->noise;  seed  rand_init's (1) */
@@ -268,6 +270,17 @@ struct filter_siggen_params {
 };
 int filter_siggen_setup(struct filter_in *master, struct filter_siggen_params const *params);
 int write_genfilter(struct filter_in *master, int n, double scale);
+/* EXTENSION: sig_gen.c's AM and DSB sources (sig_gen.c:297-314, :327-344).  libsamplerate stays with the driver; the
+ * device multiplies the carrier by (dc + m), m the envelope floats src_callback_read produces at the front end's rate.
+ * filter_siggen_modulate turns a master just set up by filter_siggen_setup into an AM (dc = 1) or DSB (dc = 0)
+ * generator: -1 after its first write_genfilter, on a master that is not generated, or for a non-finite dc.  As in the
+ * reference, a COMPLEX master then draws one Gaussian per pair and puts the noise on I only.
+ * filter_siggen_mod_pointer is where the next write's envelope goes: one float per sample (REAL) or pair (COMPLEX), in a
+ * pinned, mirrored host ring the library owns, with contiguous room for the largest n write_genfilter accepts (NULL on a
+ * master that is not modulated).  The driver passes it straight to src_callback_read; write_genfilter(master, r, scale)
+ * then commits the r envelope floats written there and generates those samples. */
+int filter_siggen_modulate(struct filter_in *master, double dc);
+float *filter_siggen_mod_pointer(struct filter_in *master);
 /* The generated energy, as filter_ingest_stats counts its statistics: never blocks, sums over the blocks whose device
  * work completed since the previous call, each block once; the first call starts collection and returns zeros.  energy
  * is the sum of samp^2 (REAL, as sig_gen.c:294) or |samp|^2 (COMPLEX) of the unscaled samples; the reference's COMPLEX

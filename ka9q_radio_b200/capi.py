@@ -95,11 +95,16 @@ def load() -> C.CDLL:
     L.kgpu_siggen_create.argtypes = [i, vp]
     L.kgpu_siggen_destroy.argtypes = [vp]
     L.kgpu_siggen_generate.argtypes = [vp, ll, l, d, vp, i, vp, vp, i, l, l, vp]
+    L.kgpu_siggen_set_modulation.argtypes = [vp, d]
+    L.kgpu_siggen_generate_mod.argtypes = [vp, ll, l, d, vp, i, vp, vp, vp, i, l, l, vp]
     L.kgpu_siggen_state.argtypes = [vp, C.c_ulonglong, vp]
     L.kgpu_siggen_angles.argtypes = [vp, vp]
     L.filter_siggen_setup.argtypes = [vp, vp]
     L.write_genfilter.argtypes = [vp, i, d]
     L.filter_siggen_stats.argtypes = [vp, vp]
+    L.filter_siggen_modulate.argtypes = [vp, d]
+    L.filter_siggen_mod_pointer.restype = vp
+    L.filter_siggen_mod_pointer.argtypes = [vp]
     L.kgpu_bank_define_ex.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_wide.argtypes = [vp, i, i, i]
     L.kgpu_bank_define_huge.argtypes = [vp, i, i, i]
@@ -253,7 +258,7 @@ class SiggenStats(C.Structure):
 
 class Siggen:
     """sig_gen.c's CW source on the device (kgpu_siggen_*): carrier freq / rate in cycles per sample (per sample^2),
-    amplitude, noise and the xoshiro256** seed as rand_init gives it (1)."""
+    amplitude, noise and the xoshiro256** seed as rand_init gives it (1); AM or DSB after modulate()."""
 
     def __init__(self, in_type: int, freq: float, amplitude: float, noise: float, rate: float = 0.0, seed: int = 1):
         self.cplx = in_type == KGPU_COMPLEX
@@ -270,6 +275,18 @@ class Siggen:
             history = count - nblocks * L
         check(load().kgpu_siggen_generate(self.h, a0, count, scale, d_chg or None, nchg, d_out, d_energy or None, nblocks, L,
                                           history, stream or None), "kgpu_siggen_generate")
+
+    def modulate(self, dc: float) -> None:
+        """AM (dc = 1) or DSB (dc = 0): from now on generate_mod() drives the generator"""
+        check(load().kgpu_siggen_set_modulation(self.h, dc), "kgpu_siggen_set_modulation")
+
+    def generate_mod(self, a0: int, count: int, scale: float, d_out: int, d_mod: int, d_energy: int = 0, nblocks: int = 0,
+                     L: int = 0, history: int | None = None, d_chg: int = 0, nchg: int = 0, stream: int = 0) -> None:
+        """generate() of a modulated generator; d_mod: one float32 envelope value per sample of the window"""
+        if history is None:
+            history = count - nblocks * L
+        check(load().kgpu_siggen_generate_mod(self.h, a0, count, scale, d_chg or None, nchg, d_out, d_mod, d_energy or None,
+                                              nblocks, L, history, stream or None), "kgpu_siggen_generate_mod")
 
     def state(self, draw: int) -> tuple[int, int, int, int]:
         """the xoshiro256** state before draw `draw` (host jump)"""

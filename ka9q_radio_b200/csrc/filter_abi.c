@@ -91,7 +91,7 @@ struct spec_slave {
  * its float ring has taken or launched a sample (ingest_of). */
 enum ingest { INGEST_NONE, INGEST_FLOAT, INGEST_INT16, INGEST_RAW, INGEST_GEN };
 
-/* The int16 or raw words of a master's stream: a mirrored, pinned host ring of `size` bytes, `group` bytes to every 8
+/* The int16 or raw words, or the AM / DSB envelope floats, of a master's stream: a mirrored, pinned host ring of `size` bytes, `group` bytes to every 8
  * samples (REAL) or I/Q pairs, written at wp; rp is the first sample (history included) of the next launch's window. */
 struct word_ring {
   char *base, *wp, *rp;
@@ -135,7 +135,7 @@ struct master_ctx {
   struct notch_state *notches_seen;
   unsigned notch_hash;
   /* what feeds the master (see check_mode); int16 and raw words go through `ring`, raw ones are then unpacked on the
-   * device from d_raw into d_win[slot] */
+   * device from d_raw into d_win[slot]; a modulated generator's envelope goes through `ring` and d_raw too */
   enum ingest mode;
   int raw_fmt; /* INGEST_RAW: the enum filter_raw_format, its row of raw_formats; else 0 */
   struct word_ring ring;
@@ -181,9 +181,11 @@ struct master_ctx {
   long sring_cap; /* samples */
   long sring_pos; /* just past the newest issued sample */
   bool sring_i16;
-  /* sig_gen's CW source (filter_siggen_setup): the device generates every window, the host ring is never written.
-   * d_gen_energy / h_gen_energy: each ring slot's block energies, folded in job order into gen_acc once asked for */
+  /* sig_gen's source (filter_siggen_setup): the device generates every window, the host ring is never written.
+   * d_gen_energy / h_gen_energy: each ring slot's block energies, folded in job order into gen_acc once asked for.
+   * gen_mod: AM or DSB (filter_siggen_modulate), the envelope floats in `ring` */
   kgpu_siggen *gen;
+  bool gen_mod;
   double *d_gen_energy, *h_gen_energy;
   bool gen_stats_on;
   unsigned long long gen_folded;
@@ -1017,6 +1019,15 @@ static void gen_fold_one(struct filter_in const *f, struct master_ctx *c) {
   c->gen_folded++;
 }
 
+/* the generator's floats of samples [a0, a0 + count) at d_out (kgpu_siggen_generate's arguments), from the envelope
+ * at d_mod (one float per sample of the window) on a modulated master */
+static int gen_window(struct master_ctx *c, long long a0, long count, double scale, struct kgpu_scale_change const *chg,
+                      int nchg, void *d_out, float const *d_mod, double *d_energy, int nblocks, long L, long history) {
+  return c->gen_mod ? kgpu_siggen_generate_mod(c->gen, a0, count, scale, chg, nchg, d_out, d_mod, d_energy, nblocks, L,
+                                               history, c->st)
+                    : kgpu_siggen_generate(c->gen, a0, count, scale, chg, nchg, d_out, d_energy, nblocks, L, history, c->st);
+}
+
 /* ---------------------------------------------------------------- spectrum device ring ------ */
 /* n samples of esz bytes from a ring (src_cap samples, position src) to the device ring at position dst, both modular */
 static int sring_copy(struct master_ctx *c, char const *src_base, long src_cap, long src, long dst, long n, size_t esz,
@@ -1056,18 +1067,24 @@ static int sring_seed(struct filter_in *f, struct master_ctx *c) {
   struct word_ring const *r = &c->ring;
   int rc = 0;
   switch (c->mode) {
-  case INGEST_GEN: { /* the host ring holds nothing: generate the last sring_cap samples again */
+  case INGEST_GEN: { /* the host float ring holds nothing: generate the last sring_cap samples again */
     double scale;
     int nc;
     rc = chg_span(c, ND, a0, a0 + n, &scale, &nc);
     struct kgpu_scale_change const *chg = nc ? c->d_chg : NULL;
-    rc = rc ? rc
-            : kgpu_siggen_generate(c->gen, a0, first, scale, chg, nc, (char *)c->d_sring + (size_t)dst * esz, NULL, 0, 0, first,
-                                   c->st);
+    float *mod = NULL; /* modulated: those samples' envelope, sent over from the envelope ring */
+    if (rc == 0 && c->gen_mod) {
+      long const cap = wring_samples(r, r->size), end = wring_samples(r, (size_t)(r->rp - r->base)) + M1;
+      long const src = ((end - n) % cap + cap) % cap;
+      rc = cudaMalloc((void **)&mod, wring_bytes(r, (size_t)n)) == cudaSuccess ? 0 : -1;
+      rc = rc ? rc : window_h2d(mod, r->base + wring_bytes(r, (size_t)src), wring_bytes(r, (size_t)n), r->base, r->size, c->st);
+    }
+    rc = rc ? rc : gen_window(c, a0, first, scale, chg, nc, (char *)c->d_sring + (size_t)dst * esz, mod, NULL, 0, 0, first);
     if (rc == 0 && dst > 0)
-      rc = kgpu_siggen_generate(c->gen, a0 + first, dst, scale, chg, nc, c->d_sring, NULL, 0, 0, dst, c->st);
+      rc = gen_window(c, a0 + first, dst, scale, chg, nc, c->d_sring, mod ? mod + first : NULL, NULL, 0, 0, dst);
     if (cudaStreamSynchronize(c->st) != cudaSuccess)
       rc = -1;
+    cudaFree(mod);
     return rc ? kgf_fail("filter_spectrum_setup: generating the device ring") : 0;
   }
   case INGEST_RAW: { /* the host ring holds raw bytes: send the last sring_cap samples' bytes over and unpack them there */
@@ -1143,11 +1160,14 @@ static int launch_input(struct filter_in *f, struct master_ctx *c, int slot, int
   }
   double s;
   int n;
-  if (c->mode == INGEST_GEN) { /* generated on the device: nothing crosses PCIe */
+  if (c->mode == INGEST_GEN) { /* generated on the device: only a modulated master's envelope crosses PCIe */
+    if (c->gen_mod && window_h2d(c->d_raw, wring_advance(&c->ring, (size_t)f->ilen * (size_t)k), wring_bytes(&c->ring, span),
+                                 c->ring.base, c->ring.size, c->st) != 0)
+      return kgf_fail("execute_filter_input: H2D of the envelope");
     if (chg_span(c, slot, a0, a0 + (long long)span, &s, &n) != 0 ||
-        kgpu_siggen_generate(c->gen, a0, (long)span, s, n ? c->d_chg : NULL, n, win,
-                             c->gen_stats_on ? c->d_gen_energy + slot : NULL, k, f->ilen, M1, c->st) != 0)
-      return kgf_fail("execute_filter_input: kgpu_siggen_generate");
+        gen_window(c, a0, (long)span, s, n ? c->d_chg : NULL, n, win, c->d_raw, c->gen_stats_on ? c->d_gen_energy + slot : NULL,
+                   k, f->ilen, M1) != 0)
+      return kgf_fail("execute_filter_input: generating the window");
     return 0;
   }
   bool const raw = c->mode == INGEST_RAW;
@@ -2193,7 +2213,7 @@ int filter_iq_records(struct filter_in *f, struct filter_iq_record *recs, int ma
 }
 
 /* ---------------------------------------------------------------- sig_gen ------------------- */
-/* EXTENSION: sig_gen's CW source on the device (see include/ka9q_gpu_filter.h), before the first write. */
+/* EXTENSION: sig_gen's source on the device (see include/ka9q_gpu_filter.h), before the first write. */
 int filter_siggen_setup(struct filter_in *f, struct filter_siggen_params const *p) {
   if (f == NULL || f->fwd_plan == NULL || p == NULL)
     return -1;
@@ -2233,8 +2253,50 @@ int write_genfilter(struct filter_in *f, int n, double scale) {
   pthread_mutex_unlock(&c->mu);
   if (rc != 0)
     return -1;
+  if (c->gen_mod)
+    wring_push(&c->ring, (size_t)n); /* the envelope the driver wrote at filter_siggen_mod_pointer */
   f->wcnt += n;
   return fire_ready_blocks(f);
+}
+
+/* EXTENSION: sig_gen's AM and DSB sources (see include/ka9q_gpu_filter.h), after filter_siggen_setup and before the
+ * first write.  The envelope ring holds the host float ring's samples for the wideband analyzer's seeding (sring_seed
+ * regenerates them), plus the largest write that may be pending or being written behind them; the device window of
+ * the envelope is d_raw, sized as raw_start sizes it. */
+int filter_siggen_modulate(struct filter_in *f, double dc) {
+  if (f == NULL || f->fwd_plan == NULL || !isfinite(dc))
+    return -1;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  if (c->mode != INGEST_GEN || c->chg_started) {
+    fprintf(stderr, "filter_siggen_modulate: %s\n", c->mode != INGEST_GEN ? "the master is not generated" : "after the first write");
+    return -1;
+  }
+  if (!c->gen_mod) {
+    static uint32_t const zero[3];
+    size_t const samples = f->input_buffer_size / c->esz; /* the host float ring's */
+    size_t const span = (size_t)(ND - 2) * (size_t)f->ilen + (size_t)f->points;
+    if (wring_open(&c->ring, page_round(2 * samples * sizeof(float)), 8 * sizeof(float), f->impulse_length - 1, zero) != 0)
+      return kgf_fail("filter_siggen_modulate: envelope ring");
+    if (cudaMalloc(&c->d_raw, span * sizeof(float)) != cudaSuccess) {
+      c->d_raw = NULL;
+      ring_free(c->ring.base, c->ring.size);
+      c->ring.base = NULL;
+      return kgf_fail("filter_siggen_modulate: device buffer");
+    }
+  }
+  if (kgpu_siggen_set_modulation(c->gen, dc) != 0)
+    return kgf_fail("filter_siggen_modulate");
+  pthread_mutex_lock(&c->mu);
+  c->gen_mod = true;
+  pthread_mutex_unlock(&c->mu);
+  return 0;
+}
+
+float *filter_siggen_mod_pointer(struct filter_in *f) {
+  if (f == NULL || f->fwd_plan == NULL)
+    return NULL;
+  struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
+  return c->mode == INGEST_GEN && c->gen_mod ? (float *)c->ring.wp : NULL;
 }
 
 /* EXTENSION: the generated energy of the blocks whose device work completed since the previous call, as

@@ -447,7 +447,7 @@ extern "C" int kgpu_iq_apply(const void *d_raw, int fmt, long long a0, long coun
   return 0;
 }
 
-// ---- sig_gen.c's CW source (siggen.cuh) ------------------------------------------------------------------------------
+// ---- sig_gen.c's CW, AM and DSB sources (siggen.cuh) -----------------------------------------------------------------
 extern "C" void kgpu_siggen_angle128(double f, uint64_t *out);  // siggen_host.c
 namespace {
 // T^(2^b), b = 0 .. 63, of xoshiro256**'s state transition, in siggen.cuh's nibble-table form; built once per process
@@ -507,6 +507,8 @@ unsigned long long splitmix64(unsigned long long *x) {  // gauss.c:24-29
 
 struct kgpu_siggen {
   bool cplx;
+  bool mod;   // AM / DSB (kgpu_siggen_set_modulation): one draw per sample, the envelope from kgpu_siggen_generate_mod
+  double dc;  // and its carrier component
   kgpu_siggen_params p;
   unsigned long long seeded[4];  // xoshiro256ss_seed (gauss.c:32-44)
   U128 F, R;
@@ -563,24 +565,37 @@ extern "C" int kgpu_siggen_angles(const kgpu_siggen *g, uint64_t *out) {
   return 0;
 }
 
-extern "C" int kgpu_siggen_generate(kgpu_siggen *g, long long a0, long count, double scale, const kgpu_scale_change *d_chg, int nchg,
-                                    void *d_out, double *d_block_energy, int nblocks, long L, long history, void *stream) {
-  int const C = g && g->cplx ? 2 : 1, S = kGenRun / C;
-  if (!g || !d_out || count < 0 || history < 0 || nblocks < 0 || nchg < 0 || (nchg && !d_chg) ||
-      (nblocks > 0 && (L < S || count != history + (long)nblocks * L)) || (a0 < 0 && std::min(-a0, (long long)count) > history))
-    return fail("kgpu_siggen_generate: bad arguments");
+extern "C" int kgpu_siggen_set_modulation(kgpu_siggen *g, double dc) {
+  if (!g || !std::isfinite(dc)) return fail("kgpu_siggen_set_modulation: bad arguments");
+  g->mod = true;
+  g->dc = dc;
+  return 0;
+}
+
+// kgpu_siggen_generate and _generate_mod: d_mod is NULL exactly when the generator is not modulated
+static int siggen_launch(kgpu_siggen *g, long long a0, long count, double scale, const kgpu_scale_change *d_chg, int nchg,
+                         void *d_out, const float *d_mod, double *d_block_energy, int nblocks, long L, long history,
+                         void *stream, char const *who) {
+  int const C = g && g->cplx ? 2 : 1;                   // floats per sample
+  int const D = g && g->cplx && !g->mod ? 2 : 1;        // draws per sample
+  int const S = kGenRun / D;                            // samples per thread
+  if (!g || !d_out || (g->mod != (d_mod != nullptr)) || count < 0 || history < 0 || nblocks < 0 || nchg < 0 ||
+      (nchg && !d_chg) || (nblocks > 0 && (L < S || count != history + (long)nblocks * L)) ||
+      (a0 < 0 && std::min(-a0, (long long)count) > history))
+    return fail("%s: bad arguments", who);
   cudaStream_t st = (cudaStream_t)stream;
   float *out = (float *)d_out;
   if (a0 < 0) {  // the samples before the stream's first: zeros, all inside the history
     long const z = (long)std::min(-a0, (long long)count);
     CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)C * (size_t)z, st));
     out += (size_t)C * (size_t)z;
+    if (d_mod) d_mod += z;
     count -= z;
     history -= z;
     a0 = 0;
   }
   long const nthreads = (count + S - 1) / S;
-  if (nthreads >= (1L << kGenJumpBits)) return fail("kgpu_siggen_generate: %ld samples exceed one launch", count);
+  if (nthreads >= (1L << kGenJumpBits)) return fail("%s: %ld samples exceed one launch", who, count);
   if (count == 0) return 0;
   long const grid = (nthreads + kGenThreads - 1) / kGenThreads;
   if (!g->d_tabs) {  // the device's jump matrices, at the first launch (create is pure host code)
@@ -598,7 +613,7 @@ extern "C" int kgpu_siggen_generate(kgpu_siggen *g, long long a0, long count, do
   }
   GenArgs a;
   uint64_t base[4];
-  kgpu_siggen_state(g, (unsigned long long)a0 * (unsigned long long)C, base);
+  kgpu_siggen_state(g, (unsigned long long)a0 * (unsigned long long)D, base);
   for (int k = 0; k < 4; k++) a.base[k] = base[k];
   a.F = g->F;
   a.R = g->R;
@@ -614,8 +629,11 @@ extern "C" int kgpu_siggen_generate(kgpu_siggen *g, long long a0, long count, do
   a.tabs = g->d_tabs;
   a.out = out;
   a.part = d_block_energy && nblocks > 0 ? g->d_part : nullptr;
-  if (g->cplx) siggen_kernel<true><<<(unsigned)grid, kGenThreads, 0, st>>>(a);
-  else siggen_kernel<false><<<(unsigned)grid, kGenThreads, 0, st>>>(a);
+  a.dc = g->dc;
+  a.mod = d_mod;
+  auto const k = g->mod ? (g->cplx ? siggen_kernel<true, true> : siggen_kernel<false, true>)
+                        : (g->cplx ? siggen_kernel<true, false> : siggen_kernel<false, false>);
+  k<<<(unsigned)grid, kGenThreads, 0, st>>>(a);
   g_launches++;
   CUDA_OK(cudaGetLastError());
   if (a.part) {
@@ -624,6 +642,19 @@ extern "C" int kgpu_siggen_generate(kgpu_siggen *g, long long a0, long count, do
     CUDA_OK(cudaGetLastError());
   }
   return 0;
+}
+
+extern "C" int kgpu_siggen_generate(kgpu_siggen *g, long long a0, long count, double scale, const kgpu_scale_change *d_chg, int nchg,
+                                    void *d_out, double *d_block_energy, int nblocks, long L, long history, void *stream) {
+  return siggen_launch(g, a0, count, scale, d_chg, nchg, d_out, nullptr, d_block_energy, nblocks, L, history, stream,
+                       "kgpu_siggen_generate");
+}
+
+extern "C" int kgpu_siggen_generate_mod(kgpu_siggen *g, long long a0, long count, double scale, const kgpu_scale_change *d_chg,
+                                        int nchg, void *d_out, const float *d_mod, double *d_block_energy, int nblocks, long L,
+                                        long history, void *stream) {
+  return siggen_launch(g, a0, count, scale, d_chg, nchg, d_out, d_mod, d_block_energy, nblocks, L, history, stream,
+                       "kgpu_siggen_generate_mod");
 }
 
 extern "C" int kgpu_device_count(void) {

@@ -16,6 +16,15 @@
 // cycle; the phase is exact modular integer arithmetic.  The chain's own rounding walks away from this by about 1e-12
 // rad after 1e8 samples, which flips the float rounding of a few samples in 1e5 by one ulp, and next to a zero of the
 // signal, where a float ulp is smaller than that, by more ulps (tests/test_siggen_cpu.py).
+//
+// AM and DSB (sig_gen.c:297-314, :327-344).  The modulated instantiation multiplies the carrier by dc + m, m the envelope
+// float libsamplerate produced for the sample (read from GenArgs::mod; dc = 1 for AM, 0 for DSB), with the products and
+// sums the reference's compiled loop performs, in its order and contraction (found in its disassembly, pinned by
+// tests/test_siggen_mod_cpu.py):
+//   REAL     samp = fma(amplitude * cr, dc + m, noise * g)
+//   COMPLEX  k = (dc + m) * amplitude;  re = fma(k, cr, noise * g),  im = k * ci
+// The reference draws one Gaussian per sample there, for COMPLEX too (noise on I only), so draw d is sample d and each
+// thread's run of kGenRun draws is kGenRun samples.
 #pragma once
 #include <stdint.h>
 
@@ -62,6 +71,8 @@ struct GenArgs {
   unsigned long long const *tabs;  // kGenJumpBits jump matrices T^(kGenRun 2^b)
   float *out;
   double *part;  // 2 per thread: energy in the block of its first new sample, and in the next one
+  double dc;             // modulated: the carrier component (AM 1, DSB 0)
+  float const *mod;      // modulated: one envelope float per sample of out
 };
 
 __device__ __forceinline__ unsigned long long rotl64(unsigned long long x, int k) { return (x << k) | (x >> (64 - k)); }
@@ -106,10 +117,11 @@ __device__ __forceinline__ void gf2_apply(unsigned long long const *__restrict__
   s[3] = y3;
 }
 
-template <bool CPLX>
+// MOD: the AM / DSB instantiation (one draw per sample, the envelope from a.mod)
+template <bool CPLX, bool MOD>
 __global__ void __launch_bounds__(kGenThreads) siggen_kernel(GenArgs a) {
   constexpr int C = CPLX ? 2 : 1;
-  constexpr int S = kGenRun / C;  // samples per thread
+  constexpr int S = MOD ? kGenRun : kGenRun / C;  // samples per thread
   long const t = (long)blockIdx.x * kGenThreads + threadIdx.x;
   long const i0 = t * S;
   double e_lo = 0, e_hi = 0;
@@ -140,16 +152,33 @@ __global__ void __launch_bounds__(kGenThreads) siggen_kernel(GenArgs a) {
         ph = add128(ph, inc);
         inc = add128(inc, a.R);
       }
-      // samp = amplitude * step_osc() + noise * gauss, the product by the carrier contracted into an FMA
-      double const re = carrier ? __fma_rn(a.amplitude, cr, __dmul_rn(a.noise, gauss_of(xo_next(s))))
-                                : __dmul_rn(a.noise, gauss_of(xo_next(s)));
-      double e = __dmul_rn(re, re);
-      a.out[i * C] = __double2float_rn(__dmul_rn(re, sc));
-      if constexpr (CPLX) {
-        double const im = carrier ? __fma_rn(a.amplitude, ci, __dmul_rn(a.noise, gauss_of(xo_next(s))))
-                                  : __dmul_rn(a.noise, gauss_of(xo_next(s)));
-        e = __fma_rn(im, im, e);
-        a.out[i * C + 1] = __double2float_rn(__dmul_rn(im, sc));
+      double re, e;
+      if constexpr (MOD) {
+        double const m = (double)a.mod[i];
+        double const ng = __dmul_rn(a.noise, gauss_of(xo_next(s)));
+        if constexpr (CPLX) {
+          double const k = __dmul_rn(__dadd_rn(m, a.dc), a.amplitude);
+          re = __fma_rn(k, cr, ng);
+          double const im = __dmul_rn(k, ci);
+          e = __fma_rn(im, im, __dmul_rn(re, re));
+          a.out[2 * i + 1] = __double2float_rn(__dmul_rn(im, sc));
+        } else {
+          re = __fma_rn(__dmul_rn(a.amplitude, cr), __dadd_rn(m, a.dc), ng);
+          e = __dmul_rn(re, re);
+        }
+        a.out[i * C] = __double2float_rn(__dmul_rn(re, sc));
+      } else {
+        // samp = amplitude * step_osc() + noise * gauss, the product by the carrier contracted into an FMA
+        re = carrier ? __fma_rn(a.amplitude, cr, __dmul_rn(a.noise, gauss_of(xo_next(s))))
+                     : __dmul_rn(a.noise, gauss_of(xo_next(s)));
+        e = __dmul_rn(re, re);
+        a.out[i * C] = __double2float_rn(__dmul_rn(re, sc));
+        if constexpr (CPLX) {
+          double const im = carrier ? __fma_rn(a.amplitude, ci, __dmul_rn(a.noise, gauss_of(xo_next(s))))
+                                    : __dmul_rn(a.noise, gauss_of(xo_next(s)));
+          e = __fma_rn(im, im, e);
+          a.out[i * C + 1] = __double2float_rn(__dmul_rn(im, sc));
+        }
       }
       if (i >= a.history) {
         if ((i - a.history) / a.L == blk0) e_lo += e;
