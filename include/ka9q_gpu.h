@@ -348,6 +348,31 @@ int kgpu_bank_fm_front(kgpu_bank *b, const void *d_out, long out_pitch, int nblo
 
 /* Push pending channel changes (shift/filter/enable) to the device now, ordered after `stream`. */
 int kgpu_bank_commit(kgpu_bank *b, void *stream);
+
+/* A small master (small_master.cuh): the forward transform and every slave of one block in one CTA, one kernel launch per
+ * write, for radiod's per-channel secondary masters (filter2, the wfm / stereod / rdsd composite, packetd, ctcss).  Its
+ * envelope: Nc (N for COMPLEX, N/2 for REAL, with L and N even) has factors 2, 3, 5, 7 and at most 28 812 points; at most
+ * KGPU_SMALL_MAX_SLAVES slaves, each of a point count with the same bounds.  The caller owns the window, the spectrum
+ * slots (kgpu_small_spec_stride float2 per block, kgpu_master_spec_stride's layout) and the output rows. */
+#define KGPU_SMALL_MAX_SLAVES 8
+typedef struct kgpu_small kgpu_small;
+long kgpu_small_smem(int L, int M, int in_type); /* host only: the forward's shared memory in bytes, -1 outside the envelope */
+kgpu_small *kgpu_small_create(int L, int M, int in_type);
+void kgpu_small_destroy(kgpu_small *m);
+long kgpu_small_spec_stride(kgpu_small const *m);
+int kgpu_small_define(kgpu_small *m, int idx, int olen, int out_type); /* the slave's points, or -1 */
+int kgpu_small_undefine(kgpu_small *m, int idx);
+/* set_filter's design and response transform, bitwise kgpu_bank_set_filter's; the response (points float2) is copied to
+ * `response`.  Synchronises `stream` first: launches queued on it may still read the old response. */
+int kgpu_small_set_filter(kgpu_small *m, int idx, double low, double high, double kaiser_beta, float *response, void *stream);
+int kgpu_small_set_slave(kgpu_small *m, int idx, int shift, int isb); /* used by the next kgpu_small_run */
+long kgpu_small_out_offset(kgpu_small const *m, int idx); /* float2 offset of slave idx in an output row */
+long kgpu_small_out_stride(kgpu_small const *m);          /* float2 of one output row */
+/* nblocks blocks from d_win (block b's window starts L samples after block b-1's): spectra into d_spec, every slave with a
+ * response into d_out (rows out_pitch float2 apart).  only >= 0: d_win is not read and slave `only` alone is recomputed
+ * from the spectra already in d_spec (after a retune). */
+int kgpu_small_run(kgpu_small *m, const void *d_win, int nblocks, void *d_spec, void *d_out, long out_pitch, int only,
+                   void *stream);
 /* Testing aid: 0 forces the generic runtime-plan kernels even where a compile-time specialised
  * kernel exists (both are parity-tested); it takes effect at the next launch, also for existing masters. Default 1.
  * Masters running the extended pair (kgpu_master_create_ex) have no specialised kernels and ignore it.

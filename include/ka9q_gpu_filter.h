@@ -8,6 +8,7 @@
  *
  *   entry point                   replaces (reference file:line)
  *   create_filter_input           filter.c:186-269   master: ring + forward plan  -> device plans
+ *   create_filter_input_small     (EXTENSION) the same for a small secondary master: one kernel per write, no bank
  *   create_filter_output          filter.c:298-415   slave: response/ifft plan    -> bank slot
  *   execute_filter_input          filter.c:558-651   queue forward FFT            -> H2D + 2 kernels
  *   execute_filter_output         filter.c:663-921   wait, slice*response, IFFT   -> batched kernel
@@ -124,6 +125,26 @@ extern double FFTW_plan_timelimit;
 extern int64_t Min_fft_time, Max_fft_time, Avg_fft_time, Mean_dev;
 
 int create_filter_input(struct filter_in *master, int L, int M, enum filtertype in_type);
+/* EXTENSION: create_filter_input for a master small enough for one CTA: radiod's per-channel secondary masters (filter2
+ * of CW and ISB channels, radio.c:1583; the wfm / stereod / rdsd composite, wfm.c:70; packetd; ctcss).  Each write that
+ * completes k blocks costs the window's H2D, one kernel, one D2H of the slaves' outputs and one event per block, and the
+ * host state is sized to the master: no channel bank, nothing per KGF_MAX_SLAVES.  Envelope: Nc (N for COMPLEX, N/2 for
+ * REAL, which needs even L and N) has factors 2, 3, 5, 7 and at most 28 812 points; outside it -1 is returned without
+ * touching *master, and the caller calls create_filter_input as before.  The filter_in fields mean what they always mean,
+ * and create_filter_output, set_filter, execute_filter_output(_batch), write_rfilter / write_cfilter, put_*filter and
+ * delete_filter_* keep the reference's semantics (laps, no response, hot response swaps, k-block writes).  The slaves'
+ * responses are bitwise a default master's.  On such a master:
+ *   - at most 8 slaves, COMPLEX or REAL output, each of a point count (olen N / L) with the same bounds as Nc;
+ *   - these return -1 with a message: SPECTRUM slaves, beam slaves (execute_filter_output), execute_filter_output_tuned,
+ *     filter_output_untune, filter_input_enable_noise, both spectrum analyzers, and every int16, raw, I/Q corrected and
+ *     generated ingest entry point (pointer-returning ones return NULL); filter_noise_estimate returns NAN;
+ *   - in.notches is not read (only the front end has notches, radio.c:601), and fdomain[] is allocated but never written
+ *     (only estimate_noise reads it, and only on the front end). */
+int create_filter_input_small(struct filter_in *master, int L, int M, enum filtertype in_type);
+/* Pure host code: the host and device bytes a create_filter_input_small master of this geometry allocates with max_slaves
+ * slaves of olen <= L (an upper bound: ring, fdomain[], context, window, ND spectra, ND output rows, responses and the
+ * slaves' own buffers), or -1 outside the envelope or for max_slaves outside 0..8. */
+long filter_small_master_bytes(int L, int M, enum filtertype in_type, int max_slaves);
 int create_filter_output(struct filter_out *slave, struct filter_in *master, int olen, enum filtertype out_type);
 int execute_filter_input(struct filter_in *master);
 int execute_filter_output(struct filter_out *slave, int shift);

@@ -53,21 +53,26 @@ __device__ __forceinline__ float2 beam_product(ChanAux const &ax, float2 const *
 // REAL-output slave (filter.c:794-809): element si (0 <= si <= ns/2) of the half spectrum is master bin si + shift
 // (d.q0) times the response.  The c2r inverse implies the Hermitian extension: slot si takes it (with the imaginary part
 // dropped at si = 0 and 2 si = ns, as FFTW ignores it), slot ns - si its conjugate.  The reference's "Nyquist zero"
-// (filter.c:911) lands on index (sb+1)/2 of the HALF spectrum; so does ours.
-__device__ __forceinline__ float2 real_half(ChanArgs const &a, ChanDesc const &d, float2 const *X, float2 const *R, int si) {
+// (filter.c:911) lands on index (sb+1)/2 of the HALF spectrum; so does ours.  x(q) loads master bin q.
+template <class LoadX>
+__device__ __forceinline__ float2 real_half_at(ChanArgs const &a, ChanDesc const &d, LoadX x, float2 const *R, int si) {
   int const sb = d.points / 2 + 1, m = a.m_bins, mi = si + d.q0;
   float2 v = make_float2(0.f, 0.f);
   if (!a.wrap) {
-    if (mi >= 0 && mi < m) v = cmul(__ldg(X + mi), __ldg(R + si));
+    if (mi >= 0 && mi < m) v = cmul(x(mi), __ldg(R + si));
   } else if (mi >= -(m / 2) && mi < m / 2) {
     int q1 = mi % m, q2 = (m - mi) % m;
     if (q1 < 0) q1 += m;
     if (q2 < 0) q2 += m;
-    float2 const xa = __ldg(X + q1), xb = __ldg(X + q2);
+    float2 const xa = x(q1), xb = x(q2);
     v = cmul(__ldg(R + si), make_float2(xa.x + xb.x, xa.y - xb.y));
   }
   if (si == (sb + 1) / 2) v = make_float2(0.f, 0.f);
   return v;
+}
+// The same from a spectrum no kernel of the launch writes (read-only loads).
+__device__ __forceinline__ float2 real_half(ChanArgs const &a, ChanDesc const &d, float2 const *X, float2 const *R, int si) {
+  return real_half_at(a, d, [X](int q) { return __ldg(X + q); }, R, si);
 }
 
 // ISB (filter.c:895-909), for 0 < p < ns/2: (S[p], S[ns-p]) <- (S[p] + conj S[ns-p], S[ns-p] - conj S[p]).  The

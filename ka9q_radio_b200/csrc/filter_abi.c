@@ -99,6 +99,7 @@ struct word_ring {
 };
 
 struct master_ctx {
+  bool small; /* false; a small master's context (struct small_ctx) starts with true */
   kgpu_master *km;
   kgpu_bank *bank;
   cudaStream_t st, st_one, st_d2h; /* pipeline, single-channel recompute, device->host copies */
@@ -330,9 +331,12 @@ static int nb_append(struct slave_ctx *sc, void const *d_src, int olen, cudaStre
   return 0;
 }
 
+static void small_teardown(struct filter_in *master);
 static void master_teardown(struct filter_in *master) {
   struct master_ctx *c = (struct master_ctx *)master->fwd_plan;
-  if (c) {
+  if (c && c->small) {
+    small_teardown(master);
+  } else if (c) {
     cudaStreamSynchronize(c->st);
     cudaStreamSynchronize(c->st_one);
     cudaStreamSynchronize(c->st_d2h);
@@ -393,6 +397,306 @@ static void master_teardown(struct filter_in *master) {
   }
   ring_free(master->input_buffer, master->input_buffer_size);
   master->input_buffer = NULL;
+}
+
+/* ---------------------------------------------------------------- small masters ------------- */
+/* A master made by create_filter_input_small: one small_master_kernel launch per write (kgpu_small_run), no channel bank.
+ * Its host state is what the filter.h semantics need and nothing sized by KGF_MAX_SLAVES: the float ring, a stream, ND
+ * events, ND pinned output rows for its (at most KGPU_SMALL_MAX_SLAVES) slaves, and what each slot's launch used per
+ * slave.  Device: one window, ND spectrum slots, ND output rows, the slaves' responses. */
+struct small_ctx {
+  bool small; /* true: see master_ctx */
+  kgpu_small *ks;
+  cudaStream_t st;
+  cudaEvent_t done[ND];
+  pthread_mutex_t mu;
+  size_t esz;
+  void *d_win;
+  float complex *d_spec; /* ND * spec_stride */
+  long spec_stride;
+  float complex *d_out, *h_out; /* ND rows of out_pitch float2 */
+  long out_pitch;
+  struct filter_out *slots[KGPU_SMALL_MAX_SLAVES];
+  unsigned ver[KGPU_SMALL_MAX_SLAVES];
+  int cur_shift[KGPU_SMALL_MAX_SLAVES];
+  bool cur_isb[KGPU_SMALL_MAX_SLAVES];
+  struct snap snap[ND][KGPU_SMALL_MAX_SLAVES];
+};
+
+static bool is_small(struct filter_in const *f) { return f && f->fwd_plan && *(bool const *)f->fwd_plan; }
+/* -1 with a message: `who` is not served on a small master (see create_filter_input_small) */
+static int small_refuses(char const *who) {
+  fprintf(stderr, "%s: not served on a master made by create_filter_input_small\n", who);
+  return -1;
+}
+
+/* the window bytes one launch sends: up to ND-1 consecutive blocks (fire_ready_blocks) */
+static size_t small_win_bytes(int L, int M, size_t esz) { return esz * ((size_t)(ND - 2) * (size_t)L + (size_t)(L + M - 1)); }
+/* output row pitch for slaves of at most `points` points each (olen <= points) */
+static long small_row_pitch(int nslaves, long points) { return ((long)nslaves * points + 3) / 4 * 4; }
+
+long filter_small_master_bytes(int L, int M, enum filtertype in_type, int max_slaves) {
+  if ((in_type != REAL && in_type != COMPLEX) || max_slaves < 0 || max_slaves > KGPU_SMALL_MAX_SLAVES ||
+      kgpu_small_smem(L, M, in_type == REAL ? KGPU_REAL : KGPU_COMPLEX) < 0)
+    return -1;
+  long const N = (long)L + M - 1, bins = in_type == COMPLEX ? N : N / 2 + 1, stride = (bins + 3) / 4 * 4;
+  size_t const esz = in_type == COMPLEX ? sizeof(float complex) : sizeof(float);
+  long const pitch = small_row_pitch(max_slaves, N); /* a slave of olen <= L has at most N points */
+  long const host = (long)sizeof(struct small_ctx) + (long)page_round((size_t)ND * (size_t)N * esz) /* float ring */
+                    + ND * bins * (long)sizeof(float complex)                                      /* fdomain[] */
+                    + ND * pitch * (long)sizeof(float complex)                                     /* output rows */
+                    + (long)max_slaves * N * (long)(sizeof(float complex) + sizeof(float complex) + 2 * sizeof(float complex));
+                    /* per slave: response, fdomain, own output buffer (upper bound) */
+  long const dev = (long)small_win_bytes(L, M, esz) + ND * stride * (long)sizeof(float complex) +
+                   ND * pitch * (long)sizeof(float complex) + (long)max_slaves * N * (long)sizeof(float complex);
+  return host + dev;
+}
+
+static void small_teardown(struct filter_in *master) {
+  struct small_ctx *c = (struct small_ctx *)master->fwd_plan;
+  cudaStreamSynchronize(c->st);
+  for (int i = 0; i < ND; i++)
+    cudaEventDestroy(c->done[i]);
+  cudaFree(c->d_win);
+  cudaFree(c->d_spec);
+  cudaFree(c->d_out);
+  cudaFreeHost(c->h_out);
+  kgpu_small_destroy(c->ks);
+  cudaStreamDestroy(c->st);
+  pthread_mutex_destroy(&c->mu);
+  free(c);
+  master->fwd_plan = NULL;
+}
+
+/* create_filter_input for a master one CTA serves (filter.c:186-269 semantics); -1 without touching *master outside
+ * the envelope of kgpu_small_smem */
+int create_filter_input_small(struct filter_in *master, int const L, int const M, enum filtertype const in_type) {
+  if (master == NULL || (in_type != REAL && in_type != COMPLEX) ||
+      kgpu_small_smem(L, M, in_type == REAL ? KGPU_REAL : KGPU_COMPLEX) < 0)
+    return -1;
+  if (master->init && is_small(master) && master->ilen == L && master->impulse_length == M && in_type == master->in_type)
+    return 0; /* unchanged (filter.c:191) */
+  struct small_ctx *c = calloc(1, sizeof *c);
+  if (!c)
+    return -1;
+  c->small = true;
+  c->ks = kgpu_small_create(L, M, in_type == REAL ? KGPU_REAL : KGPU_COMPLEX);
+  if (!c->ks) {
+    fprintf(stderr, "create_filter_input_small(L=%d M=%d): %s\n", L, M, kgpu_last_error());
+    free(c);
+    return -1;
+  }
+  if (master->init && master->fwd_plan)
+    master_teardown(master);
+  int const N = L + M - 1;
+  int const bins = (in_type == COMPLEX) ? N : N / 2 + 1;
+  c->esz = (in_type == COMPLEX) ? sizeof(float complex) : sizeof(float);
+  c->spec_stride = kgpu_small_spec_stride(c->ks);
+  pthread_mutex_init(&c->mu, NULL);
+  bool ok = cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking) == cudaSuccess;
+  ok = ok && cudaMalloc(&c->d_win, small_win_bytes(L, M, c->esz)) == cudaSuccess;
+  ok = ok && cudaMalloc((void **)&c->d_spec, sizeof(float complex) * (size_t)c->spec_stride * ND) == cudaSuccess;
+  for (int i = 0; ok && i < ND; i++)
+    ok = cudaEventCreateWithFlags(&c->done[i], cudaEventDisableTiming) == cudaSuccess;
+  master->fwd_plan = (fftwf_plan)c;
+  master->points = N;
+  master->perform_inline = (N_worker_threads == 0);
+  master->bins = bins;
+  master->ilen = L;
+  master->impulse_length = M;
+  master->in_type = in_type;
+  master->wcnt = 0;
+  master->next_jobnum = 0;
+  master->sample_index = 0;
+  for (int i = 0; i < ND; i++) { /* allocated for the caller's layout; no launch copies the spectrum back */
+    ok = ok && cudaHostAlloc((void **)&master->fdomain[i], sizeof(float complex) * (size_t)bins, cudaHostAllocPortable) ==
+                   cudaSuccess;
+    if (ok)
+      memset(master->fdomain[i], 0, sizeof(float complex) * (size_t)bins);
+    master->completed_jobs[i] = UINT_MAX; /* filter.c:214 */
+  }
+  master->input_buffer_size = page_round((size_t)ND * N * c->esz);
+  master->input_buffer = ok ? ring_alloc(master->input_buffer_size) : NULL;
+  ok = ok && master->input_buffer != NULL;
+  if (!ok) {
+    fprintf(stderr, "create_filter_input_small(L=%d M=%d): device/host allocation failed: %s\n", L, M,
+            cudaGetErrorString(cudaGetLastError()));
+    master_teardown(master);
+    return -1;
+  }
+  if (in_type == COMPLEX) { /* filter.c:243-244 */
+    master->input_read_pointer.c = master->input_buffer;
+    master->input_write_pointer.c = master->input_read_pointer.c + (M - 1);
+    master->input_read_pointer.r = master->input_write_pointer.r = NULL;
+  } else {
+    master->input_read_pointer.r = master->input_buffer;
+    master->input_write_pointer.r = master->input_read_pointer.r + (M - 1);
+    master->input_read_pointer.c = master->input_write_pointer.c = NULL;
+  }
+  if (!master->init) {
+    pthread_mutex_init(&master->filter_mutex, NULL);
+    pthread_cond_init(&master->filter_cond, NULL);
+    master->init = true;
+  }
+  master->owner = pthread_self();
+  return 0;
+}
+
+/* the output rows for the slaves now defined (c->mu held) */
+static int small_rows(struct small_ctx *c) {
+  long const need = kgpu_small_out_stride(c->ks);
+  if (need <= c->out_pitch)
+    return 0;
+  cudaStreamSynchronize(c->st);
+  cudaFree(c->d_out);
+  cudaFreeHost(c->h_out);
+  c->d_out = NULL;
+  c->h_out = NULL;
+  c->out_pitch = 0;
+  for (int s = 0; s < ND; s++)
+    for (int i = 0; i < KGPU_SMALL_MAX_SLAVES; i++)
+      c->snap[s][i].ok = false;
+  if (cudaMalloc((void **)&c->d_out, sizeof(float complex) * (size_t)need * ND) != cudaSuccess ||
+      cudaHostAlloc((void **)&c->h_out, sizeof(float complex) * (size_t)need * ND, cudaHostAllocPortable) != cudaSuccess)
+    return -1;
+  c->out_pitch = need;
+  return 0;
+}
+
+/* create_filter_output on a small master: a slot among its KGPU_SMALL_MAX_SLAVES (filter.c:298-415 semantics) */
+static int small_create_output(struct filter_out *slave, struct filter_in *master, int len, enum filtertype out_type) {
+  if (out_type != COMPLEX && out_type != REAL)
+    return small_refuses("create_filter_output (SPECTRUM)");
+  struct small_ctx *c = (struct small_ctx *)master->fwd_plan;
+  struct slave_ctx *sc = (struct slave_ctx *)slave->rev_plan;
+  if (slave->init && slave->master != master) /* a slave moves between masters only through delete_filter_output */
+    return -1;
+  if (!slave->init) {
+    pthread_mutex_init(&slave->response_mutex, NULL);
+    slave->init = true;
+  }
+  pthread_mutex_lock(&c->mu);
+  if (!sc) {
+    int idx = -1;
+    for (int i = 0; i < KGPU_SMALL_MAX_SLAVES && idx < 0; i++)
+      if (c->slots[i] == NULL)
+        idx = i;
+    if (idx < 0) {
+      pthread_mutex_unlock(&c->mu);
+      fprintf(stderr, "create_filter_output: a small master serves at most %d slaves\n", KGPU_SMALL_MAX_SLAVES);
+      return -1;
+    }
+    sc = calloc(1, sizeof *sc);
+    if (!sc) {
+      pthread_mutex_unlock(&c->mu);
+      return -1;
+    }
+    sc->idx = idx;
+    c->slots[idx] = slave;
+    slave->rev_plan = (fftwf_plan)sc;
+  }
+  cudaStreamSynchronize(c->st);
+  int const pts = kgpu_small_define(c->ks, sc->idx, len, out_type == REAL ? KGPU_REAL : KGPU_COMPLEX);
+  c->ver[sc->idx]++;
+  int const rows = pts > 0 ? small_rows(c) : 0;
+  pthread_mutex_unlock(&c->mu);
+  if (pts <= 0 || rows != 0) {
+    fprintf(stderr, "create_filter_output: %s\n", kgpu_last_error());
+    return -1;
+  }
+  pthread_mutex_lock(&slave->response_mutex);
+  free(slave->response);
+  slave->response = NULL;
+  pthread_mutex_unlock(&slave->response_mutex);
+  free(slave->fdomain);
+  free(sc->own);
+  slave->olen = len;
+  slave->points = pts;
+  slave->master = master;
+  slave->out_type = out_type;
+  set_filter_weights(slave, 1.0, 0.0);
+  slave->bins = out_type == COMPLEX ? pts : pts / 2 + 1;
+  size_t const osz = out_type == COMPLEX ? sizeof(float complex) : sizeof(float);
+  sc->own = cache_aligned(osz * (size_t)pts);
+  slave->fdomain = cache_aligned(sizeof(float complex) * (size_t)slave->bins);
+  if (!slave->fdomain || !sc->own)
+    return -1;
+  memset(sc->own, 0, osz * (size_t)pts);
+  if (out_type == COMPLEX) {
+    slave->output_buffer.c = sc->own;
+    slave->output.c = slave->output_buffer.c + slave->bins - len; /* filter.c:357 */
+    slave->output_buffer.r = slave->output.r = NULL;
+  } else {
+    slave->output_buffer.r = sc->own;
+    slave->output.r = slave->output_buffer.r + slave->points - len; /* filter.c:385 */
+    slave->output_buffer.c = slave->output.c = NULL;
+  }
+  slave->next_jobnum = master->next_jobnum;
+  return 0;
+}
+
+/* k consecutive blocks as one launch: the window's H2D (two copies at the ring's end), small_master_kernel, one D2H of
+ * the output rows, one event per block */
+static int small_execute(struct filter_in *const f, int const k) {
+  struct small_ctx *c = (struct small_ctx *)f->fwd_plan;
+  pthread_mutex_lock(&c->mu);
+  unsigned const jobnum = f->next_jobnum;
+  int const slot = (int)(jobnum % ND);
+  for (int j = 0; j < k; j++) { /* the slots' previous occupants (job - ND) must have drained */
+    cudaEventSynchronize(c->done[slot + j]);
+    for (int i = 0; i < KGPU_SMALL_MAX_SLAVES; i++)
+      c->snap[slot + j][i].ok = false;
+  }
+  void **const rp = f->in_type == COMPLEX ? (void **)&f->input_read_pointer.c : (void **)&f->input_read_pointer.r;
+  char const *const src = *rp;
+  *rp = (char *)*rp + c->esz * (size_t)f->ilen * (size_t)k;
+  kgf_ring_wrap(rp, f->input_buffer, f->input_buffer_size);
+  size_t const span = (size_t)(k - 1) * (size_t)f->ilen + (size_t)f->points;
+  float complex *spec = c->d_spec + (size_t)slot * (size_t)c->spec_stride;
+  float complex *d_row = c->d_out ? c->d_out + (size_t)slot * (size_t)c->out_pitch : NULL;
+  float complex *h_row = c->h_out ? c->h_out + (size_t)slot * (size_t)c->out_pitch : NULL;
+  int rc = 0;
+  if (window_h2d(c->d_win, src, c->esz * span, f->input_buffer, f->input_buffer_size, c->st) != 0)
+    rc = kgf_fail("execute_filter_input: H2D of the window");
+  /* a master without slaves still transforms: a slave created later recomputes from the stored spectrum */
+  float complex dummy_row;
+  if (rc == 0 && kgpu_small_run(c->ks, c->d_win, k, spec, d_row ? (void *)d_row : (void *)&dummy_row, c->out_pitch, -1, c->st) != 0)
+    rc = kgf_fail("execute_filter_input: kgpu_small_run");
+  if (rc == 0 && h_row &&
+      cudaMemcpyAsync(h_row, d_row, sizeof(float complex) * (size_t)(k * c->out_pitch), cudaMemcpyDeviceToHost, c->st) !=
+          cudaSuccess)
+    rc = kgf_fail("execute_filter_input: D2H of the outputs");
+  if (rc == 0)
+    for (int i = 0; i < KGPU_SMALL_MAX_SLAVES; i++) {
+      struct filter_out *o = c->slots[i];
+      if (!o || !o->response)
+        continue;
+      for (int j = 0; j < k; j++) {
+        struct snap *s = &c->snap[slot + j][i];
+        s->shift = c->cur_shift[i];
+        s->isb = c->cur_isb[i];
+        s->ver = c->ver[i];
+        s->off = kgpu_small_out_offset(c->ks, i);
+        s->ok = true;
+      }
+    }
+  for (int j = 0; j < k; j++)
+    cudaEventRecord(c->done[slot + j], c->st);
+  pthread_mutex_unlock(&c->mu);
+
+  pthread_mutex_lock(&f->filter_mutex);
+  f->owner = pthread_self();
+  for (int j = 0; j < k; j++) {
+    f->samples_by_job[slot + j] = f->sample_index;
+    f->completed_jobs[slot + j] = jobnum + (unsigned)j; /* "complete" == issued; consumers wait on the slot's event */
+    f->sample_index += (uint64_t)f->ilen;
+  }
+  f->next_jobnum += (unsigned)k;
+  pthread_cond_broadcast(&f->filter_cond);
+  pthread_mutex_unlock(&f->filter_mutex);
+  if (f->perform_inline)
+    cudaEventSynchronize(c->done[slot + k - 1]);
+  return rc;
 }
 
 /* ---------------------------------------------------------------- create_filter_input ------- */
@@ -508,6 +812,8 @@ int create_filter_output(struct filter_out *slave, struct filter_in *master, int
     return -1;
   if (slave->master == master && slave->olen == len && slave->out_type == out_type && slave->init)
     goto done;
+  if (is_small(master))
+    return small_create_output(slave, master, len, out_type);
   if (out_type == SPECTRUM)
     len = 0;
   struct master_ctx *c = (struct master_ctx *)master->fwd_plan;
@@ -1198,6 +1504,8 @@ static int launch_input(struct filter_in *f, struct master_ctx *c, int slot, int
 /* k consecutive blocks (jobs next_jobnum .. +k-1, ring slots without wrap) as one device launch sequence.
  * filter.c:558-651 (+ run_fft :485-555) */
 static int execute_filter_input_n(struct filter_in *const f, int const k) {
+  if (is_small(f))
+    return small_execute(f, k);
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
   pthread_mutex_lock(&c->mu);
   unsigned const jobnum = f->next_jobnum;
@@ -1515,6 +1823,52 @@ static int deliver(struct filter_out *slave, struct master_ctx *c, unsigned job,
   return rc;
 }
 
+/* Deliver job `job` of a small master to the slave: from the launch's output row if it used exactly these parameters,
+ * else that slave recomputed alone from the job's stored spectrum into its run of the row.  filter.c:703-921 */
+static int small_deliver(struct filter_out *slave, unsigned job, int shift) {
+  struct small_ctx *c = (struct small_ctx *)slave->master->fwd_plan;
+  if (cudaEventSynchronize(c->done[job % ND]) != cudaSuccess)
+    return kgf_fail("execute_filter_output: waiting for the block");
+  struct slave_ctx *sc = (struct slave_ctx *)slave->rev_plan;
+  if (sc == NULL || sc->own == NULL)
+    return -1;
+  if (slave->beam)
+    return small_refuses("execute_filter_output (beam)");
+  if (slave->response == NULL) /* no filter yet: leave the output alone (filter.c:715-718) */
+    return 0;
+  int const slot = (int)(job % ND), i = sc->idx;
+  size_t const obytes = (slave->out_type == REAL ? sizeof(float) : sizeof(float complex)) * (size_t)slave->olen;
+  int rc = 0;
+  pthread_mutex_lock(&c->mu);
+  struct snap *s = &c->snap[slot][i];
+  if (!(s->ok && s->shift == shift && s->ver == c->ver[i] && s->isb == slave->isb)) {
+    c->cur_shift[i] = shift; /* the next launches use them too */
+    c->cur_isb[i] = slave->isb;
+    long const off = kgpu_small_out_offset(c->ks, i);
+    float complex *d_row = c->d_out + (size_t)slot * (size_t)c->out_pitch;
+    if (kgpu_small_set_slave(c->ks, i, shift, slave->isb) != 0 ||
+        kgpu_small_run(c->ks, NULL, 1, c->d_spec + (size_t)slot * (size_t)c->spec_stride, d_row, c->out_pitch, i, c->st) != 0 ||
+        cudaMemcpyAsync(c->h_out + (size_t)slot * (size_t)c->out_pitch + off, d_row + off, obytes, cudaMemcpyDeviceToHost,
+                        c->st) != cudaSuccess ||
+        cudaStreamSynchronize(c->st) != cudaSuccess) {
+      rc = kgf_fail("execute_filter_output: recomputing the slave");
+    } else {
+      s->shift = shift;
+      s->isb = slave->isb;
+      s->ver = c->ver[i];
+      s->off = off;
+      s->ok = true;
+    }
+  }
+  if (rc == 0) {
+    own_output(slave, sc);
+    memcpy(slave->out_type == REAL ? (void *)slave->output.r : (void *)slave->output.c,
+           c->h_out + (size_t)slot * (size_t)c->out_pitch + s->off, obytes);
+  }
+  pthread_mutex_unlock(&c->mu);
+  return rc;
+}
+
 /* filter.c:663-921 */
 int execute_filter_output(struct filter_out *const slave, int const shift) {
   if (slave == NULL)
@@ -1527,6 +1881,8 @@ int execute_filter_output(struct filter_out *const slave, int const shift) {
   int const t = take_job(slave, master, &job);
   if (t != 0)
     return t < 0 ? -1 : 0;
+  if (c->small)
+    return small_deliver(slave, job, shift);
   if (cudaEventSynchronize(c->done[job % ND]) != cudaSuccess)
     return kgf_fail("execute_filter_output: waiting for the block");
   if (slave->out_type == SPECTRUM)
@@ -1555,6 +1911,11 @@ int execute_filter_output_batch(struct filter_out *const *slaves, int const *shi
     int const t = take_job(slave, slave->master, &job);
     if (t != 0) {
       if (t < 0)
+        rc = -1;
+      continue;
+    }
+    if (c->small) {
+      if (small_deliver(slave, job, shifts[i]) != 0)
         rc = -1;
       continue;
     }
@@ -1588,6 +1949,8 @@ int execute_filter_output_batch(struct filter_out *const *slaves, int const *shi
  * doppler_rate in Hz/s.  *bb_power receives chan->sig.bb_power.  The caller then skips its own step_osc loop. */
 int execute_filter_output_tuned(struct filter_out *slave, int shift, double remainder, double samprate, double doppler_rate,
                                 double *bb_power) {
+  if (slave && is_small(slave->master))
+    return small_refuses("execute_filter_output_tuned");
   if (slave == NULL || slave->master == NULL || slave->master->fwd_plan == NULL || !(samprate > 0))
     return -1;
   struct filter_in *master = slave->master;
@@ -1635,6 +1998,8 @@ int execute_filter_output_tuned(struct filter_out *slave, int shift, double rema
 }
 /* back to the plain filter.h behaviour for this slave */
 int filter_output_untune(struct filter_out *slave) {
+  if (slave && is_small(slave->master))
+    return small_refuses("filter_output_untune");
   if (slave == NULL || slave->master == NULL || slave->master->fwd_plan == NULL || slave->rev_plan == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
@@ -1654,6 +2019,8 @@ int filter_output_untune(struct filter_out *slave) {
  * device for all slaves; samprate = Frontend.samprate.  filter_noise_estimate() then returns the value for the block
  * the slave's last execute_filter_output delivered (NAN for a block that had to be recomputed alone). */
 int filter_input_enable_noise(struct filter_in *master, double samprate) {
+  if (is_small(master))
+    return small_refuses("filter_input_enable_noise");
   if (master == NULL || master->fwd_plan == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)master->fwd_plan;
@@ -1664,6 +2031,10 @@ int filter_input_enable_noise(struct filter_in *master, double samprate) {
   return 0;
 }
 double filter_noise_estimate(struct filter_out const *slave) {
+  if (slave && is_small(slave->master)) {
+    small_refuses("filter_noise_estimate");
+    return NAN;
+  }
   if (slave == NULL || slave->rev_plan == NULL)
     return NAN;
   return ((struct slave_ctx const *)slave->rev_plan)->last_n0;
@@ -1681,15 +2052,25 @@ int set_filter(struct filter_out *const slave, double low, double high, double c
   float complex *host = cache_aligned(sizeof(float complex) * (size_t)slave->points);
   if (!host)
     return -1;
-  pthread_mutex_lock(&c->mu);
-  /* only this master's pipeline stream is synchronised: a retune of one channel must not stall other masters
-   * (filter2 / wfm composite masters of other channel threads) the way a device-wide synchronisation would */
-  int rc = kgpu_bank_set_filter_on(c->bank, sc->idx, low, high, kaiser_beta, c->st);
-  if (rc == 0)
-    rc = kgpu_bank_get_response(c->bank, sc->idx, (float *)host) > 0 ? 0 : -1;
-  if (rc == 0)
-    c->ver[sc->idx]++;
-  pthread_mutex_unlock(&c->mu);
+  int rc;
+  if (c->small) {
+    struct small_ctx *k = (struct small_ctx *)c;
+    pthread_mutex_lock(&k->mu);
+    rc = kgpu_small_set_filter(k->ks, sc->idx, low, high, kaiser_beta, (float *)host, k->st);
+    if (rc == 0)
+      k->ver[sc->idx]++;
+    pthread_mutex_unlock(&k->mu);
+  } else {
+    pthread_mutex_lock(&c->mu);
+    /* only this master's pipeline stream is synchronised: a retune of one channel must not stall other masters
+     * (filter2 / wfm composite masters of other channel threads) the way a device-wide synchronisation would */
+    rc = kgpu_bank_set_filter_on(c->bank, sc->idx, low, high, kaiser_beta, c->st);
+    if (rc == 0)
+      rc = kgpu_bank_get_response(c->bank, sc->idx, (float *)host) > 0 ? 0 : -1;
+    if (rc == 0)
+      c->ver[sc->idx]++;
+    pthread_mutex_unlock(&c->mu);
+  }
   if (rc != 0) {
     free(host);
     return -1;
@@ -1714,6 +2095,8 @@ int set_filter_weights(struct filter_out *out, double complex i_weight, double c
 /* EXTENSION: wideband_poll (spectrum.c:308-522) on the device for a SPECTRUM slave.  fft_n floats of window, as
  * generate_window() leaves them.  -1 (and the CPU loop stays with the caller) for lengths the analyzer cannot serve. */
 int filter_spectrum_setup(struct filter_out *slave, int fft_n, int bin_count, float const *window) {
+  if (slave && is_small(slave->master))
+    return small_refuses("filter_spectrum_setup");
   if (slave == NULL || slave->out_type != SPECTRUM || slave->master == NULL || slave->master->fwd_plan == NULL ||
       window == NULL || bin_count < 1)
     return -1;
@@ -1756,6 +2139,8 @@ int filter_spectrum_setup(struct filter_out *slave, int fft_n, int bin_count, fl
  * (frontend->samples at spectrum.c:365 / :425).  bin_data: bin_count floats, as wideband_poll leaves them. */
 int filter_spectrum_poll(struct filter_out *slave, int shift, int fft_avg, double overlap, float *bin_data,
                          uint64_t *end_sample) {
+  if (slave && is_small(slave->master))
+    return small_refuses("filter_spectrum_poll");
   if (slave == NULL || slave->master == NULL || slave->master->fwd_plan == NULL || bin_data == NULL)
     return -1;
   struct filter_in *f = slave->master;
@@ -1795,6 +2180,8 @@ int filter_spectrum_poll(struct filter_out *slave, int shift, int fft_avg, doubl
 /* EXTENSION: narrowband_poll (spectrum.c:206-306) on the device for a COMPLEX slave.  fft_n floats of window, as
  * generate_window() leaves them.  -1 (and the CPU loop stays with the caller) when the device cannot serve the slave. */
 int filter_spectrum_narrow_setup(struct filter_out *slave, int fft_n, int bin_count, float const *window) {
+  if (slave && is_small(slave->master))
+    return small_refuses("filter_spectrum_narrow_setup");
   if (slave == NULL || slave->out_type != COMPLEX || slave->rev_plan == NULL || slave->master == NULL ||
       slave->master->fwd_plan == NULL || window == NULL || bin_count < 1 || bin_count > fft_n)
     return -1;
@@ -1833,6 +2220,8 @@ int filter_spectrum_narrow_setup(struct filter_out *slave, int fft_n, int bin_co
  * the write index at 0; a larger size keeps [0, old size), zeroes the rest and leaves the index; a smaller one does
  * nothing.  Call it where demod_spectrum would grow its ring, before downconvert() delivers the block. */
 int filter_spectrum_narrow_reserve(struct filter_out *slave, long ring_samples) {
+  if (slave && is_small(slave->master))
+    return small_refuses("filter_spectrum_narrow_reserve");
   if (slave == NULL || slave->rev_plan == NULL || slave->master == NULL || slave->master->fwd_plan == NULL ||
       ring_samples < 1)
     return -1;
@@ -1866,6 +2255,8 @@ int filter_spectrum_narrow_reserve(struct filter_out *slave, long ring_samples) 
  * bin_data, as narrowband_poll leaves them before its base / step scaling (spectrum.c:284-305), which stays with the
  * caller.  -1 before the first reserve.  One poller per slave. */
 int filter_spectrum_narrow_poll(struct filter_out *slave, int fft_avg, double overlap, float *bin_data) {
+  if (slave && is_small(slave->master))
+    return small_refuses("filter_spectrum_narrow_poll");
   if (slave == NULL || slave->rev_plan == NULL || slave->master == NULL || slave->master->fwd_plan == NULL ||
       bin_data == NULL)
     return -1;
@@ -1893,6 +2284,8 @@ int filter_spectrum_narrow_poll(struct filter_out *slave, int fft_avg, double ov
 /* EXTENSION: a host copy of the slave's ring (up to cap samples) with its size and write index, e.g. for a caller that
  * hands the analysis back to its CPU loop.  Returns the ring size, 0 before the first reserve, -1 on error. */
 long filter_spectrum_narrow_ring(struct filter_out *slave, float complex *ring, long cap, long *ring_idx) {
+  if (slave && is_small(slave->master))
+    return (long)small_refuses("filter_spectrum_narrow_ring");
   if (slave == NULL || slave->rev_plan == NULL || slave->master == NULL || slave->master->fwd_plan == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
@@ -1920,13 +2313,23 @@ int delete_filter_output(struct filter_out *slave) { /* filter.c:943-957 */
   if (slave == NULL)
     return -1;
   struct slave_ctx *sc = (struct slave_ctx *)slave->rev_plan;
-  if (slave->out_type == SPECTRUM && slave->master && slave->master->fwd_plan) {
+  if (sc && is_small(slave->master)) {
+    struct small_ctx *c = (struct small_ctx *)slave->master->fwd_plan;
+    pthread_mutex_lock(&c->mu);
+    cudaStreamSynchronize(c->st);
+    kgpu_small_undefine(c->ks, sc->idx);
+    c->slots[sc->idx] = NULL;
+    c->ver[sc->idx]++;
+    for (int s = 0; s < ND; s++)
+      c->snap[s][sc->idx].ok = false;
+    pthread_mutex_unlock(&c->mu);
+  } else if (slave->out_type == SPECTRUM && slave->master && slave->master->fwd_plan) {
     struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
     pthread_mutex_lock(&c->mu);
     spec_slave_drop(c, slave);
     pthread_mutex_unlock(&c->mu);
   }
-  if (sc && slave->master && slave->master->fwd_plan) {
+  if (sc && slave->master && slave->master->fwd_plan && !is_small(slave->master)) {
     struct master_ctx *c = (struct master_ctx *)slave->master->fwd_plan;
     pthread_mutex_lock(&c->mu);
     cudaStreamSynchronize(c->st);
@@ -1967,7 +2370,7 @@ int delete_filter_input(struct filter_in *master) { /* filter.c:930-942 */
 /* ---------------------------------------------------------------- write_*filter ------------- */
 /* filter.c:1093-1134: n floats or float pairs of esz bytes to the float ring at its write pointer *wp */
 static int write_floats(struct filter_in *f, void **wp, void const *buffer, int size, size_t esz, char const *who) {
-  if (f->fwd_plan == NULL || check_mode(f, (struct master_ctx *)f->fwd_plan, INGEST_FLOAT, false, who) != 0)
+  if (f->fwd_plan == NULL || (!is_small(f) && check_mode(f, (struct master_ctx *)f->fwd_plan, INGEST_FLOAT, false, who) != 0))
     return -1;
   if ((f->wcnt + size) * esz >= f->input_buffer_size)
     return -1;
@@ -1987,6 +2390,8 @@ int write_rfilter(struct filter_in *f, float const *buffer, int size) {
 /* EXTENSION: raw ADC words straight to the device; conversion (rx888.c:753-767) happens in fwd_cols.
  * samples == NULL: the caller already wrote them through filter_i16_write_pointer() (the zero-copy driver path). */
 int write_i16filter(struct filter_in *f, int16_t const *samples, int n, float scale, bool derandomize) {
+  if (is_small(f))
+    return small_refuses("write_i16filter");
   if (f == NULL || f->fwd_plan == NULL || n < 0)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
@@ -2009,6 +2414,10 @@ int write_i16filter(struct filter_in *f, int16_t const *samples, int n, float sc
 /* where a driver may deposit the next raw samples itself (mirrored, pinned ring: up to one block contiguous),
  * e.g. as the libusb transfer buffer of rx888.c:797-826; publish with write_i16filter(f, NULL, n, ...) */
 int16_t *filter_i16_write_pointer(struct filter_in *f) {
+  if (is_small(f)) {
+    small_refuses("filter_i16_write_pointer");
+    return NULL;
+  }
   if (f == NULL || f->fwd_plan == NULL)
     return NULL;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
@@ -2080,6 +2489,8 @@ static int raw_commit(struct filter_in *f, struct master_ctx *c, int n) {
  * airspyhf.c:292-325, fobos.c:395-426) get their buffers from their vendor libraries, so there is no zero-copy write
  * pointer: the bytes are copied into the raw ring. */
 int write_rawfilter(struct filter_in *f, void const *samples, int n, int format, double scale) {
+  if (is_small(f))
+    return small_refuses("write_rawfilter");
   if (f == NULL || f->fwd_plan == NULL || samples == NULL || n < 0)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
@@ -2092,6 +2503,8 @@ int write_rawfilter(struct filter_in *f, void const *samples, int n, int format,
 /* EXTENSION: SDRplay's separate I and Q arrays (sdrplay.c:1234-1246), interleaved into the FILTER_RAW_S16 ring: a copy
  * like write_rawfilter's memcpy, after which the pairs are an S16 write like any other. */
 int write_rawfilter_planar(struct filter_in *f, int16_t const *i, int16_t const *q, int n, double scale) {
+  if (is_small(f))
+    return small_refuses("write_rawfilter_planar");
   if (f == NULL || f->fwd_plan == NULL || i == NULL || q == NULL || n < 0)
     return -1;
   if (f->in_type != COMPLEX) {
@@ -2113,6 +2526,8 @@ int write_rawfilter_planar(struct filter_in *f, int16_t const *i, int16_t const 
  * include/ka9q_gpu_filter.h).  The slots about to be reused are folded in by execute_filter_input_n, which has already
  * waited for them; this call folds, in job order, whatever else has completed, without waiting. */
 int filter_ingest_stats(struct filter_in *f, struct filter_ingest_stats *stats) {
+  if (is_small(f))
+    return small_refuses("filter_ingest_stats");
   if (f == NULL || f->fwd_plan == NULL || stats == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
@@ -2148,6 +2563,8 @@ int filter_ingest_stats(struct filter_in *f, struct filter_ingest_stats *stats) 
 /* EXTENSION: HackRF's and FUNcube's DC and I/Q correction on the device (see include/ka9q_gpu_filter.h): the raw ring,
  * the table of writes and the initial coefficient set, before the first write. */
 int filter_iq_correction_setup(struct filter_in *f, int format, struct filter_iq_params const *p) {
+  if (is_small(f))
+    return small_refuses("filter_iq_correction_setup");
   struct raw_format const *rf = format_row(format);
   if (f == NULL || f->fwd_plan == NULL || p == NULL || rf == NULL || rf->path != RAW_IQ)
     return -1;
@@ -2175,6 +2592,8 @@ int filter_iq_correction_setup(struct filter_in *f, int format, struct filter_iq
  * about to be reused are taken in by execute_filter_input_n, which has already waited for them; this call takes in, in
  * job order, whatever else has completed, without waiting. */
 int filter_iq_records(struct filter_in *f, struct filter_iq_record *recs, int max) {
+  if (is_small(f))
+    return small_refuses("filter_iq_records");
   if (f == NULL || f->fwd_plan == NULL || (recs == NULL && max > 0))
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
@@ -2215,6 +2634,8 @@ int filter_iq_records(struct filter_in *f, struct filter_iq_record *recs, int ma
 /* ---------------------------------------------------------------- sig_gen ------------------- */
 /* EXTENSION: sig_gen's source on the device (see include/ka9q_gpu_filter.h), before the first write. */
 int filter_siggen_setup(struct filter_in *f, struct filter_siggen_params const *p) {
+  if (is_small(f))
+    return small_refuses("filter_siggen_setup");
   if (f == NULL || f->fwd_plan == NULL || p == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
@@ -2241,6 +2662,8 @@ int filter_siggen_setup(struct filter_in *f, struct filter_siggen_params const *
 /* EXTENSION: advance a generated master by n samples (REAL) or pairs (COMPLEX), stored with this write's scale; fires
  * the blocks they complete as write_rfilter does. */
 int write_genfilter(struct filter_in *f, int n, double scale) {
+  if (is_small(f))
+    return small_refuses("write_genfilter");
   if (f == NULL || f->fwd_plan == NULL || n < 0)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
@@ -2264,6 +2687,8 @@ int write_genfilter(struct filter_in *f, int n, double scale) {
  * regenerates them), plus the largest write that may be pending or being written behind them; the device window of
  * the envelope is d_raw, sized as raw_start sizes it. */
 int filter_siggen_modulate(struct filter_in *f, double dc) {
+  if (is_small(f))
+    return small_refuses("filter_siggen_modulate");
   if (f == NULL || f->fwd_plan == NULL || !isfinite(dc))
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
@@ -2293,6 +2718,10 @@ int filter_siggen_modulate(struct filter_in *f, double dc) {
 }
 
 float *filter_siggen_mod_pointer(struct filter_in *f) {
+  if (is_small(f)) {
+    small_refuses("filter_siggen_mod_pointer");
+    return NULL;
+  }
   if (f == NULL || f->fwd_plan == NULL)
     return NULL;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;
@@ -2302,6 +2731,8 @@ float *filter_siggen_mod_pointer(struct filter_in *f) {
 /* EXTENSION: the generated energy of the blocks whose device work completed since the previous call, as
  * filter_ingest_stats counts them. */
 int filter_siggen_stats(struct filter_in *f, struct filter_siggen_stats *stats) {
+  if (is_small(f))
+    return small_refuses("filter_siggen_stats");
   if (f == NULL || f->fwd_plan == NULL || stats == NULL)
     return -1;
   struct master_ctx *c = (struct master_ctx *)f->fwd_plan;

@@ -20,6 +20,7 @@
 #include "chan_kernels.cuh"
 #include "chan_huge.cuh"
 #include "chan_wide.cuh"
+#include "small_master.cuh"
 #include "fwd_kernels.cuh"
 #include "noise_kernel.cuh"
 #include "plan.cuh"
@@ -2084,8 +2085,9 @@ static void *bank_scratch(kgpu_bank *b, cudaStream_t st, size_t bytes) {
   return grow(s, bytes, st, "bank scratch") ? nullptr : s.p;
 }
 
-static void resolve_walk(kgpu_master const *m, ChanHost const &c, ChanDesc &d) {
-  int const ns = c.points, mb = m->bins, half = ns / 2;
+// in_type, mb: the master's type and bins
+static void resolve_walk(int in_type, int mb, ChanHost const &c, ChanDesc &d) {
+  int const ns = c.points, half = ns / 2;
   long const shift = c.shift;
   d.zlead = 0;
   d.ncopy = 0;
@@ -2096,7 +2098,7 @@ static void resolve_walk(kgpu_master const *m, ChanHost const &c, ChanDesc &d) {
     d.ncopy = 1;
     return;
   }
-  if (m->in_type == KGPU_REAL) {
+  if (in_type == KGPU_REAL) {
     if (shift >= 0) {  // filter.c:819-855
       long const start = shift - half;
       long const z = std::min<long>(std::max<long>(0, -start), ns);
@@ -2161,7 +2163,7 @@ static int bank_commit(kgpu_bank *b, cudaStream_t st) {
     off += c.real_out ? (c.olen + 1) / 2 : c.olen;
     if (c.enabled && c.has_response) {
       d.plan = c.geom->plan;
-      resolve_walk(b->m, c, d);
+      resolve_walk(b->m->in_type, b->m->bins, c, d);
       b->max_points = std::max(b->max_points, c.points);
     }
   }
@@ -2316,6 +2318,38 @@ extern "C" int kgpu_bank_define_any(kgpu_bank *b, int idx, int olen, int out_typ
   return bank_define("kgpu_bank_define_any", b, idx, olen, out_type, CP_BLUESTEIN);
 }
 
+// The forward transform of one response in place on stream st (set_filter's fftwf_execute, filter.c:1030), for the paths
+// whose transform runs in one CTA: direct, wide and extended.  1: another path (the caller's own code).
+static int response_transform_cta(float2 *dst, ChanGeom const &g, int points, cudaStream_t st) {
+  size_t const sm = sizeof(float2) * (size_t)points;  // the narrow paths' transform in shared memory
+  switch (g.r.path) {
+    case CP_DIRECT:
+      if (allow_smem((const void *)response_fft_kernel, sm)) return -1;
+      response_fft_kernel<<<1, 32, sm, st>>>(dst, g.plan);
+      break;
+    case CP_WIDE: {
+      size_t const smw = (size_t)wide_smem_bytes(g.wide.n1, g.wide.n2);
+      if (allow_smem((const void *)response_wide_kernel, smw)) return -1;
+      response_wide_kernel<<<1, kWideThreads, smw, st>>>(dst, g.wide);
+      break;
+    }
+    case CP_EXTENDED:
+      if (g.r.narrow) {
+        if (allow_smem((const void *)response_fft_ext, sm)) return -1;
+        response_fft_ext<<<1, 32, sm, st>>>(dst, g.ext);
+      } else {
+        size_t const smw = (size_t)wide_smem_bytes(g.wide_ext.g.n1, g.wide_ext.g.n2);
+        if (allow_smem((const void *)response_wide_ext, smw)) return -1;
+        response_wide_ext<<<1, kWideThreads, smw, st>>>(dst, g.wide_ext);
+      }
+      break;
+    default:
+      return 1;
+  }
+  g_launches++;
+  return 0;
+}
+
 // st == nullptr: legacy entry points, whole-device synchronisation (any stream may be using the response);
 // otherwise only `st` is synchronised: the caller guarantees that every launch reading this bank is ordered on it
 static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *host, bool transform, cudaStream_t st = nullptr,
@@ -2328,20 +2362,12 @@ static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *ho
   CUDA_OK(cudaMemcpyAsync(dst, host, sizeof(float2) * (size_t)c.points, cudaMemcpyHostToDevice, st));
   if (transform) {
     ChanGeom const &g = *c.geom;
-    size_t const sm = sizeof(float2) * (size_t)c.points;  // the narrow paths' transform in shared memory
     switch (g.r.path) {
       case CP_DIRECT:
-        if (allow_smem((const void *)response_fft_kernel, sm)) return -1;
-        response_fft_kernel<<<1, 32, sm, st>>>(dst, g.plan);
-        g_launches++;
+      case CP_WIDE:
+      case CP_EXTENDED:
+        if (response_transform_cta(dst, g, c.points, st)) return -1;
         break;
-      case CP_WIDE: {
-        size_t const smw = (size_t)wide_smem_bytes(g.wide.n1, g.wide.n2);
-        if (allow_smem((const void *)response_wide_kernel, smw)) return -1;
-        response_wide_kernel<<<1, kWideThreads, smw, st>>>(dst, g.wide);
-        g_launches++;
-        break;
-      }
       case CP_HUGE: {
         float2 *scr = (float2 *)bank_scratch(b, st, sizeof(float2) * (size_t)c.points);
         if (!scr) return -1;
@@ -2352,17 +2378,6 @@ static int upload_taps_and_transform(kgpu_bank *b, ChanHost &c, float2 const *ho
         g_launches += 2;
         break;
       }
-      case CP_EXTENDED:
-        if (g.r.narrow) {
-          if (allow_smem((const void *)response_fft_ext, sm)) return -1;
-          response_fft_ext<<<1, 32, sm, st>>>(dst, g.ext);
-        } else {
-          size_t const smw = (size_t)wide_smem_bytes(g.wide_ext.g.n1, g.wide_ext.g.n2);
-          if (allow_smem((const void *)response_wide_ext, smw)) return -1;
-          response_wide_ext<<<1, kWideThreads, smw, st>>>(dst, g.wide_ext);
-        }
-        g_launches++;
-        break;
       case CP_BLUESTEIN: {  // one block of the masters' chain: a COMPLEX master of `points` with hop 0, in place
         kgpu_master *im = bank_bluestein_master(b, st, g.r.blue.P);
         if (!im) return -1;
@@ -2782,6 +2797,217 @@ extern "C" int kgpu_bank_fm_front(kgpu_bank *b, const void *d_out, long out_pitc
 extern "C" int kgpu_bank_commit(kgpu_bank *b, void *stream) {
   if (!b) return fail("kgpu_bank_commit: bad arguments");
   return bank_commit(b, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------ small masters -------------
+// A master whose forward transform and every slave's inverse fit one CTA (small_master.cuh): radiod's per-channel
+// secondary masters.  It owns its slaves' responses and geometry; the caller (filter_abi.c) owns the ring, the spectrum
+// slots and the output rows.  No bank: each launch passes every slave's walk by value.
+struct SmallSlaveHost {
+  bool defined = false, real_out = false, has_response = false, isb = false;
+  int olen = 0, points = 0, shift = 0;
+  WideGeom const *g = nullptr;  // the inverse's four-step geometry
+  float2 *d_resp = nullptr;     // points float2
+};
+struct kgpu_small {
+  int L, M, N, in_type, bins, nc;
+  long spec_stride;
+  WideGeom const *fg;
+  SmallSlaveHost s[kSmallMaxSlaves];
+};
+
+// A length one CTA transforms: factors 2, 3, 5, 7, at most kMaxWideChanPoints, a four-step split that fits shared memory.
+// The shared memory it needs, or -1.  Host only.
+static long small_len_smem(long n) {
+  Split2 sp;
+  if (n < 2 || n > kMaxWideChanPoints || !smooth7(n) || !choose_split(n, &sp) || sp.n1 < 2 || sp.n2 < 2) return -1;
+  long const bytes = wide_smem_bytes(sp.n1, sp.n2);
+  return bytes <= kChanSmemLimit ? bytes : -1;
+}
+// The four-step geometry of a length small_len_smem accepts, per device, built once and never freed (like g_geom).
+static WideGeom const *small_geom(int points) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) {
+    fail("cudaGetDevice: %s", cudaGetErrorString(cudaGetLastError()));
+    return nullptr;
+  }
+  static std::mutex mu;
+  static std::map<std::pair<int, int>, WideGeom> geoms;
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = geoms.find({dev, points});
+  if (it != geoms.end()) return &it->second;
+  Split2 sp;
+  if (small_len_smem(points) < 0 || !choose_split(points, &sp)) {
+    fail("%d points: not a one-CTA transform length", points);
+    return nullptr;
+  }
+  WideGeom g{sp.n1, sp.n2, wide_pitch(sp.n2), get_tile_plan(sp.n1), get_tile_plan(sp.n2), nullptr};
+  if (g.plan1 < 0 || g.plan2 < 0 || wide_twiddles(g, *host_tile_plan(g.plan2))) return nullptr;
+  return &(geoms[{dev, points}] = g);
+}
+
+extern "C" long kgpu_small_smem(int L, int M, int in_type) {
+  if (L < 1 || M < 1 || (in_type != KGPU_REAL && in_type != KGPU_COMPLEX)) return -1;
+  long const N = (long)L + M - 1;
+  if (in_type == KGPU_REAL && ((L & 1) || (N & 1))) return -1;
+  return small_len_smem(in_type == KGPU_REAL ? N / 2 : N);
+}
+
+extern "C" kgpu_small *kgpu_small_create(int L, int M, int in_type) {
+  if (kgpu_small_smem(L, M, in_type) < 0) {
+    fail("kgpu_small_create(L=%d M=%d): outside the one-CTA envelope (Nc with factors 2, 3, 5, 7, at most %d points)", L, M,
+         kMaxWideChanPoints);
+    return nullptr;
+  }
+  kgpu_small *m = new kgpu_small;
+  m->L = L;
+  m->M = M;
+  m->N = L + M - 1;
+  m->in_type = in_type;
+  m->bins = in_type == KGPU_COMPLEX ? m->N : m->N / 2 + 1;
+  m->nc = in_type == KGPU_COMPLEX ? m->N : m->N / 2;
+  m->spec_stride = ((long)m->bins + 3) / 4 * 4;
+  m->fg = small_geom(m->nc);
+  if (!m->fg) {
+    delete m;
+    return nullptr;
+  }
+  return m;
+}
+extern "C" void kgpu_small_destroy(kgpu_small *m) {
+  if (!m) return;
+  for (auto &s : m->s) cudaFree(s.d_resp);
+  delete m;
+}
+extern "C" long kgpu_small_spec_stride(kgpu_small const *m) { return m ? m->spec_stride : -1; }
+
+static bool small_bad(kgpu_small const *m, int idx) { return !m || idx < 0 || idx >= kSmallMaxSlaves; }
+
+extern "C" int kgpu_small_define(kgpu_small *m, int idx, int olen, int out_type) {
+  if (small_bad(m, idx) || olen < 1 || (out_type != KGPU_COMPLEX && out_type != KGPU_REAL))
+    return fail("kgpu_small_define: bad arguments");
+  long const num = (long)olen * m->N;
+  if (num % m->L) return fail("invalid output length %d for N=%d L=%d (filter.c:312-316)", olen, m->N, m->L);
+  int const points = (int)(num / m->L);
+  if (out_type == KGPU_REAL && (points & 1))
+    return fail("kgpu_small_define: REAL-output slaves need an even number of points (got %d)", points);
+  WideGeom const *g = small_geom(points);
+  if (!g) return fail("kgpu_small_define: %d-point slave is outside the one-CTA envelope", points);
+  SmallSlaveHost &s = m->s[idx];
+  if (!(s.defined && s.points == points)) {
+    cudaFree(s.d_resp);
+    s.d_resp = nullptr;
+    CUDA_OK(cudaMalloc(&s.d_resp, sizeof(float2) * (size_t)points));
+    s.has_response = false;
+  }
+  s.defined = true;
+  s.real_out = out_type == KGPU_REAL;
+  s.olen = olen;
+  s.points = points;
+  s.g = g;
+  return points;
+}
+extern "C" int kgpu_small_undefine(kgpu_small *m, int idx) {
+  if (small_bad(m, idx)) return fail("kgpu_small_undefine: bad arguments");
+  cudaFree(m->s[idx].d_resp);
+  m->s[idx] = SmallSlaveHost{};
+  return 0;
+}
+
+// set_filter for slave idx on stream st: the bank's Kaiser design and response transform (bitwise the bank's response),
+// copied to `response` (points float2).  Waits for st before the swap: queued launches may still read the old one.
+extern "C" int kgpu_small_set_filter(kgpu_small *m, int idx, double low, double high, double kaiser_beta, float *response,
+                                     void *stream) {
+  if (small_bad(m, idx) || !m->s[idx].defined || !response) return fail("kgpu_small_set_filter: slave not defined");
+  SmallSlaveHost &s = m->s[idx];
+  cudaStream_t const st = (cudaStream_t)stream;
+  if (s.real_out) {  // filter edges may not cross DC for a real output (filter.c:971-975)
+    low = fabs(low);
+    high = fabs(high);
+  }
+  std::vector<float2> taps;
+  if (design_taps(s.points, s.olen, m->N, m->in_type == KGPU_REAL, low, high, kaiser_beta, taps))
+    return fail("kgpu_small_set_filter: rejected (NaN or M < 2), cf. filter.c:969,989");
+  ChanRoute r;
+  if (chan_route(s.points, CP_EXTENDED, "kgpu_small_set_filter", &r)) return -1;
+  ChanGeom const *g = chan_geom(s.points, r);
+  if (!g) return -1;
+  CUDA_OK(cudaStreamSynchronize(st));
+  CUDA_OK(cudaMemcpyAsync(s.d_resp, taps.data(), sizeof(float2) * taps.size(), cudaMemcpyHostToDevice, st));
+  if (response_transform_cta(s.d_resp, *g, s.points, st)) return fail("kgpu_small_set_filter: no one-CTA response transform");
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaMemcpyAsync(response, s.d_resp, sizeof(float2) * (size_t)s.points, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  s.has_response = true;
+  return 0;
+}
+extern "C" int kgpu_small_set_slave(kgpu_small *m, int idx, int shift, int isb) {
+  if (small_bad(m, idx) || !m->s[idx].defined) return fail("kgpu_small_set_slave: slave not defined");
+  m->s[idx].shift = shift;
+  m->s[idx].isb = isb != 0;
+  return 0;
+}
+// Output rows: slave i's olen float2 (COMPLEX) or olen floats in (olen + 1) / 2 float2 (REAL) at kgpu_small_out_offset,
+// in slave order; a row is kgpu_small_out_stride float2.
+extern "C" long kgpu_small_out_offset(kgpu_small const *m, int idx) {
+  if (small_bad(m, idx)) return -1;
+  long off = 0;
+  for (int i = 0; i < idx; i++)
+    if (m->s[i].defined) off += m->s[i].real_out ? (m->s[i].olen + 1) / 2 : m->s[i].olen;
+  return off;
+}
+extern "C" long kgpu_small_out_stride(kgpu_small const *m) {
+  if (!m) return -1;
+  long off = 0;
+  for (auto const &s : m->s)
+    if (s.defined) off += s.real_out ? (s.olen + 1) / 2 : s.olen;
+  return (off + 3) / 4 * 4;
+}
+
+extern "C" int kgpu_small_run(kgpu_small *m, const void *d_win, int nblocks, void *d_spec, void *d_out, long out_pitch, int only,
+                              void *stream) {
+  if (!m || nblocks < 1 || !d_spec || !d_out || only >= kSmallMaxSlaves || (only < 0 && !d_win))
+    return fail("kgpu_small_run: bad arguments");
+  SmallArgs a{};
+  a.in = d_win;
+  a.hop = m->in_type == KGPU_REAL ? m->L / 2 : m->L;
+  a.fg = *m->fg;
+  a.real = m->in_type == KGPU_REAL;
+  a.spec = (float2 *)d_spec;
+  a.spec_stride = m->spec_stride;
+  a.m_bins = m->bins;
+  a.out = (float2 *)d_out;
+  a.out_stride = out_pitch;
+  a.nslaves = kSmallMaxSlaves;
+  a.only = only;
+  long smem = only < 0 ? wide_smem_bytes(a.fg.n1, a.fg.n2) : 0, off = 0;
+  for (int i = 0; i < kSmallMaxSlaves; i++) {
+    SmallSlaveHost const &h = m->s[i];
+    SmallSlave &s = a.s[i];
+    s.d.plan = -1;
+    if (!h.defined) continue;
+    s.d.out_off = off;
+    off += h.real_out ? (h.olen + 1) / 2 : h.olen;
+    if (!h.has_response || (only >= 0 && i != only)) continue;
+    ChanHost c;
+    c.points = h.points;
+    c.shift = h.shift;
+    c.real_out = h.real_out;
+    resolve_walk(m->in_type, m->bins, c, s.d);
+    s.d.plan = 0;
+    s.d.points = h.points;
+    s.d.olen = h.olen;
+    s.d.flags = h.real_out ? kChanRealOut : (h.isb ? kChanIsb : 0);
+    s.g = *h.g;
+    s.resp = h.d_resp;
+    smem = std::max(smem, wide_smem_bytes(h.g->n1, h.g->n2));
+  }
+  if (only >= 0 && a.s[only].d.plan < 0) return fail("kgpu_small_run: slave %d has no response", only);
+  if (allow_smem((const void *)small_master_kernel, (size_t)smem)) return -1;
+  small_master_kernel<<<(unsigned)nblocks, kWideThreads, (size_t)smem, (cudaStream_t)stream>>>(a);
+  g_launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
 }
 
 // pure host helpers (usable without a GPU): what the planner would pick
